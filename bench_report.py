@@ -209,7 +209,9 @@ def config_rows(torch, lib, dev, flush, peak, kind, world=1, rank=0, reps=10, fu
     ms = timeit(torch, flush, lambda: lib.pn2_gather_point(1, 1, 1, one.data_ptr(), onei.data_ptr(), oneo.data_ptr(), None), reps=max(reps, 9))
     add("harness", "timing floor: a 1-thread kernel under the same event pair + L2 flush", ms, 28)
 
-    def sa_layer(tag, xyz, feats, m, r, s, xyz_first=True):
+    BF16 = 1  # PN2_BF16
+
+    def sa_layer(tag, xyz, feats, m, r, s, xyz_first=True, bf16_rows=False):
         b, n, _ = xyz.shape
         fi = torch.empty((b, m), dtype=torch.int32, device=dev)
         nx = torch.empty((b, m, 3), dtype=torch.float32, device=dev)
@@ -247,6 +249,12 @@ def config_rows(torch, lib, dev, flush, peak, kind, world=1, rank=0, reps=10, fu
             ms = timeit(torch, flush, lambda: lib.pn2_group_point(b, n, c, m, s, feats.data_ptr(), idx.data_ptr(), gf.data_ptr(), None), reps=reps)
             add(tag, f"group_point C={c} S={s}", ms, W.bytes_group(b, n, m, s, c))
             del gf
+        if c and full and bf16_rows:  # the same gather on bfloat16 features
+            fh = feats.to(torch.bfloat16)
+            gh = torch.empty((b, m, s, c), dtype=torch.bfloat16, device=dev)
+            ms = timeit(torch, flush, lambda: lib.pn2_group_point_typed(BF16, b, n, c, m, s, fh.data_ptr(), idx.data_ptr(), gh.data_ptr(), None), reps=reps)
+            add(tag, f"group_point bf16 C={c} S={s}", ms, W.bytes_group(b, n, m, s, c, esz=2))
+            del gh
         if c and full:  # backward of the gather: atomic scatter-add (the caller's zero-fill is part of the op)
             go = torch.randn((b, m, s, c), dtype=torch.float32, device=dev)
             gp = torch.empty((b, n, c), dtype=torch.float32, device=dev)
@@ -262,6 +270,13 @@ def config_rows(torch, lib, dev, flush, peak, kind, world=1, rank=0, reps=10, fu
             ms = timeit(torch, flush, lambda: lib.pn2_group_concat(b, n, c, m, s, xyz.data_ptr(), nx.data_ptr(), feats.data_ptr(),
                                                                    idx.data_ptr(), 1 if xyz_first else 0, out.data_ptr(), None, None), reps=reps)
             add(tag, f"group_concat (fused tail) C={c}+3 S={s}", ms, 4 * b * m * s + 4 * b * min(n, m * s) * (c + 3) + 4 * b * m * s * (c + 3))
+            del out
+            if full and bf16_rows:
+                oh = torch.empty((b, m, s, 3 + c), dtype=torch.bfloat16, device=dev)
+                ms = timeit(torch, flush, lambda: lib.pn2_group_concat_typed(BF16, b, n, c, m, s, xyz.data_ptr(), nx.data_ptr(), fh.data_ptr(),
+                                                                             idx.data_ptr(), 1 if xyz_first else 0, oh.data_ptr(), None, None), reps=reps)
+                add(tag, f"group_concat (fused tail) bf16 C={c}+3 S={s}", ms, W.bytes_group_concat(b, n, m, s, c, esz=2))
+                del oh, fh
         return nx
 
     # cfg2 in the three input distributions (the driver line's own workload: --report only)
@@ -278,7 +293,7 @@ def config_rows(torch, lib, dev, flush, peak, kind, world=1, rank=0, reps=10, fu
         nx1 = sa_layer("cfg3.L1", xyz, None, L1["npoint"], r, s, xyz_first=False)
     feats = T(W.features(c3["b"], L1["npoint"], L2["c"], 103))
     for r, s in zip(L2["radii"], L2["nsamples"]):
-        sa_layer("cfg3.L2", nx1, feats, L2["npoint"], r, s, xyz_first=False)
+        sa_layer("cfg3.L2", nx1, feats, L2["npoint"], r, s, xyz_first=False, bf16_rows=True)
 
     def msg_layer(tag, x, L):
         """One pn2_sa_layer_msg_device call: the sampling pass + all three scales' ball query and xyz grouping."""
@@ -345,6 +360,27 @@ def config_rows(torch, lib, dev, flush, peak, kind, world=1, rank=0, reps=10, fu
                         2 * 4 * b * m_ * c_ + 24 * b * n_ + 4 * b * n_ * c_)
             ms = timeit(torch, flush, lambda: lib.pn2_three_nn_interpolate(b, n_, m_, c_, x1.data_ptr(), x2.data_ptr(), p2.data_ptr(), o.data_ptr(), None, None, None, None), reps=reps)
             add(f"cfg4[B={b}].FP{n_}<-{m_}", f"three_nn_interpolate (fused) C={c_}", ms, 12 * b * n_ + 12 * b * m_ + 4 * b * m_ * c_ + 4 * b * n_ * c_)
+            if full:  # bfloat16 features beside float32: three_interpolate, its deterministic gradient, the FP front end
+                tag4 = f"cfg4[B={b}].FP{n_}<-{m_}"
+                p2h, goh = p2.to(torch.bfloat16), go.to(torch.bfloat16)
+                oh = torch.empty((b, n_, c_), dtype=torch.bfloat16, device=dev)
+                gph = torch.empty((b, m_, c_), dtype=torch.bfloat16, device=dev)
+                ms = timeit(torch, flush, lambda: lib.pn2_three_interpolate_typed(BF16, b, m_, c_, n_, p2h.data_ptr(), i.data_ptr(), w.data_ptr(), oh.data_ptr(), None), reps=reps)
+                add(tag4, f"three_interpolate bf16 C={c_}", ms, W.bytes_three_interpolate(b, n_, m_, c_, esz=2))
+                ms = timeit(torch, flush, lambda: lib.pn2_three_interpolate_grad_det_typed(BF16, b, n_, c_, m_, goh.data_ptr(), i.data_ptr(), w.data_ptr(),
+                                                                                           gph.data_ptr(), dw.data_ptr(), dwb, None), reps=reps)
+                add(tag4, f"three_interpolate_grad bf16 C={c_} (deterministic, inverse index)", ms, W.bytes_three_interpolate_grad(b, n_, m_, c_, esz=2))
+                # points1: the dense level's own features, as the sem-seg network feeds them (none at the input level)
+                c1 = c4["sa"][next(k for k, lv in enumerate(levels) if lv is x1)]["c"]
+                for dt, code, esz, name in ((torch.float32, 0, 4, ""), (torch.bfloat16, BF16, 2, " bf16")):
+                    p1 = T(W.features(b, n_, c1, 106)).to(dt) if c1 else None
+                    p2d = p2 if dt == torch.float32 else p2h
+                    of = torch.empty((b, n_, c_ + c1), dtype=dt, device=dev)
+                    ms = timeit(torch, flush, lambda: lib.pn2_fp_interpolate_concat_typed(code, b, n_, m_, c_, c1, x1.data_ptr(), x2.data_ptr(),
+                                                                                          p1.data_ptr() if c1 else None, p2d.data_ptr(), of.data_ptr(), None), reps=reps)
+                    add(tag4, f"fp_interpolate_concat{name} C={c_}+{c1}", ms, W.bytes_fp_interpolate_concat(b, n_, m_, c_, c1, esz=esz))
+                    del p1, of
+                del p2h, goh, oh, gph
     if full:
         # n3: knn_point at cfg2's shape — one tiled top-k kernel against the reference's composite
         # (materialised (b,m,n) matrix + selection sort of whole rows, here as torch ops + pn2_selection_sort)

@@ -182,6 +182,43 @@ int pn2_three_nn_interpolate(int b, int n, int m, int c, const float* xyz1, cons
 int pn2_fp_interpolate_concat(int b, int n, int m, int c2, int c1, const float* xyz1, const float* xyz2,
                               const float* points1, const float* points2, float* out, void* stream);
 
+/* ---- 16-bit features (mixed precision) ----------------------------------------------------------
+ * The ops that carry FEATURES also take bfloat16 or float16 feature tensors.  Each typed entry point
+ * takes the feature element type as its first argument and otherwise the arguments of the untyped entry
+ * of the same name, feature pointers as void*.  Coordinates, weights, distances and indices stay
+ * float32 / int32.  Arithmetic is float32: features are upcast exactly, every result is the float32
+ * result of the untyped op rounded once (round to nearest even) to the feature type, and copied
+ * features are copied bit for bit.  With PN2_F32 a typed entry computes exactly what the untyped one
+ * does.  An unknown dtype code or a NULL tensor returns cudaErrorInvalidValue without a launch. */
+#define PN2_F32 0
+#define PN2_BF16 1
+#define PN2_F16 2
+
+int pn2_group_point_typed(int dtype, int b, int n, int c, int m, int nsample, const void* points, const int* idx,
+                          void* out, void* stream);
+/* The scatter-add runs into `accum` (b,n,c) float32, zero-filled by the caller; grad_points (b,n,c) in `dtype`
+ * then receives accum rounded once.  accum may be NULL for PN2_F32 (grad_points is accumulated into, zero-filled
+ * by the caller, as in pn2_group_point_grad). */
+int pn2_group_point_grad_typed(int dtype, int b, int n, int c, int m, int nsample, const void* grad_out,
+                               const int* idx, void* grad_points, float* accum, void* stream);
+/* points and out in `dtype`; the xyz channels of out are the float32 differences rounded once;
+ * grouped_xyz stays float32. */
+int pn2_group_concat_typed(int dtype, int b, int n, int c, int m, int nsample, const float* xyz,
+                           const float* new_xyz, const void* points, const int* idx, int xyz_first, void* out,
+                           float* grouped_xyz, void* stream);
+int pn2_three_interpolate_typed(int dtype, int b, int m, int c, int n, const void* points, const int* idx,
+                                const float* weight, void* out, void* stream);
+/* workspace: pn2_three_interpolate_grad_det_workspace_bytes(b, n, m), as for the untyped entry */
+int pn2_three_interpolate_grad_det_typed(int dtype, int b, int n, int c, int m, const void* grad_out,
+                                         const int* idx, const float* weight, void* grad_points, void* workspace,
+                                         size_t workspace_bytes, void* stream);
+int pn2_three_nn_interpolate_typed(int dtype, int b, int n, int m, int c, const float* xyz1, const float* xyz2,
+                                   const void* points2, void* out, float* dist, int* idx, float* weight,
+                                   void* stream);
+int pn2_fp_interpolate_concat_typed(int dtype, int b, int n, int m, int c2, int c1, const float* xyz1,
+                                    const float* xyz2, const void* points1, const void* points2, void* out,
+                                    void* stream);
+
 /* ---- the sampling+grouping half of a set-abstraction layer, device-resident ------------------ */
 
 /* query_ball_point + group_point(xyz) in ONE launch (tf_grouping_g.cu:3-57 back to back, as

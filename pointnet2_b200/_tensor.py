@@ -13,11 +13,22 @@ from contextlib import contextmanager
 import torch
 
 
-def require_cuda(t: torch.Tensor, name: str, dtype: torch.dtype) -> torch.Tensor:
+# Feature tensors may be float32, bfloat16 or float16 (the kernels compute in float32 and round once); coordinates,
+# weights and indices have a single dtype.
+FEATURE_DTYPES = (torch.float32, torch.bfloat16, torch.float16)
+
+# dtype codes of the typed entry points (include/pn2_api.h: PN2_F32, PN2_BF16, PN2_F16)
+DTYPE_CODES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2}
+
+
+def require_cuda(t: torch.Tensor, name: str, dtype) -> torch.Tensor:
+    """``dtype``: one torch.dtype or a tuple of the allowed ones."""
     if not isinstance(t, torch.Tensor):
         raise TypeError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
-    if t.dtype != dtype:
-        raise TypeError(f"{name} must be {dtype}, got {t.dtype}")
+    allowed = dtype if isinstance(dtype, tuple) else (dtype,)
+    if t.dtype not in allowed:
+        want = allowed[0] if len(allowed) == 1 else " or ".join(str(d) for d in allowed)
+        raise TypeError(f"{name} must be {want}, got {t.dtype}")
     if not t.is_cuda:
         raise RuntimeError(f"{name} must be a CUDA tensor: pointnet2_b200 has no CPU path "
                            f"(got device {t.device})")

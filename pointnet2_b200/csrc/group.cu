@@ -14,6 +14,8 @@
 // served from L2: the source tensor is at most tens of MB).
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "pn2_common.cuh"
 
 namespace pn2 {
@@ -129,12 +131,17 @@ group_rows_vec4_kernel(int n, int c4, unsigned rows_per_cloud, const float4* __r
 // LPR consecutive lanes own one row and walk its channels with stride LPR, so a warp's loads and
 // stores are runs of consecutive 4-byte words (full sectors) whatever the row width; the per-row
 // index/centroid loads are broadcasts.  No per-element division or branching.
-template <int LPR, bool HAS_XYZ>
-__global__ void __launch_bounds__(kCopyThreads)
+// T = float, or unsigned short for both 2-byte formats: features are copied as T, the xyz channels are the float32
+// differences rounded once (f16 != 0: to float16, else bfloat16; grouped_xyz stays float32).
+// The 2-byte instantiations hold twice the loaded values per lane (16 bytes of 2-byte words in 8 registers); they
+// are held to the CTAs per SM of the float ones (48 / 40 registers: 5 / 6 CTAs of 256 threads), without spilling.
+// (0 = no bound for float: even a bound of 1 CTA changes its register allocation.)
+template <int LPR, bool HAS_XYZ, typename T>
+__global__ void __launch_bounds__(kCopyThreads, sizeof(T) == 4 ? 0 : (HAS_XYZ ? 5 : 6))
 group_rows_kernel(int n, int c, int nsample, unsigned rows_per_cloud, const float* __restrict__ xyz,
-                  const float* __restrict__ new_xyz, const float* __restrict__ points,
-                  const int* __restrict__ idx, int xyz_lo, int feat_lo, float* __restrict__ out,
-                  float* __restrict__ grouped_xyz) {
+                  const float* __restrict__ new_xyz, const T* __restrict__ points,
+                  const int* __restrict__ idx, int xyz_lo, int feat_lo, T* __restrict__ out,
+                  float* __restrict__ grouped_xyz, int f16) {
     constexpr int RPW = 32 / LPR;  // rows per warp per pass
     const int lane = threadIdx.x & 31, g = lane % LPR, sub = lane / LPR;
     const unsigned cloud = blockIdx.y;
@@ -143,33 +150,34 @@ group_rows_kernel(int n, int c, int nsample, unsigned rows_per_cloud, const floa
     const unsigned warp = (blockIdx.x * kCopyThreads + threadIdx.x) >> 5;
     const size_t cloud_row0 = (size_t)cloud * rows_per_cloud;
     const int* __restrict__ cidx = idx + cloud_row0;
-    const float* __restrict__ cpts = points ? points + (size_t)cloud * n * c : nullptr;
+    const T* __restrict__ cpts = points ? points + (size_t)cloud * n * c : nullptr;
     const float* __restrict__ cxyz = HAS_XYZ ? xyz + (size_t)cloud * n * 3 : nullptr;
     // R rows per lane group and trip, U words per row and lane in flight: what limits these copies is bytes in
     // flight per SM (measured: 32 KB/SM -> 3.5 TB/s, 64 KB/SM -> 5.5 TB/s for the same gather), so all R*U loads of a
-    // trip are issued before the first store
-    constexpr int R = 2, U = 4;  // measured at C = 320 + 3: R = 2: 58 / 94 / 172 us (38 registers); R = 4: 66 / 103 / 180 us (58 registers)
+    // trip are issued before the first store.  U * sizeof(T) = 16 bytes per row and lane whatever the element size.
+    // measured (float) at C = 320 + 3: R = 2: 58 / 94 / 172 us (38 registers); R = 4: 66 / 103 / 180 us (58 registers)
+    constexpr int R = 2, U = 16 / (int)sizeof(T);
     for (unsigned r0 = (warp * RPW + sub) * R; r0 < rows_per_cloud; r0 += warps * RPW * R) {
-        const float* __restrict__ src[R];
-        float* __restrict__ d[R];
+        const T* __restrict__ src[R];
+        T* __restrict__ d[R];
         bool ok[R];
 #pragma unroll
         for (int rr = 0; rr < R; ++rr) {
             const unsigned r = r0 + rr;
             ok[rr] = r < rows_per_cloud;
             const int a = ok[rr] ? __ldg(cidx + r) : 0;
-            float* __restrict__ dst = out + (cloud_row0 + r) * w;
+            T* __restrict__ dst = out + (cloud_row0 + r) * w;
             src[rr] = cpts ? cpts + (size_t)a * c : nullptr;
             d[rr] = dst + feat_lo;
             if (HAS_XYZ && ok[rr] && g < 3) {
                 const size_t ctr = (size_t)cloud * (rows_per_cloud / (unsigned)nsample) + r / (unsigned)nsample;  // global centroid index
                 const float v = __fsub_rn(__ldg(cxyz + (size_t)a * 3 + g), __ldg(new_xyz + ctr * 3 + g));
-                __stcs(dst + xyz_lo + g, v);
+                __stcs(dst + xyz_lo + g, of_f32<T>(v, f16));
                 if (grouped_xyz) __stcs(grouped_xyz + (cloud_row0 + r) * 3 + g, v);
             }
         }
         for (int l0 = g; l0 < c; l0 += LPR * U) {
-            float v[R][U];
+            T v[R][U];
 #pragma unroll
             for (int rr = 0; rr < R; ++rr)
 #pragma unroll
@@ -292,11 +300,11 @@ group_concat_vec_kernel(int n, int c4, int nsample, unsigned rows_per_cloud, con
 
 // Narrow rows (w <= 4 floats, e.g. group_point(xyz) and the C=0 sample_and_group tail): one thread
 // per output row — the per-row index/centroid work is the cost, not the copy.
-template <bool HAS_XYZ>
+template <bool HAS_XYZ, typename T>
 __global__ void __launch_bounds__(kCopyThreads)
 group_narrow_kernel(int n, int c, int nsample, unsigned rows_per_cloud, const float* __restrict__ xyz,
-                    const float* __restrict__ new_xyz, const float* __restrict__ points,
-                    const int* __restrict__ idx, float* __restrict__ out, float* __restrict__ grouped_xyz) {
+                    const float* __restrict__ new_xyz, const T* __restrict__ points,
+                    const int* __restrict__ idx, T* __restrict__ out, float* __restrict__ grouped_xyz, int f16) {
     const unsigned cloud = blockIdx.y;
     const size_t cloud_row0 = (size_t)cloud * rows_per_cloud;
     const int* __restrict__ cidx = idx + cloud_row0;
@@ -308,35 +316,35 @@ group_narrow_kernel(int n, int c, int nsample, unsigned rows_per_cloud, const fl
             const float* __restrict__ ctr = new_xyz + ((size_t)cloud * m + r / (unsigned)nsample) * 3;
             const float v0 = __fsub_rn(__ldg(s), __ldg(ctr)), v1 = __fsub_rn(__ldg(s + 1), __ldg(ctr + 1)),
                         v2 = __fsub_rn(__ldg(s + 2), __ldg(ctr + 2));
-            float* __restrict__ d = out + (cloud_row0 + r) * 3;
-            __stcs(d, v0); __stcs(d + 1, v1); __stcs(d + 2, v2);
+            T* __restrict__ d = out + (cloud_row0 + r) * 3;
+            __stcs(d, of_f32<T>(v0, f16)); __stcs(d + 1, of_f32<T>(v1, f16)); __stcs(d + 2, of_f32<T>(v2, f16));
             if (grouped_xyz) {
                 float* __restrict__ gq = grouped_xyz + (cloud_row0 + r) * 3;
                 __stcs(gq, v0); __stcs(gq + 1, v1); __stcs(gq + 2, v2);
             }
         } else {
-            const float* __restrict__ s = points + ((size_t)cloud * n + a) * c;
-            float* __restrict__ d = out + (cloud_row0 + r) * c;
+            const T* __restrict__ s = points + ((size_t)cloud * n + a) * c;
+            T* __restrict__ d = out + (cloud_row0 + r) * c;
             for (int l = 0; l < c; ++l) __stcs(d + l, __ldg(s + l));
         }
     }
 }
 
-template <bool HAS_XYZ>
+template <bool HAS_XYZ, typename T>
 static int launch_group_rows(int b, int n, int c, int m, int nsample, const float* xyz, const float* new_xyz,
-                             const float* points, const int* idx, int xyz_lo, int feat_lo, float* out,
-                             float* grouped_xyz, cudaStream_t st) {
+                             const T* points, const int* idx, int xyz_lo, int feat_lo, T* out,
+                             float* grouped_xyz, int f16, cudaStream_t st) {
     const unsigned rpc = (unsigned)m * (unsigned)nsample;
     const int w = c + (HAS_XYZ ? 3 : 0);
     if (w <= 4 && (!HAS_XYZ || c == 0)) {
         unsigned gx = (rpc + kCopyThreads - 1) / kCopyThreads;
         const unsigned cap = ((unsigned)num_sms() * 16u + b - 1) / b;
         if (gx > cap) gx = cap;
-        group_narrow_kernel<HAS_XYZ><<<dim3(gx, b, 1), kCopyThreads, 0, st>>>(n, c, nsample, rpc, xyz, new_xyz, points, idx, out,
-                                                                                grouped_xyz);
+        group_narrow_kernel<HAS_XYZ, T><<<dim3(gx, b, 1), kCopyThreads, 0, st>>>(n, c, nsample, rpc, xyz, new_xyz, points, idx, out,
+                                                                                grouped_xyz, f16);
         return finish_launch();
     }
-    if (HAS_XYZ && c >= 8 && c <= 64 && c % 4 == 0 && aligned16(points) && aligned16(out)) {
+    if (std::is_same<T, float>::value && HAS_XYZ && c >= 8 && c <= 64 && c % 4 == 0 && aligned16(points) && aligned16(out)) {
         // vectorised tail (see group_concat_vec_kernel).  Measured: it wins at C = 64 (30.7 against 35.6 us, cfg4 SA256) and
         // loses to the row kernel below from C = 128 up (C = 320 + 3, S = 64: 125 against 94 us), so only narrow rows take it
         const int c4 = c / 4;
@@ -349,9 +357,10 @@ static int launch_group_rows(int b, int n, int c, int m, int nsample, const floa
         if (gx < 1) gx = 1;
         dim3 grid(gx, b, 1);
         const float4* p4 = reinterpret_cast<const float4*>(points);
-        if (lpr == 8) group_concat_vec_kernel<8, R><<<grid, kCopyThreads, 0, st>>>(n, c4, nsample, rpc, xyz, new_xyz, p4, idx, xyz_lo, feat_lo, out, grouped_xyz);
-        else if (lpr == 16) group_concat_vec_kernel<16, R><<<grid, kCopyThreads, 0, st>>>(n, c4, nsample, rpc, xyz, new_xyz, p4, idx, xyz_lo, feat_lo, out, grouped_xyz);
-        else group_concat_vec_kernel<32, R><<<grid, kCopyThreads, 0, st>>>(n, c4, nsample, rpc, xyz, new_xyz, p4, idx, xyz_lo, feat_lo, out, grouped_xyz);
+        float* o = reinterpret_cast<float*>(out);  // (float here: the condition above)
+        if (lpr == 8) group_concat_vec_kernel<8, R><<<grid, kCopyThreads, 0, st>>>(n, c4, nsample, rpc, xyz, new_xyz, p4, idx, xyz_lo, feat_lo, o, grouped_xyz);
+        else if (lpr == 16) group_concat_vec_kernel<16, R><<<grid, kCopyThreads, 0, st>>>(n, c4, nsample, rpc, xyz, new_xyz, p4, idx, xyz_lo, feat_lo, o, grouped_xyz);
+        else group_concat_vec_kernel<32, R><<<grid, kCopyThreads, 0, st>>>(n, c4, nsample, rpc, xyz, new_xyz, p4, idx, xyz_lo, feat_lo, o, grouped_xyz);
         return finish_launch();
     }
     const int lpr = w <= 4 ? 4 : (w <= 8 ? 8 : (w <= 16 ? 16 : 32));
@@ -362,7 +371,7 @@ static int launch_group_rows(int b, int n, int c, int m, int nsample, const floa
     if (gx < 1) gx = 1;
     dim3 grid(gx, b, 1);
 #define PN2_GROUP_ROWS(L) \
-    group_rows_kernel<L, HAS_XYZ><<<grid, kCopyThreads, 0, st>>>(n, c, nsample, rpc, xyz, new_xyz, points, idx, xyz_lo, feat_lo, out, grouped_xyz)
+    group_rows_kernel<L, HAS_XYZ, T><<<grid, kCopyThreads, 0, st>>>(n, c, nsample, rpc, xyz, new_xyz, points, idx, xyz_lo, feat_lo, out, grouped_xyz, f16)
     if (lpr == 4) PN2_GROUP_ROWS(4);
     else if (lpr == 8) PN2_GROUP_ROWS(8);
     else if (lpr == 16) PN2_GROUP_ROWS(16);
@@ -372,10 +381,11 @@ static int launch_group_rows(int b, int n, int c, int m, int nsample, const floa
 }
 
 // ---- group_point_grad: atomic scatter-add (vector red.global.add.v4.f32 when c % 4 == 0) -------
-template <typename IndexT>
+// T: element type of grad_out (read and upcast 4 at a time); the accumulator is always float32
+template <typename IndexT, typename T>
 __global__ void __launch_bounds__(kCopyThreads)
 group_point_grad_vec4_kernel(int n, int c4, IndexT rows_per_cloud, IndexT total_vec,
-                             const float4* __restrict__ grad_out, const int* __restrict__ idx,
+                             const T* __restrict__ grad_out, const int* __restrict__ idx,
                              float4* __restrict__ grad_points) {
     const IndexT stride = (IndexT)gridDim.x * kCopyThreads;
     for (IndexT v = (IndexT)blockIdx.x * kCopyThreads + threadIdx.x; v < total_vec; v += stride) {
@@ -383,15 +393,15 @@ group_point_grad_vec4_kernel(int n, int c4, IndexT rows_per_cloud, IndexT total_
         const int l = (int)(v - row * (IndexT)c4);
         const IndexT cloud = row / rows_per_cloud;
         const int a = __ldg(idx + row);
-        const float4 g = __ldcs(grad_out + v);
+        const float4 g = ldcs4(grad_out + (size_t)v * 4);
         atomicAdd(grad_points + ((size_t)cloud * n + a) * c4 + l, g);  // red.global.add.v4.f32 (sm_90+)
     }
 }
 
-template <typename IndexT>
+template <typename IndexT, typename T>
 __global__ void __launch_bounds__(kCopyThreads)
 group_point_grad_scalar_kernel(int n, int c, IndexT rows_per_cloud, IndexT total,
-                               const float* __restrict__ grad_out, const int* __restrict__ idx,
+                               const T* __restrict__ grad_out, const int* __restrict__ idx,
                                float* __restrict__ grad_points) {
     const IndexT stride = (IndexT)gridDim.x * kCopyThreads;
     for (IndexT e = (IndexT)blockIdx.x * kCopyThreads + threadIdx.x; e < total; e += stride) {
@@ -399,8 +409,17 @@ group_point_grad_scalar_kernel(int n, int c, IndexT rows_per_cloud, IndexT total
         const int l = (int)(e - row * (IndexT)c);
         const IndexT cloud = row / rows_per_cloud;
         const int a = __ldg(idx + row);
-        atomicAdd(grad_points + ((size_t)cloud * n + a) * c + l, __ldcs(grad_out + e));
+        atomicAdd(grad_points + ((size_t)cloud * n + a) * c + l, to_f32(__ldcs(grad_out + e)));
     }
+}
+
+// the float32 gradient accumulator rounded once to the feature type
+template <typename T>
+__global__ void __launch_bounds__(kCopyThreads)
+round_to_kernel(unsigned long long total, const float* __restrict__ src, T* __restrict__ dst) {
+    for (unsigned long long e = (unsigned long long)blockIdx.x * kCopyThreads + threadIdx.x; e < total;
+         e += (unsigned long long)gridDim.x * kCopyThreads)
+        dst[e] = from_f32<T>(__ldcs(src + e));
 }
 
 // ---- selection_sort: one warp per (b,m) row ------------------------------------------------------
@@ -464,6 +483,101 @@ static unsigned grid_for(unsigned long long work_items, unsigned per_block) {
 }
 
 
+// ---- entry bodies, one per element type T (float, __nv_bfloat16, __half) ----------------------------
+// The 16-byte vector kernels copy bytes, so they serve every T: a row of c elements is c * sizeof(T) / 16 vectors
+// (c % 4 == 0 for float, c % 8 == 0 for the 2-byte types); other widths and misaligned bases take the row kernels.
+template <typename T>
+static int group_point_impl(int b, int n, int c, int m, int nsample, const T* points, const int* idx, T* out,
+                            cudaStream_t st) {
+    const unsigned long long rows = (unsigned long long)b * m * nsample;
+    const unsigned long long rpc = (unsigned long long)m * nsample;
+    if (((size_t)c * sizeof(T)) % 16 == 0 && aligned16(points) && aligned16(out)) {
+        const int c4 = (int)((size_t)c * sizeof(T) / 16);  // 16-byte vectors per row
+        const unsigned long long tv = rows * c4;
+        static int mode = -1, ctas_per_sm = 0;
+        if (mode < 0) {  // tuning hooks: PN2_GROUP_MODE 0 = row-batched (default), 1 = flat one-vector-per-thread
+            const char* e = getenv("PN2_GROUP_MODE");
+            mode = e ? atoi(e) : 0;
+            const char* gq = getenv("PN2_GROUP_CTAS");
+            ctas_per_sm = gq ? atoi(gq) : 16;
+        }
+        const float4* p4 = reinterpret_cast<const float4*>(points);
+        float4* o4 = reinterpret_cast<float4*>(out);
+        if (mode == 0 && rpc < (1ull << 32) && b <= 65535) {
+            const int lpr = c4 <= 4 ? 4 : (c4 <= 8 ? 8 : (c4 <= 16 ? 16 : 32));
+            constexpr int R = 4;
+            const unsigned rows_per_block = (kCopyThreads / 32) * (32 / lpr) * R;
+            unsigned gx = (unsigned)((rpc + rows_per_block - 1) / rows_per_block);
+            const unsigned cap = ((unsigned)num_sms() * (unsigned)ctas_per_sm + b - 1) / b;
+            if (gx > cap) gx = cap;
+            if (gx < 1) gx = 1;
+            dim3 grid(gx, b, 1);
+            if (lpr == 4) group_rows_vec4_kernel<4, R><<<grid, kCopyThreads, 0, st>>>(n, c4, (unsigned)rpc, p4, idx, o4);
+            else if (lpr == 8) group_rows_vec4_kernel<8, R><<<grid, kCopyThreads, 0, st>>>(n, c4, (unsigned)rpc, p4, idx, o4);
+            else if (lpr == 16) group_rows_vec4_kernel<16, R><<<grid, kCopyThreads, 0, st>>>(n, c4, (unsigned)rpc, p4, idx, o4);
+            else group_rows_vec4_kernel<32, R><<<grid, kCopyThreads, 0, st>>>(n, c4, (unsigned)rpc, p4, idx, o4);
+            return finish_launch();
+        }
+        unsigned long long blocks = (tv + kCopyThreads - 1) / kCopyThreads;
+        const unsigned long long cap = (unsigned long long)num_sms() * (unsigned long long)ctas_per_sm;
+        const unsigned grid = (unsigned)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
+        if (tv < (1ull << 31))
+            group_point_vec4_kernel<unsigned, 1><<<grid, kCopyThreads, 0, st>>>(n, c4, (unsigned)rpc, (unsigned)tv, p4, idx, o4);
+        else
+            group_point_vec4_kernel<unsigned long long, 1><<<grid, kCopyThreads, 0, st>>>(n, c4, rpc, tv, p4, idx, o4);
+    } else {
+        if (rpc >= (1ull << 32) || b > 65535) return (int)cudaErrorInvalidValue;
+        return launch_group_rows<false, T>(b, n, c, m, nsample, nullptr, nullptr, points, idx, 0, 0, out, nullptr, 0, st);
+    }
+    return finish_launch();
+}
+
+// scatter-add of grad_out (T) into the float32 accumulator (b,n,c)
+template <typename T>
+static int group_point_grad_impl(int b, int n, int c, int m, int nsample, const T* grad_out, const int* idx,
+                                 float* accum, cudaStream_t st) {
+    const unsigned long long total = (unsigned long long)b * m * nsample * c;
+    const unsigned long long rpc = (unsigned long long)m * nsample;
+    if (c % 4 == 0 && aligned_to(grad_out, 4 * sizeof(T)) && aligned16(accum)) {
+        const unsigned long long tv = total / 4;
+        const unsigned grid = grid_for(tv, kCopyThreads);
+        if (tv < (1ull << 31))
+            group_point_grad_vec4_kernel<unsigned, T><<<grid, kCopyThreads, 0, st>>>(
+                n, c / 4, (unsigned)rpc, (unsigned)tv, grad_out, idx, (float4*)accum);
+        else
+            group_point_grad_vec4_kernel<unsigned long long, T><<<grid, kCopyThreads, 0, st>>>(
+                n, c / 4, rpc, tv, grad_out, idx, (float4*)accum);
+    } else {
+        const unsigned grid = grid_for(total, kCopyThreads);
+        if (total < (1ull << 31))
+            group_point_grad_scalar_kernel<unsigned, T><<<grid, kCopyThreads, 0, st>>>(n, c, (unsigned)rpc, (unsigned)total, grad_out, idx, accum);
+        else
+            group_point_grad_scalar_kernel<unsigned long long, T><<<grid, kCopyThreads, 0, st>>>(n, c, rpc, total, grad_out, idx, accum);
+    }
+    return finish_launch();
+}
+
+template <typename T>
+static int group_point_grad_round_impl(int b, int n, int c, int m, int nsample, const void* grad_out, const int* idx,
+                                       void* grad_points, float* accum, cudaStream_t st) {
+    int rc = group_point_grad_impl<T>(b, n, c, m, nsample, static_cast<const T*>(grad_out), idx, accum, st);
+    if (rc != 0) return rc;
+    const unsigned long long total = (unsigned long long)b * n * c;
+    round_to_kernel<T><<<grid_for(total, kCopyThreads), kCopyThreads, 0, st>>>(total, accum, static_cast<T*>(grad_points));
+    return finish_launch();
+}
+
+template <typename T>
+static int group_concat_impl(int b, int n, int c, int m, int nsample, const float* xyz, const float* new_xyz,
+                             const void* points, const int* idx, int xyz_first, void* out, float* grouped_xyz, int f16,
+                             cudaStream_t st) {
+    const unsigned long long rpc = (unsigned long long)m * nsample;
+    if (rpc >= (1ull << 32) || b > 65535) return (int)cudaErrorInvalidValue;
+    const int xyz_lo = xyz_first ? 0 : c, feat_lo = xyz_first ? 3 : 0;
+    return launch_group_rows<true, T>(b, n, c, m, nsample, xyz, new_xyz, static_cast<const T*>(points), idx, xyz_lo,
+                                      feat_lo, static_cast<T*>(out), grouped_xyz, f16, st);
+}
+
 }  // namespace pn2
 
 extern "C" {
@@ -492,78 +606,45 @@ int pn2_group_point(int b, int n, int c, int m, int nsample, const float* points
                     void* stream) {
     using namespace pn2;
     if (b < 0 || n <= 0 || c < 0 || m < 0 || nsample < 0) return (int)cudaErrorInvalidValue;
-    const unsigned long long rows = (unsigned long long)b * m * nsample;
-    const unsigned long long total = rows * c;
-    if (total == 0) return 0;
+    if ((unsigned long long)b * m * nsample * c == 0) return 0;
     if (!points || !idx || !out) return (int)cudaErrorInvalidValue;
-    cudaStream_t st = as_stream(stream);
-    const unsigned long long rpc = (unsigned long long)m * nsample;
-    if (c % 4 == 0 && aligned16(points) && aligned16(out)) {
-        const unsigned long long tv = total / 4;
-        static int mode = -1, ctas_per_sm = 0;
-        if (mode < 0) {  // tuning hooks: PN2_GROUP_MODE 0 = row-batched (default), 1 = flat one-vector-per-thread
-            const char* e = getenv("PN2_GROUP_MODE");
-            mode = e ? atoi(e) : 0;
-            const char* gq = getenv("PN2_GROUP_CTAS");
-            ctas_per_sm = gq ? atoi(gq) : 16;
-        }
-        if (mode == 0 && rpc < (1ull << 32) && b <= 65535) {
-            const int c4 = c / 4;
-            const int lpr = c4 <= 4 ? 4 : (c4 <= 8 ? 8 : (c4 <= 16 ? 16 : 32));
-            constexpr int R = 4;
-            const unsigned rows_per_block = (kCopyThreads / 32) * (32 / lpr) * R;
-            unsigned gx = (unsigned)((rpc + rows_per_block - 1) / rows_per_block);
-            const unsigned cap = ((unsigned)num_sms() * (unsigned)ctas_per_sm + b - 1) / b;
-            if (gx > cap) gx = cap;
-            if (gx < 1) gx = 1;
-            dim3 grid(gx, b, 1);
-            if (lpr == 4) group_rows_vec4_kernel<4, R><<<grid, kCopyThreads, 0, st>>>(n, c4, (unsigned)rpc, (const float4*)points, idx, (float4*)out);
-            else if (lpr == 8) group_rows_vec4_kernel<8, R><<<grid, kCopyThreads, 0, st>>>(n, c4, (unsigned)rpc, (const float4*)points, idx, (float4*)out);
-            else if (lpr == 16) group_rows_vec4_kernel<16, R><<<grid, kCopyThreads, 0, st>>>(n, c4, (unsigned)rpc, (const float4*)points, idx, (float4*)out);
-            else group_rows_vec4_kernel<32, R><<<grid, kCopyThreads, 0, st>>>(n, c4, (unsigned)rpc, (const float4*)points, idx, (float4*)out);
-            return finish_launch();
-        }
-        unsigned long long blocks = (tv + kCopyThreads - 1) / kCopyThreads;
-        const unsigned long long cap = (unsigned long long)num_sms() * (unsigned long long)ctas_per_sm;
-        const unsigned grid = (unsigned)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
-        if (tv < (1ull << 31))
-            group_point_vec4_kernel<unsigned, 1><<<grid, kCopyThreads, 0, st>>>(n, c / 4, (unsigned)rpc, (unsigned)tv, (const float4*)points, idx, (float4*)out);
-        else
-            group_point_vec4_kernel<unsigned long long, 1><<<grid, kCopyThreads, 0, st>>>(n, c / 4, rpc, tv, (const float4*)points, idx, (float4*)out);
-    } else {
-        if (rpc >= (1ull << 32) || b > 65535) return (int)cudaErrorInvalidValue;
-        return launch_group_rows<false>(b, n, c, m, nsample, nullptr, nullptr, points, idx, 0, 0, out, nullptr, st);
-    }
-    return finish_launch();
+    return group_point_impl<float>(b, n, c, m, nsample, points, idx, out, as_stream(stream));
+}
+
+int pn2_group_point_typed(int dtype, int b, int n, int c, int m, int nsample, const void* points, const int* idx,
+                          void* out, void* stream) {
+    using namespace pn2;
+    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
+    if (dtype == PN2_F32) return pn2_group_point(b, n, c, m, nsample, static_cast<const float*>(points), idx, static_cast<float*>(out), stream);
+    if (b < 0 || n <= 0 || c < 0 || m < 0 || nsample < 0) return (int)cudaErrorInvalidValue;
+    if ((unsigned long long)b * m * nsample * c == 0) return 0;
+    if (!points || !idx || !out) return (int)cudaErrorInvalidValue;
+    // a bit copy: bfloat16 and float16 are both moved as unsigned short
+    return group_point_impl<unsigned short>(b, n, c, m, nsample, static_cast<const unsigned short*>(points), idx,
+                                            static_cast<unsigned short*>(out), as_stream(stream));
 }
 
 int pn2_group_point_grad(int b, int n, int c, int m, int nsample, const float* grad_out, const int* idx,
                          float* grad_points, void* stream) {
     using namespace pn2;
     if (b < 0 || n <= 0 || c < 0 || m < 0 || nsample < 0) return (int)cudaErrorInvalidValue;
-    const unsigned long long rows = (unsigned long long)b * m * nsample;
-    const unsigned long long total = rows * c;
-    if (total == 0) return 0;
+    if ((unsigned long long)b * m * nsample * c == 0) return 0;
     if (!grad_out || !idx || !grad_points) return (int)cudaErrorInvalidValue;
-    cudaStream_t st = as_stream(stream);
-    const unsigned long long rpc = (unsigned long long)m * nsample;
-    if (c % 4 == 0 && aligned16(grad_out) && aligned16(grad_points)) {
-        const unsigned long long tv = total / 4;
-        const unsigned grid = grid_for(tv, kCopyThreads);
-        if (tv < (1ull << 31))
-            group_point_grad_vec4_kernel<unsigned><<<grid, kCopyThreads, 0, st>>>(
-                n, c / 4, (unsigned)rpc, (unsigned)tv, (const float4*)grad_out, idx, (float4*)grad_points);
-        else
-            group_point_grad_vec4_kernel<unsigned long long><<<grid, kCopyThreads, 0, st>>>(
-                n, c / 4, rpc, tv, (const float4*)grad_out, idx, (float4*)grad_points);
-    } else {
-        const unsigned grid = grid_for(total, kCopyThreads);
-        if (total < (1ull << 31))
-            group_point_grad_scalar_kernel<unsigned><<<grid, kCopyThreads, 0, st>>>(n, c, (unsigned)rpc, (unsigned)total, grad_out, idx, grad_points);
-        else
-            group_point_grad_scalar_kernel<unsigned long long><<<grid, kCopyThreads, 0, st>>>(n, c, rpc, total, grad_out, idx, grad_points);
-    }
-    return finish_launch();
+    return group_point_grad_impl<float>(b, n, c, m, nsample, grad_out, idx, grad_points, as_stream(stream));
+}
+
+int pn2_group_point_grad_typed(int dtype, int b, int n, int c, int m, int nsample, const void* grad_out,
+                               const int* idx, void* grad_points, float* accum, void* stream) {
+    using namespace pn2;
+    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
+    if (dtype == PN2_F32)
+        return pn2_group_point_grad(b, n, c, m, nsample, static_cast<const float*>(grad_out), idx, static_cast<float*>(grad_points), stream);
+    if (b < 0 || n <= 0 || c < 0 || m < 0 || nsample < 0) return (int)cudaErrorInvalidValue;
+    if ((unsigned long long)b * m * nsample * c == 0) return 0;
+    if (!grad_out || !idx || !grad_points || !accum) return (int)cudaErrorInvalidValue;
+    if (dtype == PN2_BF16)
+        return group_point_grad_round_impl<__nv_bfloat16>(b, n, c, m, nsample, grad_out, idx, grad_points, accum, as_stream(stream));
+    return group_point_grad_round_impl<__half>(b, n, c, m, nsample, grad_out, idx, grad_points, accum, as_stream(stream));
 }
 
 int pn2_group_concat(int b, int n, int c, int m, int nsample, const float* xyz, const float* new_xyz,
@@ -574,10 +655,24 @@ int pn2_group_concat(int b, int n, int c, int m, int nsample, const float* xyz, 
     const unsigned long long rpc = (unsigned long long)m * nsample;
     if (b == 0 || rpc == 0) return 0;
     if (!xyz || !new_xyz || !idx || !out || (c > 0 && !points)) return (int)cudaErrorInvalidValue;
-    if (rpc >= (1ull << 32) || b > 65535) return (int)cudaErrorInvalidValue;
-    const int xyz_lo = xyz_first ? 0 : c, feat_lo = xyz_first ? 3 : 0;
-    return launch_group_rows<true>(b, n, c, m, nsample, xyz, new_xyz, points, idx, xyz_lo, feat_lo, out, grouped_xyz,
-                                   as_stream(stream));
+    return group_concat_impl<float>(b, n, c, m, nsample, xyz, new_xyz, points, idx, xyz_first, out, grouped_xyz, 0, as_stream(stream));
+}
+
+int pn2_group_concat_typed(int dtype, int b, int n, int c, int m, int nsample, const float* xyz,
+                           const float* new_xyz, const void* points, const int* idx, int xyz_first, void* out,
+                           float* grouped_xyz, void* stream) {
+    using namespace pn2;
+    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
+    if (dtype == PN2_F32)
+        return pn2_group_concat(b, n, c, m, nsample, xyz, new_xyz, static_cast<const float*>(points), idx, xyz_first,
+                                static_cast<float*>(out), grouped_xyz, stream);
+    if (b < 0 || n <= 0 || c < 0 || m < 0 || nsample < 0) return (int)cudaErrorInvalidValue;
+    const unsigned long long rpc = (unsigned long long)m * nsample;
+    if (b == 0 || rpc == 0) return 0;
+    if (!xyz || !new_xyz || !idx || !out || (c > 0 && !points)) return (int)cudaErrorInvalidValue;
+    // bfloat16 and float16 share one instance: dtype == PN2_F16 selects the format of the xyz channels
+    return group_concat_impl<unsigned short>(b, n, c, m, nsample, xyz, new_xyz, points, idx, xyz_first, out, grouped_xyz,
+                                             dtype == PN2_F16, as_stream(stream));
 }
 
 int pn2_selection_sort(int b, int n, int m, int k, const float* dist, int* outi, float* out, void* stream) {

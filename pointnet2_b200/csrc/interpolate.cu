@@ -171,15 +171,17 @@ constexpr int kItThreads = 256;
 // One thread per output float4 (U = 1): U = 4 outputs in flight per thread costs 96 registers and quarter
 // occupancy; staging channel slices of the known features in shared memory is worse still (one 160 KB CTA
 // per SM cannot hide its own slice load).
-template <typename IndexT, int U>
+// T = float, __nv_bfloat16 or __half: P = Pack4<T>::type holds 4 channels; they are upcast, interpolated in float32
+// and rounded once on the way out.
+template <typename IndexT, int U, typename T, typename P = typename Pack4<T>::type>
 __global__ void __launch_bounds__(kItThreads)
-three_interp_vec4_kernel(int m, int c4, IndexT rows_per_cloud, IndexT total_vec, const float4* __restrict__ points,
-                         const int* __restrict__ idx, const float* __restrict__ weight, float4* __restrict__ out) {
+three_interp_vec4_kernel(int m, int c4, IndexT rows_per_cloud, IndexT total_vec, const P* __restrict__ points,
+                         const int* __restrict__ idx, const float* __restrict__ weight, P* __restrict__ out) {
     const IndexT stride = (IndexT)gridDim.x * kItThreads;
     for (IndexT v0 = (IndexT)blockIdx.x * kItThreads + threadIdx.x; v0 < total_vec; v0 += stride * U) {
         int i1[U], i2[U], i3[U];
         float w1[U], w2[U], w3[U];
-        const float4* pb[U];
+        const P* pb[U];
         bool ok[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
@@ -200,9 +202,9 @@ three_interp_vec4_kernel(int m, int c4, IndexT rows_per_cloud, IndexT total_vec,
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             if (ok[u]) {
-                a[u] = __ldg(pb[u] + (size_t)i1[u] * c4);
-                b[u] = __ldg(pb[u] + (size_t)i2[u] * c4);
-                c[u] = __ldg(pb[u] + (size_t)i3[u] * c4);
+                a[u] = unpack4(__ldg(pb[u] + (size_t)i1[u] * c4), T());
+                b[u] = unpack4(__ldg(pb[u] + (size_t)i2[u] * c4), T());
+                c[u] = unpack4(__ldg(pb[u] + (size_t)i3[u] * c4), T());
             }
         }
 #pragma unroll
@@ -213,16 +215,16 @@ three_interp_vec4_kernel(int m, int c4, IndexT rows_per_cloud, IndexT total_vec,
                 o.y = interp3(a[u].y, b[u].y, c[u].y, w1[u], w2[u], w3[u]);
                 o.z = interp3(a[u].z, b[u].z, c[u].z, w1[u], w2[u], w3[u]);
                 o.w = interp3(a[u].w, b[u].w, c[u].w, w1[u], w2[u], w3[u]);
-                st_stream_f4(out + v0 + (IndexT)u * stride, o);
+                __stcs(out + v0 + (IndexT)u * stride, pack4(o, T()));
             }
         }
     }
 }
 
-template <typename IndexT>
+template <typename IndexT, typename T>
 __global__ void __launch_bounds__(kItThreads)
-three_interp_scalar_kernel(int m, int c, IndexT rows_per_cloud, IndexT total, const float* __restrict__ points,
-                           const int* __restrict__ idx, const float* __restrict__ weight, float* __restrict__ out) {
+three_interp_scalar_kernel(int m, int c, IndexT rows_per_cloud, IndexT total, const T* __restrict__ points,
+                           const int* __restrict__ idx, const float* __restrict__ weight, T* __restrict__ out) {
     const IndexT stride = (IndexT)gridDim.x * kItThreads;
     for (IndexT e = (IndexT)blockIdx.x * kItThreads + threadIdx.x; e < total; e += stride) {
         const IndexT row = e / (IndexT)c;
@@ -230,9 +232,9 @@ three_interp_scalar_kernel(int m, int c, IndexT rows_per_cloud, IndexT total, co
         const IndexT cloud = row / rows_per_cloud;
         const int* ii = idx + (size_t)row * 3;
         const float* w = weight + (size_t)row * 3;
-        const float* pb = points + (size_t)cloud * m * c + l;
-        out[e] = interp3(__ldg(pb + (size_t)__ldg(ii + 0) * c), __ldg(pb + (size_t)__ldg(ii + 1) * c),
-                         __ldg(pb + (size_t)__ldg(ii + 2) * c), __ldg(w + 0), __ldg(w + 1), __ldg(w + 2));
+        const T* pb = points + (size_t)cloud * m * c + l;
+        out[e] = from_f32<T>(interp3(to_f32(__ldg(pb + (size_t)__ldg(ii + 0) * c)), to_f32(__ldg(pb + (size_t)__ldg(ii + 1) * c)),
+                                     to_f32(__ldg(pb + (size_t)__ldg(ii + 2) * c)), __ldg(w + 0), __ldg(w + 1), __ldg(w + 2)));
     }
 }
 
@@ -320,11 +322,14 @@ __device__ __forceinline__ void scan_tile_strided(Top3& t, const KnownTile& tile
     }
 }
 
-template <int G>
+// T: element type of points1 / points2 / out: float, or unsigned short for both 2-byte formats, f16 choosing float16 or
+// bfloat16 at run time (the 3-NN phase is most of the code: one 2-byte instance per G instead of two).  Phase 2 upcasts,
+// interpolates in float32 and rounds once; points1 is copied.
+template <int G, typename T>
 __global__ void __launch_bounds__(kNnThreads)
 fp_front_kernel(int n, int m, int c2, int c1, const float* __restrict__ xyz1, const float* __restrict__ xyz2,
-                const float* __restrict__ points1, const float* __restrict__ points2, float* __restrict__ out,
-                float* __restrict__ dist_o, int* __restrict__ idx_o, float* __restrict__ weight_o) {
+                const T* __restrict__ points1, const T* __restrict__ points2, T* __restrict__ out,
+                float* __restrict__ dist_o, int* __restrict__ idx_o, float* __restrict__ weight_o, int f16) {
     constexpr int PPB = kNnThreads / G;  // unknown points per CTA
     __shared__ KnownTile s_tile;
     __shared__ int s_i[PPB][3];
@@ -385,39 +390,43 @@ fp_front_kernel(int n, int m, int c2, int c1, const float* __restrict__ xyz1, co
     if (!out) return;
     const int rows = min(PPB, n - j0);
     const int cw = c2 + c1;  // output row width
-    const float* __restrict__ pb = points2 + (size_t)cloud * m * c2;
-    const float* __restrict__ p1 = points1 ? points1 + ((size_t)cloud * n + j0) * c1 : nullptr;
-    float* __restrict__ ob = out + ((size_t)cloud * n + j0) * cw;
+    const T* __restrict__ pb = points2 + (size_t)cloud * m * c2;
+    const T* __restrict__ p1 = points1 ? points1 + ((size_t)cloud * n + j0) * c1 : nullptr;
+    T* __restrict__ ob = out + ((size_t)cloud * n + j0) * cw;
     const bool vec = ((c2 | c1) & 3) == 0 &&
-                     ((reinterpret_cast<uintptr_t>(pb) | reinterpret_cast<uintptr_t>(ob) | reinterpret_cast<uintptr_t>(p1)) & 15u) == 0;
-    if (vec) {
+                     ((reinterpret_cast<uintptr_t>(pb) | reinterpret_cast<uintptr_t>(ob) | reinterpret_cast<uintptr_t>(p1)) & (4 * sizeof(T) - 1)) == 0;
+    if (vec) {  // 4 channels per vector
+        using P = typename Pack4<T>::type;
         const int c24 = c2 >> 2, cw4 = cw >> 2, c14 = c1 >> 2;
-        const float4* pb4 = reinterpret_cast<const float4*>(pb);
-        const float4* p14 = reinterpret_cast<const float4*>(p1);
-        float4* ob4 = reinterpret_cast<float4*>(ob);
+        const P* pb4 = reinterpret_cast<const P*>(pb);
+        const P* p14 = reinterpret_cast<const P*>(p1);
+        P* ob4 = reinterpret_cast<P*>(ob);
         for (int e = tid; e < rows * cw4; e += kNnThreads) {
             const int r = e / cw4, l = e - r * cw4;
-            float4 o;
+            P o;
             if (l < c24) {
-                const float4 a = __ldg(pb4 + (size_t)s_i[r][0] * c24 + l), b = __ldg(pb4 + (size_t)s_i[r][1] * c24 + l),
-                             cc = __ldg(pb4 + (size_t)s_i[r][2] * c24 + l);
+                const float4 a = unpack4_of(__ldg(pb4 + (size_t)s_i[r][0] * c24 + l), f16),
+                             b = unpack4_of(__ldg(pb4 + (size_t)s_i[r][1] * c24 + l), f16),
+                             cc = unpack4_of(__ldg(pb4 + (size_t)s_i[r][2] * c24 + l), f16);
                 const float x1 = s_w[r][0], x2 = s_w[r][1], x3 = s_w[r][2];
-                o.x = interp3(a.x, b.x, cc.x, x1, x2, x3);
-                o.y = interp3(a.y, b.y, cc.y, x1, x2, x3);
-                o.z = interp3(a.z, b.z, cc.z, x1, x2, x3);
-                o.w = interp3(a.w, b.w, cc.w, x1, x2, x3);
+                float4 f;
+                f.x = interp3(a.x, b.x, cc.x, x1, x2, x3);
+                f.y = interp3(a.y, b.y, cc.y, x1, x2, x3);
+                f.z = interp3(a.z, b.z, cc.z, x1, x2, x3);
+                f.w = interp3(a.w, b.w, cc.w, x1, x2, x3);
+                o = pack4_of(f, T(), f16);
             } else {
-                o = __ldcs(p14 + (size_t)r * c14 + (l - c24));  // points1, read once
+                o = __ldcs(p14 + (size_t)r * c14 + (l - c24));  // points1, read once, copied as it is
             }
-            st_stream_f4(ob4 + e, o);
+            __stcs(ob4 + e, o);
         }
     } else {
         for (int e = tid; e < rows * cw; e += kNnThreads) {
             const int r = e / cw, l = e - r * cw;
-            float o;
+            T o;
             if (l < c2)
-                o = interp3(__ldg(pb + (size_t)s_i[r][0] * c2 + l), __ldg(pb + (size_t)s_i[r][1] * c2 + l),
-                            __ldg(pb + (size_t)s_i[r][2] * c2 + l), s_w[r][0], s_w[r][1], s_w[r][2]);
+                o = of_f32<T>(interp3(f32_of(__ldg(pb + (size_t)s_i[r][0] * c2 + l), f16), f32_of(__ldg(pb + (size_t)s_i[r][1] * c2 + l), f16),
+                                      f32_of(__ldg(pb + (size_t)s_i[r][2] * c2 + l), f16), s_w[r][0], s_w[r][1], s_w[r][2]), f16);
             else
                 o = __ldcs(p1 + (size_t)r * c1 + (l - c2));
             ob[e] = o;
@@ -425,29 +434,30 @@ fp_front_kernel(int n, int m, int c2, int c1, const float* __restrict__ xyz1, co
     }
 }
 
-template <int G>
-static int launch_fp_front(int b, int n, int m, int c2, int c1, const float* xyz1, const float* xyz2, const float* points1,
-                           const float* points2, float* out, float* dist, int* idx, float* weight, cudaStream_t st) {
+template <int G, typename T>
+static int launch_fp_front(int b, int n, int m, int c2, int c1, const float* xyz1, const float* xyz2, const T* points1,
+                           const T* points2, T* out, float* dist, int* idx, float* weight, int f16, cudaStream_t st) {
     constexpr int PPB = kNnThreads / G;
     dim3 grid((n + PPB - 1) / PPB, b, 1);
-    fp_front_kernel<G><<<grid, kNnThreads, 0, st>>>(n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight);
+    fp_front_kernel<G, T><<<grid, kNnThreads, 0, st>>>(n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16);
     return finish_launch();
 }
 
-static int fp_front_dispatch(int b, int n, int m, int c2, int c1, const float* xyz1, const float* xyz2, const float* points1,
-                             const float* points2, float* out, float* dist, int* idx, float* weight, cudaStream_t st) {
+template <typename T>
+static int fp_front_dispatch(int b, int n, int m, int c2, int c1, const float* xyz1, const float* xyz2, const T* points1,
+                             const T* points2, T* out, float* dist, int* idx, float* weight, int f16, cudaStream_t st) {
     // lanes per unknown point: as many as it takes to put ~2 CTAs on every SM (a CTA covers 128/G points),
     // but never more lanes than there are pairs of known points to share
     const long long pts = (long long)b * n;
     int G = 1;
     while (G < 32 && pts * G < 2LL * num_sms() * kNnThreads && 2 * G <= (m + 1) / 2) G *= 2;
     switch (G) {
-        case 1: return launch_fp_front<1>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, st);
-        case 2: return launch_fp_front<2>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, st);
-        case 4: return launch_fp_front<4>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, st);
-        case 8: return launch_fp_front<8>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, st);
-        case 16: return launch_fp_front<16>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, st);
-        default: return launch_fp_front<32>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, st);
+        case 1: return launch_fp_front<1, T>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16, st);
+        case 2: return launch_fp_front<2, T>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16, st);
+        case 4: return launch_fp_front<4, T>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16, st);
+        case 8: return launch_fp_front<8, T>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16, st);
+        case 16: return launch_fp_front<16, T>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16, st);
+        default: return launch_fp_front<32, T>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16, st);
     }
 }
 
@@ -570,11 +580,13 @@ inv_build_kernel(int n3, int m, const int* __restrict__ idx, int* __restrict__ o
 
 // one warp per known point (b, i); lanes over channels (float4 when VEC).  Lists longer than kInvSortCap are
 // queued for inv_long_kernel.
-template <bool VEC>
+// T: element type of grad_out and grad_points (upcast on load, float32 sums, rounded once on the store): float, or
+// unsigned short for both 2-byte formats with f16 choosing float16 / bfloat16 at run time (one instance for the two)
+template <bool VEC, typename T>
 __global__ void __launch_bounds__(kInvThreads)
-inv_gather_kernel(int n, int c, int m, long long warps_total, const float* __restrict__ grad_out,
+inv_gather_kernel(int n, int c, int m, long long warps_total, const T* __restrict__ grad_out,
                   const float* __restrict__ weight, const int* __restrict__ off, const int* __restrict__ entries,
-                  float* __restrict__ grad_points, int* __restrict__ long_queue) {
+                  T* __restrict__ grad_points, int* __restrict__ long_queue, int f16) {
     __shared__ int s_e[kInvThreads / 32][kInvSortCap];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const long long gw = ((long long)blockIdx.x * kInvThreads + threadIdx.x) >> 5;
@@ -588,9 +600,9 @@ inv_gather_kernel(int n, int c, int m, long long warps_total, const float* __res
         if (lane == 0) long_queue[1 + atomicAdd(long_queue, 1)] = (int)gw;  // the order of the queue does not matter
         return;
     }
-    const float* __restrict__ go = grad_out + (size_t)cloud * n * c;
+    const T* __restrict__ go = grad_out + (size_t)cloud * n * c;
     const float* __restrict__ wt = weight + (size_t)cloud * n3;
-    float* __restrict__ gp = grad_points + ((size_t)cloud * m + i) * c;
+    T* __restrict__ gp = grad_points + ((size_t)cloud * m + i) * c;
     {
         int key[8];
 #pragma unroll
@@ -610,23 +622,41 @@ inv_gather_kernel(int n, int c, int m, long long warps_total, const float* __res
         const int l = l0 + lane * W;
         if (l >= c) continue;
         float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll 4
-        for (int sidx = 0; sidx < len; ++sidx) {
-            const int e = s_e[wib][sidx];
-            const float w = __ldg(wt + e);
-            const float* __restrict__ src = go + (size_t)(e / 3) * c + l;
-            if (VEC) {
-                const float4 g = __ldg(reinterpret_cast<const float4*>(src));
-                a0 = __fadd_rn(a0, __fmul_rn(g.x, w));
-                a1 = __fadd_rn(a1, __fmul_rn(g.y, w));
-                a2 = __fadd_rn(a2, __fmul_rn(g.z, w));
-                a3 = __fadd_rn(a3, __fmul_rn(g.w, w));
-            } else {
-                a0 = __fadd_rn(a0, __fmul_rn(__ldg(src), w));
+        // H entries at a time: their raw rows are all loaded before the first is upcast and added (in ascending order);
+        // an upcast next to each load made the warp wait for the loads one by one
+        constexpr int H = 4;
+        for (int s0 = 0; s0 < len; s0 += H) {
+            typename Pack4<T>::type gv[H];
+            T gs[H];
+            float w[H];
+#pragma unroll
+            for (int u = 0; u < H; ++u) {
+                w[u] = 0.f;
+                if (s0 + u < len) {
+                    const int e = s_e[wib][s0 + u];
+                    w[u] = __ldg(wt + e);
+                    const T* __restrict__ src = go + (size_t)(e / 3) * c + l;
+                    if (VEC) gv[u] = __ldg(reinterpret_cast<const typename Pack4<T>::type*>(src));
+                    else gs[u] = __ldg(src);
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < H; ++u) {
+                if (s0 + u < len) {
+                    if (VEC) {
+                        const float4 g = unpack4_of(gv[u], f16);
+                        a0 = __fadd_rn(a0, __fmul_rn(g.x, w[u]));
+                        a1 = __fadd_rn(a1, __fmul_rn(g.y, w[u]));
+                        a2 = __fadd_rn(a2, __fmul_rn(g.z, w[u]));
+                        a3 = __fadd_rn(a3, __fmul_rn(g.w, w[u]));
+                    } else {
+                        a0 = __fadd_rn(a0, __fmul_rn(f32_of(gs[u], f16), w[u]));
+                    }
+                }
             }
         }
-        if (VEC) *reinterpret_cast<float4*>(gp + l) = make_float4(a0, a1, a2, a3);
-        else gp[l] = a0;
+        if (VEC) *reinterpret_cast<typename Pack4<T>::type*>(gp + l) = pack4_of(make_float4(a0, a1, a2, a3), T(), f16);
+        else gp[l] = of_f32<T>(a0, f16);
     }
 }
 
@@ -635,10 +665,10 @@ inv_gather_kernel(int n, int c, int m, long long warps_total, const float* __res
 // (coalesced index loads + ballot), adds the entries that point at i in that order, and the 8 partial sums are
 // combined in piece order — a fixed association, hence deterministic (it differs from one long sequential sum
 // only in rounding; short lists, the normal case, are bit-identical to the reference's loop).
-template <bool VEC>
+template <bool VEC, typename T>
 __global__ void __launch_bounds__(kInvThreads)
-inv_long_kernel(int n, int c, int m, const float* __restrict__ grad_out, const int* __restrict__ idx,
-                const float* __restrict__ weight, const int* __restrict__ long_queue, float* __restrict__ grad_points) {
+inv_long_kernel(int n, int c, int m, const T* __restrict__ grad_out, const int* __restrict__ idx,
+                const float* __restrict__ weight, const int* __restrict__ long_queue, T* __restrict__ grad_points, int f16) {
     constexpr int NW = kInvThreads / 32;
     constexpr int W = VEC ? 4 : 1;
     __shared__ float s_part[NW][32 * W];
@@ -650,10 +680,10 @@ inv_long_kernel(int n, int c, int m, const float* __restrict__ grad_out, const i
         const long long gw = long_queue[1 + q];
         const long long cloud = gw / m;
         const int i = (int)(gw - cloud * m);
-        const float* __restrict__ go = grad_out + (size_t)cloud * n * c;
+        const T* __restrict__ go = grad_out + (size_t)cloud * n * c;
         const float* __restrict__ wt = weight + (size_t)cloud * n3;
         const int* __restrict__ cidx = idx + cloud * n3;
-        float* __restrict__ gp = grad_points + ((size_t)cloud * m + i) * c;
+        T* __restrict__ gp = grad_points + ((size_t)cloud * m + i) * c;
         const int e_lo = warp * piece, e_hi = min(n3, e_lo + piece);
         for (int l0 = 0; l0 < c; l0 += 32 * W) {
             const int l = l0 + lane * W;
@@ -662,12 +692,18 @@ inv_long_kernel(int n, int c, int m, const float* __restrict__ grad_out, const i
             for (int base = e_lo; base < e_hi; base += 32) {
                 const int e = base + lane;
                 unsigned hit = __ballot_sync(kFullMask, e < e_hi && __ldg(cidx + e) == i);
-                while (hit) {  // up to 4 matching entries at a time: their rows are loaded together, then added in order
-                    int ee[4];
-                    float w[4];
-                    float4 g[4];
+                // up to H matching entries at a time: their rows are loaded together, then added in order.  Raw vectors: the
+                // 2-byte types are upcast only when added, so all H loads are in flight first (an upcast next to each load
+                // made the 16-bit kernel wait for every load in turn: 2x the float time); their smaller vectors leave the
+                // registers for 8 rows in flight (4: still 6 % behind float at cfg4 FP8192 <- 1024)
+                constexpr int H = sizeof(T) == 4 ? 4 : 8;
+                while (hit) {
+                    int ee[H];
+                    float w[H];
+                    typename Pack4<T>::type gv[H];
+                    T gs[H];
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) {
+                    for (int u = 0; u < H; ++u) {
                         ee[u] = -1;
                         if (hit) {
                             ee[u] = base + __ffs(hit) - 1;
@@ -675,24 +711,24 @@ inv_long_kernel(int n, int c, int m, const float* __restrict__ grad_out, const i
                         }
                     }
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        g[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+                    for (int u = 0; u < H; ++u) {
                         w[u] = 0.f;
                         if (ee[u] >= 0 && act) {
                             w[u] = __ldg(wt + ee[u]);
-                            const float* __restrict__ src = go + (size_t)(ee[u] / 3) * c + l;
-                            if (VEC) g[u] = __ldg(reinterpret_cast<const float4*>(src));
-                            else g[u].x = __ldg(src);
+                            const T* __restrict__ src = go + (size_t)(ee[u] / 3) * c + l;
+                            if (VEC) gv[u] = __ldg(reinterpret_cast<const typename Pack4<T>::type*>(src));
+                            else gs[u] = __ldg(src);
                         }
                     }
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) {
+                    for (int u = 0; u < H; ++u) {
                         if (ee[u] >= 0 && act) {
-                            a0 = __fadd_rn(a0, __fmul_rn(g[u].x, w[u]));
+                            const float4 g = VEC ? unpack4_of(gv[u], f16) : make_float4(f32_of(gs[u], f16), 0.f, 0.f, 0.f);
+                            a0 = __fadd_rn(a0, __fmul_rn(g.x, w[u]));
                             if (VEC) {
-                                a1 = __fadd_rn(a1, __fmul_rn(g[u].y, w[u]));
-                                a2 = __fadd_rn(a2, __fmul_rn(g[u].z, w[u]));
-                                a3 = __fadd_rn(a3, __fmul_rn(g[u].w, w[u]));
+                                a1 = __fadd_rn(a1, __fmul_rn(g.y, w[u]));
+                                a2 = __fadd_rn(a2, __fmul_rn(g.z, w[u]));
+                                a3 = __fadd_rn(a3, __fmul_rn(g.w, w[u]));
                             }
                         }
                     }
@@ -711,7 +747,7 @@ inv_long_kernel(int n, int c, int m, const float* __restrict__ grad_out, const i
                     float t = s_part[0][lane * W + u];
 #pragma unroll
                     for (int p = 1; p < NW; ++p) t = __fadd_rn(t, s_part[p][lane * W + u]);
-                    gp[l + u] = t;
+                    gp[l + u] = of_f32<T>(t, f16);
                 }
             }
             __syncthreads();
@@ -729,109 +765,38 @@ static unsigned it_grid(unsigned long long work_items, unsigned per_block) {
 
 static bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-}  // namespace pn2
-
-extern "C" {
-
-int pn2_three_nn(int b, int n, int m, const float* xyz1, const float* xyz2, float* dist, int* idx, void* stream) {
-    using namespace pn2;
-    if (b < 0 || n < 0 || m < 0) return (int)cudaErrorInvalidValue;
-    if (b == 0 || n == 0) return 0;
-    if (!xyz1 || (m > 0 && !xyz2) || !dist || !idx) return (int)cudaErrorInvalidValue;
-    if (b > 65535) return (int)cudaErrorInvalidValue;
-    dim3 grid((n + kNnThreads - 1) / kNnThreads, b, 1);
-    three_nn_kernel<<<grid, kNnThreads, 0, as_stream(stream)>>>(n, m, xyz1, xyz2, dist, idx);
-    return finish_launch();
-}
-
-int pn2_three_interpolate(int b, int m, int c, int n, const float* points, const int* idx, const float* weight,
-                          float* out, void* stream) {
-    using namespace pn2;
-    if (b < 0 || m <= 0 || c < 0 || n < 0) return (int)cudaErrorInvalidValue;
+template <typename T>
+static int three_interpolate_impl(int b, int m, int c, int n, const T* points, const int* idx, const float* weight, T* out,
+                                  cudaStream_t st) {
+    using P = typename Pack4<T>::type;
     const unsigned long long total = (unsigned long long)b * n * c;
-    if (total == 0) return 0;
-    if (!points || !idx || !weight || !out) return (int)cudaErrorInvalidValue;
-    cudaStream_t st = as_stream(stream);
-    if (c % 4 == 0 && al16(points) && al16(out)) {
+    if (c % 4 == 0 && aligned_to(points, sizeof(P)) && aligned_to(out, sizeof(P))) {
         const unsigned long long tv = total / 4;
         const unsigned grid = it_grid(tv, kItThreads);
         if (tv < (1ull << 31))
-            three_interp_vec4_kernel<unsigned, 1><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned)n, (unsigned)tv, (const float4*)points, idx, weight, (float4*)out);
+            three_interp_vec4_kernel<unsigned, 1, T><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned)n, (unsigned)tv, (const P*)points, idx, weight, (P*)out);
         else
-            three_interp_vec4_kernel<unsigned long long, 1><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned long long)n, tv, (const float4*)points, idx, weight, (float4*)out);
+            three_interp_vec4_kernel<unsigned long long, 1, T><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned long long)n, tv, (const P*)points, idx, weight, (P*)out);
     } else {
         const unsigned grid = it_grid(total, kItThreads);
         if (total < (1ull << 31))
-            three_interp_scalar_kernel<unsigned><<<grid, kItThreads, 0, st>>>(m, c, (unsigned)n, (unsigned)total, points, idx, weight, out);
+            three_interp_scalar_kernel<unsigned, T><<<grid, kItThreads, 0, st>>>(m, c, (unsigned)n, (unsigned)total, points, idx, weight, out);
         else
-            three_interp_scalar_kernel<unsigned long long><<<grid, kItThreads, 0, st>>>(m, c, (unsigned long long)n, total, points, idx, weight, out);
+            three_interp_scalar_kernel<unsigned long long, T><<<grid, kItThreads, 0, st>>>(m, c, (unsigned long long)n, total, points, idx, weight, out);
     }
     return finish_launch();
 }
 
-int pn2_three_interpolate_grad(int b, int n, int c, int m, const float* grad_out, const int* idx, const float* weight,
-                               float* grad_points, void* stream) {
-    using namespace pn2;
-    if (b < 0 || m <= 0 || c < 0 || n < 0) return (int)cudaErrorInvalidValue;
-    const unsigned long long total = (unsigned long long)b * n * c;
-    if (total == 0) return 0;
-    if (!grad_out || !idx || !weight || !grad_points) return (int)cudaErrorInvalidValue;
-    cudaStream_t st = as_stream(stream);
-    if (c % 4 == 0 && al16(grad_out) && al16(grad_points)) {
-        const unsigned long long tv = total / 4;
-        const unsigned grid = it_grid(tv, kItThreads);
-        if (tv < (1ull << 31))
-            three_interp_grad_vec4_kernel<unsigned><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned)n, (unsigned)tv, (const float4*)grad_out, idx, weight, (float4*)grad_points);
-        else
-            three_interp_grad_vec4_kernel<unsigned long long><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned long long)n, tv, (const float4*)grad_out, idx, weight, (float4*)grad_points);
-    } else {
-        const unsigned grid = it_grid(total, kItThreads);
-        if (total < (1ull << 31))
-            three_interp_grad_scalar_kernel<unsigned><<<grid, kItThreads, 0, st>>>(m, c, (unsigned)n, (unsigned)total, grad_out, idx, weight, grad_points);
-        else
-            three_interp_grad_scalar_kernel<unsigned long long><<<grid, kItThreads, 0, st>>>(m, c, (unsigned long long)n, total, grad_out, idx, weight, grad_points);
-    }
-    return finish_launch();
-}
-
-int pn2_three_nn_interpolate(int b, int n, int m, int c, const float* xyz1, const float* xyz2, const float* points2,
-                             float* out, float* dist, int* idx, float* weight, void* stream) {
-    using namespace pn2;
-    if (b < 0 || n < 0 || m <= 0 || c < 0) return (int)cudaErrorInvalidValue;
-    if (b == 0 || n == 0) return 0;
-    if (!xyz1 || !xyz2 || (c > 0 && (!points2 || !out))) return (int)cudaErrorInvalidValue;
-    if (b > 65535) return (int)cudaErrorInvalidValue;
-    return fp_front_dispatch(b, n, m, c, 0, xyz1, xyz2, nullptr, points2, c > 0 ? out : nullptr, dist, idx, weight, as_stream(stream));
-}
-
-int pn2_fp_interpolate_concat(int b, int n, int m, int c2, int c1, const float* xyz1, const float* xyz2, const float* points1,
-                              const float* points2, float* out, void* stream) {
-    using namespace pn2;
-    if (b < 0 || n < 0 || m <= 0 || c2 <= 0 || c1 < 0) return (int)cudaErrorInvalidValue;
-    if (b == 0 || n == 0) return 0;
-    if (!xyz1 || !xyz2 || !points2 || !out || (c1 > 0 && !points1)) return (int)cudaErrorInvalidValue;
-    if (b > 65535) return (int)cudaErrorInvalidValue;
-    return fp_front_dispatch(b, n, m, c2, c1, xyz1, xyz2, c1 > 0 ? points1 : nullptr, points2, out, nullptr, nullptr, nullptr,
-                             as_stream(stream));
-}
-
-size_t pn2_three_interpolate_grad_det_workspace_bytes(int b, int n, int m) {
-    if (b <= 0 || n <= 0 || m <= 0) return 0;
-    // offsets (b, m+1) + cursors (b, m) + entries (b, 3n) + queue of long lists (1 + b * ceil(3n / (cap+1))), ints
-    const size_t longs = (size_t)b * ((3 * (size_t)n) / (pn2::kInvSortCap + 1) + 1);
-    return sizeof(int) * ((size_t)b * (m + 1) + (size_t)b * m + (size_t)b * 3 * (size_t)n + 1 + longs);
-}
-
-int pn2_three_interpolate_grad_det(int b, int n, int c, int m, const float* grad_out, const int* idx, const float* weight,
-                                   float* grad_points, void* workspace, size_t workspace_bytes, void* stream) {
-    using namespace pn2;
+template <typename T>
+static int three_interpolate_grad_det_impl(int b, int n, int c, int m, const T* grad_out, const int* idx, const float* weight,
+                                           T* grad_points, void* workspace, size_t workspace_bytes, int f16, void* stream) {
     if (b < 0 || m <= 0 || c < 0 || n < 0) return (int)cudaErrorInvalidValue;
     if ((unsigned long long)b * m * c == 0) return 0;
     if (!grad_points) return (int)cudaErrorInvalidValue;
     cudaStream_t st = as_stream(stream);
-    if (n == 0) return (int)cudaMemsetAsync(grad_points, 0, sizeof(float) * (size_t)b * m * c, st);
+    if (n == 0) return (int)cudaMemsetAsync(grad_points, 0, sizeof(T) * (size_t)b * m * c, st);
     if (!grad_out || !idx || !weight || !workspace) return (int)cudaErrorInvalidValue;
-    if (workspace_bytes < pn2_three_interpolate_grad_det_workspace_bytes(b, n, m) || (long long)n * 3 > 0x7fffffffLL)
+    if (workspace_bytes < ::pn2_three_interpolate_grad_det_workspace_bytes(b, n, m) || (long long)n * 3 > 0x7fffffffLL)
         return (int)cudaErrorInvalidValue;
     int* off = static_cast<int*>(workspace);
     int* cur = off + (size_t)b * (m + 1);
@@ -866,15 +831,161 @@ int pn2_three_interpolate_grad_det(int b, int n, int c, int m, const float* grad
     if (blocks > 0x7fffffffull) return (int)cudaErrorInvalidValue;
     // long lists: a fixed grid walks the queue (usually empty: the CTAs read one word and leave)
     const unsigned long_grid = (unsigned)num_sms() * 2u;
-    if (c % 4 == 0 && al16(grad_out) && al16(grad_points)) {
-        inv_gather_kernel<true><<<(unsigned)blocks, kInvThreads, 0, st>>>(n, c, m, warps, grad_out, weight, off, entries, grad_points, long_queue);
-        inv_long_kernel<true><<<long_grid, kInvThreads, 0, st>>>(n, c, m, grad_out, idx, weight, long_queue, grad_points);
+    if (c % 4 == 0 && aligned_to(grad_out, 4 * sizeof(T)) && aligned_to(grad_points, 4 * sizeof(T))) {
+        inv_gather_kernel<true, T><<<(unsigned)blocks, kInvThreads, 0, st>>>(n, c, m, warps, grad_out, weight, off, entries, grad_points, long_queue, f16);
+        inv_long_kernel<true, T><<<long_grid, kInvThreads, 0, st>>>(n, c, m, grad_out, idx, weight, long_queue, grad_points, f16);
     } else {
-        inv_gather_kernel<false><<<(unsigned)blocks, kInvThreads, 0, st>>>(n, c, m, warps, grad_out, weight, off, entries, grad_points, long_queue);
-        inv_long_kernel<false><<<long_grid, kInvThreads, 0, st>>>(n, c, m, grad_out, idx, weight, long_queue, grad_points);
+        inv_gather_kernel<false, T><<<(unsigned)blocks, kInvThreads, 0, st>>>(n, c, m, warps, grad_out, weight, off, entries, grad_points, long_queue, f16);
+        inv_long_kernel<false, T><<<long_grid, kInvThreads, 0, st>>>(n, c, m, grad_out, idx, weight, long_queue, grad_points, f16);
     }
     count_launch(launches - 1);
     return finish_launch();
+}
+
+}  // namespace pn2
+
+extern "C" {
+
+int pn2_three_nn(int b, int n, int m, const float* xyz1, const float* xyz2, float* dist, int* idx, void* stream) {
+    using namespace pn2;
+    if (b < 0 || n < 0 || m < 0) return (int)cudaErrorInvalidValue;
+    if (b == 0 || n == 0) return 0;
+    if (!xyz1 || (m > 0 && !xyz2) || !dist || !idx) return (int)cudaErrorInvalidValue;
+    if (b > 65535) return (int)cudaErrorInvalidValue;
+    dim3 grid((n + kNnThreads - 1) / kNnThreads, b, 1);
+    three_nn_kernel<<<grid, kNnThreads, 0, as_stream(stream)>>>(n, m, xyz1, xyz2, dist, idx);
+    return finish_launch();
+}
+
+int pn2_three_interpolate(int b, int m, int c, int n, const float* points, const int* idx, const float* weight,
+                          float* out, void* stream) {
+    using namespace pn2;
+    if (b < 0 || m <= 0 || c < 0 || n < 0) return (int)cudaErrorInvalidValue;
+    const unsigned long long total = (unsigned long long)b * n * c;
+    if (total == 0) return 0;
+    if (!points || !idx || !weight || !out) return (int)cudaErrorInvalidValue;
+    return three_interpolate_impl<float>(b, m, c, n, points, idx, weight, out, as_stream(stream));
+}
+
+int pn2_three_interpolate_typed(int dtype, int b, int m, int c, int n, const void* points, const int* idx,
+                                const float* weight, void* out, void* stream) {
+    using namespace pn2;
+    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
+    if (dtype == PN2_F32) return pn2_three_interpolate(b, m, c, n, static_cast<const float*>(points), idx, weight, static_cast<float*>(out), stream);
+    if (b < 0 || m <= 0 || c < 0 || n < 0) return (int)cudaErrorInvalidValue;
+    if ((unsigned long long)b * n * c == 0) return 0;
+    if (!points || !idx || !weight || !out) return (int)cudaErrorInvalidValue;
+    if (dtype == PN2_BF16)
+        return three_interpolate_impl<__nv_bfloat16>(b, m, c, n, static_cast<const __nv_bfloat16*>(points), idx, weight,
+                                                     static_cast<__nv_bfloat16*>(out), as_stream(stream));
+    return three_interpolate_impl<__half>(b, m, c, n, static_cast<const __half*>(points), idx, weight, static_cast<__half*>(out),
+                                          as_stream(stream));
+}
+
+int pn2_three_interpolate_grad(int b, int n, int c, int m, const float* grad_out, const int* idx, const float* weight,
+                               float* grad_points, void* stream) {
+    using namespace pn2;
+    if (b < 0 || m <= 0 || c < 0 || n < 0) return (int)cudaErrorInvalidValue;
+    const unsigned long long total = (unsigned long long)b * n * c;
+    if (total == 0) return 0;
+    if (!grad_out || !idx || !weight || !grad_points) return (int)cudaErrorInvalidValue;
+    cudaStream_t st = as_stream(stream);
+    if (c % 4 == 0 && al16(grad_out) && al16(grad_points)) {
+        const unsigned long long tv = total / 4;
+        const unsigned grid = it_grid(tv, kItThreads);
+        if (tv < (1ull << 31))
+            three_interp_grad_vec4_kernel<unsigned><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned)n, (unsigned)tv, (const float4*)grad_out, idx, weight, (float4*)grad_points);
+        else
+            three_interp_grad_vec4_kernel<unsigned long long><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned long long)n, tv, (const float4*)grad_out, idx, weight, (float4*)grad_points);
+    } else {
+        const unsigned grid = it_grid(total, kItThreads);
+        if (total < (1ull << 31))
+            three_interp_grad_scalar_kernel<unsigned><<<grid, kItThreads, 0, st>>>(m, c, (unsigned)n, (unsigned)total, grad_out, idx, weight, grad_points);
+        else
+            three_interp_grad_scalar_kernel<unsigned long long><<<grid, kItThreads, 0, st>>>(m, c, (unsigned long long)n, total, grad_out, idx, weight, grad_points);
+    }
+    return finish_launch();
+}
+
+int pn2_three_nn_interpolate(int b, int n, int m, int c, const float* xyz1, const float* xyz2, const float* points2,
+                             float* out, float* dist, int* idx, float* weight, void* stream) {
+    using namespace pn2;
+    if (b < 0 || n < 0 || m <= 0 || c < 0) return (int)cudaErrorInvalidValue;
+    if (b == 0 || n == 0) return 0;
+    if (!xyz1 || !xyz2 || (c > 0 && (!points2 || !out))) return (int)cudaErrorInvalidValue;
+    if (b > 65535) return (int)cudaErrorInvalidValue;
+    return fp_front_dispatch<float>(b, n, m, c, 0, xyz1, xyz2, nullptr, points2, c > 0 ? out : nullptr, dist, idx, weight, 0, as_stream(stream));
+}
+
+int pn2_three_nn_interpolate_typed(int dtype, int b, int n, int m, int c, const float* xyz1, const float* xyz2,
+                                   const void* points2, void* out, float* dist, int* idx, float* weight,
+                                   void* stream) {
+    using namespace pn2;
+    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
+    if (dtype == PN2_F32)
+        return pn2_three_nn_interpolate(b, n, m, c, xyz1, xyz2, static_cast<const float*>(points2), static_cast<float*>(out), dist, idx,
+                                        weight, stream);
+    if (b < 0 || n < 0 || m <= 0 || c < 0) return (int)cudaErrorInvalidValue;
+    if (b == 0 || n == 0) return 0;
+    if (!xyz1 || !xyz2 || (c > 0 && (!points2 || !out))) return (int)cudaErrorInvalidValue;
+    if (b > 65535) return (int)cudaErrorInvalidValue;
+    using U16 = unsigned short;  // bfloat16 and float16 share one instance: dtype == PN2_F16 selects the format
+    return fp_front_dispatch<U16>(b, n, m, c, 0, xyz1, xyz2, nullptr, static_cast<const U16*>(points2),
+                                  c > 0 ? static_cast<U16*>(out) : nullptr, dist, idx, weight, dtype == PN2_F16, as_stream(stream));
+}
+
+int pn2_fp_interpolate_concat(int b, int n, int m, int c2, int c1, const float* xyz1, const float* xyz2, const float* points1,
+                              const float* points2, float* out, void* stream) {
+    using namespace pn2;
+    if (b < 0 || n < 0 || m <= 0 || c2 <= 0 || c1 < 0) return (int)cudaErrorInvalidValue;
+    if (b == 0 || n == 0) return 0;
+    if (!xyz1 || !xyz2 || !points2 || !out || (c1 > 0 && !points1)) return (int)cudaErrorInvalidValue;
+    if (b > 65535) return (int)cudaErrorInvalidValue;
+    return fp_front_dispatch<float>(b, n, m, c2, c1, xyz1, xyz2, c1 > 0 ? points1 : nullptr, points2, out, nullptr, nullptr, nullptr,
+                                    0, as_stream(stream));
+}
+
+int pn2_fp_interpolate_concat_typed(int dtype, int b, int n, int m, int c2, int c1, const float* xyz1,
+                                    const float* xyz2, const void* points1, const void* points2, void* out,
+                                    void* stream) {
+    using namespace pn2;
+    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
+    if (dtype == PN2_F32)
+        return pn2_fp_interpolate_concat(b, n, m, c2, c1, xyz1, xyz2, static_cast<const float*>(points1), static_cast<const float*>(points2),
+                                         static_cast<float*>(out), stream);
+    if (b < 0 || n < 0 || m <= 0 || c2 <= 0 || c1 < 0) return (int)cudaErrorInvalidValue;
+    if (b == 0 || n == 0) return 0;
+    if (!xyz1 || !xyz2 || !points2 || !out || (c1 > 0 && !points1)) return (int)cudaErrorInvalidValue;
+    if (b > 65535) return (int)cudaErrorInvalidValue;
+    using U16 = unsigned short;  // bfloat16 and float16 share one instance: dtype == PN2_F16 selects the format
+    return fp_front_dispatch<U16>(b, n, m, c2, c1, xyz1, xyz2, c1 > 0 ? static_cast<const U16*>(points1) : nullptr,
+                                  static_cast<const U16*>(points2), static_cast<U16*>(out), nullptr, nullptr, nullptr, dtype == PN2_F16,
+                                  as_stream(stream));
+}
+
+size_t pn2_three_interpolate_grad_det_workspace_bytes(int b, int n, int m) {
+    if (b <= 0 || n <= 0 || m <= 0) return 0;
+    // offsets (b, m+1) + cursors (b, m) + entries (b, 3n) + queue of long lists (1 + b * ceil(3n / (cap+1))), ints
+    const size_t longs = (size_t)b * ((3 * (size_t)n) / (pn2::kInvSortCap + 1) + 1);
+    return sizeof(int) * ((size_t)b * (m + 1) + (size_t)b * m + (size_t)b * 3 * (size_t)n + 1 + longs);
+}
+
+int pn2_three_interpolate_grad_det(int b, int n, int c, int m, const float* grad_out, const int* idx, const float* weight,
+                                   float* grad_points, void* workspace, size_t workspace_bytes, void* stream) {
+    return pn2::three_interpolate_grad_det_impl<float>(b, n, c, m, grad_out, idx, weight, grad_points, workspace, workspace_bytes, 0, stream);
+}
+
+int pn2_three_interpolate_grad_det_typed(int dtype, int b, int n, int c, int m, const void* grad_out,
+                                         const int* idx, const float* weight, void* grad_points, void* workspace,
+                                         size_t workspace_bytes, void* stream) {
+    using namespace pn2;
+    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
+    if (dtype == PN2_F32)
+        return pn2_three_interpolate_grad_det(b, n, c, m, static_cast<const float*>(grad_out), idx, weight, static_cast<float*>(grad_points),
+                                              workspace, workspace_bytes, stream);
+    using U16 = unsigned short;  // bfloat16 and float16 share one instance: dtype == PN2_F16 selects the format
+    return three_interpolate_grad_det_impl<U16>(b, n, c, m, static_cast<const U16*>(grad_out), idx, weight, static_cast<U16*>(grad_points),
+                                                workspace, workspace_bytes, dtype == PN2_F16, stream);
 }
 
 }  // extern "C"

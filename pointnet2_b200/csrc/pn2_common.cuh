@@ -1,5 +1,7 @@
 // pn2_common.cuh — shared device/host helpers for libpn2_b200 (sm_90a only).
 #pragma once
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -134,5 +136,70 @@ size_t fps_scratch_bytes(int b, int n);
 // ---- streaming memory ops ---------------------------------------------------------------------
 __device__ __forceinline__ void st_stream_f4(float4* p, float4 v) { __stcs(p, v); }
 __device__ __forceinline__ void st_stream_i4(int4* p, int4 v) { __stcs(p, v); }
+
+// ---- feature element types (PN2_F32 / PN2_BF16 / PN2_F16) -------------------------------------
+// Features may be float, bfloat16 or half; arithmetic is always float32.  Loads upcast exactly,
+// stores round once to nearest even (the rounding torch's .to(dtype) uses).
+__device__ __forceinline__ float to_f32(float x) { return x; }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 x) { return __bfloat162float(x); }
+__device__ __forceinline__ float to_f32(__half x) { return __half2float(x); }
+template <typename T> __device__ __forceinline__ T from_f32(float x);
+template <> __device__ __forceinline__ float from_f32<float>(float x) { return x; }
+template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
+template <> __device__ __forceinline__ __half from_f32<__half>(float x) { return __float2half_rn(x); }
+
+// Four consecutive elements as one vector: float4 (16 bytes) for float, uint2 (8 bytes) for 2-byte types.
+template <typename T> struct Pack4 { using type = uint2; };
+template <> struct Pack4<float> { using type = float4; };
+
+__device__ __forceinline__ float lo16_f32(unsigned w, __nv_bfloat16) { return __uint_as_float(w << 16); }
+__device__ __forceinline__ float lo16_f32(unsigned w, __half) { return __half2float(__ushort_as_half((unsigned short)(w & 0xffffu))); }
+// (the second argument only selects the element type)
+__device__ __forceinline__ float4 unpack4(float4 v, float) { return v; }
+template <typename T> __device__ __forceinline__ float4 unpack4(uint2 v, T t) {
+    return make_float4(lo16_f32(v.x, t), lo16_f32(v.x >> 16, t), lo16_f32(v.y, t), lo16_f32(v.y >> 16, t));
+}
+template <typename T> __device__ __forceinline__ unsigned short bits16(float a) {
+    const T x = from_f32<T>(a);
+    return *reinterpret_cast<const unsigned short*>(&x);
+}
+__device__ __forceinline__ float4 pack4(float4 v, float) { return v; }
+template <typename T> __device__ __forceinline__ uint2 pack4(float4 v, T) {
+    return make_uint2((unsigned)bits16<T>(v.x) | ((unsigned)bits16<T>(v.y) << 16),
+                      (unsigned)bits16<T>(v.z) | ((unsigned)bits16<T>(v.w) << 16));
+}
+
+// 4 elements at p (4 * sizeof(T)-byte aligned) upcast to float: read-only path / streaming read
+template <typename T> __device__ __forceinline__ float4 ldg4(const T* p) {
+    return unpack4(__ldg(reinterpret_cast<const typename Pack4<T>::type*>(p)), T());
+}
+template <typename T> __device__ __forceinline__ float4 ldcs4(const T* p) {
+    return unpack4(__ldcs(reinterpret_cast<const typename Pack4<T>::type*>(p)), T());
+}
+template <typename T> __device__ __forceinline__ void st4(T* p, float4 v) {
+    *reinterpret_cast<typename Pack4<T>::type*>(p) = pack4(v, T());
+}
+
+// 2-byte features whose format is a runtime flag (f16 != 0: float16, else bfloat16), held as their raw unsigned short bits:
+// one instantiation serves both where the code around the conversions is large (the FP front end's 3-NN phase).
+// The float overloads ignore the flag.
+__device__ __forceinline__ float f32_of(float x, int) { return x; }
+__device__ __forceinline__ float f32_of(unsigned short x, int f16) {
+    return f16 ? __half2float(__ushort_as_half(x)) : __uint_as_float((unsigned)x << 16);
+}
+template <typename T> __device__ __forceinline__ T of_f32(float x, int f16);
+template <> __device__ __forceinline__ float of_f32<float>(float x, int) { return x; }
+template <> __device__ __forceinline__ unsigned short of_f32<unsigned short>(float x, int f16) {
+    return f16 ? __half_as_ushort(__float2half_rn(x)) : __bfloat16_as_ushort(__float2bfloat16_rn(x));
+}
+__device__ __forceinline__ float4 unpack4_of(float4 v, int) { return v; }
+__device__ __forceinline__ float4 unpack4_of(uint2 v, int f16) { return f16 ? unpack4(v, __half()) : unpack4(v, __nv_bfloat16()); }
+__device__ __forceinline__ float4 pack4_of(float4 v, float, int) { return v; }
+__device__ __forceinline__ uint2 pack4_of(float4 v, unsigned short, int f16) {
+    return f16 ? pack4(v, __half()) : pack4(v, __nv_bfloat16());
+}
+
+inline bool aligned_to(const void* p, unsigned bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1u)) == 0; }
+inline bool valid_dtype(int dtype) { return dtype == PN2_F32 || dtype == PN2_BF16 || dtype == PN2_F16; }
 
 }  // namespace pn2

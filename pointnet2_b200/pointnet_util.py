@@ -20,30 +20,38 @@ from typing import Callable, Optional, Sequence
 import torch
 
 from . import _lib, layers
-from ._tensor import on_device, ptr, require_cuda, same_device, stream_ptr
-from .tf_grouping import group_point, knn_point, query_ball_point
+from ._tensor import DTYPE_CODES, FEATURE_DTYPES, on_device, ptr, require_cuda, same_device, stream_ptr
+from .tf_grouping import group_point, group_point_grad, knn_point, query_ball_point
 from .tf_interpolate import fp_interpolate_concat, three_interpolate, three_nn, three_nn_interpolate
 from .sa_layer import sample_group, sample_group_msg
 from .tf_sampling import farthest_point_sample, farthest_point_sample_and_gather, gather_point
 
 
 class _GroupConcat(torch.autograd.Function):
-    """out = concat(xyz[idx]-new_xyz, points[idx]) in either channel order, plus grouped_xyz."""
+    """out = concat(xyz[idx]-new_xyz, points[idx]) in either channel order, plus grouped_xyz.  out has the dtype of
+    ``points`` (float32 without points); grouped_xyz is float32."""
 
     @staticmethod
     def forward(ctx, xyz, new_xyz, points, idx, xyz_first):
         b, n, _ = xyz.shape
         _, m, s = idx.shape
         c = 0 if points is None else points.shape[2]
-        out = torch.empty((b, m, s, 3 + c), dtype=torch.float32, device=xyz.device)
+        dtype = torch.float32 if points is None else points.dtype
+        out = torch.empty((b, m, s, 3 + c), dtype=dtype, device=xyz.device)
         gxyz = torch.empty((b, m, s, 3), dtype=torch.float32, device=xyz.device)
         if out.numel():
             with on_device(xyz):
-                rc = _lib.load().pn2_group_concat(b, n, c, m, s, ptr(xyz), ptr(new_xyz), ptr(points), ptr(idx),
-                                                  1 if xyz_first else 0, ptr(out), ptr(gxyz), stream_ptr(xyz.device))
+                if dtype == torch.float32:
+                    rc = _lib.load().pn2_group_concat(b, n, c, m, s, ptr(xyz), ptr(new_xyz), ptr(points), ptr(idx),
+                                                      1 if xyz_first else 0, ptr(out), ptr(gxyz), stream_ptr(xyz.device))
+                else:
+                    rc = _lib.load().pn2_group_concat_typed(DTYPE_CODES[dtype], b, n, c, m, s, ptr(xyz), ptr(new_xyz), ptr(points),
+                                                            ptr(idx), 1 if xyz_first else 0, ptr(out), ptr(gxyz),
+                                                            stream_ptr(xyz.device))
             _lib.check(rc, "pn2_group_concat")
         ctx.save_for_backward(idx)
         ctx.meta = (b, n, c, m, s, bool(xyz_first), points is not None)
+        ctx.dtype = dtype
         return out, gxyz
 
     @staticmethod
@@ -53,7 +61,8 @@ class _GroupConcat(torch.autograd.Function):
         lib = _lib.load()
         dev = g_out.device
         lo = 0 if xyz_first else c
-        g_xyz_part = g_out[..., lo:lo + 3]
+        g_out = g_out.to(ctx.dtype)
+        g_xyz_part = g_out[..., lo:lo + 3].float()  # the coordinates' gradient is float32 (an exact upcast)
         if g_gxyz is not None:
             g_xyz_part = g_xyz_part + g_gxyz
         g_xyz_part = g_xyz_part.contiguous()
@@ -63,22 +72,23 @@ class _GroupConcat(torch.autograd.Function):
             st = stream_ptr(dev)
             _lib.check(lib.pn2_group_point_grad(b, n, 3, m, s, ptr(g_xyz_part), ptr(idx), ptr(g_xyz), st),
                        "pn2_group_point_grad")
-            if has_points:
-                g_feat = (g_out[..., 3:] if xyz_first else g_out[..., :c]).contiguous()
-                g_points = torch.zeros((b, n, c), dtype=torch.float32, device=dev)
-                _lib.check(lib.pn2_group_point_grad(b, n, c, m, s, ptr(g_feat), ptr(idx), ptr(g_points), st),
-                           "pn2_group_point_grad")
+        if has_points:
+            g_feat = (g_out[..., 3:] if xyz_first else g_out[..., :c]).contiguous()
+            g_points = group_point_grad(g_feat, idx, (b, n, c))
         g_new_xyz = -g_xyz_part.sum(dim=2)
         return g_xyz, g_new_xyz, g_points, None, None
 
 
 def group_and_concat(xyz, new_xyz, points, idx, xyz_first: bool = True):
-    """Fused tail of sample_and_group: returns (new_points (b,m,s,3+c), grouped_xyz (b,m,s,3))."""
+    """Fused tail of sample_and_group: returns (new_points (b,m,s,3+c), grouped_xyz (b,m,s,3)).
+
+    ``points`` may be float32, bfloat16 or float16: new_points then has its dtype, with the feature channels copied and
+    the xyz channels (float32 differences) rounded once; grouped_xyz is float32 in every case."""
     xyz = require_cuda(xyz, "xyz", torch.float32)
     new_xyz = require_cuda(new_xyz, "new_xyz", torch.float32)
     idx = require_cuda(idx, "idx", torch.int32)
     if points is not None:
-        points = require_cuda(points, "points", torch.float32)
+        points = require_cuda(points, "points", FEATURE_DTYPES)
         same_device(xyz, new_xyz, idx, points)
         if points.dim() != 3 or points.shape[:2] != xyz.shape[:2]:
             raise ValueError("points must be (batch_size, ndataset, channel) matching xyz")
@@ -95,7 +105,8 @@ def sample_and_group(npoint, radius, nsample, xyz, points, knn=False, use_xyz=Tr
 
     Args:
         npoint, radius, nsample: centroids to sample, ball radius, neighbours kept per centroid.
-        xyz (b, n, 3) float32; points (b, n, c) float32 or None (then the grouped xyz are the features).
+        xyz (b, n, 3) float32; points (b, n, c) float32, bfloat16 or float16, or None (then the grouped xyz are
+        the features).  new_points has the dtype of points (float32 without points).
         knn: k-nearest-neighbour grouping instead of the ball query; use_xyz: keep the centred xyz
         in front of the grouped features.
     Returns:
@@ -139,7 +150,8 @@ def sample_and_group(npoint, radius, nsample, xyz, points, knn=False, use_xyz=Tr
         new_points = grouped_xyz
     else:
         grouped_points = group_point(points, idx)
-        new_points = torch.cat([grouped_xyz, grouped_points], dim=-1) if use_xyz else grouped_points
+        # (cast back: torch.cat promotes 16-bit features to the coordinates' float32)
+        new_points = torch.cat([grouped_xyz, grouped_points], dim=-1).to(points.dtype) if use_xyz else grouped_points
     return new_xyz, new_points, idx, grouped_xyz
 
 
@@ -243,7 +255,7 @@ def pointnet_sa_module_msg(xyz, points, npoint, radius_list: Sequence[float], ns
                 if points is not None:
                     grouped_points = group_point(points, idx)
                     if use_xyz:
-                        grouped_points = torch.cat([grouped_points, grouped_xyz], dim=-1)
+                        grouped_points = torch.cat([grouped_points, grouped_xyz], dim=-1).to(points.dtype)
                 else:
                     grouped_points = grouped_xyz
         grouped_points = _apply_mlp(None if mlp_list is None else mlp_list[i], grouped_points, scope, f"conv{i}", bn, is_training, bn_decay)
@@ -259,7 +271,8 @@ def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp=None, is_training=None,
         Return: new_points (b,n1,mlp[-1]) (or (b,n1,c2+c1) when mlp is None)
     '''
     no_grad = not points2.requires_grad and (points1 is None or not points1.requires_grad)
-    if fused and no_grad and points2.shape[2] > 0:
+    same_dtype = points1 is None or points1.dtype == points2.dtype
+    if fused and no_grad and same_dtype and points2.shape[2] > 0:
         # one kernel: 3-NN, weights, interpolation and the concat of :219
         new_points1 = fp_interpolate_concat(xyz1, xyz2, points1, points2)
     else:

@@ -89,7 +89,9 @@ CFG4_SEMSEG = dict(name="cfg4_scannet_semseg", b=16, n=8192, dist="D", seed=100,
 CFG5_SWEEP = dict(name="cfg5_sweep", b=8, ns=[4096, 16384, 65536, 262144], nsample=32, radius=0.1, dist="U")
 
 
-# ---- algorithmic bytes (BASELINE.md §4): each tensor touched once, 4-byte elements --------------
+# ---- algorithmic bytes (BASELINE.md §4): each tensor touched once -------------------------------
+# `esz` is the size of a FEATURE element (4 = float32, 2 = bfloat16 / float16); coordinates, weights and indices are
+# always 4 bytes.
 def bytes_fps(b, n, m, with_new_xyz=False):
     return 12 * b * n + 4 * b * m + (12 * b * m if with_new_xyz else 0)
 
@@ -102,16 +104,30 @@ def bytes_ball_query(b, n, m, s):
     return 12 * b * n + 12 * b * m + 4 * b * m * s + 4 * b * m
 
 
-def bytes_group(b, n, m, s, c):
-    return 4 * b * m * s + 4 * b * min(n, m * s) * c + 4 * b * m * s * c
+def bytes_group(b, n, m, s, c, esz=4):
+    return 4 * b * m * s + esz * b * min(n, m * s) * c + esz * b * m * s * c
 
 
 def bytes_three_nn(b, n, m):
     return 12 * b * n + 12 * b * m + 24 * b * n
 
 
-def bytes_three_interpolate(b, n, m, c):
-    return 4 * b * m * c + 24 * b * n + 4 * b * n * c
+def bytes_three_interpolate(b, n, m, c, esz=4):
+    return esz * b * m * c + 24 * b * n + esz * b * n * c
+
+
+def bytes_group_concat(b, n, m, s, c, esz=4):
+    """group_concat: idx, xyz + features of the distinct source rows, (3 + c)-wide output rows."""
+    return 4 * b * m * s + (12 + esz * c) * b * min(n, m * s) + esz * b * m * s * (3 + c)
+
+
+def bytes_three_interpolate_grad(b, n, m, c, esz=4):
+    """three_interpolate's gradient: grad_out read, grad_points written (read-modify-write for the atomics)."""
+    return 2 * esz * b * m * c + 24 * b * n + esz * b * n * c
+
+
+def bytes_fp_interpolate_concat(b, n, m, c2, c1, esz=4):
+    return 12 * b * n + 12 * b * m + esz * b * m * c2 + esz * b * n * c1 + esz * b * n * (c2 + c1)
 
 
 def bytes_sa_layer(b, n, m, s, c=3):

@@ -20,10 +20,10 @@ WATCH = [("CREDUX", r"^CREDUX"), ("REDUX", r"^REDUX"), ("FADD2", r"^FADD2"), ("F
 SHOW = ["fps_cta_kernel<16, 256, 0>", "fps_cta_kernel<16, 256, 1>", "fps_cta_kernel<32, 256, 1>", "fps_cluster_kernel<16, 128, 16, 1>", "fps_cluster_kernel<32, 128, 32, 0>", "fps_cluster_kernel<32, 128, 32, 1>", "fps_cluster_kernel<32, 512, 16, 1>",
         "fps_cluster_big_kernel<52, 512, 16, 0>", "fps_cluster_big_kernel<52, 512, 16, 1>",
         "ball_group_kernel", "knn_kernel", "ball_query_kernel<16>", "bq_grid_build_kernel", "bq_grid_query_kernel",
-        "group_rows_vec4_kernel<32, 4>", "group_narrow_kernel<0>", "group_rows_kernel<32, true>", "group_concat_vec_kernel<16, 2>",
-        "group_point_grad_vec4_kernel<unsigned int>", "three_nn_kernel", "fp_front_kernel<1>", "fp_front_kernel<8>",
-        "three_interp_vec4_kernel<unsigned int, 1>", "three_interp_grad_vec4_kernel<unsigned int>", "inv_build_kernel",
-        "inv_gather_kernel<true>", "inv_long_kernel<true>", "selection_sort_kernel", "prob_cumsum_kernel", "prob_search_kernel"]
+        "group_rows_vec4_kernel<32, 4>", "group_narrow_kernel<false, float>", "group_rows_kernel<32, true, float>", "group_concat_vec_kernel<16, 2>",
+        "group_point_grad_vec4_kernel<unsigned int, float>", "group_point_grad_vec4_kernel<unsigned int, __nv_bfloat16>", "three_nn_kernel", "fp_front_kernel<1, float>", "fp_front_kernel<8, float>", "fp_front_kernel<8, unsigned short>", "group_rows_kernel<32, true, unsigned short>",
+        "three_interp_vec4_kernel<unsigned int, 1, float, float4>", "three_interp_vec4_kernel<unsigned int, 1, __nv_bfloat16, uint2>", "three_interp_grad_vec4_kernel<unsigned int>", "inv_build_kernel",
+        "inv_gather_kernel<true, float>", "inv_long_kernel<true, float>", "inv_gather_kernel<true, unsigned short>", "inv_long_kernel<true, unsigned short>", "selection_sort_kernel", "prob_cumsum_kernel", "prob_search_kernel"]
 
 
 def demangle(names):
@@ -74,6 +74,7 @@ def main():
             lines.append(f"{nice}\n    REG {u.get('REG')}  STACK {u.get('STACK')}  SHARED {u.get('SHARED')}  instructions {total[k]}\n    "
                          + "  ".join(f"{w}:{c[w]}" for w, _ in WATCH if c[w]))
     out = os.path.join(ROOT, "profiles", "r2_sass_audit.txt")
+    os.makedirs(os.path.dirname(out), exist_ok=True)
     with open(out, "w") as f:
         f.write("\n".join(lines) + "\n")
     print(open(out).read())

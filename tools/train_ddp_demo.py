@@ -9,6 +9,7 @@ Adam, lr 1e-3 decayed 0.7x every 200000 samples (floored at 1e-5), batch-norm de
 min(0.99, 1 - 0.5 * 0.5^(samples/200000)).
 
     python tools/train_ddp_demo.py --steps 20                                   # one GPU
+    python tools/train_ddp_demo.py --steps 30 --amp bf16                        # bf16 autocast
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 \
         tools/train_ddp_demo.py --steps 20                                      # one rank per GPU
 
@@ -76,6 +77,8 @@ def main() -> None:
     ap.add_argument("--lr", type=float, default=1e-3)
     ap.add_argument("--decay-step", type=float, default=200000)
     ap.add_argument("--json", type=str, default=None)
+    ap.add_argument("--amp", choices=["none", "bf16", "fp16"], default="none",
+                    help="mixed precision: torch.autocast in bfloat16, or float16 with a GradScaler")
     args = ap.parse_args()
 
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -100,6 +103,8 @@ def main() -> None:
     model = model.to(dev)
     net = torch.nn.parallel.DistributedDataParallel(model, device_ids=[local]) if world > 1 else model
     opt = torch.optim.Adam(net.parameters(), lr=args.lr)
+    amp_dtype = {"none": None, "bf16": torch.bfloat16, "fp16": torch.float16}[args.amp]
+    scaler = torch.amp.GradScaler("cuda") if args.amp == "fp16" else None
 
     rs = np.random.RandomState(1234)  # the same global batch stream on every rank; each takes its slice
     losses, t_steps = [], []
@@ -115,15 +120,21 @@ def main() -> None:
         torch.cuda.synchronize(dev)
         t0 = time.perf_counter()
         net.train()
-        pred, _ = net(xyz)
-        if args.model == "sem_seg":  # per-point labels: the cloud's class everywhere, unit weights
-            lab_pt = lab[:, None].expand(-1, args.num_point)
-            loss = nets.sem_seg_loss(pred, lab_pt, torch.ones_like(lab_pt, dtype=torch.float32))
-        else:
-            loss = nets.cls_loss(pred, lab)
+        with torch.autocast(device_type="cuda", dtype=amp_dtype, enabled=amp_dtype is not None):
+            pred, _ = net(xyz)
+            if args.model == "sem_seg":  # per-point labels: the cloud's class everywhere, unit weights
+                lab_pt = lab[:, None].expand(-1, args.num_point)
+                loss = nets.sem_seg_loss(pred, lab_pt, torch.ones_like(lab_pt, dtype=torch.float32))
+            else:
+                loss = nets.cls_loss(pred, lab)
         opt.zero_grad(set_to_none=True)
-        loss.backward()  # DDP all-reduces (averages) the gradients over NCCL here
-        opt.step()
+        if scaler is not None:
+            scaler.scale(loss).backward()  # DDP all-reduces (averages) the gradients over NCCL here
+            scaler.step(opt)
+            scaler.update()
+        else:
+            loss.backward()  # DDP all-reduces (averages) the gradients over NCCL here
+            opt.step()
         torch.cuda.synchronize(dev)
         t_steps.append(time.perf_counter() - t0)
         lv = loss.detach()
@@ -146,7 +157,7 @@ def main() -> None:
         k = max(1, args.steps // 4)
         first, last = float(np.mean(losses[:k])), float(np.mean(losses[-k:]))
         steady = t_steps[min(3, len(t_steps) - 1):]
-        out = {"model": args.model, "world": world, "global_batch": args.batch, "num_point": args.num_point,
+        out = {"model": args.model, "amp": args.amp, "world": world, "global_batch": args.batch, "num_point": args.num_point,
                "steps": args.steps, "loss_first": first, "loss_last": last, "loss_decreased": last < first,
                "weights_identical_across_ranks": same, "ms_per_step_wallclock": 1e3 * float(np.median(steady)),
                "clouds_per_s": args.batch / float(np.median(steady)), "data": "synthetic parametric shapes"}
