@@ -217,6 +217,20 @@ def config_rows(torch, lib, dev, flush, peak, kind, world=1, rank=0, reps=10, fu
         nx = torch.empty((b, m, 3), dtype=torch.float32, device=dev)
         ms = timeit(torch, flush, lambda: lib.pn2_fps_gather(b, n, m, xyz.data_ptr(), None, fi.data_ptr(), nx.data_ptr(), None), reps=reps)
         add(tag, "fps+gather", ms, W.bytes_fps(b, n, m, True), dict(pairs_per_s=b * (m - 1) * n / (ms * 1e-3), us_per_iter=1e3 * ms / max(m - 1, 1)))
+        if full and tag.startswith("cfg2"):  # gather_point's backward: atomics (with the zero-fill) and the ordered sums
+            og, ig = torch.randn((b, m, 3), device=dev), torch.empty((b, n, 3), device=dev)
+
+            def ggrad():
+                ig.zero_()
+                lib.pn2_gather_point_grad(b, n, m, og.data_ptr(), fi.data_ptr(), ig.data_ptr(), None)
+            ms = timeit(torch, flush, ggrad, reps=reps)
+            add(tag, "gather_point_grad (atomics, incl. zero-fill)", ms, 4 * b * m + 12 * b * m + 2 * 12 * b * n)
+            gwsb = int(lib.pn2_group_point_grad_det_workspace_bytes(b, n, m, 1))
+            gws = torch.empty(gwsb, dtype=torch.uint8, device=dev)
+            ms = timeit(torch, flush, lambda: lib.pn2_gather_point_grad_det(b, n, m, og.data_ptr(), fi.data_ptr(), ig.data_ptr(), gws.data_ptr(),
+                                                                            gwsb, None), reps=reps)
+            add(tag, "gather_point_grad (deterministic, inverse index)", ms, 4 * b * m + 12 * b * m + 12 * b * n)
+            del og, ig, gws
         idx = torch.empty((b, m, s), dtype=torch.int32, device=dev)
         cnt = torch.empty((b, m), dtype=torch.int32, device=dev)
         wsb = int(lib.pn2_query_ball_point_workspace_bytes(b, n))
@@ -264,7 +278,24 @@ def config_rows(torch, lib, dev, flush, peak, kind, world=1, rank=0, reps=10, fu
                 lib.pn2_group_point_grad(b, n, c, m, s, go.data_ptr(), idx.data_ptr(), gp.data_ptr(), None)
             ms = timeit(torch, flush, grad, reps=reps)
             add(tag, f"group_point_grad C={c} S={s} (incl. zero-fill)", ms, 4 * b * m * s + 4 * b * m * s * c + 2 * 4 * b * n * c)
-            del go, gp
+            # the ordered sums of deterministic mode: each output written once, no zero-fill
+            gwsb = int(lib.pn2_group_point_grad_det_workspace_bytes(b, n, m, s))
+            gws = torch.empty(gwsb, dtype=torch.uint8, device=dev)
+            ms = timeit(torch, flush, lambda: lib.pn2_group_point_grad_det(b, n, c, m, s, go.data_ptr(), idx.data_ptr(), gp.data_ptr(),
+                                                                           gws.data_ptr(), gwsb, None), reps=reps)
+            add(tag, f"group_point_grad C={c} S={s} (deterministic, inverse index)", ms, 4 * b * m * s + 4 * b * m * s * c + 4 * b * n * c)
+            goh, gph = go.to(torch.bfloat16), torch.empty((b, n, c), dtype=torch.bfloat16, device=dev)
+
+            def grad_h():
+                gp.zero_()  # the float32 accumulator
+                lib.pn2_group_point_grad_typed(BF16, b, n, c, m, s, goh.data_ptr(), idx.data_ptr(), gph.data_ptr(), gp.data_ptr(), None)
+            ms = timeit(torch, flush, grad_h, reps=reps)
+            add(tag, f"group_point_grad bf16 C={c} S={s} (incl. zero-fill and rounding pass)", ms,
+                4 * b * m * s + 2 * b * m * s * c + 3 * 4 * b * n * c + 2 * b * n * c)
+            ms = timeit(torch, flush, lambda: lib.pn2_group_point_grad_det_typed(BF16, b, n, c, m, s, goh.data_ptr(), idx.data_ptr(), gph.data_ptr(),
+                                                                                 gws.data_ptr(), gwsb, None), reps=reps)
+            add(tag, f"group_point_grad bf16 C={c} S={s} (deterministic, inverse index)", ms, 4 * b * m * s + 2 * b * m * s * c + 2 * b * n * c)
+            del go, gp, goh, gph, gws
         if c:
             out = torch.empty((b, m, s, 3 + c), dtype=torch.float32, device=dev)
             ms = timeit(torch, flush, lambda: lib.pn2_group_concat(b, n, c, m, s, xyz.data_ptr(), nx.data_ptr(), feats.data_ptr(),

@@ -68,6 +68,11 @@ int pn2_gather_point(int b, int n, int m, const float* inp, const int* idx, floa
 /* scatteraddpointLauncher(b,n,m,out_g,idx,inp_g), tf_sampling_g.cu:209-211.
  * inp_g (b,n,3) must be zero-filled by the caller. */
 int pn2_gather_point_grad(int b, int n, int m, const float* out_g, const int* idx, float* inp_g, void* stream);
+/* The same gradient WITHOUT atomics: pn2_group_point_grad_det with c = 3, nsample = 1, i.e. inp_g[b,i,:] is the
+ * sum of out_g[b,j,:] over the j with idx[b,j] == i in ascending j.  inp_g (b,n,3) is overwritten.
+ * workspace: pn2_group_point_grad_det_workspace_bytes(b, n, m, 1). */
+int pn2_gather_point_grad_det(int b, int n, int m, const float* out_g, const int* idx, float* inp_g,
+                              void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- grouping (replaces tf_ops/grouping/tf_grouping_g.cu launchers) ----------------------- */
 
@@ -111,6 +116,16 @@ int pn2_group_point(int b, int n, int c, int m, int nsample, const float* points
  * grad_points (b,n,c) must be zero-filled by the caller. */
 int pn2_group_point_grad(int b, int n, int c, int m, int nsample, const float* grad_out,
                          const int* idx, float* grad_points, void* stream);
+
+/* The same gradient WITHOUT atomics, for reproducible training: an inverse index (which entries e = j*nsample + k
+ * point at each data point) is built in `workspace` (pn2_group_point_grad_det_workspace_bytes(b,n,m,nsample) bytes),
+ * then each data point's rows are added in ascending e, the order group_point_grad_cpu (query_ball_point.cpp:70-84)
+ * adds them: the result is run-to-run deterministic and bit-identical to that function for any list length.
+ * grad_points (b,n,c) is overwritten (rows no entry references become 0): no zero-fill needed.
+ * m*nsample >= 2^31 or a workspace that is too small returns cudaErrorInvalidValue without a launch. */
+size_t pn2_group_point_grad_det_workspace_bytes(int b, int n, int m, int nsample);
+int pn2_group_point_grad_det(int b, int n, int c, int m, int nsample, const float* grad_out, const int* idx,
+                             float* grad_points, void* workspace, size_t workspace_bytes, void* stream);
 
 /* selectionSortLauncher(b,n,m,k,dist,outi,out), tf_grouping_g.cu:129-132 (select_top_k).
  * dist (b,m,n); outi (b,m,n) i32, out (b,m,n) f32: the first k columns hold the k smallest values
@@ -201,6 +216,11 @@ int pn2_group_point_typed(int dtype, int b, int n, int c, int m, int nsample, co
  * by the caller, as in pn2_group_point_grad). */
 int pn2_group_point_grad_typed(int dtype, int b, int n, int c, int m, int nsample, const void* grad_out,
                                const int* idx, void* grad_points, float* accum, void* stream);
+/* float32 sums in the same order as the untyped entry, rounded once; no accumulator.
+ * workspace: pn2_group_point_grad_det_workspace_bytes(b, n, m, nsample) */
+int pn2_group_point_grad_det_typed(int dtype, int b, int n, int c, int m, int nsample, const void* grad_out,
+                                   const int* idx, void* grad_points, void* workspace, size_t workspace_bytes,
+                                   void* stream);
 /* points and out in `dtype`; the xyz channels of out are the float32 differences rounded once;
  * grouped_xyz stays float32. */
 int pn2_group_concat_typed(int dtype, int b, int n, int c, int m, int nsample, const float* xyz,

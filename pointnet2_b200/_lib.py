@@ -21,6 +21,7 @@ _SIGNATURES = {
     "pn2_prob_sample": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P]),
     "pn2_gather_point": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P]),
     "pn2_gather_point_grad": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P]),
+    "pn2_gather_point_grad_det": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_query_ball_point": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P]),
     "pn2_query_ball_point_workspace_bytes": (c_size_t, [c_int, c_int]),
     "pn2_query_ball_point_ws": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, c_size_t, _P]),
@@ -28,6 +29,8 @@ _SIGNATURES = {
     "pn2_query_ball_point_prebuilt": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_group_point": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
     "pn2_group_point_grad": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
+    "pn2_group_point_grad_det_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "pn2_group_point_grad_det": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_selection_sort": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
     "pn2_knn_point": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
     "pn2_three_nn": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P]),
@@ -41,6 +44,7 @@ _SIGNATURES = {
     # 16-bit features: the untyped entry's arguments behind a leading dtype code (PN2_F32 / PN2_BF16 / PN2_F16)
     "pn2_group_point_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
     "pn2_group_point_grad_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
+    "pn2_group_point_grad_det_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_group_concat_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int, _P, _P, _P]),
     "pn2_three_interpolate_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
     "pn2_three_interpolate_grad_det_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_size_t, _P]),

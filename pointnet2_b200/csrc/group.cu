@@ -567,6 +567,20 @@ static int group_point_grad_round_impl(int b, int n, int c, int m, int nsample, 
     return finish_launch();
 }
 
+// the ordered-sum gradient (no atomics): T = float, or unsigned short for both 2-byte formats (f16 selects float16)
+template <typename T>
+static int group_point_grad_det_impl(int b, int n, int c, int m, int nsample, const T* grad_out, const int* idx,
+                                     T* grad_points, void* workspace, size_t workspace_bytes, int f16, cudaStream_t st) {
+    if (b < 0 || n <= 0 || c < 0 || m < 0 || nsample < 0) return (int)cudaErrorInvalidValue;
+    if ((unsigned long long)b * n * c == 0) return 0;
+    if (!grad_points) return (int)cudaErrorInvalidValue;
+    const long long ne = (long long)m * nsample;  // entries per cloud
+    if (ne == 0) return (int)cudaMemsetAsync(grad_points, 0, sizeof(T) * (size_t)b * n * c, st);
+    if (!grad_out || !idx || !workspace) return (int)cudaErrorInvalidValue;
+    if (ne > 0x7fffffffLL || workspace_bytes < inv_workspace_bytes(b, ne, n)) return (int)cudaErrorInvalidValue;
+    return inv_sum_rows_det<T>(b, (int)ne, c, n, grad_out, idx, grad_points, workspace, f16, st);
+}
+
 template <typename T>
 static int group_concat_impl(int b, int n, int c, int m, int nsample, const float* xyz, const float* new_xyz,
                              const void* points, const int* idx, int xyz_first, void* out, float* grouped_xyz, int f16,
@@ -600,6 +614,12 @@ int pn2_gather_point_grad(int b, int n, int m, const float* out_g, const int* id
     const long long total = (long long)b * m;
     gather_point_grad_kernel<<<grid_for(total, kCopyThreads), kCopyThreads, 0, as_stream(stream)>>>(n, m, total, out_g, idx, inp_g);
     return finish_launch();
+}
+
+int pn2_gather_point_grad_det(int b, int n, int m, const float* out_g, const int* idx, float* inp_g, void* workspace,
+                              size_t workspace_bytes, void* stream) {
+    return pn2::group_point_grad_det_impl<float>(b, n, 3, m, 1, out_g, idx, inp_g, workspace, workspace_bytes, 0,
+                                                 pn2::as_stream(stream));
 }
 
 int pn2_group_point(int b, int n, int c, int m, int nsample, const float* points, const int* idx, float* out,
@@ -645,6 +665,30 @@ int pn2_group_point_grad_typed(int dtype, int b, int n, int c, int m, int nsampl
     if (dtype == PN2_BF16)
         return group_point_grad_round_impl<__nv_bfloat16>(b, n, c, m, nsample, grad_out, idx, grad_points, accum, as_stream(stream));
     return group_point_grad_round_impl<__half>(b, n, c, m, nsample, grad_out, idx, grad_points, accum, as_stream(stream));
+}
+
+size_t pn2_group_point_grad_det_workspace_bytes(int b, int n, int m, int nsample) {
+    if (b <= 0 || n <= 0 || m <= 0 || nsample <= 0) return 0;
+    return pn2::inv_workspace_bytes(b, (long long)m * nsample, n);
+}
+
+int pn2_group_point_grad_det(int b, int n, int c, int m, int nsample, const float* grad_out, const int* idx,
+                             float* grad_points, void* workspace, size_t workspace_bytes, void* stream) {
+    return pn2::group_point_grad_det_impl<float>(b, n, c, m, nsample, grad_out, idx, grad_points, workspace, workspace_bytes, 0,
+                                                 pn2::as_stream(stream));
+}
+
+int pn2_group_point_grad_det_typed(int dtype, int b, int n, int c, int m, int nsample, const void* grad_out,
+                                   const int* idx, void* grad_points, void* workspace, size_t workspace_bytes,
+                                   void* stream) {
+    using namespace pn2;
+    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
+    using U16 = unsigned short;  // bfloat16 and float16 share one instance: dtype == PN2_F16 selects the format
+    if (dtype == PN2_F32)
+        return group_point_grad_det_impl<float>(b, n, c, m, nsample, static_cast<const float*>(grad_out), idx,
+                                                static_cast<float*>(grad_points), workspace, workspace_bytes, 0, as_stream(stream));
+    return group_point_grad_det_impl<U16>(b, n, c, m, nsample, static_cast<const U16*>(grad_out), idx, static_cast<U16*>(grad_points),
+                                          workspace, workspace_bytes, dtype == PN2_F16, as_stream(stream));
 }
 
 int pn2_group_concat(int b, int n, int c, int m, int nsample, const float* xyz, const float* new_xyz,

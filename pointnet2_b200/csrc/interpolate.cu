@@ -461,39 +461,43 @@ static int fp_front_dispatch(int b, int n, int m, int c2, int c1, const float* x
     }
 }
 
-// ---- three_interpolate_grad without atomics: an inverse index, then one warp per known point ------
-// grad_points[b,i,:] = sum over the entries e = 3j+t with idx[b,j,t] == i of grad_out[b,j,:] * weight[b,j,t],
+// ---- scatter-add without atomics: an inverse index, then one warp per target row ----------------------
+// Shared by three_interpolate's gradient (weighted) and the group_point / gather_point gradients (unweighted,
+// pn2::inv_sum_rows_det).  A cloud has `ne` entries, each pointing at one of `nt` target rows:
+//   weighted:   grad_points[b,i,:] = sum over e = 3j+t with idx[b,j,t] == i of grad_out[b,j,:] * weight[b,j,t]
+//   unweighted: dst[b,i,:]         = sum over e         with idx[b,e]   == i of src[b,e,:]
 // accumulated in ASCENDING e — the very order threeinterpolate_grad_cpu (tf_interpolate.cpp:131-153: j outer,
-// t = 1,2,3 inner) adds them, each product and sum rounded on its own — so the result is not only
-// deterministic but bit-identical to the reference's CPU function, and grad_points needs no zero-fill.
-// Build: count entries per known point (int atomics), exclusive scan per cloud, fill the CSR lists (order
-// inside a list is arbitrary), then every warp sorts its own list (<= 128 entries: bitonic sort in
-// registers; longer lists — degenerate layers where most unknown points share a neighbour — are served
-// by an index-ordered scan of the cloud's entries instead).
+// t = 1,2,3 inner) and group_point_grad_cpu (query_ball_point.cpp:70-84: j, k ascending) add them, each product and
+// sum rounded on its own — so the result is not only deterministic but bit-identical to the reference's CPU
+// functions, and the output needs no zero-fill.
+// Build: count entries per target (int atomics), exclusive scan per cloud, fill the CSR lists (order inside a list
+// is arbitrary), then every warp sorts its own list (<= 256 entries: bitonic sort in registers).  Longer lists are
+// queued: inv_long_kernel (weighted) and inv_long_seq_kernel (unweighted) serve them with an index-ordered scan of
+// the cloud's entries.
 constexpr int kInvThreads = 256;
 constexpr int kInvSortCap = 256;
 
 __global__ void __launch_bounds__(kInvThreads)
-inv_count_kernel(int n3, int m, long long total, const int* __restrict__ idx, int* __restrict__ cnt) {
+inv_count_kernel(int ne, int nt, long long total, const int* __restrict__ idx, int* __restrict__ cnt) {
     for (long long e = (long long)blockIdx.x * kInvThreads + threadIdx.x; e < total; e += (long long)gridDim.x * kInvThreads) {
-        const long long cloud = e / n3;
-        atomicAdd(cnt + cloud * (m + 1) + __ldg(idx + e), 1);
+        const long long cloud = e / ne;
+        atomicAdd(cnt + cloud * (nt + 1) + __ldg(idx + e), 1);
     }
 }
 
-// one CTA per cloud: off[i] = exclusive prefix of cnt[i], i = 0..m (off[m] = 3n); cur[i] = off[i]
+// one CTA per cloud: off[i] = exclusive prefix of cnt[i], i = 0..nt (off[nt] = ne); cur[i] = off[i]
 __global__ void __launch_bounds__(1024)
-inv_scan_kernel(int m, int* __restrict__ cnt_off, int* __restrict__ cur) {
+inv_scan_kernel(int nt, int* __restrict__ cnt_off, int* __restrict__ cur) {
     __shared__ int s_w[32];
     __shared__ int s_carry;
-    int* __restrict__ c = cnt_off + (size_t)blockIdx.x * (m + 1);
-    int* __restrict__ cu = cur + (size_t)blockIdx.x * m;
+    int* __restrict__ c = cnt_off + (size_t)blockIdx.x * (nt + 1);
+    int* __restrict__ cu = cur + (size_t)blockIdx.x * nt;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     if (tid == 0) s_carry = 0;
     __syncthreads();
-    for (int base = 0; base <= m; base += 1024) {
+    for (int base = 0; base <= nt; base += 1024) {
         const int i = base + tid;
-        const int v = (i < m) ? c[i] : 0;
+        const int v = (i < nt) ? c[i] : 0;
         int incl = v;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
@@ -510,8 +514,8 @@ inv_scan_kernel(int m, int* __restrict__ cnt_off, int* __restrict__ cur) {
         }
         const int carry = s_carry;
         const int excl = carry + __shfl_sync(kFullMask, winc - wv, warp) + incl - v;
-        if (i <= m) c[i] = excl;
-        if (i < m) cu[i] = excl;
+        if (i <= nt) c[i] = excl;
+        if (i < nt) cu[i] = excl;
         __syncthreads();
         if (tid == 1023) s_carry = excl + v;
         __syncthreads();
@@ -519,38 +523,38 @@ inv_scan_kernel(int m, int* __restrict__ cnt_off, int* __restrict__ cur) {
 }
 
 __global__ void __launch_bounds__(kInvThreads)
-inv_fill_kernel(int n3, int m, long long total, const int* __restrict__ idx, int* __restrict__ cur, int* __restrict__ entries) {
+inv_fill_kernel(int ne, int nt, long long total, const int* __restrict__ idx, int* __restrict__ cur, int* __restrict__ entries) {
     for (long long e = (long long)blockIdx.x * kInvThreads + threadIdx.x; e < total; e += (long long)gridDim.x * kInvThreads) {
-        const long long cloud = e / n3;
-        const int pos = atomicAdd(cur + cloud * m + __ldg(idx + e), 1);
-        entries[cloud * n3 + pos] = (int)(e - cloud * n3);
+        const long long cloud = e / ne;
+        const int pos = atomicAdd(cur + cloud * nt + __ldg(idx + e), 1);
+        entries[cloud * ne + pos] = (int)(e - cloud * ne);
     }
 }
 
-// count + scan + fill of one cloud in ONE CTA, with the counters and cursors in shared memory (m <= 16000): the
+// count + scan + fill of one cloud in ONE CTA, with the counters and cursors in shared memory (nt <= 16000): the
 // inverse index of a layer costs one launch instead of two memsets and three kernels.
 constexpr int kInvBuildMaxM = 16000;
 __global__ void __launch_bounds__(1024)
-inv_build_kernel(int n3, int m, const int* __restrict__ idx, int* __restrict__ off, int* __restrict__ entries,
+inv_build_kernel(int ne, int nt, const int* __restrict__ idx, int* __restrict__ off, int* __restrict__ entries,
                  int* __restrict__ long_queue) {
-    extern __shared__ int s_c[];  // [m + 1]: counts -> exclusive offsets (kept as the fill cursors)
+    extern __shared__ int s_c[];  // [nt + 1]: counts -> exclusive offsets (kept as the fill cursors)
     __shared__ int s_w[32];
     __shared__ int s_carry;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const long long cloud = blockIdx.x;
-    const int* __restrict__ cidx = idx + cloud * n3;
-    for (int i = tid; i <= m; i += 1024) s_c[i] = 0;
+    const int* __restrict__ cidx = idx + cloud * ne;
+    for (int i = tid; i <= nt; i += 1024) s_c[i] = 0;
     if (tid == 0) {
         s_carry = 0;
         if (cloud == 0) long_queue[0] = 0;
     }
     __syncthreads();
-    for (int e = tid; e < n3; e += 1024) atomicAdd(&s_c[__ldg(cidx + e)], 1);
+    for (int e = tid; e < ne; e += 1024) atomicAdd(&s_c[__ldg(cidx + e)], 1);
     __syncthreads();
-    int* __restrict__ o = off + cloud * (m + 1);
-    for (int base = 0; base <= m; base += 1024) {
+    int* __restrict__ o = off + cloud * (nt + 1);
+    for (int base = 0; base <= nt; base += 1024) {
         const int i = base + tid;
-        const int v = (i < m) ? s_c[i] : 0;
+        const int v = (i < nt) ? s_c[i] : 0;
         int incl = v;
 #pragma unroll
         for (int sft = 1; sft < 32; sft <<= 1) {
@@ -566,7 +570,7 @@ inv_build_kernel(int n3, int m, const int* __restrict__ idx, int* __restrict__ o
             if (lane >= sft) winc += t;
         }
         const int excl = s_carry + __shfl_sync(kFullMask, winc - wv, warp) + incl - v;
-        if (i <= m) {
+        if (i <= nt) {
             o[i] = excl;
             s_c[i] = excl;
         }
@@ -574,15 +578,17 @@ inv_build_kernel(int n3, int m, const int* __restrict__ idx, int* __restrict__ o
         if (tid == 1023) s_carry = excl + v;
         __syncthreads();
     }
-    int* __restrict__ ent = entries + cloud * n3;
-    for (int e = tid; e < n3; e += 1024) ent[atomicAdd(&s_c[__ldg(cidx + e)], 1)] = e;
+    int* __restrict__ ent = entries + cloud * ne;
+    for (int e = tid; e < ne; e += 1024) ent[atomicAdd(&s_c[__ldg(cidx + e)], 1)] = e;
 }
 
-// one warp per known point (b, i); lanes over channels (float4 when VEC).  Lists longer than kInvSortCap are
-// queued for inv_long_kernel.
+// one warp per target row (b, i); lanes over channels (float4 when VEC).  Lists longer than kInvSortCap are
+// queued for the long-list kernel.
+// WEIGHTED: entry e = 3j+t adds grad_out row j times weight[e] (three_interpolate, n = unknown points, ne = 3n);
+// otherwise entry e adds grad_out row e as it is (n = ne = entries).  m = targets.
 // T: element type of grad_out and grad_points (upcast on load, float32 sums, rounded once on the store): float, or
 // unsigned short for both 2-byte formats with f16 choosing float16 / bfloat16 at run time (one instance for the two)
-template <bool VEC, typename T>
+template <bool VEC, bool WEIGHTED, typename T>
 __global__ void __launch_bounds__(kInvThreads)
 inv_gather_kernel(int n, int c, int m, long long warps_total, const T* __restrict__ grad_out,
                   const float* __restrict__ weight, const int* __restrict__ off, const int* __restrict__ entries,
@@ -593,20 +599,17 @@ inv_gather_kernel(int n, int c, int m, long long warps_total, const T* __restric
     if (gw >= warps_total) return;
     const long long cloud = gw / m;
     const int i = (int)(gw - cloud * m);
-    const int n3 = 3 * n;
+    const int ne = WEIGHTED ? 3 * n : n;
     const int* __restrict__ o = off + cloud * (m + 1);
     const int beg = o[i], len = o[i + 1] - beg;
     if (len > kInvSortCap) {  // warp-uniform
         if (lane == 0) long_queue[1 + atomicAdd(long_queue, 1)] = (int)gw;  // the order of the queue does not matter
         return;
     }
-    const T* __restrict__ go = grad_out + (size_t)cloud * n * c;
-    const float* __restrict__ wt = weight + (size_t)cloud * n3;
-    T* __restrict__ gp = grad_points + ((size_t)cloud * m + i) * c;
     {
         int key[8];
 #pragma unroll
-        for (int q = 0; q < 8; ++q) key[q] = (32 * q + lane < len) ? __ldg(entries + cloud * n3 + beg + 32 * q + lane) : 0x7fffffff;
+        for (int q = 0; q < 8; ++q) key[q] = (32 * q + lane < len) ? __ldg(entries + cloud * ne + beg + 32 * q + lane) : 0x7fffffff;
         const int nreg = (len + 31) >> 5;
         if (nreg <= 1) bitonic_sort_keys<1, 8>(key, lane);
         else if (nreg == 2) bitonic_sort_keys<2, 8>(key, lane);
@@ -617,6 +620,9 @@ inv_gather_kernel(int n, int c, int m, long long warps_total, const T* __restric
             if (32 * q + lane < len) s_e[wib][32 * q + lane] = key[q];
         __syncwarp();
     }
+    const T* __restrict__ go = grad_out + (size_t)cloud * n * c;
+    const float* __restrict__ wt = WEIGHTED ? weight + (size_t)cloud * ne : nullptr;
+    T* __restrict__ gp = grad_points + ((size_t)cloud * m + i) * c;
     constexpr int W = VEC ? 4 : 1;
     for (int l0 = 0; l0 < c; l0 += 32 * W) {  // 128 (VEC) or 32 channels per pass
         const int l = l0 + lane * W;
@@ -634,8 +640,8 @@ inv_gather_kernel(int n, int c, int m, long long warps_total, const T* __restric
                 w[u] = 0.f;
                 if (s0 + u < len) {
                     const int e = s_e[wib][s0 + u];
-                    w[u] = __ldg(wt + e);
-                    const T* __restrict__ src = go + (size_t)(e / 3) * c + l;
+                    if (WEIGHTED) w[u] = __ldg(wt + e);
+                    const T* __restrict__ src = go + (size_t)(WEIGHTED ? e / 3 : e) * c + l;
                     if (VEC) gv[u] = __ldg(reinterpret_cast<const typename Pack4<T>::type*>(src));
                     else gs[u] = __ldg(src);
                 }
@@ -645,18 +651,122 @@ inv_gather_kernel(int n, int c, int m, long long warps_total, const T* __restric
                 if (s0 + u < len) {
                     if (VEC) {
                         const float4 g = unpack4_of(gv[u], f16);
-                        a0 = __fadd_rn(a0, __fmul_rn(g.x, w[u]));
-                        a1 = __fadd_rn(a1, __fmul_rn(g.y, w[u]));
-                        a2 = __fadd_rn(a2, __fmul_rn(g.z, w[u]));
-                        a3 = __fadd_rn(a3, __fmul_rn(g.w, w[u]));
+                        a0 = __fadd_rn(a0, WEIGHTED ? __fmul_rn(g.x, w[u]) : g.x);
+                        a1 = __fadd_rn(a1, WEIGHTED ? __fmul_rn(g.y, w[u]) : g.y);
+                        a2 = __fadd_rn(a2, WEIGHTED ? __fmul_rn(g.z, w[u]) : g.z);
+                        a3 = __fadd_rn(a3, WEIGHTED ? __fmul_rn(g.w, w[u]) : g.w);
                     } else {
-                        a0 = __fadd_rn(a0, __fmul_rn(f32_of(gs[u], f16), w[u]));
+                        const float g = f32_of(gs[u], f16);
+                        a0 = __fadd_rn(a0, WEIGHTED ? __fmul_rn(g, w[u]) : g);
                     }
                 }
             }
         }
         if (VEC) *reinterpret_cast<typename Pack4<T>::type*>(gp + l) = pack4_of(make_float4(a0, a1, a2, a3), T(), f16);
         else gp[l] = of_f32<T>(a0, f16);
+    }
+}
+
+// Long lists of the unweighted sum, in plain ascending entry order like the short ones (the group_point and
+// gather_point gradients are bit-identical to the reference's loop at any list length; at cls_msg layer 2 up to 5 %
+// of the entries sit in lists longer than 256).  One CTA per list: it scans the cloud's entries in order, kSeqScan per
+// thread and step, compacts the ones that point at i into shared memory in that order (ballot, then a popc prefix
+// over the (step, warp) slots), and when the buffer is full every thread adds the buffered rows to its own channels
+// in one chain.
+constexpr int kSeqScan = 8;
+constexpr int kSeqBuf = 2 * kSeqScan * kInvThreads;  // room for one more step whenever a step starts
+// (the bound of 1 CTA per SM lifts the register budget: without it ptxas kept the VEC instances at 64 and spilled)
+template <bool VEC, typename T>
+__global__ void __launch_bounds__(kInvThreads, 1)
+inv_long_seq_kernel(int ne, int c, int m, const T* __restrict__ grad_out, const int* __restrict__ idx,
+                    const int* __restrict__ long_queue, T* __restrict__ grad_points, int f16) {
+    constexpr int NW = kInvThreads / 32;
+    constexpr int W = VEC ? 4 : 1;
+    constexpr int H = sizeof(T) == 4 ? 4 : 8;  // rows in flight per thread, as in inv_long_kernel
+    __shared__ int s_list[kSeqBuf];
+    __shared__ int s_cnt[kSeqScan * NW];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const unsigned below = (1u << lane) - 1u;
+    const int nq = long_queue[0];
+    for (int q = blockIdx.x; q < nq; q += gridDim.x) {
+        const long long gw = long_queue[1 + q];
+        const long long cloud = gw / m;
+        const int i = (int)(gw - cloud * m);
+        const T* __restrict__ go = grad_out + (size_t)cloud * ne * c;
+        const int* __restrict__ cidx = idx + cloud * ne;
+        T* __restrict__ gp = grad_points + ((size_t)cloud * m + i) * c;
+        for (int l0 = 0; l0 < c; l0 += kInvThreads * W) {
+            const int l = l0 + tid * W;
+            const bool act = l < c;
+            float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+            long long e0 = 0;
+            while (e0 < ne) {
+                int cnt = 0;  // CTA-uniform
+                while (e0 < ne && cnt <= kSeqBuf - kSeqScan * kInvThreads) {
+                    int v[kSeqScan];
+#pragma unroll
+                    for (int u = 0; u < kSeqScan; ++u) {
+                        const long long e = e0 + u * kInvThreads + tid;
+                        v[u] = e < ne ? __ldg(cidx + e) : -1;
+                    }
+                    unsigned hits = 0, rank[kSeqScan];  // rank: matches of this step's slot u in the lanes below
+#pragma unroll
+                    for (int u = 0; u < kSeqScan; ++u) {
+                        const unsigned bal = __ballot_sync(kFullMask, v[u] == i);
+                        hits |= (v[u] == i ? 1u : 0u) << u;
+                        rank[u] = __popc(bal & below);
+                        if (lane == 0) s_cnt[u * NW + warp] = __popc(bal);
+                    }
+                    __syncthreads();
+#pragma unroll
+                    for (int u = 0; u < kSeqScan; ++u) {
+                        int pos = cnt;
+#pragma unroll
+                        for (int w = 0; w < NW; ++w) {
+                            const int k = s_cnt[u * NW + w];
+                            pos += w < warp ? k : 0;
+                            cnt += k;
+                        }
+                        if (hits >> u & 1u) s_list[pos + rank[u]] = (int)(e0 + u * kInvThreads + tid);
+                    }
+                    e0 += kSeqScan * kInvThreads;
+                    __syncthreads();
+                }
+                if (act) {
+                    for (int s0 = 0; s0 < cnt; s0 += H) {
+                        typename Pack4<T>::type gv[H];
+                        T gs[H];
+#pragma unroll
+                        for (int u = 0; u < H; ++u) {
+                            if (s0 + u < cnt) {
+                                const T* __restrict__ src = go + (size_t)s_list[s0 + u] * c + l;
+                                if (VEC) gv[u] = __ldg(reinterpret_cast<const typename Pack4<T>::type*>(src));
+                                else gs[u] = __ldg(src);
+                            }
+                        }
+#pragma unroll
+                        for (int u = 0; u < H; ++u) {
+                            if (s0 + u < cnt) {
+                                if (VEC) {
+                                    const float4 g = unpack4_of(gv[u], f16);
+                                    a0 = __fadd_rn(a0, g.x);
+                                    a1 = __fadd_rn(a1, g.y);
+                                    a2 = __fadd_rn(a2, g.z);
+                                    a3 = __fadd_rn(a3, g.w);
+                                } else {
+                                    a0 = __fadd_rn(a0, f32_of(gs[u], f16));
+                                }
+                            }
+                        }
+                    }
+                }
+                __syncthreads();  // s_list is refilled
+            }
+            if (act) {
+                if (VEC) *reinterpret_cast<typename Pack4<T>::type*>(gp + l) = pack4_of(make_float4(a0, a1, a2, a3), T(), f16);
+                else gp[l] = of_f32<T>(a0, f16);
+            }
+        }
     }
 }
 
@@ -787,6 +897,68 @@ static int three_interpolate_impl(int b, int m, int c, int n, const T* points, c
     return finish_launch();
 }
 
+size_t inv_workspace_bytes(int b, long long ne, int nt) {
+    // offsets (b, nt+1) + cursors (b, nt) + entries (b, ne) + queue of long lists (1 + b * (ne / (cap+1) + 1)), ints
+    const size_t longs = (size_t)b * ((size_t)ne / (kInvSortCap + 1) + 1);
+    return sizeof(int) * ((size_t)b * (nt + 1) + (size_t)b * nt + (size_t)b * (size_t)ne + 1 + longs);
+}
+
+// Inverse index of the b clouds' entries over nt targets, built in `workspace` (inv_workspace_bytes), then the ordered
+// sums.  Weighted: source rows n = ne / 3 (three_interpolate); unweighted: n = ne.  The arguments are checked by the caller.
+template <bool WEIGHTED, typename T>
+static int inv_scatter_det(int b, int n, int ne, int c, int nt, const T* grad_out, const int* idx, const float* weight,
+                           T* grad_points, void* workspace, int f16, cudaStream_t st) {
+    const long long warps = (long long)b * nt;
+    const unsigned long long blocks = ((unsigned long long)warps * 32 + kInvThreads - 1) / kInvThreads;
+    if (blocks > 0x7fffffffull) return (int)cudaErrorInvalidValue;
+    int* off = static_cast<int*>(workspace);
+    int* cur = off + (size_t)b * (nt + 1);
+    int* entries = cur + (size_t)b * nt;
+    int* long_queue = entries + (size_t)b * (size_t)ne;  // [0] = count, then (cloud * nt + i) of every list > kInvSortCap
+    int launches = 2;
+    if (nt <= kInvBuildMaxM) {
+        static std::atomic<unsigned long long> attr_done{0ull};
+        int dev = 0;
+        cudaError_t e = cudaGetDevice(&dev);
+        if (e != cudaSuccess) return (int)e;
+        if (dev >= 64 || !(attr_done.load(std::memory_order_acquire) & (1ull << dev))) {
+            e = cudaFuncSetAttribute(inv_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(int) * (kInvBuildMaxM + 1));
+            if (e != cudaSuccess) return (int)e;
+            if (dev < 64) attr_done.fetch_or(1ull << dev, std::memory_order_release);
+        }
+        inv_build_kernel<<<b, 1024, sizeof(int) * (size_t)(nt + 1), st>>>(ne, nt, idx, off, entries, long_queue);
+        launches += 1;
+    } else {
+        cudaError_t e = cudaMemsetAsync(off, 0, sizeof(int) * (size_t)b * (nt + 1), st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(long_queue, 0, sizeof(int), st);
+        if (e != cudaSuccess) return (int)e;
+        const long long total = (long long)b * ne;
+        const unsigned g1 = it_grid((unsigned long long)total, kInvThreads);
+        inv_count_kernel<<<g1, kInvThreads, 0, st>>>(ne, nt, total, idx, off);
+        inv_scan_kernel<<<b, 1024, 0, st>>>(nt, off, cur);
+        inv_fill_kernel<<<g1, kInvThreads, 0, st>>>(ne, nt, total, idx, cur, entries);
+        launches += 3;
+    }
+    // long lists: a fixed grid walks the queue (usually empty: the CTAs read one word and leave)
+    const unsigned long_grid = (unsigned)num_sms() * 2u;
+    const bool vec = c % 4 == 0 && aligned_to(grad_out, 4 * sizeof(T)) && aligned_to(grad_points, 4 * sizeof(T));
+#define PN2_INV_SUMS(VEC)                                                                                                     \
+    inv_gather_kernel<VEC, WEIGHTED, T><<<(unsigned)blocks, kInvThreads, 0, st>>>(n, c, nt, warps, grad_out, weight, off, entries, \
+                                                                                  grad_points, long_queue, f16);            \
+    if constexpr (WEIGHTED)                                                                                                   \
+        inv_long_kernel<VEC, T><<<long_grid, kInvThreads, 0, st>>>(n, c, nt, grad_out, idx, weight, long_queue, grad_points, f16); \
+    else                                                                                                                      \
+        inv_long_seq_kernel<VEC, T><<<long_grid, kInvThreads, 0, st>>>(ne, c, nt, grad_out, idx, long_queue, grad_points, f16)
+    if (vec) {
+        PN2_INV_SUMS(true);
+    } else {
+        PN2_INV_SUMS(false);
+    }
+#undef PN2_INV_SUMS
+    count_launch(launches - 1);
+    return finish_launch();
+}
+
 template <typename T>
 static int three_interpolate_grad_det_impl(int b, int n, int c, int m, const T* grad_out, const int* idx, const float* weight,
                                            T* grad_points, void* workspace, size_t workspace_bytes, int f16, void* stream) {
@@ -798,49 +970,18 @@ static int three_interpolate_grad_det_impl(int b, int n, int c, int m, const T* 
     if (!grad_out || !idx || !weight || !workspace) return (int)cudaErrorInvalidValue;
     if (workspace_bytes < ::pn2_three_interpolate_grad_det_workspace_bytes(b, n, m) || (long long)n * 3 > 0x7fffffffLL)
         return (int)cudaErrorInvalidValue;
-    int* off = static_cast<int*>(workspace);
-    int* cur = off + (size_t)b * (m + 1);
-    int* entries = cur + (size_t)b * m;
-    int* long_queue = entries + (size_t)b * 3 * (size_t)n;  // [0] = count, then (cloud * m + i) of every list > kInvSortCap
-    int launches = 2;
-    if (m <= kInvBuildMaxM) {
-        static std::atomic<unsigned long long> attr_done{0ull};
-        int dev = 0;
-        cudaError_t e = cudaGetDevice(&dev);
-        if (e != cudaSuccess) return (int)e;
-        if (dev >= 64 || !(attr_done.load(std::memory_order_acquire) & (1ull << dev))) {
-            e = cudaFuncSetAttribute(inv_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(int) * (kInvBuildMaxM + 1));
-            if (e != cudaSuccess) return (int)e;
-            if (dev < 64) attr_done.fetch_or(1ull << dev, std::memory_order_release);
-        }
-        inv_build_kernel<<<b, 1024, sizeof(int) * (size_t)(m + 1), st>>>(3 * n, m, idx, off, entries, long_queue);
-        launches += 1;
-    } else {
-        cudaError_t e = cudaMemsetAsync(off, 0, sizeof(int) * (size_t)b * (m + 1), st);
-        if (e == cudaSuccess) e = cudaMemsetAsync(long_queue, 0, sizeof(int), st);
-        if (e != cudaSuccess) return (int)e;
-        const long long total = (long long)b * n * 3;
-        const unsigned g1 = it_grid((unsigned long long)total, kInvThreads);
-        inv_count_kernel<<<g1, kInvThreads, 0, st>>>(3 * n, m, total, idx, off);
-        inv_scan_kernel<<<b, 1024, 0, st>>>(m, off, cur);
-        inv_fill_kernel<<<g1, kInvThreads, 0, st>>>(3 * n, m, total, idx, cur, entries);
-        launches += 3;
-    }
-    const long long warps = (long long)b * m;
-    const unsigned long long blocks = ((unsigned long long)warps * 32 + kInvThreads - 1) / kInvThreads;
-    if (blocks > 0x7fffffffull) return (int)cudaErrorInvalidValue;
-    // long lists: a fixed grid walks the queue (usually empty: the CTAs read one word and leave)
-    const unsigned long_grid = (unsigned)num_sms() * 2u;
-    if (c % 4 == 0 && aligned_to(grad_out, 4 * sizeof(T)) && aligned_to(grad_points, 4 * sizeof(T))) {
-        inv_gather_kernel<true, T><<<(unsigned)blocks, kInvThreads, 0, st>>>(n, c, m, warps, grad_out, weight, off, entries, grad_points, long_queue, f16);
-        inv_long_kernel<true, T><<<long_grid, kInvThreads, 0, st>>>(n, c, m, grad_out, idx, weight, long_queue, grad_points, f16);
-    } else {
-        inv_gather_kernel<false, T><<<(unsigned)blocks, kInvThreads, 0, st>>>(n, c, m, warps, grad_out, weight, off, entries, grad_points, long_queue, f16);
-        inv_long_kernel<false, T><<<long_grid, kInvThreads, 0, st>>>(n, c, m, grad_out, idx, weight, long_queue, grad_points, f16);
-    }
-    count_launch(launches - 1);
-    return finish_launch();
+    return inv_scatter_det<true, T>(b, n, 3 * n, c, m, grad_out, idx, weight, grad_points, workspace, f16, st);
 }
+
+// explicit instances for the group_point / gather_point gradients (group.cu)
+template <typename T>
+int inv_sum_rows_det(int b, int ne, int c, int nt, const T* src, const int* idx, T* dst, void* workspace, int f16,
+                     cudaStream_t st) {
+    return inv_scatter_det<false, T>(b, ne, ne, c, nt, src, idx, nullptr, dst, workspace, f16, st);
+}
+template int inv_sum_rows_det<float>(int, int, int, int, const float*, const int*, float*, void*, int, cudaStream_t);
+template int inv_sum_rows_det<unsigned short>(int, int, int, int, const unsigned short*, const int*, unsigned short*, void*, int,
+                                              cudaStream_t);
 
 }  // namespace pn2
 
@@ -965,9 +1106,7 @@ int pn2_fp_interpolate_concat_typed(int dtype, int b, int n, int m, int c2, int 
 
 size_t pn2_three_interpolate_grad_det_workspace_bytes(int b, int n, int m) {
     if (b <= 0 || n <= 0 || m <= 0) return 0;
-    // offsets (b, m+1) + cursors (b, m) + entries (b, 3n) + queue of long lists (1 + b * ceil(3n / (cap+1))), ints
-    const size_t longs = (size_t)b * ((3 * (size_t)n) / (pn2::kInvSortCap + 1) + 1);
-    return sizeof(int) * ((size_t)b * (m + 1) + (size_t)b * m + (size_t)b * 3 * (size_t)n + 1 + longs);
+    return pn2::inv_workspace_bytes(b, 3 * (long long)n, m);
 }
 
 int pn2_three_interpolate_grad_det(int b, int n, int c, int m, const float* grad_out, const int* idx, const float* weight,

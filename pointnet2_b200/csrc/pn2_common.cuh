@@ -133,6 +133,14 @@ int fps_dispatch(int b, int n, int m, const float* inp, float* temp, int* out, f
 bool fps_single_cta(int b, int n);
 size_t fps_scratch_bytes(int b, int n);
 
+// ordered-sum scatter through an inverse index (interpolate.cu), shared by three_interpolate's gradient and the
+// group_point / gather_point gradients: dst[b, i, :] = sum of the rows src[b, e, :] with idx[b, e] == i, e ascending, in
+// float32, rounded once to T (unsigned short: f16 != 0 float16, else bfloat16).  Every dst row is written (0 if no entry
+// points at it).  b clouds of ne entries over nt targets; workspace of inv_workspace_bytes(b, ne, nt) bytes.
+size_t inv_workspace_bytes(int b, long long ne, int nt);
+template <typename T>
+int inv_sum_rows_det(int b, int ne, int c, int nt, const T* src, const int* idx, T* dst, void* workspace, int f16, cudaStream_t st);
+
 // ---- streaming memory ops ---------------------------------------------------------------------
 __device__ __forceinline__ void st_stream_f4(float4* p, float4 v) { __stcs(p, v); }
 __device__ __forceinline__ void st_stream_i4(int4* p, int4 v) { __stcs(p, v); }

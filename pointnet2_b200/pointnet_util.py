@@ -58,24 +58,21 @@ class _GroupConcat(torch.autograd.Function):
     def backward(ctx, g_out, g_gxyz):
         (idx,) = ctx.saved_tensors
         b, n, c, m, s, xyz_first, has_points = ctx.meta
-        lib = _lib.load()
-        dev = g_out.device
         lo = 0 if xyz_first else c
         g_out = g_out.to(ctx.dtype)
-        g_xyz_part = g_out[..., lo:lo + 3].float()  # the coordinates' gradient is float32 (an exact upcast)
-        if g_gxyz is not None:
-            g_xyz_part = g_xyz_part + g_gxyz
-        g_xyz_part = g_xyz_part.contiguous()
-        g_xyz = torch.zeros((b, n, 3), dtype=torch.float32, device=dev)
-        g_points = None
-        with on_device(g_out):
-            st = stream_ptr(dev)
-            _lib.check(lib.pn2_group_point_grad(b, n, 3, m, s, ptr(g_xyz_part), ptr(idx), ptr(g_xyz), st),
-                       "pn2_group_point_grad")
+        g_xyz = g_new_xyz = g_points = None
+        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:  # in the networks the coordinates need none
+            g_xyz_part = g_out[..., lo:lo + 3].float()  # the coordinates' gradient is float32 (an exact upcast)
+            if g_gxyz is not None:
+                g_xyz_part = g_xyz_part + g_gxyz
+            g_xyz_part = g_xyz_part.contiguous()
+            if ctx.needs_input_grad[0]:
+                g_xyz = group_point_grad(g_xyz_part, idx, (b, n, 3))
+            if ctx.needs_input_grad[1]:
+                g_new_xyz = -g_xyz_part.sum(dim=2)
         if has_points:
             g_feat = (g_out[..., 3:] if xyz_first else g_out[..., :c]).contiguous()
             g_points = group_point_grad(g_feat, idx, (b, n, c))
-        g_new_xyz = -g_xyz_part.sum(dim=2)
         return g_xyz, g_new_xyz, g_points, None, None
 
 

@@ -113,10 +113,23 @@ class _GroupPoint(torch.autograd.Function):
 
 def group_point_grad(grad_out: torch.Tensor, idx: torch.Tensor, shape) -> torch.Tensor:
     """Backward of group_point: scatter-add of ``grad_out`` (B, M, S, C) into a (B, N, C) gradient of
-    ``grad_out``'s dtype.  Float32 atomics in every case; a 16-bit gradient is the float32 sum rounded once."""
+    ``grad_out``'s dtype; a 16-bit gradient is the float32 sum rounded once.  Float32 atomics, unless
+    ``torch.are_deterministic_algorithms_enabled()``: then every point's rows are added in ascending (j, k) order, run to
+    run identical and bit-identical to the reference's group_point_grad_cpu."""
     b, n, c = shape
     _, m, s = idx.shape
     dev = grad_out.device
+    if torch.are_deterministic_algorithms_enabled():
+        grad_points = torch.empty((b, n, c), dtype=grad_out.dtype, device=dev)  # every element is written
+        if grad_points.numel():
+            lib = _lib.load()
+            with on_device(grad_out):
+                wsb = int(lib.pn2_group_point_grad_det_workspace_bytes(b, n, max(m, 1), max(s, 1)))
+                ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+                rc = lib.pn2_group_point_grad_det_typed(DTYPE_CODES[grad_out.dtype], b, n, c, m, s, ptr(grad_out), ptr(idx),
+                                                        ptr(grad_points), ptr(ws), wsb, stream_ptr(dev))
+            _lib.check(rc, "pn2_group_point_grad_det")
+        return grad_points
     # zero-filled by the caller, as GroupPointGradGpuOp does (tf_grouping.cpp:204)
     accum = torch.zeros((b, n, c), dtype=torch.float32, device=dev)
     if grad_out.dtype == torch.float32:

@@ -45,7 +45,7 @@ def three_nn(xyz1: torch.Tensor, xyz2: torch.Tensor):
 # pn2_three_interpolate_grad, the reference's own semantics on a GPU).
 # bfloat16 / float16 gradients always take the deterministic path (pn2_three_interpolate_grad_det_typed: float32 sums
 # in the same order, rounded once): atomics on 16-bit values would need a float32 accumulator and a rounding pass
-# as well, and would gain nothing.
+# as well, and would gain nothing.  So does every gradient while torch.are_deterministic_algorithms_enabled().
 DETERMINISTIC_GRAD = True
 
 
@@ -87,7 +87,7 @@ class _ThreeInterpolate(torch.autograd.Function):
                                                                   ptr(weight), ptr(grad_points), ptr(ws), wsb, stream_ptr(dev))
                 _lib.check(rc, "pn2_three_interpolate_grad_det")
             return grad_points, None, None
-        if DETERMINISTIC_GRAD and b * m * c:
+        if (DETERMINISTIC_GRAD or torch.are_deterministic_algorithms_enabled()) and b * m * c:
             # inverse index + ordered accumulation: deterministic, bit-identical to threeinterpolate_grad_cpu
             # (tf_interpolate.cpp:131-153), and ~3x faster than the atomics at the sem-seg sizes
             grad_points = torch.empty((b, m, c), dtype=torch.float32, device=dev)

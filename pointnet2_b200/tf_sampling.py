@@ -123,12 +123,23 @@ class _GatherPoint(torch.autograd.Function):
         (idx,) = ctx.saved_tensors
         b, m = idx.shape
         out_g = out_g.contiguous()
+        lib = _lib.load()
+        if torch.are_deterministic_algorithms_enabled():
+            # no atomics: each point's rows added in ascending j, every element of inp_g written
+            inp_g = torch.empty((b, ctx.n, 3), dtype=torch.float32, device=out_g.device)
+            if inp_g.numel():
+                with on_device(out_g):
+                    wsb = int(lib.pn2_group_point_grad_det_workspace_bytes(b, ctx.n, max(m, 1), 1))
+                    ws = torch.empty(wsb, dtype=torch.uint8, device=out_g.device)
+                    rc = lib.pn2_gather_point_grad_det(b, ctx.n, m, ptr(out_g), ptr(idx), ptr(inp_g), ptr(ws), wsb,
+                                                       stream_ptr(out_g.device))
+                _lib.check(rc, "pn2_gather_point_grad_det")
+            return inp_g, None
         # the caller zero-fills, as GatherPointGradGpuOp does (tf_sampling.cpp:174)
         inp_g = torch.zeros((b, ctx.n, 3), dtype=torch.float32, device=out_g.device)
         if b * m:
             with on_device(out_g):
-                rc = _lib.load().pn2_gather_point_grad(b, ctx.n, m, ptr(out_g), ptr(idx), ptr(inp_g),
-                                                       stream_ptr(out_g.device))
+                rc = lib.pn2_gather_point_grad(b, ctx.n, m, ptr(out_g), ptr(idx), ptr(inp_g), stream_ptr(out_g.device))
             _lib.check(rc, "pn2_gather_point_grad")
         return inp_g, None
 
@@ -136,7 +147,8 @@ class _GatherPoint(torch.autograd.Function):
 def gather_point(inp: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
     """Row gather of coordinates: ``out[b, j, :] = inp[b, idx[b, j], :]``.
 
-    ``inp`` float32 (B, N, 3); ``idx`` int32 (B, M).  Returns float32 (B, M, 3).  Differentiable in ``inp``.
+    ``inp`` float32 (B, N, 3); ``idx`` int32 (B, M).  Returns float32 (B, M, 3).  Differentiable in ``inp``: float
+    atomics, or, when ``torch.are_deterministic_algorithms_enabled()``, ordered sums (ascending j, run to run identical).
     Reference: tf_sampling.py:29-37 -> gatherpointKernel (tf_sampling_g.cu:172-181);
     gradient tf_sampling.py:43-47 -> scatteraddpointKernel (:183-192).
     """

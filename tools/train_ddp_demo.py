@@ -10,6 +10,7 @@ min(0.99, 1 - 0.5 * 0.5^(samples/200000)).
 
     python tools/train_ddp_demo.py --steps 20                                   # one GPU
     python tools/train_ddp_demo.py --steps 30 --amp bf16                        # bf16 autocast
+    python tools/train_ddp_demo.py --steps 5 --deterministic                    # reproducible: prints a weights hash
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 \
         tools/train_ddp_demo.py --steps 20                                      # one rank per GPU
 
@@ -20,6 +21,7 @@ loss has something to learn and the demo can assert that it goes down.
 from __future__ import annotations
 
 import argparse
+import hashlib
 import json
 import os
 import sys
@@ -79,7 +81,12 @@ def main() -> None:
     ap.add_argument("--json", type=str, default=None)
     ap.add_argument("--amp", choices=["none", "bf16", "fp16"], default="none",
                     help="mixed precision: torch.autocast in bfloat16, or float16 with a GradScaler")
+    ap.add_argument("--deterministic", action="store_true",
+                    help="torch.use_deterministic_algorithms(True): run-to-run identical weights; prints their SHA-256")
     args = ap.parse_args()
+    if args.deterministic:
+        os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")  # read when cuBLAS starts: before the first matmul
+        torch.use_deterministic_algorithms(True)
 
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -160,7 +167,13 @@ def main() -> None:
         out = {"model": args.model, "amp": args.amp, "world": world, "global_batch": args.batch, "num_point": args.num_point,
                "steps": args.steps, "loss_first": first, "loss_last": last, "loss_decreased": last < first,
                "weights_identical_across_ranks": same, "ms_per_step_wallclock": 1e3 * float(np.median(steady)),
-               "clouds_per_s": args.batch / float(np.median(steady)), "data": "synthetic parametric shapes"}
+               "clouds_per_s": args.batch / float(np.median(steady)), "data": "synthetic parametric shapes",
+               "deterministic": args.deterministic}
+        if args.deterministic:
+            h = hashlib.sha256()
+            for p in model.parameters():
+                h.update(p.detach().cpu().numpy().tobytes())
+            out["weights_sha256"] = h.hexdigest()
         print(json.dumps(out))
         if args.json:
             with open(args.json, "w") as f:
