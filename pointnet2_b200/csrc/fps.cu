@@ -93,16 +93,14 @@ __device__ __forceinline__ void st_async_u32(unsigned remote_addr, unsigned v, u
 }
 
 // ---- per-thread step: update P register-resident points against the last pick ------------------
-// D = number of distinct reference slots (k mod 512) one thread's points fall into: thread t of a
-// T-thread CTA owns k = t + j*T, so for T < 512 its slots cycle with period D = 512/T.  The scan
-// visits the points in tie-break order (slot ascending, then k ascending): for each slot residue
-// r = j mod D in turn, j ascending — so the strict '>' keeps the reference's winner.
-template <int P, int D = 1, int PT = P>
+// DD = number of distinct reference slots (k mod 512) one thread's points fall into (ScanOrder::DD).  The
+// scan visits the points in tie-break order (slot ascending, then k ascending): for each slot residue
+// r = j mod DD in turn, j ascending — so the strict '>' keeps the reference's winner.
+template <int P, int DD = 1, int PT = P>
 __device__ __forceinline__ void fps_step(const float (&px)[P], const float (&py)[P], const float (&pz)[P],
                                          float (&td)[PT], float x1, float y1, float z1, float& best, int& bj) {
     best = -1.0f;
     bj = 0;
-    constexpr int DD = (D < P) ? D : P;
 #pragma unroll
     for (int r = 0; r < DD; ++r) {
 #pragma unroll
@@ -153,6 +151,83 @@ __device__ __forceinline__ unsigned long long f2_fma(unsigned long long a, unsig
     return f2_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 
+// Packed pair update: the running minima of the H register-resident pairs (X, Y, Z)[h] = points 2h, 2h + 1 against
+// the last pick (x1, y1, z1), d2_fma_pattern on both halves.
+template <int H, int P>
+__device__ __forceinline__ void pair_update(const unsigned long long (&X)[H], const unsigned long long (&Y)[H],
+                                            const unsigned long long (&Z)[H], float (&td)[P], float x1, float y1, float z1) {
+    const unsigned long long X1 = f2_pack(x1, x1), Y1 = f2_pack(y1, y1), Z1 = f2_pack(z1, z1);
+#pragma unroll
+    for (int h = 0; h < H; ++h) {
+        const unsigned long long dx = f2_sub(X[h], X1), dy = f2_sub(Y[h], Y1), dz = f2_sub(Z[h], Z1);
+        const unsigned long long d = f2_fma(dz, dz, f2_fma(dx, dx, f2_mul(dy, dy)));  // d2_fma_pattern on both halves
+        float d0, d1;
+        f2_unpack(d, d0, d1);
+        td[2 * h] = fminf(d0, td[2 * h]);
+        td[2 * h + 1] = fminf(d1, td[2 * h + 1]);
+    }
+}
+
+// ---- streamed points of the cluster kernels: shared-memory float4 groups [(g*3 + c)*T + t], .x..w = four consecutive
+// points of thread t.  Groups [G0, G1) hold the thread's points J0 + 4*(g - G0) + u, whose running minima are in td.
+template <int G0, int G1, int J0, int T, int P>
+__device__ __forceinline__ void stream_update_packed(const float4* __restrict__ s4, int tid, float (&td)[P], float x1,
+                                                     float y1, float z1) {
+    const unsigned long long X1 = f2_pack(x1, x1), Y1 = f2_pack(y1, y1), Z1 = f2_pack(z1, z1);
+#pragma unroll
+    for (int g = G0; g < G1; ++g) {
+        const float4 X = s4[(g * 3 + 0) * T + tid], Y = s4[(g * 3 + 1) * T + tid], Z = s4[(g * 3 + 2) * T + tid];
+        const unsigned long long xa = f2_pack(X.x, X.y), xb = f2_pack(X.z, X.w), ya = f2_pack(Y.x, Y.y),
+                                 yb = f2_pack(Y.z, Y.w), za = f2_pack(Z.x, Z.y), zb = f2_pack(Z.z, Z.w);
+        const unsigned long long dxa = f2_sub(xa, X1), dya = f2_sub(ya, Y1), dza = f2_sub(za, Z1);
+        const unsigned long long dxb = f2_sub(xb, X1), dyb = f2_sub(yb, Y1), dzb = f2_sub(zb, Z1);
+        const unsigned long long da = f2_fma(dza, dza, f2_fma(dxa, dxa, f2_mul(dya, dya)));
+        const unsigned long long db = f2_fma(dzb, dzb, f2_fma(dxb, dxb, f2_mul(dyb, dyb)));
+        float d0, d1, d2, d3;
+        f2_unpack(da, d0, d1);
+        f2_unpack(db, d2, d3);
+        const int j = J0 + 4 * (g - G0);
+        td[j + 0] = fminf(d0, td[j + 0]);
+        td[j + 1] = fminf(d1, td[j + 1]);
+        td[j + 2] = fminf(d2, td[j + 2]);
+        td[j + 3] = fminf(d3, td[j + 3]);
+    }
+}
+// The plain form continues fps_step's scan (best, bj) over the streamed points, which follow the register-resident ones
+// in tie-break order.
+template <int G0, int G1, int J0, int T, int P>
+__device__ __forceinline__ void stream_update(const float4* __restrict__ s4, int tid, float (&td)[P], float x1, float y1,
+                                              float z1, float& best, int& bj) {
+#pragma unroll
+    for (int g = G0; g < G1; ++g) {
+        const float4 X = s4[(g * 3 + 0) * T + tid], Y = s4[(g * 3 + 1) * T + tid], Z = s4[(g * 3 + 2) * T + tid];
+        const float xs[4] = {X.x, X.y, X.z, X.w}, ys[4] = {Y.x, Y.y, Y.z, Y.w}, zs[4] = {Z.x, Z.y, Z.z, Z.w};
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const int j = J0 + 4 * (g - G0) + u;
+            const float d = d2_fma_pattern(xs[u], ys[u], zs[u], x1, y1, z1);
+            const float d2 = fminf(d, td[j]);
+            td[j] = d2;
+            if (d2 > best) {
+                best = d2;
+                bj = j;
+            }
+        }
+    }
+}
+
+// Pick `it` of a single-CTA chain: its index, and its coordinates when the caller asked for them.  The cluster kernels
+// and the global fallback store the index first and keep their own stores: the other order compiles to other code.
+__device__ __forceinline__ void write_pick(int* __restrict__ out, float* __restrict__ oxyz, int it, int idx, float x,
+                                          float y, float z) {
+    if (oxyz) {
+        oxyz[3 * it + 0] = x;
+        oxyz[3 * it + 1] = y;
+        oxyz[3 * it + 2] = z;
+    }
+    out[it] = idx;
+}
+
 // Lexicographic (max hi, then min lo) over the warp; every lane gets the result.
 __device__ __forceinline__ void warp_max_min_pair(unsigned& hi, unsigned& lo) {
     const unsigned mh = __reduce_max_sync(kFullMask, hi);
@@ -165,6 +240,8 @@ __device__ __forceinline__ void warp_max_min_pair(unsigned& hi, unsigned& lo) {
 // Register slot e of thread t holds point k = t + j(e)*T, with j(e) running through the thread's points in the
 // reference's tie-break order (slot k mod 512 ascending, then k ascending; see fps_step).  The tie-break word of
 // that point splits into the thread's own part tb_encode(t) and a compile-time constant tbj(e) with disjoint bits.
+// D = number of distinct reference slots (k mod 512) of thread t's points k = t + j*T: for T < 512 they cycle with
+// period D = 512/T, and a thread with P < D points sees DD = P of them.
 template <int P, int T>
 struct ScanOrder {
     static constexpr int D = (T >= 512) ? 1 : 512 / T;
@@ -267,30 +344,14 @@ __device__ __forceinline__ void fps_chain_packed(int n, int m, const float* __re
     const unsigned tp = (tid < n) ? tb_encode((unsigned)tid) : 0xffffffffu;
 
     float x1 = src[0], y1 = src[1], z1 = src[2];
-    if (tid == 0) {
-        if (oxyz) {
-            oxyz[0] = x1;
-            oxyz[1] = y1;
-            oxyz[2] = z1;
-        }
-        out[0] = 0;
-    }
+    if (tid == 0) write_pick(out, oxyz, 0, 0, x1, y1, z1);
     // key slots of warps that do not exist stay (value 0, word ~0): the cross-warp reduction reads all 32 without a test
     if (tid < 64) (&s_keys[0][0])[tid] = make_uint2(0xffffffffu, 0u);
     __syncthreads();
 
 #pragma unroll 2
     for (int it = 1; it < m; ++it) {
-        const unsigned long long X1 = f2_pack(x1, x1), Y1 = f2_pack(y1, y1), Z1 = f2_pack(z1, z1);
-#pragma unroll
-        for (int h = 0; h < H; ++h) {
-            const unsigned long long dx = f2_sub(X[h], X1), dy = f2_sub(Y[h], Y1), dz = f2_sub(Z[h], Z1);
-            const unsigned long long d = f2_fma(dz, dz, f2_fma(dx, dx, f2_mul(dy, dy)));  // d2_fma_pattern on both halves
-            float d0, d1;
-            f2_unpack(d, d0, d1);
-            td[2 * h] = fminf(d0, td[2 * h]);
-            td[2 * h + 1] = fminf(d1, td[2 * h + 1]);
-        }
+        pair_update(X, Y, Z, td, x1, y1, z1);
         // running minima are never NaN (fminf drops a NaN distance) and never -0, so == and the unsigned order of
         // the float bits are exact
         float g[G];
@@ -331,14 +392,7 @@ __device__ __forceinline__ void fps_chain_packed(int n, int m, const float* __re
         x1 = src[3 * old + 0];
         y1 = src[3 * old + 1];
         z1 = src[3 * old + 2];
-        if (tid == 0) {
-            if (oxyz) {
-                oxyz[3 * it + 0] = x1;
-                oxyz[3 * it + 1] = y1;
-                oxyz[3 * it + 2] = z1;
-            }
-            out[it] = old;
-        }
+        if (tid == 0) write_pick(out, oxyz, it, old, x1, y1, z1);
     }
 }
 
@@ -359,8 +413,6 @@ __global__ void __launch_bounds__(T, 1)
 fps_cta_kernel(int n, int m, const float* __restrict__ xyz, int* __restrict__ idx_out,
                float* __restrict__ new_xyz, int sentinel) {
     static_assert(T % 512 == 0 || 512 % T == 0, "T must divide or be a multiple of the reference's 512 slots");
-    constexpr int NW = T / 32;
-    constexpr int D = (T >= 512) ? 1 : 512 / T;
     __shared__ uint2 s_keys[2][32];
     extern __shared__ __align__(16) float s_xyz[];
 
@@ -415,61 +467,95 @@ fps_cta_kernel(int n, int m, const float* __restrict__ xyz, int* __restrict__ id
     if constexpr (V == 1) {
         fps_chain_packed<P, T>(n, m, src, out, oxyz, s_keys);
     } else {
-    float px[P], py[P], pz[P], td[P];
+        // the plain chain stays in the kernel body: moved into a function of its own, it compiles to differently
+        // scheduled code
+        constexpr int NW = T / 32;
+        float px[P], py[P], pz[P], td[P];
+#pragma unroll
+        for (int j = 0; j < P; ++j) {
+            const int k = tid + j * T;
+            if (k < n) {
+                px[j] = src[3 * k + 0];
+                py[j] = src[3 * k + 1];
+                pz[j] = src[3 * k + 2];
+                td[j] = 1e38f;
+            } else {
+                px[j] = py[j] = pz[j] = 0.0f;
+                td[j] = -1.0f;
+            }
+        }
+
+        float x1 = src[0], y1 = src[1], z1 = src[2];
+        if (tid == 0) write_pick(out, oxyz, 0, 0, x1, y1, z1);
+
+        for (int it = 1; it < m; ++it) {
+            float best;
+            int bj;
+            fps_step<P, ScanOrder<P, T>::DD>(px, py, pz, td, x1, y1, z1, best, bj);
+            unsigned hi = 0u, lo = 0u;
+            if (best >= 0.0f) {
+                hi = __float_as_uint(best);
+                lo = ~tb_encode((unsigned)(tid + bj * T));
+            }
+            warp_max_pair(hi, lo);
+            const int buf = it & 1;
+            if (lane == 0) s_keys[buf][warp] = make_uint2(lo, hi);
+            __syncthreads();
+            uint2 e = (lane < NW) ? s_keys[buf][lane] : make_uint2(0u, 0u);
+            unsigned gh = e.y, gl = e.x;
+            warp_max_pair(gh, gl);
+            const int old = (int)tb_decode(~gl);
+            x1 = src[3 * old + 0];
+            y1 = src[3 * old + 1];
+            z1 = src[3 * old + 2];
+            if (tid == 0) write_pick(out, oxyz, it, old, x1, y1, z1);
+        }
+    }
+}
+
+// ---- pieces of the two cluster kernels ---------------------------------------------------------------------------
+// Two step mbarriers, alternating by step parity; each step thread 0 arrives once, expecting the C messages' bytes.
+__device__ __forceinline__ void init_step_mbars(unsigned long long (&s_mbar)[2]) {
+    mbar_init(smem_addr(&s_mbar[0]), 1);
+    mbar_init(smem_addr(&s_mbar[1]), 1);
+    fence_mbar_init_cluster();
+}
+
+// This thread's points k = t + T*(rank + C*j), j < P: running minimum 1e38 (padding: coordinates 0, minimum -1), the
+// coordinates of j < PR into registers, and every point to keep(j, x, y, z) for the CTA's shared-memory copy.
+template <int P, int PR, int T, class Keep>
+__device__ __forceinline__ void load_points(const float* __restrict__ pts, int n, long long C, unsigned rank, int tid,
+                                            float (&px)[PR], float (&py)[PR], float (&pz)[PR], float (&td)[P], Keep keep) {
 #pragma unroll
     for (int j = 0; j < P; ++j) {
-        const int k = tid + j * T;
+        const long long k = (long long)tid + (long long)T * (rank + C * j);
+        float x = 0.f, y = 0.f, z = 0.f, t = -1.0f;
         if (k < n) {
-            px[j] = src[3 * k + 0];
-            py[j] = src[3 * k + 1];
-            pz[j] = src[3 * k + 2];
-            td[j] = 1e38f;
-        } else {
-            px[j] = py[j] = pz[j] = 0.0f;
-            td[j] = -1.0f;
+            x = pts[3 * k + 0];
+            y = pts[3 * k + 1];
+            z = pts[3 * k + 2];
+            t = 1e38f;
+        }
+        td[j] = t;
+        keep(j, x, y, z);
+        if (j < PR) {
+            px[j] = x;
+            py[j] = y;
+            pz[j] = z;
         }
     }
+}
 
-    float x1 = src[0], y1 = src[1], z1 = src[2];
-    if (tid == 0) {
-        if (oxyz) {
-            oxyz[0] = x1;
-            oxyz[1] = y1;
-            oxyz[2] = z1;
-        }
-        out[0] = 0;
+// The register-resident coordinates as packed pairs for the packed update (the scalar copies are then dead).
+template <int H, int PR>
+__device__ __forceinline__ void pack_pairs(const float (&px)[PR], const float (&py)[PR], const float (&pz)[PR],
+                                           unsigned long long (&X)[H], unsigned long long (&Y)[H], unsigned long long (&Z)[H]) {
+#pragma unroll
+    for (int h = 0; h < H; ++h) {
+        X[h] = f2_pack(px[2 * h], px[2 * h + 1]);
+        Y[h] = f2_pack(py[2 * h], py[2 * h + 1]);
+        Z[h] = f2_pack(pz[2 * h], pz[2 * h + 1]);
     }
-
-    for (int it = 1; it < m; ++it) {
-        float best;
-        int bj;
-        fps_step<P, D>(px, py, pz, td, x1, y1, z1, best, bj);
-        unsigned hi = 0u, lo = 0u;
-        if (best >= 0.0f) {
-            hi = __float_as_uint(best);
-            lo = ~tb_encode((unsigned)(tid + bj * T));
-        }
-        warp_max_pair(hi, lo);
-        const int buf = it & 1;
-        if (lane == 0) s_keys[buf][warp] = make_uint2(lo, hi);
-        __syncthreads();
-        uint2 e = (lane < NW) ? s_keys[buf][lane] : make_uint2(0u, 0u);
-        unsigned gh = e.y, gl = e.x;
-        warp_max_pair(gh, gl);
-        const int old = (int)tb_decode(~gl);
-        x1 = src[3 * old + 0];
-        y1 = src[3 * old + 1];
-        z1 = src[3 * old + 2];
-        if (tid == 0) {
-            if (oxyz) {
-                oxyz[3 * it + 0] = x1;
-                oxyz[3 * it + 1] = y1;
-                oxyz[3 * it + 2] = z1;
-            }
-            out[it] = old;
-        }
-    }
-    }  // V == 0
 }
 
 // =================================================================================================
@@ -514,11 +600,7 @@ fps_cluster_kernel(int n, int m, int log2c, const float* __restrict__ xyz, int* 
     int* __restrict__ out = idx_out + (size_t)cloud * m;
     float* __restrict__ oxyz = new_xyz ? new_xyz + (size_t)cloud * m * 3 : nullptr;
 
-    if (tid == 0) {
-        mbar_init(smem_addr(&s_mbar[0]), 1);
-        mbar_init(smem_addr(&s_mbar[1]), 1);
-        fence_mbar_init_cluster();
-    }
+    if (tid == 0) init_step_mbars(s_mbar);
 
     auto slot_addr = [&](int j, int t, int c) -> int {  // float index of coordinate c of local point (j, t)
         if constexpr (STREAM) return ((((j >> 2) * 3 + c) * T + t) << 2) + (j & 3);
@@ -526,37 +608,16 @@ fps_cluster_kernel(int n, int m, int log2c, const float* __restrict__ xyz, int* 
     };
 
     float px[PR], py[PR], pz[PR], td[P];
-#pragma unroll
-    for (int j = 0; j < P; ++j) {
-        const long long k = (long long)tid + (long long)T * (rank + (long long)C * j);
-        float x = 0.f, y = 0.f, z = 0.f, t = -1.0f;
-        if (k < n) {
-            x = pts[3 * k + 0];
-            y = pts[3 * k + 1];
-            z = pts[3 * k + 2];
-            t = 1e38f;
-        }
-        td[j] = t;
+    load_points<P, PR, T>(pts, n, C, rank, tid, px, py, pz, td, [&](int j, float x, float y, float z) {
         s_pts[slot_addr(j, tid, 0)] = x;
         s_pts[slot_addr(j, tid, 1)] = y;
         s_pts[slot_addr(j, tid, 2)] = z;
-        if (j < PR) {
-            px[j] = x;
-            py[j] = y;
-            pz[j] = z;
-        }
-    }
-    // V == 1: the register-resident coordinates as packed pairs (the scalar copies above are then dead)
+    });
     constexpr int HR = (V == 1) ? PR / 2 : 1;
     unsigned long long X2[HR], Y2[HR], Z2[HR];
     unsigned tpc = 0u, jshift = 0u;
     if constexpr (V == 1) {
-#pragma unroll
-        for (int h = 0; h < HR; ++h) {
-            X2[h] = f2_pack(px[2 * h], px[2 * h + 1]);
-            Y2[h] = f2_pack(py[2 * h], py[2 * h + 1]);
-            Z2[h] = f2_pack(pz[2 * h], pz[2 * h + 1]);
-        }
+        pack_pairs(px, py, pz, X2, Y2, Z2);
         const unsigned base = (unsigned)tid + (unsigned)T * rank;  // this thread's point j = 0
         tpc = (base < (unsigned)n) ? tb_encode(base) : 0xffffffffu;  // all ones: a thread without points sends key (0, 0)
         unsigned log2t = 0;
@@ -587,67 +648,23 @@ fps_cluster_kernel(int n, int m, int log2c, const float* __restrict__ xyz, int* 
 
         unsigned hi = 0u, lo = 0u;
         if constexpr (V == 1) {
-            const unsigned long long X1 = f2_pack(x1, x1), Y1 = f2_pack(y1, y1), Z1 = f2_pack(z1, z1);
-#pragma unroll
-            for (int h = 0; h < PR / 2; ++h) {
-                const unsigned long long dx = f2_sub(X2[h], X1), dy = f2_sub(Y2[h], Y1), dz = f2_sub(Z2[h], Z1);
-                const unsigned long long d = f2_fma(dz, dz, f2_fma(dx, dx, f2_mul(dy, dy)));
-                float d0, d1;
-                f2_unpack(d, d0, d1);
-                td[2 * h] = fminf(d0, td[2 * h]);
-                td[2 * h + 1] = fminf(d1, td[2 * h + 1]);
-            }
-            if constexpr (STREAM) {
-#pragma unroll
-                for (int g = PR / 4; g < P / 4; ++g) {
-                    const float4 X = s4[(g * 3 + 0) * T + tid], Y = s4[(g * 3 + 1) * T + tid], Z = s4[(g * 3 + 2) * T + tid];
-                    const unsigned long long xa = f2_pack(X.x, X.y), xb = f2_pack(X.z, X.w), ya = f2_pack(Y.x, Y.y),
-                                             yb = f2_pack(Y.z, Y.w), za = f2_pack(Z.x, Z.y), zb = f2_pack(Z.z, Z.w);
-                    const unsigned long long dxa = f2_sub(xa, X1), dya = f2_sub(ya, Y1), dza = f2_sub(za, Z1);
-                    const unsigned long long dxb = f2_sub(xb, X1), dyb = f2_sub(yb, Y1), dzb = f2_sub(zb, Z1);
-                    const unsigned long long da = f2_fma(dza, dza, f2_fma(dxa, dxa, f2_mul(dya, dya)));
-                    const unsigned long long db = f2_fma(dzb, dzb, f2_fma(dxb, dxb, f2_mul(dyb, dyb)));
-                    float d0, d1, d2, d3;
-                    f2_unpack(da, d0, d1);
-                    f2_unpack(db, d2, d3);
-                    td[4 * g + 0] = fminf(d0, td[4 * g + 0]);
-                    td[4 * g + 1] = fminf(d1, td[4 * g + 1]);
-                    td[4 * g + 2] = fminf(d2, td[4 * g + 2]);
-                    td[4 * g + 3] = fminf(d3, td[4 * g + 3]);
-                }
-            }
+            pair_update(X2, Y2, Z2, td, x1, y1, z1);
+            if constexpr (STREAM) stream_update_packed<PR / 4, P / 4, PR, T>(s4, tid, td, x1, y1, z1);
             float mx;
             int pos;
             value_argmax_first<P>(td, mx, pos);
             hi = __float_as_uint(mx);
             lo = ~(tpc | ((unsigned)pos << jshift));
         } else {
-        float best;
-        int bj;
-        fps_step<PR, 1, P>(px, py, pz, td, x1, y1, z1, best, bj);  // the PR register-resident points
-        if constexpr (STREAM) {
-#pragma unroll
-            for (int g = PR / 4; g < P / 4; ++g) {
-                const float4 X = s4[(g * 3 + 0) * T + tid], Y = s4[(g * 3 + 1) * T + tid], Z = s4[(g * 3 + 2) * T + tid];
-                const float xs[4] = {X.x, X.y, X.z, X.w}, ys[4] = {Y.x, Y.y, Y.z, Y.w}, zs[4] = {Z.x, Z.y, Z.z, Z.w};
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int j = 4 * g + u;
-                    const float d = d2_fma_pattern(xs[u], ys[u], zs[u], x1, y1, z1);
-                    const float d2 = fminf(d, td[j]);
-                    td[j] = d2;
-                    if (d2 > best) {
-                        best = d2;
-                        bj = j;
-                    }
-                }
+            float best;
+            int bj;
+            fps_step<PR, 1, P>(px, py, pz, td, x1, y1, z1, best, bj);  // the PR register-resident points
+            if constexpr (STREAM) stream_update<PR / 4, P / 4, PR, T>(s4, tid, td, x1, y1, z1, best, bj);
+            if (best >= 0.0f) {
+                hi = __float_as_uint(best);
+                lo = ~tb_encode((unsigned)(tid + T * (rank + C * bj)));
             }
         }
-        if (best >= 0.0f) {
-            hi = __float_as_uint(best);
-            lo = ~tb_encode((unsigned)(tid + T * (rank + C * bj)));
-        }
-        }  // V == 0
         warp_max_pair(hi, lo);
         if (lane == 0) s_keys[buf][warp] = make_uint2(lo, hi);
         __syncthreads();
@@ -740,46 +757,22 @@ fps_cluster_big_kernel(int n, int m, int C, const float* __restrict__ xyz, int* 
     int* __restrict__ out = idx_out + (size_t)cloud * m;
     float* __restrict__ oxyz = new_xyz ? new_xyz + (size_t)cloud * m * 3 : nullptr;
 
-    if (tid == 0) {
-        mbar_init(smem_addr(&s_mbar[0]), 1);
-        mbar_init(smem_addr(&s_mbar[1]), 1);
-        fence_mbar_init_cluster();
-    }
+    if (tid == 0) init_step_mbars(s_mbar);
 
     float px[PR], py[PR], pz[PR], td[P];
-#pragma unroll
-    for (int j = 0; j < P; ++j) {
-        const long long k = (long long)tid + (long long)T * (rank + (long long)C * j);
-        float x = 0.f, y = 0.f, z = 0.f, t = -1.0f;
-        if (k < n) {
-            x = pts[3 * k + 0];
-            y = pts[3 * k + 1];
-            z = pts[3 * k + 2];
-            t = 1e38f;
-        }
-        td[j] = t;
-        if (j < PR) {
-            px[j] = x;
-            py[j] = y;
-            pz[j] = z;
-        } else {
+    load_points<P, PR, T>(pts, n, C, rank, tid, px, py, pz, td, [&](int j, float x, float y, float z) {
+        if (j >= PR) {
             const int g = (j - PR) >> 2, u = (j - PR) & 3;
             s_pts[(((g * 3 + 0) * T + tid) << 2) + u] = x;
             s_pts[(((g * 3 + 1) * T + tid) << 2) + u] = y;
             s_pts[(((g * 3 + 2) * T + tid) << 2) + u] = z;
         }
-    }
-    // V == 1: the register-resident coordinates as packed pairs (the scalar copies above are then dead)
+    });
     constexpr int HR = (V == 1) ? PR / 2 : 1;
     unsigned long long X2[HR], Y2[HR], Z2[HR];
     unsigned tpc = 0u, jstep = 0u;
     if constexpr (V == 1) {
-#pragma unroll
-        for (int h = 0; h < HR; ++h) {
-            X2[h] = f2_pack(px[2 * h], px[2 * h + 1]);
-            Y2[h] = f2_pack(py[2 * h], py[2 * h + 1]);
-            Z2[h] = f2_pack(pz[2 * h], pz[2 * h + 1]);
-        }
+        pack_pairs(px, py, pz, X2, Y2, Z2);
         const unsigned base = (unsigned)tid + (unsigned)T * rank;  // this thread's point j = 0
         tpc = (base < (unsigned)n) ? tb_encode(base) : 0xffffffffu;  // all ones: a thread without points sends key (0, 0)
         jstep = (unsigned)C * (unsigned)(T / 512);                   // k >> 9 grows by this per j; base >> 9 < jstep
@@ -809,63 +802,22 @@ fps_cluster_big_kernel(int n, int m, int C, const float* __restrict__ xyz, int* 
         int bj = 0;
         unsigned myhi = 0u, mylo = 0u;
         if constexpr (V == 1) {
-            const unsigned long long X1 = f2_pack(x1, x1), Y1 = f2_pack(y1, y1), Z1 = f2_pack(z1, z1);
-#pragma unroll
-            for (int h = 0; h < PR / 2; ++h) {
-                const unsigned long long dx = f2_sub(X2[h], X1), dy = f2_sub(Y2[h], Y1), dz = f2_sub(Z2[h], Z1);
-                const unsigned long long d = f2_fma(dz, dz, f2_fma(dx, dx, f2_mul(dy, dy)));
-                float d0, d1;
-                f2_unpack(d, d0, d1);
-                td[2 * h] = fminf(d0, td[2 * h]);
-                td[2 * h + 1] = fminf(d1, td[2 * h + 1]);
-            }
-#pragma unroll
-            for (int g = 0; g < NG; ++g) {
-                const float4 X = s4[(g * 3 + 0) * T + tid], Y = s4[(g * 3 + 1) * T + tid], Z = s4[(g * 3 + 2) * T + tid];
-                const unsigned long long xa = f2_pack(X.x, X.y), xb = f2_pack(X.z, X.w), ya = f2_pack(Y.x, Y.y),
-                                         yb = f2_pack(Y.z, Y.w), za = f2_pack(Z.x, Z.y), zb = f2_pack(Z.z, Z.w);
-                const unsigned long long dxa = f2_sub(xa, X1), dya = f2_sub(ya, Y1), dza = f2_sub(za, Z1);
-                const unsigned long long dxb = f2_sub(xb, X1), dyb = f2_sub(yb, Y1), dzb = f2_sub(zb, Z1);
-                const unsigned long long da = f2_fma(dza, dza, f2_fma(dxa, dxa, f2_mul(dya, dya)));
-                const unsigned long long db = f2_fma(dzb, dzb, f2_fma(dxb, dxb, f2_mul(dyb, dyb)));
-                float d0, d1, d2, d3;
-                f2_unpack(da, d0, d1);
-                f2_unpack(db, d2, d3);
-                const int j = PR + 4 * g;
-                td[j + 0] = fminf(d0, td[j + 0]);
-                td[j + 1] = fminf(d1, td[j + 1]);
-                td[j + 2] = fminf(d2, td[j + 2]);
-                td[j + 3] = fminf(d3, td[j + 3]);
-            }
+            pair_update(X2, Y2, Z2, td, x1, y1, z1);
+            stream_update_packed<0, NG, PR, T>(s4, tid, td, x1, y1, z1);
             float mx;
             value_argmax_first<P>(td, mx, bj);
             myhi = __float_as_uint(mx);
             mylo = ~(tpc + (unsigned)bj * jstep);  // tpc all ones (no points): the sum wraps to bj*jstep - 1, masked below
             if (tpc == 0xffffffffu) mylo = 0u;
         } else {
-        float best;
-        fps_step<PR, 1, P>(px, py, pz, td, x1, y1, z1, best, bj);
-#pragma unroll
-        for (int g = 0; g < NG; ++g) {
-            const float4 X = s4[(g * 3 + 0) * T + tid], Y = s4[(g * 3 + 1) * T + tid], Z = s4[(g * 3 + 2) * T + tid];
-            const float xs[4] = {X.x, X.y, X.z, X.w}, ys[4] = {Y.x, Y.y, Y.z, Y.w}, zs[4] = {Z.x, Z.y, Z.z, Z.w};
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const int j = PR + 4 * g + u;
-                const float d = d2_fma_pattern(xs[u], ys[u], zs[u], x1, y1, z1);
-                const float d2 = fminf(d, td[j]);
-                td[j] = d2;
-                if (d2 > best) {
-                    best = d2;
-                    bj = j;
-                }
+            float best;
+            fps_step<PR, 1, P>(px, py, pz, td, x1, y1, z1, best, bj);
+            stream_update<0, NG, PR, T>(s4, tid, td, x1, y1, z1, best, bj);
+            if (best >= 0.0f) {
+                myhi = __float_as_uint(best);
+                mylo = ~tb_encode((unsigned)(tid + T * (rank + uc * bj)));
             }
         }
-        if (best >= 0.0f) {
-            myhi = __float_as_uint(best);
-            mylo = ~tb_encode((unsigned)(tid + T * (rank + uc * bj)));
-        }
-        }  // V == 0
         unsigned hi = myhi, lo = mylo;
         warp_max_pair(hi, lo);
         if (lane == 0) s_keys[buf][warp] = make_uint2(lo, hi);
@@ -1034,6 +986,13 @@ static std::atomic<int> g_fps_packed{kFpsPackedDefault};
 constexpr int kFpsPackedClusterDefault = 1;
 static std::atomic<int> g_fps_packed_cluster{kFpsPackedClusterDefault};
 
+// The chain an override names in the two low bits of `threads` (T is a multiple of 128): +1 packed, +2 plain, +0 the
+// built-in choice `builtin`.
+static int override_chain(int threads, int builtin) {
+    const int chain = threads & 3;
+    return chain == 1 ? 1 : (chain == 2 ? 0 : builtin);
+}
+
 static unsigned long long pack_cfg(int threads, int ppt, int cluster) {
     if (threads <= 0) return 0ull;
     return ((unsigned long long)threads << 40) | ((unsigned long long)(ppt & 0xfffff) << 20) | (unsigned long long)(cluster + 64);
@@ -1082,76 +1041,12 @@ static int launch_cta(int b, int n, int m, const float* inp, int* out, float* ne
     return finish_launch();
 }
 
-template <int P, int T, int PR, int V>
-static int launch_cluster(int C, int b, int n, int m, const float* inp, int* out, float* new_xyz, cudaStream_t st) {
-    static AttrOnce once;
-    auto kern = fps_cluster_kernel<P, T, PR, V>;
-    const size_t dyn = (size_t)3 * P * T * sizeof(float);
-    if (dyn > 200 * 1024) return (int)cudaErrorInvalidValue;
-    cudaError_t e = ensure_attrs(once, kern, dyn, true);
-    if (e != cudaSuccess) return (int)e;
-    int log2c = 0;
-    while ((1 << log2c) < C) ++log2c;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)b * C, 1, 1);
-    cfg.blockDim = dim3(T, 1, 1);
-    cfg.dynamicSmemBytes = dyn;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = C;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    e = cudaLaunchKernelEx(&cfg, kern, n, m, log2c, inp, out, new_xyz);
-    count_launch();
-    if (e != cudaSuccess) return (int)e;
-    return (int)cudaGetLastError();
-}
-
-// How many clusters of this kernel the device can hold at once (cudaOccupancyMaxActiveClusters): the
-// planner must keep every cloud's cluster co-resident — a cluster that has to wait for a second wave
-// doubles the time of the whole call.
-template <int P, int T, int PR, int V>
-static int cluster_capacity(int C) {
-    static std::atomic<int> cache[5][64];  // [log2 C][device]; 0 = not asked yet
-    int log2c = 0;
-    while ((1 << log2c) < C) ++log2c;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64 || log2c > 4) return 0;
-    const int hit = cache[log2c][dev].load(std::memory_order_relaxed);
-    if (hit) return hit > 0 ? hit : 0;
-    static AttrOnce once;
-    auto kern = fps_cluster_kernel<P, T, PR, V>;
-    const size_t dyn = (size_t)3 * P * T * sizeof(float);
-    if (dyn > 200 * 1024 || ensure_attrs(once, kern, dyn, true) != cudaSuccess) return 0;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)C * (unsigned)num_sms(), 1, 1);
-    cfg.blockDim = dim3(T, 1, 1);
-    cfg.dynamicSmemBytes = dyn;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = C;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    int num = 0;
-    if (cudaOccupancyMaxActiveClusters(&num, kern, &cfg) != cudaSuccess) {
-        (void)cudaGetLastError();
-        num = 0;
-    }
-    cache[log2c][dev].store(num > 0 ? num : -1, std::memory_order_relaxed);
-    return num;
-}
-
-template <int P, int T, int PR>
-static cudaLaunchConfig_t big_config(int C, int clusters, cudaLaunchAttribute* attr, cudaStream_t st) {
+// `clusters` thread-block clusters of C CTAs of T threads
+static cudaLaunchConfig_t cluster_config(int clusters, int C, int T, size_t dyn, cudaStream_t st, cudaLaunchAttribute* attr) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((unsigned)clusters * (unsigned)C, 1, 1);
     cfg.blockDim = dim3(T, 1, 1);
-    cfg.dynamicSmemBytes = (size_t)3 * (P - PR) * T * sizeof(float);
+    cfg.dynamicSmemBytes = dyn;
     cfg.stream = st;
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = C;
@@ -1162,41 +1057,75 @@ static cudaLaunchConfig_t big_config(int C, int clusters, cudaLaunchAttribute* a
     return cfg;
 }
 
+// The two cluster kernels: fps_cluster_kernel keeps a shared-memory copy of every point (at most 200 KB),
+// fps_cluster_big_kernel of the streamed points only (at most 226 KB).
 template <int P, int T, int PR, int V>
-static int launch_cluster_big(int C, int b, int n, int m, const float* inp, int* out, float* new_xyz, cudaStream_t st) {
+struct ClusterKernel {
+    static constexpr size_t dyn = (size_t)3 * P * T * sizeof(float), max_dyn = 200 * 1024;
+    static constexpr int threads = T;
+    static auto kernel() { return fps_cluster_kernel<P, T, PR, V>; }
+};
+template <int P, int T, int PR, int V>
+struct ClusterBigKernel {
+    static constexpr size_t dyn = (size_t)3 * (P - PR) * T * sizeof(float), max_dyn = 226 * 1024;
+    static constexpr int threads = T;
+    static auto kernel() { return fps_cluster_big_kernel<P, T, PR, V>; }
+};
+
+// cluster_arg: log2 C for fps_cluster_kernel, C for fps_cluster_big_kernel
+template <class K>
+static int launch_cluster(int C, int cluster_arg, int b, int n, int m, const float* inp, int* out, float* new_xyz,
+                          cudaStream_t st) {
     static AttrOnce once;
-    auto kern = fps_cluster_big_kernel<P, T, PR, V>;
-    cudaLaunchAttribute attr[1];
-    cudaLaunchConfig_t cfg = big_config<P, T, PR>(C, b, attr, st);
-    if (cfg.dynamicSmemBytes > 226 * 1024) return (int)cudaErrorInvalidValue;
-    cudaError_t e = ensure_attrs(once, kern, cfg.dynamicSmemBytes, true);
+    if (K::dyn > K::max_dyn) return (int)cudaErrorInvalidValue;
+    cudaError_t e = ensure_attrs(once, K::kernel(), K::dyn, true);
     if (e != cudaSuccess) return (int)e;
-    e = cudaLaunchKernelEx(&cfg, kern, n, m, C, inp, out, new_xyz);
+    cudaLaunchAttribute attr[1];
+    const cudaLaunchConfig_t cfg = cluster_config(b, C, K::threads, K::dyn, st, attr);
+    e = cudaLaunchKernelEx(&cfg, K::kernel(), n, m, cluster_arg, inp, out, new_xyz);
     count_launch();
     if (e != cudaSuccess) return (int)e;
     return (int)cudaGetLastError();
 }
 
-template <int P, int T, int PR, int V>
-static int cluster_big_capacity(int C) {
+// How many clusters of C CTAs of this kernel the device can hold at once (cudaOccupancyMaxActiveClusters): the
+// planner must keep every cloud's cluster co-resident — a cluster that has to wait for a second wave doubles the time
+// of the whole call.
+template <class K>
+static int cluster_capacity(int C) {
     static std::atomic<int> cache[17][64];  // [C][device]; 0 = not asked yet
     int dev = 0;
     if (C < 2 || C > 16 || cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 0;
     const int hit = cache[C][dev].load(std::memory_order_relaxed);
     if (hit) return hit > 0 ? hit : 0;
     static AttrOnce once;
-    auto kern = fps_cluster_big_kernel<P, T, PR, V>;
+    if (K::dyn > K::max_dyn || ensure_attrs(once, K::kernel(), K::dyn, true) != cudaSuccess) return 0;
     cudaLaunchAttribute attr[1];
-    cudaLaunchConfig_t cfg = big_config<P, T, PR>(C, num_sms(), attr, nullptr);
-    if (cfg.dynamicSmemBytes > 226 * 1024 || ensure_attrs(once, kern, cfg.dynamicSmemBytes, true) != cudaSuccess) return 0;
+    const cudaLaunchConfig_t cfg = cluster_config(num_sms(), C, K::threads, K::dyn, nullptr, attr);
     int num = 0;
-    if (cudaOccupancyMaxActiveClusters(&num, kern, &cfg) != cudaSuccess) {
+    if (cudaOccupancyMaxActiveClusters(&num, K::kernel(), &cfg) != cudaSuccess) {
         (void)cudaGetLastError();
         num = 0;
     }
     cache[C][dev].store(num > 0 ? num : -1, std::memory_order_relaxed);
     return num;
 }
+
+// ---- every kernel instantiation, listed once ------------------------------------------------------------------------
+// X(P, T, packed): fps_cta_kernel<P, T, 0>, and <P, T, 1> where `packed` (the packed chain needs P >= 8)
+#define PN2_FPS_CTA_KERNELS(X)                                                                       \
+    X(1, 128, 0) X(2, 128, 0) X(4, 128, 0) X(8, 128, 1) X(16, 128, 1) X(32, 128, 1)                  \
+    X(1, 256, 0) X(2, 256, 0) X(4, 256, 0) X(8, 256, 1) X(16, 256, 1) X(32, 256, 1)                  \
+    X(1, 512, 0) X(2, 512, 0) X(4, 512, 0) X(8, 512, 1) X(16, 512, 1)                                \
+    X(1, 1024, 0) X(2, 1024, 0) X(4, 1024, 0) X(8, 1024, 1)
+// X(P, T, PR, packed): fps_cluster_kernel<P, T, PR, 0>, and <P, T, PR, 1> where `packed` (needs P % 4 == 0)
+#define PN2_FPS_CLUSTER_KERNELS(X)                                                                   \
+    X(4, 128, 4, 1) X(8, 128, 8, 1) X(16, 128, 16, 1) X(32, 128, 32, 1)                              \
+    X(2, 256, 2, 0) X(4, 256, 4, 1) X(8, 256, 8, 1) X(16, 256, 16, 1) X(32, 256, 32, 1)              \
+    X(1, 512, 1, 0) X(2, 512, 2, 0) X(4, 512, 4, 1) X(8, 512, 8, 1) X(16, 512, 16, 1) X(32, 512, 16, 1) \
+    X(2, 1024, 2, 0) X(4, 1024, 4, 1) X(8, 1024, 8, 1)
+// X(P, PR): fps_cluster_big_kernel<P, 512, PR, 0> and <P, 512, PR, 1>
+#define PN2_FPS_BIG_KERNELS(X) X(44, 16) X(48, 12) X(52, 16)
 
 struct FpsPlan {
     int threads, ppt, cluster;  // cluster == 0: global-scratch fallback; 1: single CTA; >= 2: thread-block cluster
@@ -1230,12 +1159,9 @@ static FpsPlan plan_fps(int b, int n) {
         p.threads = (int)(ov >> 40);
         p.ppt = (int)((ov >> 20) & 0xfffff);
         p.cluster = (int)(ov & 0xfffff) - 64;
-        const int chain = p.threads & 3;  // cluster plans: chain named in the low bits of `threads`
+        p.packed = override_chain(p.threads, (p.cluster >= 2) ? packed_cluster : packed);
         p.threads &= ~3;
         p.pr = (p.ppt >= 32 && p.threads >= 512) ? 16 : p.ppt;  // ppt > 32: the register + shared-memory kernel
-        p.packed = (p.cluster >= 2) ? packed_cluster : packed;
-        if (chain == 1) p.packed = 1;
-        if (chain == 2) p.packed = 0;
         if (p.cluster == -1 || p.cluster == -2) {  // single CTA with the chain named explicitly
             p.packed = (p.cluster == -2) ? 1 : 0;
             p.cluster = 1;
@@ -1318,17 +1244,6 @@ static FpsPlan plan_fps(int b, int n) {
     return {1024, 0, 0, 0};
 }
 
-#define PN2_TRY_CTA(PP, TT) \
-    if (plan.ppt == PP && plan.threads == TT) return launch_cta<PP, TT, 0>(b, n, m, inp, out, new_xyz, sentinel, st);
-#define PN2_TRY_CTA_PACKED(PP, TT) \
-    if (plan.packed && plan.ppt == PP && plan.threads == TT) return launch_cta<PP, TT, 1>(b, n, m, inp, out, new_xyz, sentinel, st);
-#define PN2_TRY_CLU(PP, TT, PRR) \
-    if (plan.ppt == PP && plan.threads == TT && plan.pr == PRR) \
-        return launch_cluster<PP, TT, PRR, 0>(plan.cluster, b, n, m, inp, out, new_xyz, st);
-#define PN2_TRY_CLU_PACKED(PP, TT, PRR) \
-    if (plan.packed && plan.ppt == PP && plan.threads == TT && plan.pr == PRR) \
-        return launch_cluster<PP, TT, PRR, 1>(plan.cluster, b, n, m, inp, out, new_xyz, st);
-
 bool fps_single_cta(int b, int n) { return plan_fps(b, n).cluster == 1; }
 
 size_t fps_scratch_bytes(int b, int n) {
@@ -1347,85 +1262,37 @@ int fps_dispatch(int b, int n, int m, const float* inp, float* temp, int* out, f
         if (cap < n) return (int)cudaErrorInvalidValue;
     }
     if (plan.cluster == 1) {
-        PN2_TRY_CTA_PACKED(8, 128)
-        PN2_TRY_CTA_PACKED(16, 128)
-        PN2_TRY_CTA_PACKED(32, 128)
-        PN2_TRY_CTA_PACKED(8, 256)
-        PN2_TRY_CTA_PACKED(16, 256)
-        PN2_TRY_CTA_PACKED(32, 256)
-        PN2_TRY_CTA_PACKED(8, 512)
-        PN2_TRY_CTA_PACKED(16, 512)
-        PN2_TRY_CTA_PACKED(8, 1024)
-        PN2_TRY_CTA(1, 128)
-        PN2_TRY_CTA(2, 128)
-        PN2_TRY_CTA(4, 128)
-        PN2_TRY_CTA(8, 128)
-        PN2_TRY_CTA(16, 128)
-        PN2_TRY_CTA(32, 128)
-        PN2_TRY_CTA(1, 256)
-        PN2_TRY_CTA(2, 256)
-        PN2_TRY_CTA(4, 256)
-        PN2_TRY_CTA(8, 256)
-        PN2_TRY_CTA(16, 256)
-        PN2_TRY_CTA(32, 256)
-        PN2_TRY_CTA(1, 512)
-        PN2_TRY_CTA(2, 512)
-        PN2_TRY_CTA(4, 512)
-        PN2_TRY_CTA(8, 512)
-        PN2_TRY_CTA(16, 512)
-        PN2_TRY_CTA(1, 1024)
-        PN2_TRY_CTA(2, 1024)
-        PN2_TRY_CTA(4, 1024)
-        PN2_TRY_CTA(8, 1024)
+#define PN2_TRY(P, T, PK)                                                                           \
+    if (plan.ppt == P && plan.threads == T)                                                                 \
+        return (PK && plan.packed) ? launch_cta<P, T, PK>(b, n, m, inp, out, new_xyz, sentinel, st)         \
+                                   : launch_cta<P, T, 0>(b, n, m, inp, out, new_xyz, sentinel, st);
+        PN2_FPS_CTA_KERNELS(PN2_TRY)
+#undef PN2_TRY
         return (int)cudaErrorInvalidValue;
     }
-    if (plan.cluster >= 2 && plan.ppt > 32) {  // register + shared-memory kernel, any cluster size
-        if (plan.cluster > 16 || plan.threads != 512) return (int)cudaErrorInvalidValue;
-        if (plan.packed) {
-            if (plan.ppt == 44) return launch_cluster_big<44, 512, 16, 1>(plan.cluster, b, n, m, inp, out, new_xyz, st);
-            if (plan.ppt == 48) return launch_cluster_big<48, 512, 12, 1>(plan.cluster, b, n, m, inp, out, new_xyz, st);
-            if (plan.ppt == 52) return launch_cluster_big<52, 512, 16, 1>(plan.cluster, b, n, m, inp, out, new_xyz, st);
-        }
-        if (plan.ppt == 44) return launch_cluster_big<44, 512, 16, 0>(plan.cluster, b, n, m, inp, out, new_xyz, st);
-        if (plan.ppt == 48) return launch_cluster_big<48, 512, 12, 0>(plan.cluster, b, n, m, inp, out, new_xyz, st);
-        if (plan.ppt == 52) return launch_cluster_big<52, 512, 16, 0>(plan.cluster, b, n, m, inp, out, new_xyz, st);
+    const int C = plan.cluster;
+    if (C >= 2 && plan.ppt > 32) {  // register + shared-memory kernel, any cluster size
+        if (C > 16 || plan.threads != 512) return (int)cudaErrorInvalidValue;
+#define PN2_TRY(P, PR)                                                                                       \
+    if (plan.ppt == P)                                                                                               \
+        return plan.packed ? launch_cluster<ClusterBigKernel<P, 512, PR, 1>>(C, C, b, n, m, inp, out, new_xyz, st)  \
+                           : launch_cluster<ClusterBigKernel<P, 512, PR, 0>>(C, C, b, n, m, inp, out, new_xyz, st);
+        PN2_FPS_BIG_KERNELS(PN2_TRY)
+#undef PN2_TRY
         return (int)cudaErrorInvalidValue;
     }
-    if (plan.cluster >= 2) {
-        if (plan.cluster > 16 || (plan.cluster & (plan.cluster - 1))) return (int)cudaErrorInvalidValue;
-        if (((long long)plan.cluster * plan.threads) % 512 != 0) return (int)cudaErrorInvalidValue;
-        PN2_TRY_CLU_PACKED(4, 128, 4)
-        PN2_TRY_CLU_PACKED(8, 128, 8)
-        PN2_TRY_CLU_PACKED(16, 128, 16)
-        PN2_TRY_CLU_PACKED(32, 128, 32)
-        PN2_TRY_CLU_PACKED(4, 256, 4)
-        PN2_TRY_CLU_PACKED(8, 256, 8)
-        PN2_TRY_CLU_PACKED(16, 256, 16)
-        PN2_TRY_CLU_PACKED(32, 256, 32)
-        PN2_TRY_CLU_PACKED(4, 512, 4)
-        PN2_TRY_CLU_PACKED(8, 512, 8)
-        PN2_TRY_CLU_PACKED(16, 512, 16)
-        PN2_TRY_CLU_PACKED(32, 512, 16)
-        PN2_TRY_CLU_PACKED(4, 1024, 4)
-        PN2_TRY_CLU_PACKED(8, 1024, 8)
-        PN2_TRY_CLU(4, 128, 4)
-        PN2_TRY_CLU(8, 128, 8)
-        PN2_TRY_CLU(16, 128, 16)
-        PN2_TRY_CLU(32, 128, 32)
-        PN2_TRY_CLU(2, 256, 2)
-        PN2_TRY_CLU(4, 256, 4)
-        PN2_TRY_CLU(8, 256, 8)
-        PN2_TRY_CLU(16, 256, 16)
-        PN2_TRY_CLU(32, 256, 32)
-        PN2_TRY_CLU(1, 512, 1)
-        PN2_TRY_CLU(2, 512, 2)
-        PN2_TRY_CLU(4, 512, 4)
-        PN2_TRY_CLU(8, 512, 8)
-        PN2_TRY_CLU(16, 512, 16)
-        PN2_TRY_CLU(32, 512, 16)
-        PN2_TRY_CLU(2, 1024, 2)
-        PN2_TRY_CLU(4, 1024, 4)
-        PN2_TRY_CLU(8, 1024, 8)
+    if (C >= 2) {
+        if (C > 16 || (C & (C - 1))) return (int)cudaErrorInvalidValue;
+        if (((long long)C * plan.threads) % 512 != 0) return (int)cudaErrorInvalidValue;
+        int log2c = 0;
+        while ((1 << log2c) < C) ++log2c;
+#define PN2_TRY(P, T, PR, PK)                                                                                 \
+    if (plan.ppt == P && plan.threads == T && plan.pr == PR)                                                  \
+        return (PK && plan.packed)                                                                            \
+                   ? launch_cluster<ClusterKernel<P, T, PR, PK>>(C, log2c, b, n, m, inp, out, new_xyz, st)    \
+                   : launch_cluster<ClusterKernel<P, T, PR, 0>>(C, log2c, b, n, m, inp, out, new_xyz, st);
+        PN2_FPS_CLUSTER_KERNELS(PN2_TRY)
+#undef PN2_TRY
         return (int)cudaErrorInvalidValue;
     }
     // global-scratch fallback: needs the reference's (32, n) float scratch (tf_sampling_g.cu:202)
@@ -1435,52 +1302,20 @@ int fps_dispatch(int b, int n, int m, const float* inp, float* temp, int* out, f
     return finish_launch();
 }
 
-#define PN2_CAP_CLU(PP, TT, PRR) \
-    if (ppt == PP && threads == TT) return cluster_capacity<PP, TT, PRR, 0>(cluster);
-#define PN2_CAP_CLU_PACKED(PP, TT, PRR) \
-    if (packed && ppt == PP && threads == TT) return cluster_capacity<PP, TT, PRR, 1>(cluster);
 int fps_cluster_capacity(int threads, int ppt, int cluster, int packed) {
-    if (packed) {
-        if (threads == 512 && ppt == 44) return cluster_big_capacity<44, 512, 16, 1>(cluster);
-        if (threads == 512 && ppt == 48) return cluster_big_capacity<48, 512, 12, 1>(cluster);
-        if (threads == 512 && ppt == 52) return cluster_big_capacity<52, 512, 16, 1>(cluster);
-    }
-    if (threads == 512 && ppt == 44) return cluster_big_capacity<44, 512, 16, 0>(cluster);
-    if (threads == 512 && ppt == 48) return cluster_big_capacity<48, 512, 12, 0>(cluster);
-    if (threads == 512 && ppt == 52) return cluster_big_capacity<52, 512, 16, 0>(cluster);
+#define PN2_CAP(P, PR)                                                                                      \
+    if (threads == 512 && ppt == P)                                                                         \
+        return packed ? cluster_capacity<ClusterBigKernel<P, 512, PR, 1>>(cluster)                          \
+                      : cluster_capacity<ClusterBigKernel<P, 512, PR, 0>>(cluster);
+    PN2_FPS_BIG_KERNELS(PN2_CAP)
+#undef PN2_CAP
     if (cluster < 2 || cluster > 16 || (cluster & (cluster - 1))) return 0;
-    PN2_CAP_CLU_PACKED(4, 128, 4)
-    PN2_CAP_CLU_PACKED(8, 128, 8)
-    PN2_CAP_CLU_PACKED(16, 128, 16)
-    PN2_CAP_CLU_PACKED(32, 128, 32)
-    PN2_CAP_CLU_PACKED(4, 256, 4)
-    PN2_CAP_CLU_PACKED(8, 256, 8)
-    PN2_CAP_CLU_PACKED(16, 256, 16)
-    PN2_CAP_CLU_PACKED(32, 256, 32)
-    PN2_CAP_CLU_PACKED(4, 512, 4)
-    PN2_CAP_CLU_PACKED(8, 512, 8)
-    PN2_CAP_CLU_PACKED(16, 512, 16)
-    PN2_CAP_CLU_PACKED(32, 512, 16)
-    PN2_CAP_CLU_PACKED(4, 1024, 4)
-    PN2_CAP_CLU_PACKED(8, 1024, 8)
-    PN2_CAP_CLU(4, 128, 4)
-    PN2_CAP_CLU(8, 128, 8)
-    PN2_CAP_CLU(16, 128, 16)
-    PN2_CAP_CLU(32, 128, 32)
-    PN2_CAP_CLU(2, 256, 2)
-    PN2_CAP_CLU(4, 256, 4)
-    PN2_CAP_CLU(8, 256, 8)
-    PN2_CAP_CLU(16, 256, 16)
-    PN2_CAP_CLU(32, 256, 32)
-    PN2_CAP_CLU(1, 512, 1)
-    PN2_CAP_CLU(2, 512, 2)
-    PN2_CAP_CLU(4, 512, 4)
-    PN2_CAP_CLU(8, 512, 8)
-    PN2_CAP_CLU(16, 512, 16)
-    PN2_CAP_CLU(32, 512, 16)
-    PN2_CAP_CLU(2, 1024, 2)
-    PN2_CAP_CLU(4, 1024, 4)
-    PN2_CAP_CLU(8, 1024, 8)
+#define PN2_CAP(P, T, PR, PK)                                                                               \
+    if (ppt == P && threads == T)                                                                           \
+        return (PK && packed) ? cluster_capacity<ClusterKernel<P, T, PR, PK>>(cluster)                      \
+                              : cluster_capacity<ClusterKernel<P, T, PR, 0>>(cluster);
+    PN2_FPS_CLUSTER_KERNELS(PN2_CAP)
+#undef PN2_CAP
     return 0;
 }
 
@@ -1489,8 +1324,7 @@ int fps_cluster_capacity(int threads, int ppt, int cluster, int packed) {
 extern "C" {
 
 int pn2_fps_cluster_capacity(int threads, int points_per_thread, int cluster) {
-    const int chain = threads & 3;  // as in pn2_set_fps_config: +1 packed chain, +2 plain chain, +0 the built-in choice
-    const int packed = chain == 1 ? 1 : (chain == 2 ? 0 : pn2::g_fps_packed_cluster.load(std::memory_order_relaxed));
+    const int packed = pn2::override_chain(threads, pn2::g_fps_packed_cluster.load(std::memory_order_relaxed));
     return pn2::fps_cluster_capacity(threads & ~3, points_per_thread, cluster, packed);
 }
 
