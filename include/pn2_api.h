@@ -54,6 +54,18 @@ size_t pn2_fps_scratch_bytes(int b, int n);
  * launch; the pair sample_and_group always issues, utils/pointnet_util.py:40). new_xyz may be NULL. */
 int pn2_fps_gather(int b, int n, int m, const float* inp, float* temp, int* out, float* new_xyz, void* stream);
 
+/* Variable-size clouds.  The *_ragged entries take a padded batch: xyz (b,n,3) with n the row stride, and
+ * lengths (b,) int32, a DEVICE array: cloud i is its first lengths[i] rows.  Cloud i then gets exactly what the
+ * entry without lengths computes on that cloud alone called with n = lengths[i], bit for bit; the padding rows are
+ * never read (they may hold NaN, inf or anything else).  The library never reads `lengths` on the host, so every
+ * call stays asynchronous and capturable in a CUDA graph: each kernel clamps the value it reads to [1, n], and the
+ * kernel variant (and so the cost) is chosen from n.  lengths == NULL means every cloud has n points. */
+
+/* pn2_fps_gather on ragged clouds: out (b,m) indices < lengths[i]; new_xyz (b,m,3) or NULL.  temp as for
+ * pn2_fps_gather: pn2_fps_scratch_bytes(b, n) bytes. */
+int pn2_fps_gather_ragged(int b, int n, int m, const float* inp, const int* lengths, float* temp, int* out,
+                          float* new_xyz, void* stream);
+
 /* probsampleLauncher(b,n,m,inp_p,inp_r,temp,out), tf_sampling_g.cu:198-201 (ProbSample op,
  * tf_sampling.cpp:66-92).  inp_p (b,n) f32 unnormalised probabilities; inp_r (b,m) f32 uniform
  * draws in [0,1]; temp (b,n) f32 caller-provided scratch that receives the cumulative sums (the
@@ -106,6 +118,13 @@ int pn2_ball_grid_build(int b, int n, float radius, int nsample, const float* xy
 int pn2_query_ball_point_prebuilt(int b, int n, int m, float radius, int nsample, const float* xyz1,
                                   const float* xyz2, int* idx, int* pts_cnt, const void* workspace,
                                   size_t workspace_bytes, void* stream);
+
+/* pn2_query_ball_point_ws on ragged data clouds (see pn2_fps_gather_ragged): lengths1 (b,) device int32, the
+ * lengths of xyz1; the queries xyz2 are dense.  Same paths (chosen from n) and the same workspace query,
+ * pn2_query_ball_point_workspace_bytes(b, n).  Every index in idx is < lengths1[i]. */
+int pn2_query_ball_point_ragged(int b, int n, int m, float radius, int nsample, const float* xyz1,
+                                const int* lengths1, const float* xyz2, int* idx, int* pts_cnt, void* workspace,
+                                size_t workspace_bytes, void* stream);
 
 /* groupPointLauncher(b,n,c,m,nsample,points,idx,out), tf_grouping_g.cu:133-136.
  * points (b,n,c); idx (b,m,nsample); out (b,m,nsample,c). */
@@ -278,6 +297,17 @@ void pn2_set_sa_consumer_ctas(int ctas_per_cloud);
 int pn2_sa_layer_device(int b, int n, int m, float radius, int nsample, const float* xyz, int* fps_idx,
                         float* new_xyz, int* idx, int* pts_cnt, float* grouped_xyz, int center,
                         void* workspace, size_t workspace_bytes, void* stream);
+/* The two layer calls on ragged clouds (see pn2_fps_gather_ragged): `lengths` (b,) device int32 after xyz,
+ * otherwise the arguments, paths and workspace of the calls above.  Both the overlapped path and the sequential
+ * one honour the lengths; every output index is < lengths[i], so the grouping and any later layer need none. */
+int pn2_sa_layer_device_ragged(int b, int n, int m, float radius, int nsample, const float* xyz,
+                               const int* lengths, int* fps_idx, float* new_xyz, int* idx, int* pts_cnt,
+                               float* grouped_xyz, int center, void* workspace, size_t workspace_bytes,
+                               void* stream);
+int pn2_sa_layer_msg_device_ragged(int b, int n, int m, int nscales, const float* radii, const int* nsamples,
+                                   const float* xyz, const int* lengths, int* fps_idx, float* new_xyz,
+                                   int* const* idx, int* const* pts_cnt, float* const* grouped_xyz, int center,
+                                   void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- host-buffer entry point (the reference feeds numpy through feed_dict) ----------------- */
 

@@ -35,6 +35,44 @@ def require_cuda(t: torch.Tensor, name: str, dtype) -> torch.Tensor:
     return t if t.is_contiguous() else t.contiguous()
 
 
+_INT_DTYPES = (torch.int8, torch.int16, torch.int32, torch.int64, torch.uint8)
+
+
+def device_lengths(lengths, b: int, n: int, device: torch.device, op: str):
+    """Per-cloud lengths of a padded (b, n, 3) batch as the (b,) int32 tensor on ``device`` the ragged entries take,
+    or None for ``lengths=None`` (every cloud has n points).
+
+    A tensor on ``device`` is used as is (another integer dtype is converted on the device) and never read back: the
+    kernels clamp its values to [1, n], so the call stays asynchronous and capturable in a CUDA graph.  A CPU tensor, a
+    numpy array or a Python sequence is checked here — shape (b,), 1 <= l <= n, else ValueError, as the reference's
+    OP_REQUIRES would — and then copied to the device."""
+    if lengths is None:
+        return None
+    if isinstance(lengths, torch.Tensor) and lengths.is_cuda:
+        if lengths.device != device:
+            raise RuntimeError(f"all tensors must be on the same device ({device} vs {lengths.device})")
+        if lengths.dtype not in _INT_DTYPES:
+            raise TypeError(f"{op} expects integer lengths, got {lengths.dtype}")
+        if tuple(lengths.shape) != (b,):
+            raise ValueError(f"{op} expects (batch_size,) lengths shape ({b},), got {tuple(lengths.shape)}")
+        return lengths.to(torch.int32).contiguous()
+    if isinstance(lengths, torch.Tensor):
+        if lengths.dtype not in _INT_DTYPES:
+            raise TypeError(f"{op} expects integer lengths, got {lengths.dtype}")
+        host = lengths.detach().to(torch.int64)
+    else:
+        import numpy as np
+        arr = np.asarray(lengths)
+        if arr.size and not np.issubdtype(arr.dtype, np.integer):
+            raise TypeError(f"{op} expects integer lengths, got {arr.dtype}")
+        host = torch.from_numpy(arr.astype(np.int64).reshape(arr.shape))
+    if tuple(host.shape) != (b,):
+        raise ValueError(f"{op} expects (batch_size,) lengths shape ({b},), got {tuple(host.shape)}")
+    if b and (int(host.min()) < 1 or int(host.max()) > n):
+        raise ValueError(f"{op} expects 1 <= lengths <= {n} (the padded number of points), got {host.tolist()}")
+    return host.to(torch.int32).to(device)
+
+
 def same_device(*ts: torch.Tensor) -> None:
     dev = ts[0].device
     for t in ts[1:]:

@@ -66,7 +66,7 @@ template <int G>
 __global__ void __launch_bounds__(kBqThreads)
 ball_query_kernel(int n, int m, float thr, int nsample, const float* __restrict__ xyz1,
                   const float* __restrict__ xyz2, int* __restrict__ idx, int* __restrict__ pts_cnt,
-                  const int* __restrict__ grid_params, int grid_stride) {
+                  const int* __restrict__ grid_params, int grid_stride, const int* __restrict__ lengths) {
     // clouds the uniform-grid path serves (flag written by bq_grid_build_kernel) are skipped here
     if (grid_params && grid_params[(size_t)blockIdx.y * grid_stride] != 0 &&
         batch_uses_grid(grid_params, (size_t)grid_stride, (int)gridDim.y))
@@ -87,6 +87,7 @@ ball_query_kernel(int n, int m, float thr, int nsample, const float* __restrict_
     const bool valid = q < m;
 
     const float* __restrict__ data = xyz1 + (size_t)cloud * n * 3;
+    n = cloud_length(lengths, cloud, n);  // the row stride is used up: from here on n is this cloud's length
     float qx = 0.f, qy = 0.f, qz = 0.f;
     if (valid) {
         const float* qp = xyz2 + ((size_t)cloud * m + q) * 3;
@@ -171,11 +172,11 @@ ball_query_kernel(int n, int m, float thr, int nsample, const float* __restrict_
 }
 
 template <int G>
-static int launch_bq(int b, int n, int m, float thr, int nsample, const float* xyz1, const float* xyz2, int* idx,
-                     int* pts_cnt, const int* grid_params, int grid_stride, cudaStream_t st) {
+static int launch_bq(int b, int n, int m, float thr, int nsample, const float* xyz1, const int* lengths, const float* xyz2,
+                     int* idx, int* pts_cnt, const int* grid_params, int grid_stride, cudaStream_t st) {
     constexpr int QPB = kBqThreads / G;
     dim3 grid((m + QPB - 1) / QPB, b, 1);
-    ball_query_kernel<G><<<grid, kBqThreads, 0, st>>>(n, m, thr, nsample, xyz1, xyz2, idx, pts_cnt, grid_params, grid_stride);
+    ball_query_kernel<G><<<grid, kBqThreads, 0, st>>>(n, m, thr, nsample, xyz1, xyz2, idx, pts_cnt, grid_params, grid_stride, lengths);
     return finish_launch();
 }
 
@@ -197,16 +198,33 @@ static int pick_group(int b, int m) {
     return G;
 }
 
-int launch_ball_query_brute(int b, int n, int m, float thr, int nsample, const float* xyz1, const float* xyz2,
-                            int* idx, int* pts_cnt, const int* grid_params, int grid_stride, cudaStream_t st) {
+int launch_ball_query_brute(int b, int n, int m, float thr, int nsample, const float* xyz1, const int* lengths,
+                            const float* xyz2, int* idx, int* pts_cnt, const int* grid_params, int grid_stride,
+                            cudaStream_t st) {
     switch (pick_group(b, m)) {
-        case 1: return launch_bq<1>(b, n, m, thr, nsample, xyz1, xyz2, idx, pts_cnt, grid_params, grid_stride, st);
-        case 2: return launch_bq<2>(b, n, m, thr, nsample, xyz1, xyz2, idx, pts_cnt, grid_params, grid_stride, st);
-        case 4: return launch_bq<4>(b, n, m, thr, nsample, xyz1, xyz2, idx, pts_cnt, grid_params, grid_stride, st);
-        case 8: return launch_bq<8>(b, n, m, thr, nsample, xyz1, xyz2, idx, pts_cnt, grid_params, grid_stride, st);
-        case 16: return launch_bq<16>(b, n, m, thr, nsample, xyz1, xyz2, idx, pts_cnt, grid_params, grid_stride, st);
-        default: return launch_bq<32>(b, n, m, thr, nsample, xyz1, xyz2, idx, pts_cnt, grid_params, grid_stride, st);
+        case 1: return launch_bq<1>(b, n, m, thr, nsample, xyz1, lengths, xyz2, idx, pts_cnt, grid_params, grid_stride, st);
+        case 2: return launch_bq<2>(b, n, m, thr, nsample, xyz1, lengths, xyz2, idx, pts_cnt, grid_params, grid_stride, st);
+        case 4: return launch_bq<4>(b, n, m, thr, nsample, xyz1, lengths, xyz2, idx, pts_cnt, grid_params, grid_stride, st);
+        case 8: return launch_bq<8>(b, n, m, thr, nsample, xyz1, lengths, xyz2, idx, pts_cnt, grid_params, grid_stride, st);
+        case 16: return launch_bq<16>(b, n, m, thr, nsample, xyz1, lengths, xyz2, idx, pts_cnt, grid_params, grid_stride, st);
+        default: return launch_bq<32>(b, n, m, thr, nsample, xyz1, lengths, xyz2, idx, pts_cnt, grid_params, grid_stride, st);
     }
+}
+
+// pn2_query_ball_point on the clouds' first lengths[b] points (lengths == NULL: all n)
+int query_ball_point_brute(int b, int n, int m, float radius, int nsample, const float* xyz1, const int* lengths,
+                           const float* xyz2, int* idx, int* pts_cnt, cudaStream_t st) {
+    if (b < 0 || n <= 0 || m < 0 || nsample <= 0 || !(radius > 0.0f)) return (int)cudaErrorInvalidValue;
+    if (b == 0 || m == 0) return 0;
+    if (!xyz1 || !xyz2 || !idx || !pts_cnt) return (int)cudaErrorInvalidValue;
+    if (b > 65535) return (int)cudaErrorInvalidValue;
+    const float thr = pn2_ball_threshold(radius);
+    if (thr < 0.0f) {  // radius <= 1e-20f: the reference's test can never pass
+        cudaError_t e = cudaMemsetAsync(idx, 0, sizeof(int) * (size_t)b * m * nsample, st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(pts_cnt, 0, sizeof(int) * (size_t)b * m, st);
+        return (int)e;
+    }
+    return launch_ball_query_brute(b, n, m, thr, nsample, xyz1, lengths, xyz2, idx, pts_cnt, nullptr, 0, st);
 }
 
 }  // namespace pn2
@@ -234,19 +252,7 @@ void pn2_set_bq_group(int lanes_per_query) { pn2::g_bq_group = lanes_per_query; 
 
 int pn2_query_ball_point(int b, int n, int m, float radius, int nsample, const float* xyz1, const float* xyz2,
                          int* idx, int* pts_cnt, void* stream) {
-    using namespace pn2;
-    if (b < 0 || n <= 0 || m < 0 || nsample <= 0 || !(radius > 0.0f)) return (int)cudaErrorInvalidValue;
-    if (b == 0 || m == 0) return 0;
-    if (!xyz1 || !xyz2 || !idx || !pts_cnt) return (int)cudaErrorInvalidValue;
-    if (b > 65535) return (int)cudaErrorInvalidValue;
-    cudaStream_t st = as_stream(stream);
-    const float thr = pn2_ball_threshold(radius);
-    if (thr < 0.0f) {  // radius <= 1e-20f: the reference's test can never pass
-        cudaError_t e = cudaMemsetAsync(idx, 0, sizeof(int) * (size_t)b * m * nsample, st);
-        if (e == cudaSuccess) e = cudaMemsetAsync(pts_cnt, 0, sizeof(int) * (size_t)b * m, st);
-        return (int)e;
-    }
-    return launch_ball_query_brute(b, n, m, thr, nsample, xyz1, xyz2, idx, pts_cnt, nullptr, 0, st);
+    return pn2::query_ball_point_brute(b, n, m, radius, nsample, xyz1, nullptr, xyz2, idx, pts_cnt, pn2::as_stream(stream));
 }
 
 }  // extern "C"

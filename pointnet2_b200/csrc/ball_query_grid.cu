@@ -52,7 +52,8 @@ __device__ __forceinline__ float wmax(float v) {
 }
 
 __global__ void __launch_bounds__(kGbThreads, 1)
-bq_grid_build_kernel(int n, float radius, int nsample, const float* __restrict__ xyz1, int* __restrict__ ws, size_t ws_stride) {
+bq_grid_build_kernel(int n, float radius, int nsample, const float* __restrict__ xyz1, int* __restrict__ ws, size_t ws_stride,
+                     const int* __restrict__ lengths) {
     constexpr int T = kGbThreads, NW = T / 32;
     constexpr int MAXC = kGridMaxDim * kGridMaxDim * kGridMaxDim;
     __shared__ float s_red[6][32];
@@ -65,6 +66,7 @@ bq_grid_build_kernel(int n, float radius, int nsample, const float* __restrict__
     int* __restrict__ params = ws + (size_t)cloud * ws_stride;
     int* __restrict__ sorted_idx = params + kGridParamInts;
     int* __restrict__ cell_start = sorted_idx + n;
+    n = cloud_length(lengths, cloud, n);  // the layout above is sized for the stride; from here on n is the cloud's length
 
     float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
     for (int k = tid; k < n; k += T) {
@@ -201,7 +203,7 @@ bq_grid_build_kernel(int n, float radius, int nsample, const float* __restrict__
 __global__ void __launch_bounds__(kGqThreads)
 bq_grid_query_kernel(int n, int m, float thr, int nsample, const float* __restrict__ xyz1,
                      const float* __restrict__ xyz2, int* __restrict__ idx, int* __restrict__ pts_cnt,
-                     const int* __restrict__ ws, size_t ws_stride) {
+                     const int* __restrict__ ws, size_t ws_stride, const int* __restrict__ lengths) {
     __shared__ int s_hits[kGqThreads / 32][kHitCap];
     __shared__ int s_first[kGqThreads / 32];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -217,6 +219,7 @@ bq_grid_query_kernel(int n, int m, float thr, int nsample, const float* __restri
     const int* __restrict__ sorted_idx = params + kGridParamInts;
     const int* __restrict__ cell_start = sorted_idx + n;
     const float* __restrict__ data = xyz1 + (size_t)cloud * n * 3;
+    n = cloud_length(lengths, cloud, n);  // the grid holds only these points; the ordered scan below stops here too
     const float* qp = xyz2 + ((size_t)cloud * m + q) * 3;
     const float qx = qp[0], qy = qp[1], qz = qp[2];
     int* __restrict__ row = idx + ((size_t)cloud * m + q) * nsample;
@@ -303,6 +306,60 @@ bq_grid_query_kernel(int n, int m, float thr, int nsample, const float* __restri
 
 static int g_bq_mode = 0;  // 0 auto (shared-memory grid kernel when the cloud fits it), 1 brute force only, 2 the global-memory grid path
 
+// The grid build / query / whole-path entries below, on the clouds' first lengths[b] points (lengths == NULL: all n).
+static int ball_grid_build(int b, int n, float radius, int nsample, const float* xyz1, const int* lengths, void* workspace,
+                           size_t workspace_bytes, cudaStream_t st) {
+    if (b <= 0 || n <= 0 || nsample <= 0 || !(radius > 0.0f) || !xyz1 || !workspace) return (int)cudaErrorInvalidValue;
+    const size_t need = pn2_query_ball_point_workspace_bytes(b, n);
+    if (need == 0 || workspace_bytes < need || b > 65535) return (int)cudaErrorInvalidValue;
+    bq_grid_build_kernel<<<b, kGbThreads, 0, st>>>(n, radius, nsample, xyz1, static_cast<int*>(workspace),
+                                                   grid_ws_ints_per_cloud(n), lengths);
+    return finish_launch();
+}
+
+static int query_ball_point_prebuilt(int b, int n, int m, float radius, int nsample, const float* xyz1, const int* lengths,
+                                     const float* xyz2, int* idx, int* pts_cnt, const void* workspace, size_t workspace_bytes,
+                                     cudaStream_t st) {
+    if (b < 0 || n <= 0 || m < 0 || nsample <= 0 || !(radius > 0.0f)) return (int)cudaErrorInvalidValue;
+    if (b == 0 || m == 0) return 0;
+    if (!xyz1 || !xyz2 || !idx || !pts_cnt || !workspace) return (int)cudaErrorInvalidValue;
+    const size_t need = pn2_query_ball_point_workspace_bytes(b, n);
+    const float thr = pn2_ball_threshold(radius);
+    if (need == 0 || workspace_bytes < need || b > 65535 || thr < 0.0f) return (int)cudaErrorInvalidValue;
+    const int* ws = static_cast<const int*>(workspace);
+    const size_t stride = grid_ws_ints_per_cloud(n);
+    dim3 grid((m + kGqThreads / 32 - 1) / (kGqThreads / 32), b, 1);
+    bq_grid_query_kernel<<<grid, kGqThreads, 0, st>>>(n, m, thr, nsample, xyz1, xyz2, idx, pts_cnt, ws, stride, lengths);
+    int rc = finish_launch();
+    if (rc) return rc;
+    // clouds the build kernel did not flag for the grid are done by the brute-force kernel
+    return launch_ball_query_brute(b, n, m, thr, nsample, xyz1, lengths, xyz2, idx, pts_cnt, ws, (int)stride, st);
+}
+
+int query_ball_point_ws(int b, int n, int m, float radius, int nsample, const float* xyz1, const int* lengths,
+                        const float* xyz2, int* idx, int* pts_cnt, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+    if (b < 0 || n <= 0 || m < 0 || nsample <= 0 || !(radius > 0.0f)) return (int)cudaErrorInvalidValue;
+    if (b == 0 || m == 0) return 0;
+    if (!xyz1 || !xyz2 || !idx || !pts_cnt) return (int)cudaErrorInvalidValue;
+    const size_t need = pn2_query_ball_point_workspace_bytes(b, n);
+    const float thr = pn2_ball_threshold(radius);
+    // clouds that fit the shared-memory grid of sa_fused.cu (n <= 9700): one launch that builds the grid in shared
+    // memory and serves the queries from it — one launch instead of build + query + brute-force back to back from
+    // n = 2048 up; no workspace needed
+    if (g_bq_mode == 0 && n >= kGridMinN && pn2_ball_group_fits(n) && thr >= 0.0f) {
+        // ... when there are queries enough to pay for the grids (every CTA builds its own): below ~4096 queries the
+        // packed brute-force kernel is ahead (r2_report.json, cfg4 SA1024 at B = 2: 2048 queries x 8192 points,
+        // 0.0246 ms against 0.0287)
+        if ((long long)b * m >= 4096) return ball_group(b, n, m, radius, nsample, xyz1, lengths, xyz2, idx, pts_cnt, nullptr, 0, st);
+        return query_ball_point_brute(b, n, m, radius, nsample, xyz1, lengths, xyz2, idx, pts_cnt, st);
+    }
+    if (g_bq_mode == 1 || !workspace || need == 0 || workspace_bytes < need || thr < 0.0f || b > 65535)
+        return query_ball_point_brute(b, n, m, radius, nsample, xyz1, lengths, xyz2, idx, pts_cnt, st);
+    int rc = ball_grid_build(b, n, radius, nsample, xyz1, lengths, workspace, workspace_bytes, st);
+    if (rc) return rc;
+    return query_ball_point_prebuilt(b, n, m, radius, nsample, xyz1, lengths, xyz2, idx, pts_cnt, workspace, workspace_bytes, st);
+}
+
 }  // namespace pn2
 
 extern "C" {
@@ -318,58 +375,26 @@ size_t pn2_query_ball_point_workspace_bytes(int b, int n) {
 // run it on a second stream while farthest point sampling is still producing the queries.
 int pn2_ball_grid_build(int b, int n, float radius, int nsample, const float* xyz1, void* workspace,
                         size_t workspace_bytes, void* stream) {
-    using namespace pn2;
-    if (b <= 0 || n <= 0 || nsample <= 0 || !(radius > 0.0f) || !xyz1 || !workspace) return (int)cudaErrorInvalidValue;
-    const size_t need = pn2_query_ball_point_workspace_bytes(b, n);
-    if (need == 0 || workspace_bytes < need || b > 65535) return (int)cudaErrorInvalidValue;
-    bq_grid_build_kernel<<<b, kGbThreads, 0, as_stream(stream)>>>(n, radius, nsample, xyz1, static_cast<int*>(workspace),
-                                                                   grid_ws_ints_per_cloud(n));
-    return finish_launch();
+    return pn2::ball_grid_build(b, n, radius, nsample, xyz1, nullptr, workspace, workspace_bytes, pn2::as_stream(stream));
 }
 
 int pn2_query_ball_point_prebuilt(int b, int n, int m, float radius, int nsample, const float* xyz1, const float* xyz2,
                                   int* idx, int* pts_cnt, const void* workspace, size_t workspace_bytes, void* stream) {
-    using namespace pn2;
-    if (b < 0 || n <= 0 || m < 0 || nsample <= 0 || !(radius > 0.0f)) return (int)cudaErrorInvalidValue;
-    if (b == 0 || m == 0) return 0;
-    if (!xyz1 || !xyz2 || !idx || !pts_cnt || !workspace) return (int)cudaErrorInvalidValue;
-    const size_t need = pn2_query_ball_point_workspace_bytes(b, n);
-    const float thr = pn2_ball_threshold(radius);
-    if (need == 0 || workspace_bytes < need || b > 65535 || thr < 0.0f) return (int)cudaErrorInvalidValue;
-    cudaStream_t st = as_stream(stream);
-    const int* ws = static_cast<const int*>(workspace);
-    const size_t stride = grid_ws_ints_per_cloud(n);
-    dim3 grid((m + kGqThreads / 32 - 1) / (kGqThreads / 32), b, 1);
-    bq_grid_query_kernel<<<grid, kGqThreads, 0, st>>>(n, m, thr, nsample, xyz1, xyz2, idx, pts_cnt, ws, stride);
-    int rc = finish_launch();
-    if (rc) return rc;
-    // clouds the build kernel did not flag for the grid are done by the brute-force kernel
-    return launch_ball_query_brute(b, n, m, thr, nsample, xyz1, xyz2, idx, pts_cnt, ws, (int)stride, st);
+    return pn2::query_ball_point_prebuilt(b, n, m, radius, nsample, xyz1, nullptr, xyz2, idx, pts_cnt, workspace, workspace_bytes,
+                                          pn2::as_stream(stream));
 }
 
 int pn2_query_ball_point_ws(int b, int n, int m, float radius, int nsample, const float* xyz1, const float* xyz2,
                             int* idx, int* pts_cnt, void* workspace, size_t workspace_bytes, void* stream) {
-    using namespace pn2;
-    if (b < 0 || n <= 0 || m < 0 || nsample <= 0 || !(radius > 0.0f)) return (int)cudaErrorInvalidValue;
-    if (b == 0 || m == 0) return 0;
-    if (!xyz1 || !xyz2 || !idx || !pts_cnt) return (int)cudaErrorInvalidValue;
-    const size_t need = pn2_query_ball_point_workspace_bytes(b, n);
-    const float thr = pn2_ball_threshold(radius);
-    // clouds that fit the shared-memory grid of sa_fused.cu (n <= 9700): one launch that builds the grid in shared
-    // memory and serves the queries from it — one launch instead of build + query + brute-force back to back from
-    // n = 2048 up; no workspace needed
-    if (g_bq_mode == 0 && n >= kGridMinN && pn2_ball_group_fits(n) && thr >= 0.0f) {
-        // ... when there are queries enough to pay for the grids (every CTA builds its own): below ~4096 queries the
-        // packed brute-force kernel is ahead (r2_report.json, cfg4 SA1024 at B = 2: 2048 queries x 8192 points,
-        // 0.0246 ms against 0.0287)
-        if ((long long)b * m >= 4096) return pn2_ball_group(b, n, m, radius, nsample, xyz1, xyz2, idx, pts_cnt, nullptr, 0, stream);
-        return pn2_query_ball_point(b, n, m, radius, nsample, xyz1, xyz2, idx, pts_cnt, stream);
-    }
-    if (g_bq_mode == 1 || !workspace || need == 0 || workspace_bytes < need || thr < 0.0f || b > 65535)
-        return pn2_query_ball_point(b, n, m, radius, nsample, xyz1, xyz2, idx, pts_cnt, stream);
-    int rc = pn2_ball_grid_build(b, n, radius, nsample, xyz1, workspace, workspace_bytes, stream);
-    if (rc) return rc;
-    return pn2_query_ball_point_prebuilt(b, n, m, radius, nsample, xyz1, xyz2, idx, pts_cnt, workspace, workspace_bytes, stream);
+    return pn2::query_ball_point_ws(b, n, m, radius, nsample, xyz1, nullptr, xyz2, idx, pts_cnt, workspace, workspace_bytes,
+                                    pn2::as_stream(stream));
+}
+
+int pn2_query_ball_point_ragged(int b, int n, int m, float radius, int nsample, const float* xyz1, const int* lengths1,
+                                const float* xyz2, int* idx, int* pts_cnt, void* workspace, size_t workspace_bytes,
+                                void* stream) {
+    return pn2::query_ball_point_ws(b, n, m, radius, nsample, xyz1, lengths1, xyz2, idx, pts_cnt, workspace, workspace_bytes,
+                                    pn2::as_stream(stream));
 }
 
 }  // extern "C"

@@ -408,10 +408,14 @@ __device__ __forceinline__ void fps_chain_packed(int n, int m, const float* __re
 // (sa_fused.cu) can consume the picks while this chain is still running — no fence in the loop.
 // =================================================================================================
 // V = 0: the plain chain (fps_step); V = 1: fps_chain_packed.  Same prologue, same outputs bit for bit.
-template <int P, int T, int V = 0>
+// L (ragged batch): the cloud is its first cloud_length(lengths, ...) rows and n is only the row stride.  Every kernel
+// below reads the length once, in its prologue, and from there on treats the rows beyond it as the padding slots of a
+// short cloud.  L is a template flag so that the instances without lengths compile to the code they always did (a
+// runtime test perturbs the register allocation of the chains).
+template <int P, int T, int V = 0, bool L = false>
 __global__ void __launch_bounds__(T, 1)
 fps_cta_kernel(int n, int m, const float* __restrict__ xyz, int* __restrict__ idx_out,
-               float* __restrict__ new_xyz, int sentinel) {
+               float* __restrict__ new_xyz, int sentinel, const int* __restrict__ lengths) {
     static_assert(T % 512 == 0 || 512 % T == 0, "T must divide or be a multiple of the reference's 512 slots");
     __shared__ uint2 s_keys[2][32];
     extern __shared__ __align__(16) float s_xyz[];
@@ -421,11 +425,12 @@ fps_cta_kernel(int n, int m, const float* __restrict__ xyz, int* __restrict__ id
     const float* __restrict__ pts = xyz + (size_t)cloud * n * 3;
     int* __restrict__ out = idx_out + (size_t)cloud * m;
     float* __restrict__ oxyz = new_xyz ? new_xyz + (size_t)cloud * m * 3 : nullptr;
+    const int nb = L ? cloud_length(lengths, cloud, n) : n;
 
     // The cloud comes in as 16-byte loads, up to 12 per thread in flight before the first one is consumed, and the
     // sentinel fill with its fence runs under them.  (Measured against the 4-byte copy loop this replaces: 0.3 us of
     // the 332 us kernel at cfg2 — the prologue is not where the time goes; kept because it is the shorter chain.)
-    const int total = 3 * n;
+    const int total = 3 * nb;
     const bool vec = (reinterpret_cast<size_t>(pts) & 15) == 0;  // always when n % 4 == 0
     const int nv = vec ? (total >> 2) : 0;
     const float4* __restrict__ p4 = reinterpret_cast<const float4*>(pts);
@@ -465,7 +470,7 @@ fps_cta_kernel(int n, int m, const float* __restrict__ xyz, int* __restrict__ id
     const float* __restrict__ src = s_xyz;
 
     if constexpr (V == 1) {
-        fps_chain_packed<P, T>(n, m, src, out, oxyz, s_keys);
+        fps_chain_packed<P, T>(nb, m, src, out, oxyz, s_keys);
     } else {
         // the plain chain stays in the kernel body: moved into a function of its own, it compiles to differently
         // scheduled code
@@ -474,7 +479,7 @@ fps_cta_kernel(int n, int m, const float* __restrict__ xyz, int* __restrict__ id
 #pragma unroll
         for (int j = 0; j < P; ++j) {
             const int k = tid + j * T;
-            if (k < n) {
+            if (k < nb) {
                 px[j] = src[3 * k + 0];
                 py[j] = src[3 * k + 1];
                 pz[j] = src[3 * k + 2];
@@ -577,10 +582,10 @@ __device__ __forceinline__ void pack_pairs(const float (&px)[PR], const float (&
 // V = 1 (P % 4 == 0): the per-thread update of fps_chain_packed — packed FP32x2 distances, value-only maximum,
 // position by value_argmax_first; a thread's points are already in tie-break order here (one slot per thread), and
 // the tie-break word of point j is tb_encode(t + T*rank) | j << (log2(C*T) - 9).  The exchange is unchanged.
-template <int P, int T, int PR, int V = 0>
+template <int P, int T, int PR, int V = 0, bool L = false>
 __global__ void __launch_bounds__(T, 1)
 fps_cluster_kernel(int n, int m, int log2c, const float* __restrict__ xyz, int* __restrict__ idx_out,
-                   float* __restrict__ new_xyz) {
+                   float* __restrict__ new_xyz, const int* __restrict__ lengths) {
     static_assert(T % 512 == 0 || 512 % T == 0, "T must divide or be a multiple of 512");
     static_assert(PR == P || (PR % 4 == 0 && P % 4 == 0 && PR < P), "streamed points come in groups of four");
     static_assert(V == 0 || (P % 4 == 0 && PR % 2 == 0), "the packed update works on pairs and groups of four");
@@ -599,6 +604,7 @@ fps_cluster_kernel(int n, int m, int log2c, const float* __restrict__ xyz, int* 
     const float* __restrict__ pts = xyz + (size_t)cloud * n * 3;
     int* __restrict__ out = idx_out + (size_t)cloud * m;
     float* __restrict__ oxyz = new_xyz ? new_xyz + (size_t)cloud * m * 3 : nullptr;
+    const int nb = L ? cloud_length(lengths, cloud, n) : n;
 
     if (tid == 0) init_step_mbars(s_mbar);
 
@@ -608,7 +614,7 @@ fps_cluster_kernel(int n, int m, int log2c, const float* __restrict__ xyz, int* 
     };
 
     float px[PR], py[PR], pz[PR], td[P];
-    load_points<P, PR, T>(pts, n, C, rank, tid, px, py, pz, td, [&](int j, float x, float y, float z) {
+    load_points<P, PR, T>(pts, nb, C, rank, tid, px, py, pz, td, [&](int j, float x, float y, float z) {
         s_pts[slot_addr(j, tid, 0)] = x;
         s_pts[slot_addr(j, tid, 1)] = y;
         s_pts[slot_addr(j, tid, 2)] = z;
@@ -619,7 +625,7 @@ fps_cluster_kernel(int n, int m, int log2c, const float* __restrict__ xyz, int* 
     if constexpr (V == 1) {
         pack_pairs(px, py, pz, X2, Y2, Z2);
         const unsigned base = (unsigned)tid + (unsigned)T * rank;  // this thread's point j = 0
-        tpc = (base < (unsigned)n) ? tb_encode(base) : 0xffffffffu;  // all ones: a thread without points sends key (0, 0)
+        tpc = (base < (unsigned)nb) ? tb_encode(base) : 0xffffffffu;  // all ones: a thread without points sends key (0, 0)
         unsigned log2t = 0;
         while ((1u << log2t) < (unsigned)T) ++log2t;
         jshift = (unsigned)log2c + log2t - 9u;  // C*T is a multiple of 512 (checked by the dispatcher)
@@ -734,10 +740,10 @@ fps_cluster_kernel(int n, int m, int log2c, const float* __restrict__ xyz, int* 
 // =================================================================================================
 // V = 1: packed update + value_argmax_first, as in fps_cluster_kernel; the tie-break word of point j is
 // tb_encode(t + T*rank) + j*(C*T/512) (C*T is a multiple of 512 for every C because T is).
-template <int P, int T, int PR, int V = 0>
+template <int P, int T, int PR, int V = 0, bool L = false>
 __global__ void __launch_bounds__(T, 1)
 fps_cluster_big_kernel(int n, int m, int C, const float* __restrict__ xyz, int* __restrict__ idx_out,
-                       float* __restrict__ new_xyz) {
+                       float* __restrict__ new_xyz, const int* __restrict__ lengths) {
     static_assert(T % 512 == 0, "every thread's points must share one reference slot for any cluster size");
     static_assert(PR < P && (P - PR) % 4 == 0, "streamed points come in groups of four");
     static_assert(V == 0 || (P % 4 == 0 && PR % 4 == 0), "the packed update works on pairs and groups of four");
@@ -756,11 +762,12 @@ fps_cluster_big_kernel(int n, int m, int C, const float* __restrict__ xyz, int* 
     const float* __restrict__ pts = xyz + (size_t)cloud * n * 3;
     int* __restrict__ out = idx_out + (size_t)cloud * m;
     float* __restrict__ oxyz = new_xyz ? new_xyz + (size_t)cloud * m * 3 : nullptr;
+    const int nb = L ? cloud_length(lengths, cloud, n) : n;
 
     if (tid == 0) init_step_mbars(s_mbar);
 
     float px[PR], py[PR], pz[PR], td[P];
-    load_points<P, PR, T>(pts, n, C, rank, tid, px, py, pz, td, [&](int j, float x, float y, float z) {
+    load_points<P, PR, T>(pts, nb, C, rank, tid, px, py, pz, td, [&](int j, float x, float y, float z) {
         if (j >= PR) {
             const int g = (j - PR) >> 2, u = (j - PR) & 3;
             s_pts[(((g * 3 + 0) * T + tid) << 2) + u] = x;
@@ -774,7 +781,7 @@ fps_cluster_big_kernel(int n, int m, int C, const float* __restrict__ xyz, int* 
     if constexpr (V == 1) {
         pack_pairs(px, py, pz, X2, Y2, Z2);
         const unsigned base = (unsigned)tid + (unsigned)T * rank;  // this thread's point j = 0
-        tpc = (base < (unsigned)n) ? tb_encode(base) : 0xffffffffu;  // all ones: a thread without points sends key (0, 0)
+        tpc = (base < (unsigned)nb) ? tb_encode(base) : 0xffffffffu;  // all ones: a thread without points sends key (0, 0)
         jstep = (unsigned)C * (unsigned)(T / 512);                   // k >> 9 grows by this per j; base >> 9 < jstep
     }
 
@@ -910,7 +917,7 @@ fps_cluster_big_kernel(int n, int m, int C, const float* __restrict__ xyz, int* 
 template <int T>
 __global__ void __launch_bounds__(T, 1)
 fps_global_kernel(int b, int n, int m, const float* __restrict__ xyz, float* __restrict__ temp,
-                  int* __restrict__ idx_out, float* __restrict__ new_xyz) {
+                  int* __restrict__ idx_out, float* __restrict__ new_xyz, const int* __restrict__ lengths) {
     constexpr int NW = T / 32;
     __shared__ uint2 s_keys[2][32];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -919,7 +926,8 @@ fps_global_kernel(int b, int n, int m, const float* __restrict__ xyz, float* __r
         const float* __restrict__ pts = xyz + (size_t)cloud * n * 3;
         int* __restrict__ out = idx_out + (size_t)cloud * m;
         float* __restrict__ oxyz = new_xyz ? new_xyz + (size_t)cloud * m * 3 : nullptr;
-        for (int k = tid; k < n; k += T) td[k] = 1e38f;
+        const int nb = cloud_length(lengths, cloud, n);
+        for (int k = tid; k < nb; k += T) td[k] = 1e38f;
         float x1 = pts[0], y1 = pts[1], z1 = pts[2];
         if (tid == 0) {
             out[0] = 0;
@@ -933,7 +941,7 @@ fps_global_kernel(int b, int n, int m, const float* __restrict__ xyz, float* __r
         for (int it = 1; it < m; ++it) {
             float best = -1.0f;
             int bk = 0;
-            for (int k = tid; k < n; k += T) {  // T % 512 == 0: one slot per thread, ascending k
+            for (int k = tid; k < nb; k += T) {  // T % 512 == 0: one slot per thread, ascending k
                 const float d = d2_fma_pattern(pts[3 * (size_t)k], pts[3 * (size_t)k + 1], pts[3 * (size_t)k + 2], x1, y1, z1);
                 const float d2 = fminf(d, td[k]);
                 td[k] = d2;
@@ -1022,9 +1030,10 @@ static cudaError_t ensure_attrs(AttrOnce& once, K kern, size_t dyn, bool nonport
 }
 
 template <int P, int T, int V>
-static int launch_cta(int b, int n, int m, const float* inp, int* out, float* new_xyz, int sentinel, cudaStream_t st) {
-    static AttrOnce once;
-    auto kern = fps_cta_kernel<P, T, V>;
+static int launch_cta(int b, int n, int m, const float* inp, const int* lengths, int* out, float* new_xyz, int sentinel,
+                      cudaStream_t st) {
+    static AttrOnce once[2];  // [ragged]
+    auto kern = lengths ? fps_cta_kernel<P, T, V, true> : fps_cta_kernel<P, T, V, false>;
     // the opt-in is set for the largest cloud this instantiation can serve, so one call per device is enough
     size_t dyn = (size_t)n * 3 * sizeof(float);
     if (dyn > 200 * 1024) return (int)cudaErrorInvalidValue;
@@ -1035,9 +1044,9 @@ static int launch_cta(int b, int n, int m, const float* inp, int* out, float* ne
     // memory makes that placement impossible; the other SMs are there for the other batches.
     constexpr size_t kExclusive = 116 * 1024;
     if (2 * b <= num_sms() && dyn < kExclusive) dyn = kExclusive;
-    cudaError_t e = ensure_attrs(once, kern, 200 * 1024, false);
+    cudaError_t e = ensure_attrs(once[lengths ? 1 : 0], kern, 200 * 1024, false);
     if (e != cudaSuccess) return (int)e;
-    kern<<<b, T, dyn, st>>>(n, m, inp, out, new_xyz, sentinel);
+    kern<<<b, T, dyn, st>>>(n, m, inp, out, new_xyz, sentinel, lengths);
     return finish_launch();
 }
 
@@ -1063,26 +1072,29 @@ template <int P, int T, int PR, int V>
 struct ClusterKernel {
     static constexpr size_t dyn = (size_t)3 * P * T * sizeof(float), max_dyn = 200 * 1024;
     static constexpr int threads = T;
-    static auto kernel() { return fps_cluster_kernel<P, T, PR, V>; }
+    static auto kernel(bool ragged = false) { return ragged ? fps_cluster_kernel<P, T, PR, V, true> : fps_cluster_kernel<P, T, PR, V, false>; }
 };
 template <int P, int T, int PR, int V>
 struct ClusterBigKernel {
     static constexpr size_t dyn = (size_t)3 * (P - PR) * T * sizeof(float), max_dyn = 226 * 1024;
     static constexpr int threads = T;
-    static auto kernel() { return fps_cluster_big_kernel<P, T, PR, V>; }
+    static auto kernel(bool ragged = false) {
+        return ragged ? fps_cluster_big_kernel<P, T, PR, V, true> : fps_cluster_big_kernel<P, T, PR, V, false>;
+    }
 };
 
 // cluster_arg: log2 C for fps_cluster_kernel, C for fps_cluster_big_kernel
 template <class K>
-static int launch_cluster(int C, int cluster_arg, int b, int n, int m, const float* inp, int* out, float* new_xyz,
-                          cudaStream_t st) {
-    static AttrOnce once;
+static int launch_cluster(int C, int cluster_arg, int b, int n, int m, const float* inp, const int* lengths, int* out,
+                          float* new_xyz, cudaStream_t st) {
+    static AttrOnce once[2];  // [ragged]
     if (K::dyn > K::max_dyn) return (int)cudaErrorInvalidValue;
-    cudaError_t e = ensure_attrs(once, K::kernel(), K::dyn, true);
+    const bool ragged = lengths != nullptr;
+    cudaError_t e = ensure_attrs(once[ragged ? 1 : 0], K::kernel(ragged), K::dyn, true);
     if (e != cudaSuccess) return (int)e;
     cudaLaunchAttribute attr[1];
     const cudaLaunchConfig_t cfg = cluster_config(b, C, K::threads, K::dyn, st, attr);
-    e = cudaLaunchKernelEx(&cfg, K::kernel(), n, m, cluster_arg, inp, out, new_xyz);
+    e = cudaLaunchKernelEx(&cfg, K::kernel(ragged), n, m, cluster_arg, inp, out, new_xyz, lengths);
     count_launch();
     if (e != cudaSuccess) return (int)e;
     return (int)cudaGetLastError();
@@ -1251,7 +1263,8 @@ size_t fps_scratch_bytes(int b, int n) {
     return plan_fps(b, n).cluster == 0 ? sizeof(float) * (size_t)(b < 32 ? b : 32) * (size_t)n : 0;
 }
 
-int fps_dispatch(int b, int n, int m, const float* inp, float* temp, int* out, float* new_xyz, int sentinel, cudaStream_t st) {
+int fps_dispatch(int b, int n, int m, const float* inp, const int* lengths, float* temp, int* out, float* new_xyz,
+                 int sentinel, cudaStream_t st) {
     if (b < 0 || n <= 0 || m < 0) return (int)cudaErrorInvalidValue;
     if (b == 0 || m == 0) return 0;
     if (!inp || !out) return (int)cudaErrorInvalidValue;
@@ -1264,8 +1277,8 @@ int fps_dispatch(int b, int n, int m, const float* inp, float* temp, int* out, f
     if (plan.cluster == 1) {
 #define PN2_TRY(P, T, PK)                                                                           \
     if (plan.ppt == P && plan.threads == T)                                                                 \
-        return (PK && plan.packed) ? launch_cta<P, T, PK>(b, n, m, inp, out, new_xyz, sentinel, st)         \
-                                   : launch_cta<P, T, 0>(b, n, m, inp, out, new_xyz, sentinel, st);
+        return (PK && plan.packed) ? launch_cta<P, T, PK>(b, n, m, inp, lengths, out, new_xyz, sentinel, st)         \
+                                   : launch_cta<P, T, 0>(b, n, m, inp, lengths, out, new_xyz, sentinel, st);
         PN2_FPS_CTA_KERNELS(PN2_TRY)
 #undef PN2_TRY
         return (int)cudaErrorInvalidValue;
@@ -1275,8 +1288,8 @@ int fps_dispatch(int b, int n, int m, const float* inp, float* temp, int* out, f
         if (C > 16 || plan.threads != 512) return (int)cudaErrorInvalidValue;
 #define PN2_TRY(P, PR)                                                                                       \
     if (plan.ppt == P)                                                                                               \
-        return plan.packed ? launch_cluster<ClusterBigKernel<P, 512, PR, 1>>(C, C, b, n, m, inp, out, new_xyz, st)  \
-                           : launch_cluster<ClusterBigKernel<P, 512, PR, 0>>(C, C, b, n, m, inp, out, new_xyz, st);
+        return plan.packed ? launch_cluster<ClusterBigKernel<P, 512, PR, 1>>(C, C, b, n, m, inp, lengths, out, new_xyz, st)  \
+                           : launch_cluster<ClusterBigKernel<P, 512, PR, 0>>(C, C, b, n, m, inp, lengths, out, new_xyz, st);
         PN2_FPS_BIG_KERNELS(PN2_TRY)
 #undef PN2_TRY
         return (int)cudaErrorInvalidValue;
@@ -1289,8 +1302,8 @@ int fps_dispatch(int b, int n, int m, const float* inp, float* temp, int* out, f
 #define PN2_TRY(P, T, PR, PK)                                                                                 \
     if (plan.ppt == P && plan.threads == T && plan.pr == PR)                                                  \
         return (PK && plan.packed)                                                                            \
-                   ? launch_cluster<ClusterKernel<P, T, PR, PK>>(C, log2c, b, n, m, inp, out, new_xyz, st)    \
-                   : launch_cluster<ClusterKernel<P, T, PR, 0>>(C, log2c, b, n, m, inp, out, new_xyz, st);
+                   ? launch_cluster<ClusterKernel<P, T, PR, PK>>(C, log2c, b, n, m, inp, lengths, out, new_xyz, st)    \
+                   : launch_cluster<ClusterKernel<P, T, PR, 0>>(C, log2c, b, n, m, inp, lengths, out, new_xyz, st);
         PN2_FPS_CLUSTER_KERNELS(PN2_TRY)
 #undef PN2_TRY
         return (int)cudaErrorInvalidValue;
@@ -1298,7 +1311,7 @@ int fps_dispatch(int b, int n, int m, const float* inp, float* temp, int* out, f
     // global-scratch fallback: needs the reference's (32, n) float scratch (tf_sampling_g.cu:202)
     if (!temp) return (int)cudaErrorInvalidValue;
     int grid = b < 32 ? b : 32;
-    fps_global_kernel<1024><<<grid, 1024, 0, st>>>(b, n, m, inp, temp, out, new_xyz);
+    fps_global_kernel<1024><<<grid, 1024, 0, st>>>(b, n, m, inp, temp, out, new_xyz, lengths);
     return finish_launch();
 }
 
@@ -1329,11 +1342,16 @@ int pn2_fps_cluster_capacity(int threads, int points_per_thread, int cluster) {
 }
 
 int pn2_fps(int b, int n, int m, const float* inp, float* temp, int* out, void* stream) {
-    return pn2::fps_dispatch(b, n, m, inp, temp, out, nullptr, 0, pn2::as_stream(stream));
+    return pn2::fps_dispatch(b, n, m, inp, nullptr, temp, out, nullptr, 0, pn2::as_stream(stream));
 }
 
 int pn2_fps_gather(int b, int n, int m, const float* inp, float* temp, int* out, float* new_xyz, void* stream) {
-    return pn2::fps_dispatch(b, n, m, inp, temp, out, new_xyz, 0, pn2::as_stream(stream));
+    return pn2::fps_dispatch(b, n, m, inp, nullptr, temp, out, new_xyz, 0, pn2::as_stream(stream));
+}
+
+int pn2_fps_gather_ragged(int b, int n, int m, const float* inp, const int* lengths, float* temp, int* out, float* new_xyz,
+                          void* stream) {
+    return pn2::fps_dispatch(b, n, m, inp, lengths, temp, out, new_xyz, 0, pn2::as_stream(stream));
 }
 
 size_t pn2_fps_scratch_bytes(int b, int n) { return pn2::fps_scratch_bytes(b, n); }

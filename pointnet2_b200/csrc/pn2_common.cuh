@@ -62,6 +62,14 @@ __device__ __forceinline__ float d2_nofma(float ax, float ay, float az, float bx
     return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
 }
 
+// ---- per-cloud lengths -----------------------------------------------------------------------
+// Points of cloud `cloud` in a padded (b, n, 3) batch: lengths[cloud] clamped to [1, n] (a value out of range can
+// never make a kernel read outside its row), or n when the batch has no lengths (lengths == NULL).  n stays the
+// row stride; rows k >= the length are padding that no kernel reads.
+__device__ __forceinline__ int cloud_length(const int* __restrict__ lengths, int cloud, int n) {
+    return lengths ? min(max(__ldg(lengths + cloud), 1), n) : n;
+}
+
 // ---- warp helpers ----------------------------------------------------------------------------
 // Batch-level rule of the uniform-grid ball query, evaluated identically by the grid kernel and by
 // the brute-force kernel (each warp on its own, no barrier): the two kernels run back to back on one
@@ -122,14 +130,25 @@ __device__ __forceinline__ void bitonic_sort_keys(int (&key)[KMAX], int lane) {
 }
 
 // brute-force ball query launcher (ball_query.cu); clouds whose grid_params[cloud*grid_stride] != 0
-// are skipped (they are served by the uniform-grid kernels of ball_query_grid.cu)
-int launch_ball_query_brute(int b, int n, int m, float thr, int nsample, const float* xyz1, const float* xyz2,
-                            int* idx, int* pts_cnt, const int* grid_params, int grid_stride, cudaStream_t st);
+// are skipped (they are served by the uniform-grid kernels of ball_query_grid.cu).  lengths (b,) of xyz1 or NULL.
+int launch_ball_query_brute(int b, int n, int m, float thr, int nsample, const float* xyz1, const int* lengths,
+                            const float* xyz2, int* idx, int* pts_cnt, const int* grid_params, int grid_stride,
+                            cudaStream_t st);
+// pn2_query_ball_point (ball_query.cu), pn2_query_ball_point_ws (ball_query_grid.cu) and pn2_ball_group (sa_fused.cu) with
+// the lengths of xyz1 (NULL: every cloud has n points)
+int query_ball_point_brute(int b, int n, int m, float radius, int nsample, const float* xyz1, const int* lengths,
+                           const float* xyz2, int* idx, int* pts_cnt, cudaStream_t st);
+int query_ball_point_ws(int b, int n, int m, float radius, int nsample, const float* xyz1, const int* lengths,
+                        const float* xyz2, int* idx, int* pts_cnt, void* workspace, size_t workspace_bytes, cudaStream_t st);
+int ball_group(int b, int n, int m, float radius, int nsample, const float* xyz1, const int* lengths, const float* xyz2, int* idx,
+               int* pts_cnt, float* grouped_xyz, int center, cudaStream_t st);
 
 // farthest point sampling dispatch (fps.cu), shared with the fused set-abstraction layer (sa_fused.cu).
 // sentinel != 0: single-CTA plans only (ask fps_single_cta first) — the kernel pre-fills `out` with -1 and
 // signals programmatic launch completion so that a dependent grid can consume the picks as they appear.
-int fps_dispatch(int b, int n, int m, const float* inp, float* temp, int* out, float* new_xyz, int sentinel, cudaStream_t st);
+// lengths (b,) device int32 or NULL (see cloud_length); the plan is chosen from n either way.
+int fps_dispatch(int b, int n, int m, const float* inp, const int* lengths, float* temp, int* out, float* new_xyz,
+                 int sentinel, cudaStream_t st);
 bool fps_single_cta(int b, int n);
 size_t fps_scratch_bytes(int b, int n);
 

@@ -81,11 +81,14 @@ __device__ __forceinline__ int ld_volatile_s32(const int* p) {
 // xyz1 (b,n,3) data.  Queries: xyz2 (b,m,3), or — when q_idx != NULL — the data points
 // xyz1[b, q_idx[b,j]], where q_idx (b,m) is being filled by a concurrently running sampling kernel
 // (-1 = not produced yet).  idx (b,m,nsample), pts_cnt (b,m), grouped (b,m,nsample,3) or NULL.
+// L (ragged batch): cloud i is its first cloud_length(lengths, i, n) points.  A template flag, so that the instance
+// without lengths compiles to the code it always did.
+template <bool L>
 __global__ void __launch_bounds__(kBgThreads, 1)
 ball_group_kernel(int n, int m, float radius, float thr, int nsample, const float* __restrict__ xyz1,
                   const float* __restrict__ xyz2, const int* q_idx, int* __restrict__ idx,
                   int* __restrict__ pts_cnt, float* __restrict__ grouped, int center, int ctas_per_cloud,
-                  int wait_primary, int trigger_next) {
+                  int wait_primary, int trigger_next, const int* __restrict__ lengths) {
     constexpr int T = kBgThreads, NW = kBgWarps;
     extern __shared__ __align__(16) unsigned char s_raw[];
     float4* __restrict__ s_pts = reinterpret_cast<float4*>(s_raw);                     // [n]
@@ -104,6 +107,10 @@ ball_group_kernel(int n, int m, float radius, float thr, int nsample, const floa
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int cloud = blockIdx.x / ctas_per_cloud, part = blockIdx.x - cloud * ctas_per_cloud;
     const float* __restrict__ pts = xyz1 + (size_t)cloud * n * 3;
+    // The shared-memory layout above is sized for the row stride; from here on n is this cloud's length: only its
+    // points are boxed, binned and scanned (the layout choice below may then differ from a dense call; the results
+    // cannot)
+    if (L) n = cloud_length(lengths, cloud, n);
 
     // ---- bounding box (a NaN coordinate makes the box infinite: such clouds take the ordered scan,
     //      the only path that reproduces "a NaN point is a hit in every ball", tf_grouping_g.cu:24-25)
@@ -472,12 +479,12 @@ ball_group_kernel(int n, int m, float radius, float thr, int nsample, const floa
 }
 
 struct BgOnce {
-    std::atomic<long long> max_dyn[64];  // per device: largest dynamic shared memory the kernel may request (0 = not asked yet)
+    std::atomic<long long> max_dyn[2][64];  // [ragged][device]: largest dynamic shared memory the kernel may request (0 = not asked yet)
 };
 
-static int launch_ball_group(int b, int n, int m, float radius, float thr, int nsample, const float* xyz1, const float* xyz2,
-                             const int* q_idx, int* idx, int* pts_cnt, float* grouped, int center, int ctas_per_cloud,
-                             bool dependent, bool trigger_next, cudaStream_t st) {
+static int launch_ball_group(int b, int n, int m, float radius, float thr, int nsample, const float* xyz1, const int* lengths,
+                             const float* xyz2, const int* q_idx, int* idx, int* pts_cnt, float* grouped, int center,
+                             int ctas_per_cloud, bool dependent, bool trigger_next, cudaStream_t st) {
     static BgOnce once;
     size_t dyn = bg_smem_bytes(n);
     if (dyn > kBgSmemMax) return (int)cudaErrorInvalidValue;
@@ -486,18 +493,20 @@ static int launch_ball_group(int b, int n, int m, float radius, float thr, int n
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return (int)e;
     if (dev < 0 || dev >= 64) return (int)cudaErrorInvalidDevice;
-    long long max_dyn = once.max_dyn[dev].load(std::memory_order_acquire);
+    const int ragged = lengths ? 1 : 0;
+    auto kern = ragged ? ball_group_kernel<true> : ball_group_kernel<false>;
+    long long max_dyn = once.max_dyn[ragged][dev].load(std::memory_order_acquire);
     if (max_dyn == 0) {
         int optin = 0;
         cudaFuncAttributes fa;
         e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-        if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, ball_group_kernel);
+        if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, kern);
         if (e != cudaSuccess) return (int)e;
         max_dyn = (long long)optin - (long long)fa.sharedSizeBytes;
         if (max_dyn < (long long)kBgSmemMax) return (int)cudaErrorInvalidValue;
-        e = cudaFuncSetAttribute(ball_group_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_dyn);
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_dyn);
         if (e != cudaSuccess) return (int)e;
-        once.max_dyn[dev].store(max_dyn, std::memory_order_release);
+        once.max_dyn[ragged][dev].store(max_dyn, std::memory_order_release);
     }
     // Overlapped with the sampling kernel, the consumer must have an SM to ITSELF: a 1024-thread CTA next
     // to a sampling CTA would take issue slots from the serial chain the whole layer waits for (measured:
@@ -515,8 +524,8 @@ static int launch_ball_group(int b, int n, int m, float radius, float thr, int n
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = dependent ? 1 : 0;
-    e = cudaLaunchKernelEx(&cfg, ball_group_kernel, n, m, radius, thr, nsample, xyz1, xyz2, q_idx, idx, pts_cnt, grouped, center,
-                           ctas_per_cloud, dependent ? 1 : 0, trigger_next ? 1 : 0);
+    e = cudaLaunchKernelEx(&cfg, kern, n, m, radius, thr, nsample, xyz1, xyz2, q_idx, idx, pts_cnt, grouped, center,
+                           ctas_per_cloud, dependent ? 1 : 0, trigger_next ? 1 : 0, lengths);
     count_launch();
     if (e != cudaSuccess) return (int)e;
     return (int)cudaGetLastError();
@@ -537,17 +546,9 @@ static int sa_consumer_ctas(int b, int nscales) {
     return r < 1 ? 1 : r;
 }
 
-}  // namespace pn2
-
-extern "C" {
-
-int pn2_ball_group_fits(int n) {
-    return (n > 0 && n < (1 << pn2::kBgPosBits) && pn2::bg_smem_bytes(n) <= pn2::kBgSmemMax) ? 1 : 0;
-}
-
-int pn2_ball_group(int b, int n, int m, float radius, int nsample, const float* xyz1, const float* xyz2, int* idx,
-                   int* pts_cnt, float* grouped_xyz, int center, void* stream) {
-    using namespace pn2;
+// pn2_ball_group on the clouds' first lengths[b] points (lengths == NULL: all n)
+int ball_group(int b, int n, int m, float radius, int nsample, const float* xyz1, const int* lengths, const float* xyz2, int* idx,
+               int* pts_cnt, float* grouped_xyz, int center, cudaStream_t st) {
     if (b < 0 || n <= 0 || m < 0 || nsample <= 0 || !(radius > 0.0f)) return (int)cudaErrorInvalidValue;
     if (b == 0 || m == 0) return 0;
     if (!xyz1 || !xyz2 || !idx || !pts_cnt) return (int)cudaErrorInvalidValue;
@@ -560,8 +561,66 @@ int pn2_ball_group(int b, int n, int m, float radius, int nsample, const float* 
     const int rmax = (m + kBgWarps - 1) / kBgWarps;
     if (r > rmax) r = rmax;
     if (r < 1) r = 1;
-    return launch_ball_group(b, n, m, radius, thr, nsample, xyz1, xyz2, nullptr, idx, pts_cnt, grouped_xyz, center, r, false, false,
-                             as_stream(stream));
+    return launch_ball_group(b, n, m, radius, thr, nsample, xyz1, lengths, xyz2, nullptr, idx, pts_cnt, grouped_xyz, center, r, false,
+                             false, st);
+}
+
+// pn2_sa_layer_msg_device on the clouds' first lengths[b] points (lengths == NULL: all n)
+static int sa_layer_msg(int b, int n, int m, int nscales, const float* radii, const int* nsamples, const float* xyz,
+                        const int* lengths, int* fps_idx, float* new_xyz, int* const* idx, int* const* pts_cnt,
+                        float* const* grouped_xyz, int center, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+    if (b < 0 || n <= 0 || m < 0 || nscales <= 0 || nscales > 16 || !radii || !nsamples || !idx || !pts_cnt)
+        return (int)cudaErrorInvalidValue;
+    for (int k = 0; k < nscales; ++k)
+        if (nsamples[k] <= 0 || !(radii[k] > 0.0f) || !idx[k] || !pts_cnt[k]) return (int)cudaErrorInvalidValue;
+    if (b == 0 || m == 0) return 0;
+    if (!xyz || !fps_idx || !new_xyz) return (int)cudaErrorInvalidValue;
+    bool overlapped = fps_single_cta(b, n) && pn2_ball_group_fits(n);
+    for (int k = 0; k < nscales; ++k) overlapped = overlapped && pn2_ball_threshold(radii[k]) >= 0.0f;
+    if (overlapped) {
+        // sampling (one CTA per cloud) + one dependent ball_group grid per scale, chained so that all of them
+        // are resident while the sampling chain runs
+        int rc = fps_dispatch(b, n, m, xyz, lengths, nullptr, fps_idx, new_xyz, /*sentinel=*/1, st);
+        const int r = sa_consumer_ctas(b, nscales);
+        for (int k = 0; k < nscales && rc == 0; ++k)
+            rc = launch_ball_group(b, n, m, radii[k], pn2_ball_threshold(radii[k]), nsamples[k], xyz, lengths, nullptr, fps_idx, idx[k],
+                                   pts_cnt[k], grouped_xyz ? grouped_xyz[k] : nullptr, center, r, true, k + 1 < nscales, st);
+        return rc;
+    }
+    // sequential path (clustered / global-scratch sampling, or clouds too large for the in-smem grid); every index the
+    // sampling and the ball query return is below the cloud's length, so the grouping needs no lengths
+    const size_t fps_b = align256(pn2_fps_scratch_bytes(b, n)), bq_b = pn2_query_ball_point_workspace_bytes(b, n);
+    char* ws = static_cast<char*>(workspace);
+    float* temp = nullptr;
+    void* bq_ws = nullptr;
+    if (fps_b) {
+        if (!ws || workspace_bytes < fps_b) return (int)cudaErrorInvalidValue;
+        temp = reinterpret_cast<float*>(ws);
+    }
+    if (bq_b && ws && workspace_bytes >= fps_b + bq_b) bq_ws = ws + fps_b;
+    void* stream = static_cast<void*>(st);
+    int rc = fps_dispatch(b, n, m, xyz, lengths, temp, fps_idx, new_xyz, 0, st);
+    for (int k = 0; k < nscales && rc == 0; ++k) {
+        rc = query_ball_point_ws(b, n, m, radii[k], nsamples[k], xyz, lengths, new_xyz, idx[k], pts_cnt[k], bq_ws, bq_ws ? bq_b : 0, st);
+        float* g = grouped_xyz ? grouped_xyz[k] : nullptr;
+        if (rc || !g) continue;
+        rc = center ? pn2_group_concat(b, n, 0, m, nsamples[k], xyz, new_xyz, nullptr, idx[k], 1, g, nullptr, stream)
+                    : pn2_group_point(b, n, 3, m, nsamples[k], xyz, idx[k], g, stream);
+    }
+    return rc;
+}
+
+}  // namespace pn2
+
+extern "C" {
+
+int pn2_ball_group_fits(int n) {
+    return (n > 0 && n < (1 << pn2::kBgPosBits) && pn2::bg_smem_bytes(n) <= pn2::kBgSmemMax) ? 1 : 0;
+}
+
+int pn2_ball_group(int b, int n, int m, float radius, int nsample, const float* xyz1, const float* xyz2, int* idx,
+                   int* pts_cnt, float* grouped_xyz, int center, void* stream) {
+    return pn2::ball_group(b, n, m, radius, nsample, xyz1, nullptr, xyz2, idx, pts_cnt, grouped_xyz, center, pn2::as_stream(stream));
 }
 
 size_t pn2_sa_layer_device_workspace_bytes(int b, int n, int m, int nsample) {
@@ -575,56 +634,33 @@ size_t pn2_sa_layer_device_workspace_bytes(int b, int n, int m, int nsample) {
 int pn2_sa_layer_msg_device(int b, int n, int m, int nscales, const float* radii, const int* nsamples, const float* xyz,
                             int* fps_idx, float* new_xyz, int* const* idx, int* const* pts_cnt, float* const* grouped_xyz,
                             int center, void* workspace, size_t workspace_bytes, void* stream) {
-    using namespace pn2;
-    if (b < 0 || n <= 0 || m < 0 || nscales <= 0 || nscales > 16 || !radii || !nsamples || !idx || !pts_cnt)
-        return (int)cudaErrorInvalidValue;
-    for (int k = 0; k < nscales; ++k)
-        if (nsamples[k] <= 0 || !(radii[k] > 0.0f) || !idx[k] || !pts_cnt[k]) return (int)cudaErrorInvalidValue;
-    if (b == 0 || m == 0) return 0;
-    if (!xyz || !fps_idx || !new_xyz) return (int)cudaErrorInvalidValue;
-    cudaStream_t st = as_stream(stream);
-    bool overlapped = fps_single_cta(b, n) && pn2_ball_group_fits(n);
-    for (int k = 0; k < nscales; ++k) overlapped = overlapped && pn2_ball_threshold(radii[k]) >= 0.0f;
-    if (overlapped) {
-        // sampling (one CTA per cloud) + one dependent ball_group grid per scale, chained so that all of them
-        // are resident while the sampling chain runs
-        int rc = fps_dispatch(b, n, m, xyz, nullptr, fps_idx, new_xyz, /*sentinel=*/1, st);
-        const int r = sa_consumer_ctas(b, nscales);
-        for (int k = 0; k < nscales && rc == 0; ++k)
-            rc = launch_ball_group(b, n, m, radii[k], pn2_ball_threshold(radii[k]), nsamples[k], xyz, nullptr, fps_idx, idx[k], pts_cnt[k],
-                                   grouped_xyz ? grouped_xyz[k] : nullptr, center, r, true, k + 1 < nscales, st);
-        return rc;
-    }
-    // sequential path (clustered / global-scratch sampling, or clouds too large for the in-smem grid)
-    const size_t fps_b = align256(pn2_fps_scratch_bytes(b, n)), bq_b = pn2_query_ball_point_workspace_bytes(b, n);
-    char* ws = static_cast<char*>(workspace);
-    float* temp = nullptr;
-    void* bq_ws = nullptr;
-    if (fps_b) {
-        if (!ws || workspace_bytes < fps_b) return (int)cudaErrorInvalidValue;
-        temp = reinterpret_cast<float*>(ws);
-    }
-    if (bq_b && ws && workspace_bytes >= fps_b + bq_b) bq_ws = ws + fps_b;
-    int rc = pn2_fps_gather(b, n, m, xyz, temp, fps_idx, new_xyz, stream);
-    for (int k = 0; k < nscales && rc == 0; ++k) {
-        rc = pn2_query_ball_point_ws(b, n, m, radii[k], nsamples[k], xyz, new_xyz, idx[k], pts_cnt[k], bq_ws, bq_ws ? bq_b : 0, stream);
-        float* g = grouped_xyz ? grouped_xyz[k] : nullptr;
-        if (rc || !g) continue;
-        rc = center ? pn2_group_concat(b, n, 0, m, nsamples[k], xyz, new_xyz, nullptr, idx[k], 1, g, nullptr, stream)
-                    : pn2_group_point(b, n, 3, m, nsamples[k], xyz, idx[k], g, stream);
-    }
-    return rc;
+    return pn2::sa_layer_msg(b, n, m, nscales, radii, nsamples, xyz, nullptr, fps_idx, new_xyz, idx, pts_cnt, grouped_xyz, center,
+                             workspace, workspace_bytes, pn2::as_stream(stream));
+}
+
+int pn2_sa_layer_msg_device_ragged(int b, int n, int m, int nscales, const float* radii, const int* nsamples, const float* xyz,
+                                   const int* lengths, int* fps_idx, float* new_xyz, int* const* idx, int* const* pts_cnt,
+                                   float* const* grouped_xyz, int center, void* workspace, size_t workspace_bytes, void* stream) {
+    return pn2::sa_layer_msg(b, n, m, nscales, radii, nsamples, xyz, lengths, fps_idx, new_xyz, idx, pts_cnt, grouped_xyz, center,
+                             workspace, workspace_bytes, pn2::as_stream(stream));
+}
+
+int pn2_sa_layer_device_ragged(int b, int n, int m, float radius, int nsample, const float* xyz, const int* lengths, int* fps_idx,
+                               float* new_xyz, int* idx, int* pts_cnt, float* grouped_xyz, int center, void* workspace,
+                               size_t workspace_bytes, void* stream) {
+    if (!idx || !pts_cnt) return (int)cudaErrorInvalidValue;
+    int* idxs[1] = {idx};
+    int* cnts[1] = {pts_cnt};
+    float* grps[1] = {grouped_xyz};
+    return pn2_sa_layer_msg_device_ragged(b, n, m, 1, &radius, &nsample, xyz, lengths, fps_idx, new_xyz, idxs, cnts,
+                                          grouped_xyz ? grps : nullptr, center, workspace, workspace_bytes, stream);
 }
 
 int pn2_sa_layer_device(int b, int n, int m, float radius, int nsample, const float* xyz, int* fps_idx, float* new_xyz,
                         int* idx, int* pts_cnt, float* grouped_xyz, int center, void* workspace, size_t workspace_bytes,
                         void* stream) {
-    if (!idx || !pts_cnt) return (int)cudaErrorInvalidValue;
-    int* idxs[1] = {idx};
-    int* cnts[1] = {pts_cnt};
-    float* grps[1] = {grouped_xyz};
-    return pn2_sa_layer_msg_device(b, n, m, 1, &radius, &nsample, xyz, fps_idx, new_xyz, idxs, cnts, grouped_xyz ? grps : nullptr, center,
-                                   workspace, workspace_bytes, stream);
+    return pn2_sa_layer_device_ragged(b, n, m, radius, nsample, xyz, nullptr, fps_idx, new_xyz, idx, pts_cnt, grouped_xyz, center,
+                                      workspace, workspace_bytes, stream);
 }
 
 void pn2_set_sa_consumer_ctas(int ctas_per_cloud) { pn2::g_sa_consumer_ctas.store(ctas_per_cloud, std::memory_order_relaxed); }

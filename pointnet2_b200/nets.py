@@ -38,9 +38,10 @@ class SetAbstraction(nn.Module):
         self.mlp2 = SharedMLP(pooled, mlp2, bn) if mlp2 else None
         self.out_channels = self.mlp2.out_channels if self.mlp2 else pooled
 
-    def forward(self, xyz, points):
+    def forward(self, xyz, points, lengths=None):
         return pointnet_sa_module(xyz, points, self.npoint, self.radius, self.nsample, self.mlp, self.mlp2,
-                                  group_all=self.group_all, pooling=self.pooling, knn=self.knn, use_xyz=self.use_xyz)
+                                  group_all=self.group_all, pooling=self.pooling, knn=self.knn, use_xyz=self.use_xyz,
+                                  lengths=lengths)
 
 
 class SetAbstractionMSG(nn.Module):
@@ -54,9 +55,9 @@ class SetAbstractionMSG(nn.Module):
         self.mlps = nn.ModuleList(SharedMLP(cin, w, bn) for w in mlp_list)
         self.out_channels = sum(m.out_channels for m in self.mlps)
 
-    def forward(self, xyz, points):
+    def forward(self, xyz, points, lengths=None):
         return pointnet_sa_module_msg(xyz, points, self.npoint, self.radius_list, self.nsample_list, list(self.mlps),
-                                      use_xyz=self.use_xyz)
+                                      use_xyz=self.use_xyz, lengths=lengths)
 
 
 class FeaturePropagation(nn.Module):
@@ -85,7 +86,10 @@ class _ClsHead(nn.Module):
 
 
 class PointNet2ClsSSG(nn.Module):
-    """Classification net, input (B,N,3) -> logits (B,num_class). models/pointnet2_cls_ssg.py:20-43."""
+    """Classification net, input (B,N,3) -> logits (B,num_class). models/pointnet2_cls_ssg.py:20-43.
+    ``lengths`` (B,), optional: cloud i is ``point_cloud[i, :lengths[i]]`` (variable-size clouds padded to N).  Only
+    the first level sees the padding: it samples 512 centroids per cloud from the real points, and every later level
+    is dense."""
 
     def __init__(self, num_class: int = 40):
         super().__init__()
@@ -94,16 +98,16 @@ class PointNet2ClsSSG(nn.Module):
         self.sa3 = SetAbstraction(256, None, None, None, [256, 512, 1024], group_all=True)
         self.head = _ClsHead(1024, num_class, keep_prob=0.5)
 
-    def forward(self, point_cloud):
+    def forward(self, point_cloud, lengths=None):
         end_points = {"l0_xyz": point_cloud}
-        l1_xyz, l1_points, _ = self.sa1(point_cloud, None)
+        l1_xyz, l1_points, _ = self.sa1(point_cloud, None, lengths)
         l2_xyz, l2_points, _ = self.sa2(l1_xyz, l1_points)
         _, l3_points, _ = self.sa3(l2_xyz, l2_points)
         return self.head(l3_points.reshape(point_cloud.shape[0], -1)), end_points
 
 
 class PointNet2ClsMSG(nn.Module):
-    """Multi-scale classification net. models/pointnet2_cls_msg.py:18-38."""
+    """Multi-scale classification net. models/pointnet2_cls_msg.py:18-38.  ``lengths``: as for PointNet2ClsSSG."""
 
     def __init__(self, num_class: int = 40):
         super().__init__()
@@ -113,8 +117,8 @@ class PointNet2ClsMSG(nn.Module):
         self.sa3 = SetAbstraction(self.sa2.out_channels, None, None, None, [256, 512, 1024], group_all=True)
         self.head = _ClsHead(1024, num_class, keep_prob=0.4)
 
-    def forward(self, point_cloud):
-        l1_xyz, l1_points = self.sa1(point_cloud, None)
+    def forward(self, point_cloud, lengths=None):
+        l1_xyz, l1_points = self.sa1(point_cloud, None, lengths)
         l2_xyz, l2_points = self.sa2(l1_xyz, l1_points)
         _, l3_points, _ = self.sa3(l2_xyz, l2_points)
         return self.head(l3_points.reshape(point_cloud.shape[0], -1)), {}

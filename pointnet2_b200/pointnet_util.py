@@ -96,7 +96,12 @@ def group_and_concat(xyz, new_xyz, points, idx, xyz_first: bool = True):
     return _GroupConcat.apply(xyz, new_xyz, points, idx, xyz_first)
 
 
-def sample_and_group(npoint, radius, nsample, xyz, points, knn=False, use_xyz=True, fused=True):
+def _no_lengths_with(lengths, what: str) -> None:
+    if lengths is not None:
+        raise ValueError(f"lengths (variable-size clouds) are not supported with {what}")
+
+
+def sample_and_group(npoint, radius, nsample, xyz, points, knn=False, use_xyz=True, fused=True, *, lengths=None):
     """Sampling + grouping half of a set-abstraction layer (same positional arguments and return
     tuple as the reference's sample_and_group, utils/pointnet_util.py:22-56).
 
@@ -110,16 +115,22 @@ def sample_and_group(npoint, radius, nsample, xyz, points, knn=False, use_xyz=Tr
         new_xyz (b, npoint, 3), new_points (b, npoint, nsample, 3 + c) [c alone when use_xyz is False],
         idx (b, npoint, nsample) int32 into the n input points, grouped_xyz (b, npoint, nsample, 3)
         centred on new_xyz.
+        lengths: optional (b,) integers: cloud i is ``xyz[i, :lengths[i]]`` (and ``points[i, :lengths[i]]``), padded to
+        n.  Sampling and the ball query then see each cloud alone; every index is below its length, so the grouping
+        never reads the padding.  Not with knn (ValueError).
 
     ``fused=True`` uses the overlapped sampling+grouping layer (sa_layer.sample_group) and the
     single-pass concat kernel; ``fused=False`` issues the reference's op sequence one by one.  Both
     return identical values.
     """
+    if knn:
+        _no_lengths_with(lengths, "knn grouping")
     no_grad_xyz = not xyz.requires_grad
     if fused and no_grad_xyz and not knn:
         # one call: FPS + gather + ball query (+ centred grouped xyz when they are the whole output)
         need_g = points is None or not use_xyz
-        _, new_xyz, idx, _, grouped_xyz = sample_group(npoint, radius, nsample, xyz, center=True, want_grouped=need_g)
+        _, new_xyz, idx, _, grouped_xyz = sample_group(npoint, radius, nsample, xyz, center=True, want_grouped=need_g,
+                                                       lengths=lengths)
         if points is None:
             return new_xyz, grouped_xyz, idx, grouped_xyz
         if not use_xyz:
@@ -127,13 +138,13 @@ def sample_and_group(npoint, radius, nsample, xyz, points, knn=False, use_xyz=Tr
         new_points, grouped_xyz = group_and_concat(xyz, new_xyz, points, idx, xyz_first=True)
         return new_xyz, new_points, idx, grouped_xyz
     if fused and no_grad_xyz:
-        _, new_xyz = farthest_point_sample_and_gather(npoint, xyz)
+        _, new_xyz = farthest_point_sample_and_gather(npoint, xyz, lengths=lengths)
     else:
-        new_xyz = gather_point(xyz, farthest_point_sample(npoint, xyz))
+        new_xyz = gather_point(xyz, farthest_point_sample(npoint, xyz, lengths=lengths))
     if knn:
         _, idx = knn_point(nsample, xyz, new_xyz)
     else:
-        idx, _ = query_ball_point(radius, nsample, xyz, new_xyz)
+        idx, _ = query_ball_point(radius, nsample, xyz, new_xyz, lengths=lengths)
     if fused:
         feats = points if (points is not None and use_xyz) else None
         if points is not None and not use_xyz:
@@ -183,7 +194,8 @@ def _apply_mlp(mlp, t: torch.Tensor, scope=None, name="mlp", bn=True, is_trainin
 
 
 def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp=None, mlp2=None, group_all=False, is_training=None,
-                       bn_decay=None, scope=None, bn=True, pooling='max', knn=False, use_xyz=True, use_nchw=False, fused=True):
+                       bn_decay=None, scope=None, bn=True, pooling='max', knn=False, use_xyz=True, use_nchw=False, fused=True,
+                       lengths=None):
     ''' PointNet Set Abstraction (SA) Module — same positional arguments as the reference
         (utils/pointnet_util.py:87-154), so its call sites run unchanged, e.g. models/pointnet2_sem_seg.py:28:
             pointnet_sa_module(l0_xyz, l0_points, npoint=1024, radius=0.1, nsample=32, mlp=[32,32,64], mlp2=None,
@@ -191,13 +203,16 @@ def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp=None, mlp2=None
         mlp / mlp2: lists of output widths (layers live in the variable-scope registry, layers.scoped_mlp; is_training
         and bn_decay set their mode and batch-norm momentum), or callables on a (batch, npoint, nsample, channel) tensor,
         or None.  use_nchw is accepted and ignored (a layout hint for TensorFlow's conv2d).
+        lengths: optional (b,) per-cloud point counts of a padded batch (see sample_and_group); the outputs are dense.
+        Not with group_all or knn (ValueError).
         Return: new_xyz (b,npoint,3), new_points (b,npoint,channels), idx (b,npoint,nsample)
     '''
     if group_all:
+        _no_lengths_with(lengths, "group_all (the max-pool over every point would need a mask)")
         new_xyz, new_points, idx, grouped_xyz = sample_and_group_all(xyz, points, use_xyz)
     else:
         new_xyz, new_points, idx, grouped_xyz = sample_and_group(npoint, radius, nsample, xyz, points, knn, use_xyz,
-                                                                 fused=fused)
+                                                                 fused=fused, lengths=lengths)
     new_points = _apply_mlp(mlp, new_points, scope, "conv", bn, is_training, bn_decay)
     if pooling == 'max':
         new_points = new_points.max(dim=2, keepdim=True).values
@@ -217,23 +232,25 @@ def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp=None, mlp2=None
 
 
 def pointnet_sa_module_msg(xyz, points, npoint, radius_list: Sequence[float], nsample_list: Sequence[int], mlp_list=None,
-                           is_training=None, bn_decay=None, scope=None, bn=True, use_xyz=True, use_nchw=False, fused=True):
+                           is_training=None, bn_decay=None, scope=None, bn=True, use_xyz=True, use_nchw=False, fused=True,
+                           lengths=None):
     ''' PointNet Set Abstraction (SA) module with Multi-Scale Grouping — same positional arguments as the
         reference (utils/pointnet_util.py:156-196).  One FPS+gather, then per scale: ball query, group,
         centre, concat in the MSG order [features, xyz] (:184), MLP, max-pool; scales concatenated.
         mlp_list: per scale a list of output widths (scope registry), a callable, or None.
+        lengths: optional (b,) per-cloud point counts of a padded batch (see sample_and_group); the outputs are dense.
         Return: new_xyz (b,npoint,3), new_points (b,npoint,sum of channels)
     '''
     pre = None
     if fused and not xyz.requires_grad and (points is None or use_xyz):
         # one call: the sampling pass and every scale's ball query (+ centred grouped xyz when they are the features)
         _, new_xyz, idx_list, _, gxyz_list = sample_group_msg(npoint, radius_list, nsample_list, xyz, center=True,
-                                                              want_grouped=points is None)
+                                                              want_grouped=points is None, lengths=lengths)
         pre = (idx_list, gxyz_list)
     elif fused and not xyz.requires_grad:
-        _, new_xyz = farthest_point_sample_and_gather(npoint, xyz)
+        _, new_xyz = farthest_point_sample_and_gather(npoint, xyz, lengths=lengths)
     else:
-        new_xyz = gather_point(xyz, farthest_point_sample(npoint, xyz))
+        new_xyz = gather_point(xyz, farthest_point_sample(npoint, xyz, lengths=lengths))
     new_points_list = []
     for i in range(len(radius_list)):
         radius, nsample = radius_list[i], nsample_list[i]
@@ -244,7 +261,7 @@ def pointnet_sa_module_msg(xyz, points, npoint, radius_list: Sequence[float], ns
             else:
                 grouped_points, _ = group_and_concat(xyz, new_xyz, points, idx, xyz_first=False)
         else:
-            idx, pts_cnt = query_ball_point(radius, nsample, xyz, new_xyz)
+            idx, pts_cnt = query_ball_point(radius, nsample, xyz, new_xyz, lengths=lengths)
             if fused and (points is None or use_xyz):
                 grouped_points, _ = group_and_concat(xyz, new_xyz, points, idx, xyz_first=False)
             else:

@@ -20,7 +20,7 @@ import collections
 import torch
 
 from . import _lib
-from ._tensor import on_device, ptr, require_cuda, same_device, stream_ptr
+from ._tensor import device_lengths, on_device, ptr, require_cuda, same_device, stream_ptr
 
 
 def _check_layer_args(npoint, radius, nsample, xyz):
@@ -40,16 +40,20 @@ def _check_layer_args(npoint, radius, nsample, xyz):
 
 
 def sample_group(npoint: int, radius: float, nsample: int, xyz: torch.Tensor, center: bool = True,
-                 want_grouped: bool = True):
+                 want_grouped: bool = True, *, lengths=None):
     """FPS + gather_point + query_ball_point + group_point(xyz) [- new_xyz] in one call.
 
     Returns (fps_idx (b,npoint) i32, new_xyz (b,npoint,3), idx (b,npoint,nsample) i32,
     pts_cnt (b,npoint) i32, grouped_xyz (b,npoint,nsample,3) or None).  ``center=True`` subtracts the
     centroid (the reference's ``grouped_xyz -= tile(new_xyz)``, :46); no gradients.
+    ``lengths`` (b,) integers, optional: cloud i is ``xyz[i, :lengths[i]]``; each cloud then gets exactly what this
+    call returns for it alone, and every index is below its length.  A device tensor is never read on the host, so
+    the call can be captured in a CUDA graph and replayed with new lengths written into the same tensor.
     """
     npoint, radius, nsample, xyz = _check_layer_args(npoint, radius, nsample, xyz)
     b, n, _ = xyz.shape
     dev = xyz.device
+    lens = device_lengths(lengths, b, n, dev, "sample_group")
     fps_idx = torch.empty((b, npoint), dtype=torch.int32, device=dev)
     new_xyz = torch.empty((b, npoint, 3), dtype=torch.float32, device=dev)
     idx = torch.empty((b, npoint, nsample), dtype=torch.int32, device=dev)
@@ -61,15 +65,22 @@ def sample_group(npoint: int, radius: float, nsample: int, xyz: torch.Tensor, ce
     with on_device(xyz):
         wsb = int(lib.pn2_sa_layer_device_workspace_bytes(b, n, npoint, nsample))
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev) if wsb else None
-        rc = lib.pn2_sa_layer_device(b, n, npoint, radius, nsample, ptr(xyz.detach()), ptr(fps_idx), ptr(new_xyz), ptr(idx),
-                                     ptr(pts_cnt), ptr(grouped), 1 if center else 0, ptr(ws), wsb, stream_ptr(dev))
+        if lens is None:
+            rc = lib.pn2_sa_layer_device(b, n, npoint, radius, nsample, ptr(xyz.detach()), ptr(fps_idx), ptr(new_xyz), ptr(idx),
+                                         ptr(pts_cnt), ptr(grouped), 1 if center else 0, ptr(ws), wsb, stream_ptr(dev))
+        else:
+            rc = lib.pn2_sa_layer_device_ragged(b, n, npoint, radius, nsample, ptr(xyz.detach()), ptr(lens), ptr(fps_idx),
+                                                ptr(new_xyz), ptr(idx), ptr(pts_cnt), ptr(grouped), 1 if center else 0, ptr(ws),
+                                                wsb, stream_ptr(dev))
     _lib.check(rc, "pn2_sa_layer_device")
     return fps_idx, new_xyz, idx, pts_cnt, grouped
 
 
-def sample_group_msg(npoint: int, radius_list, nsample_list, xyz: torch.Tensor, center: bool = True, want_grouped: bool = True):
+def sample_group_msg(npoint: int, radius_list, nsample_list, xyz: torch.Tensor, center: bool = True, want_grouped: bool = True,
+                     *, lengths=None):
     """The multi-scale form (pointnet_sa_module_msg, utils/pointnet_util.py:156-196): ONE sampling pass, then a
     ball query + xyz grouping per scale — one C-ABI call, every scale's grouping grid overlapping the sampling chain.
+    ``lengths``: as for sample_group.
 
     Returns (fps_idx, new_xyz, [idx_k], [pts_cnt_k], [grouped_xyz_k] or None)."""
     import ctypes
@@ -81,6 +92,7 @@ def sample_group_msg(npoint: int, radius_list, nsample_list, xyz: torch.Tensor, 
         _check_layer_args(npoint, r, s, xyz)
     b, n, _ = xyz.shape
     dev = xyz.device
+    lens = device_lengths(lengths, b, n, dev, "sample_group_msg")
     fps_idx = torch.empty((b, npoint), dtype=torch.int32, device=dev)
     new_xyz = torch.empty((b, npoint, 3), dtype=torch.float32, device=dev)
     idx = [torch.empty((b, npoint, int(s)), dtype=torch.int32, device=dev) for s in nsample_list]
@@ -97,8 +109,13 @@ def sample_group_msg(npoint: int, radius_list, nsample_list, xyz: torch.Tensor, 
     with on_device(xyz):
         wsb = int(lib.pn2_sa_layer_device_workspace_bytes(b, n, npoint, max(int(s) for s in nsample_list)))
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev) if wsb else None
-        rc = lib.pn2_sa_layer_msg_device(b, n, npoint, k, radii, nsamples, ptr(xyz.detach()), ptr(fps_idx), ptr(new_xyz), pidx, pcnt, pgrp,
-                                         1 if center else 0, ptr(ws), wsb, stream_ptr(dev))
+        if lens is None:
+            rc = lib.pn2_sa_layer_msg_device(b, n, npoint, k, radii, nsamples, ptr(xyz.detach()), ptr(fps_idx), ptr(new_xyz), pidx,
+                                             pcnt, pgrp, 1 if center else 0, ptr(ws), wsb, stream_ptr(dev))
+        else:
+            rc = lib.pn2_sa_layer_msg_device_ragged(b, n, npoint, k, radii, nsamples, ptr(xyz.detach()), ptr(lens), ptr(fps_idx),
+                                                    ptr(new_xyz), pidx, pcnt, pgrp, 1 if center else 0, ptr(ws), wsb,
+                                                    stream_ptr(dev))
     _lib.check(rc, "pn2_sa_layer_msg_device")
     return fps_idx, new_xyz, idx, cnt, grouped
 

@@ -9,16 +9,18 @@ from __future__ import annotations
 import torch
 
 from . import _lib
-from ._tensor import DTYPE_CODES, FEATURE_DTYPES, on_device, ptr, require_cuda, same_device, stream_ptr
+from ._tensor import DTYPE_CODES, FEATURE_DTYPES, device_lengths, on_device, ptr, require_cuda, same_device, stream_ptr
 
 
-def query_ball_point(radius: float, nsample: int, xyz1: torch.Tensor, xyz2: torch.Tensor):
+def query_ball_point(radius: float, nsample: int, xyz1: torch.Tensor, xyz2: torch.Tensor, *, lengths=None):
     """For every query centre, the first ``nsample`` data points (ascending index) closer than ``radius``.
 
     Arguments: ``radius`` of the ball; ``nsample`` row length; ``xyz1`` float32 (B, N, 3), the cloud that is
     searched; ``xyz2`` float32 (B, M, 3), the ball centres.
     Returns ``idx`` int32 (B, M, nsample) — positions in ``xyz1``, short rows padded with their first hit — and
     ``pts_cnt`` int32 (B, M), how many distinct hits each row holds.
+    ``lengths`` (B,) integers, optional: the data cloud b is ``xyz1[b, :lengths[b]]`` (variable-size clouds padded to
+    N); each row is then exactly what this function returns for that cloud alone, and the padding rows are never read.
     Reference: tf_grouping.py:8-20 -> QueryBallPointGpuOp (tf_grouping.cpp:67-106) ->
     query_ball_point_gpu (tf_grouping_g.cu:3-36).  Rows with no point in the ball (undefined in the
     reference) come back as zeros with pts_cnt 0.
@@ -40,13 +42,18 @@ def query_ball_point(radius: float, nsample: int, xyz1: torch.Tensor, xyz2: torc
     m = xyz2.shape[1]
     if n <= 0 and b * m:
         raise ValueError("QueryBallPoint expects a non-empty xyz1")
+    lens = device_lengths(lengths, b, n, xyz1.device, "QueryBallPoint")
     idx = torch.empty((b, m, nsample), dtype=torch.int32, device=xyz1.device)
     pts_cnt = torch.empty((b, m), dtype=torch.int32, device=xyz1.device)
     if b * m:
         lib = _lib.load()
         with on_device(xyz1):
             ws_bytes = int(lib.pn2_query_ball_point_workspace_bytes(b, n))
-            if ws_bytes:  # sparse balls are served through a uniform grid built in this scratch
+            if lens is not None:  # same paths as below; the library takes the lengths to every kernel
+                ws = torch.empty(ws_bytes, dtype=torch.uint8, device=xyz1.device) if ws_bytes else None
+                rc = lib.pn2_query_ball_point_ragged(b, n, m, radius, nsample, ptr(xyz1), ptr(lens), ptr(xyz2), ptr(idx),
+                                                     ptr(pts_cnt), ptr(ws), ws_bytes, stream_ptr(xyz1.device))
+            elif ws_bytes:  # sparse balls are served through a uniform grid built in this scratch
                 ws = torch.empty(ws_bytes, dtype=torch.uint8, device=xyz1.device)
                 rc = lib.pn2_query_ball_point_ws(b, n, m, radius, nsample, ptr(xyz1), ptr(xyz2), ptr(idx), ptr(pts_cnt),
                                                  ptr(ws), ws_bytes, stream_ptr(xyz1.device))

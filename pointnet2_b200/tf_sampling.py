@@ -13,7 +13,7 @@ from __future__ import annotations
 import torch
 
 from . import _lib
-from ._tensor import on_device, ptr, require_cuda, same_device, stream_ptr
+from ._tensor import device_lengths, on_device, ptr, require_cuda, same_device, stream_ptr
 
 
 def _check_xyz(t: torch.Tensor, name: str, op: str) -> None:
@@ -50,10 +50,13 @@ def prob_sample(inp: torch.Tensor, inpr: torch.Tensor) -> torch.Tensor:
     return out
 
 
-def farthest_point_sample(npoint: int, inp: torch.Tensor) -> torch.Tensor:
+def farthest_point_sample(npoint: int, inp: torch.Tensor, *, lengths=None) -> torch.Tensor:
     """Farthest point sampling: ``npoint`` picks per cloud, each the point farthest from everything picked so far.
 
     ``inp`` float32 (B, N, 3).  Returns int32 (B, npoint), positions in ``inp``; the first pick is point 0.
+    ``lengths`` (B,) integers, optional: cloud b is ``inp[b, :lengths[b]]`` (variable-size clouds padded to N; see
+    ``_tensor.device_lengths`` for the accepted forms).  Its picks are then exactly those of this function on that
+    cloud alone, all below lengths[b]; the padding rows are never read.
     Reference: tf_sampling.py:48-56 -> FarthestPointSampleGpuOp (tf_sampling.cpp:95-123) ->
     farthestpointsamplingKernel (tf_sampling_g.cu:105-170).  Deterministic, starts at index 0.
     """
@@ -65,6 +68,7 @@ def farthest_point_sample(npoint: int, inp: torch.Tensor) -> torch.Tensor:
     b, n, _ = inp.shape
     if n <= 0:
         raise ValueError("FarthestPointSample expects at least one point per batch entry")
+    lens = device_lengths(lengths, b, n, inp.device, "FarthestPointSample")
     out = torch.empty((b, npoint), dtype=torch.int32, device=inp.device)
     if b == 0:
         return out
@@ -74,14 +78,17 @@ def farthest_point_sample(npoint: int, inp: torch.Tensor) -> torch.Tensor:
         # (32, n) float scratch (tf_sampling.cpp:115); the library says how much
         tb = int(lib.pn2_fps_scratch_bytes(b, n))
         temp = torch.empty(tb, dtype=torch.uint8, device=inp.device) if tb else None
-        rc = lib.pn2_fps(b, n, npoint, ptr(inp), ptr(temp), ptr(out), stream_ptr(inp.device))
+        if lens is None:
+            rc = lib.pn2_fps(b, n, npoint, ptr(inp), ptr(temp), ptr(out), stream_ptr(inp.device))
+        else:
+            rc = lib.pn2_fps_gather_ragged(b, n, npoint, ptr(inp), ptr(lens), ptr(temp), ptr(out), None, stream_ptr(inp.device))
     _lib.check(rc, "pn2_fps")
     return out
 
 
-def farthest_point_sample_and_gather(npoint: int, inp: torch.Tensor):
+def farthest_point_sample_and_gather(npoint: int, inp: torch.Tensor, *, lengths=None):
     """FPS and gather_point in one launch: returns (idx (b,npoint) int32, new_xyz (b,npoint,3)).
-    Equivalent to ``idx = farthest_point_sample(npoint, inp); gather_point(inp, idx)``
+    Equivalent to ``idx = farthest_point_sample(npoint, inp, lengths=lengths); gather_point(inp, idx)``
     (utils/pointnet_util.py:40); new_xyz carries no gradient here."""
     npoint = int(npoint)
     if npoint <= 0:
@@ -91,6 +98,7 @@ def farthest_point_sample_and_gather(npoint: int, inp: torch.Tensor):
     b, n, _ = inp.shape
     if n <= 0:
         raise ValueError("FarthestPointSample expects at least one point per batch entry")
+    lens = device_lengths(lengths, b, n, inp.device, "FarthestPointSample")
     idx = torch.empty((b, npoint), dtype=torch.int32, device=inp.device)
     new_xyz = torch.empty((b, npoint, 3), dtype=torch.float32, device=inp.device)
     if b == 0:
@@ -99,7 +107,11 @@ def farthest_point_sample_and_gather(npoint: int, inp: torch.Tensor):
     with on_device(inp):
         tb = int(lib.pn2_fps_scratch_bytes(b, n))
         temp = torch.empty(tb, dtype=torch.uint8, device=inp.device) if tb else None
-        rc = lib.pn2_fps_gather(b, n, npoint, ptr(inp), ptr(temp), ptr(idx), ptr(new_xyz), stream_ptr(inp.device))
+        if lens is None:
+            rc = lib.pn2_fps_gather(b, n, npoint, ptr(inp), ptr(temp), ptr(idx), ptr(new_xyz), stream_ptr(inp.device))
+        else:
+            rc = lib.pn2_fps_gather_ragged(b, n, npoint, ptr(inp), ptr(lens), ptr(temp), ptr(idx), ptr(new_xyz),
+                                           stream_ptr(inp.device))
     _lib.check(rc, "pn2_fps_gather")
     return idx, new_xyz
 
