@@ -258,6 +258,34 @@ int pn2_fp_interpolate_concat_typed(int dtype, int b, int n, int m, int c2, int 
                                     const float* xyz2, const void* points1, const void* points2, void* out,
                                     void* stream);
 
+/* Interpolation onto ragged clouds (see pn2_fps_gather_ragged): lengths1 (b,) device int32, the lengths of the UNKNOWN
+ * side (xyz1, points1, and the n rows of idx / weight / dist / out / grad_out); the known side (xyz2, points, points2) is
+ * dense.  Every real row j < lengths1[i] of every output is bit for bit what the entry without lengths computes for it.
+ * Padding rows are never read (xyz1, points1 and grad_out may hold NaN or inf there) and hold a fixed filler:
+ * idx 0 and dist +inf (the missing-neighbour filler), weight 0, and 0 in every feature output (the points1 half of
+ * pn2_fp_interpolate_concat_ragged_typed included).  The gradients into the known features equal those of the call on
+ * the truncated clouds: bit for bit for the deterministic one (same workspace formula), within float-atomic rounding for
+ * the atomic one.  lengths1 == NULL is the entry without lengths.  lengths1 goes after xyz1, or after weight where there
+ * is no xyz1. */
+int pn2_three_nn_ragged(int b, int n, int m, const float* xyz1, const int* lengths1, const float* xyz2, float* dist,
+                        int* idx, void* stream);
+int pn2_three_nn_interpolate_ragged_typed(int dtype, int b, int n, int m, int c, const float* xyz1, const int* lengths1,
+                                          const float* xyz2, const void* points2, void* out, float* dist, int* idx,
+                                          float* weight, void* stream);
+int pn2_fp_interpolate_concat_ragged_typed(int dtype, int b, int n, int m, int c2, int c1, const float* xyz1,
+                                           const int* lengths1, const float* xyz2, const void* points1,
+                                           const void* points2, void* out, void* stream);
+int pn2_three_interpolate_ragged_typed(int dtype, int b, int m, int c, int n, const void* points, const int* idx,
+                                       const float* weight, const int* lengths1, void* out, void* stream);
+/* float32, float atomics: grad_points (b,m,c) zero-filled by the caller, as for pn2_three_interpolate_grad */
+int pn2_three_interpolate_grad_ragged(int b, int n, int c, int m, const float* grad_out, const int* idx,
+                                      const float* weight, const int* lengths1, float* grad_points, void* stream);
+/* workspace: pn2_three_interpolate_grad_det_workspace_bytes(b, n, m), n the padded size */
+int pn2_three_interpolate_grad_det_ragged_typed(int dtype, int b, int n, int c, int m, const void* grad_out,
+                                                const int* idx, const float* weight, const int* lengths1,
+                                                void* grad_points, void* workspace, size_t workspace_bytes,
+                                                void* stream);
+
 /* ---- the sampling+grouping half of a set-abstraction layer, device-resident ------------------ */
 
 /* query_ball_point + group_point(xyz) in ONE launch (tf_grouping_g.cu:3-57 back to back, as

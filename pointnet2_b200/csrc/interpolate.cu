@@ -129,14 +129,28 @@ __device__ __forceinline__ void scan_tile(Top3& t, const KnownTile& tile, int tp
 }
 
 // One thread per unknown point; known points broadcast from shared memory.
+// L (ragged unknown side): cloud i's unknown points are its first cloud_length(lengths, i, n) rows.  A template flag, so
+// that the instance without lengths compiles to the code it always did.  Padding rows get the (+inf, 0) filler; a CTA
+// made only of padding writes it and leaves before the known-point loop (CTA-uniform: the cloud is blockIdx.y).
+template <bool L>
 __global__ void __launch_bounds__(kNnThreads)
 three_nn_kernel(int n, int m, const float* __restrict__ xyz1, const float* __restrict__ xyz2,
-                float* __restrict__ dist, int* __restrict__ idx) {
+                float* __restrict__ dist, int* __restrict__ idx, const int* __restrict__ lengths) {
     __shared__ KnownTile s_tile;
     const int tid = threadIdx.x;
     const int cloud = blockIdx.y;
     const int j = blockIdx.x * kNnThreads + tid;
-    const bool valid = j < n;
+    const int len = L ? cloud_length(lengths, cloud, n) : n;
+    const bool valid = j < len;
+    if (L && (int)(blockIdx.x * kNnThreads) >= len) {
+        if (j < n) {
+            float* dd = dist + ((size_t)cloud * n + j) * 3;
+            int* ii = idx + ((size_t)cloud * n + j) * 3;
+            dd[0] = dd[1] = dd[2] = INFINITY;
+            ii[0] = ii[1] = ii[2] = 0;
+        }
+        return;
+    }
     const float* __restrict__ known = xyz2 + (size_t)cloud * m * 3;
     float ux = 0.f, uy = 0.f, uz = 0.f;
     if (valid) {
@@ -153,7 +167,8 @@ three_nn_kernel(int n, int m, const float* __restrict__ xyz1, const float* __res
         __syncthreads();
         scan_tile(t, s_tile, tp_pad, base, ux, uy, uz);
     }
-    if (valid) {
+    if (L && !valid) top3_init(t);  // a padding row of a partly filled CTA: the filler
+    if (L ? j < n : valid) {
         float* dd = dist + ((size_t)cloud * n + j) * 3;
         int* ii = idx + ((size_t)cloud * n + j) * 3;
         dd[0] = t.d1; dd[1] = t.d2; dd[2] = t.d3;
@@ -173,16 +188,19 @@ constexpr int kItThreads = 256;
 // per SM cannot hide its own slice load).
 // T = float, __nv_bfloat16 or __half: P = Pack4<T>::type holds 4 channels; they are upcast, interpolated in float32
 // and rounded once on the way out.
-template <typename IndexT, int U, typename T, typename P = typename Pack4<T>::type>
+// L (ragged unknown side, lengths (b,) of the n rows per cloud): padding rows j >= the cloud's length write zeros and read
+// neither idx nor weight.  A template flag, as in three_nn_kernel.
+template <typename IndexT, int U, typename T, bool L = false, typename P = typename Pack4<T>::type>
 __global__ void __launch_bounds__(kItThreads)
 three_interp_vec4_kernel(int m, int c4, IndexT rows_per_cloud, IndexT total_vec, const P* __restrict__ points,
-                         const int* __restrict__ idx, const float* __restrict__ weight, P* __restrict__ out) {
+                         const int* __restrict__ idx, const float* __restrict__ weight, P* __restrict__ out,
+                         const int* __restrict__ lengths) {
     const IndexT stride = (IndexT)gridDim.x * kItThreads;
     for (IndexT v0 = (IndexT)blockIdx.x * kItThreads + threadIdx.x; v0 < total_vec; v0 += stride * U) {
         int i1[U], i2[U], i3[U];
         float w1[U], w2[U], w3[U];
         const P* pb[U];
-        bool ok[U];
+        bool ok[U], pad[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             const IndexT v = v0 + (IndexT)u * stride;
@@ -190,6 +208,13 @@ three_interp_vec4_kernel(int m, int c4, IndexT rows_per_cloud, IndexT total_vec,
             const IndexT row = ok[u] ? v / (IndexT)c4 : 0;
             const int l = ok[u] ? (int)(v - row * (IndexT)c4) : 0;
             const IndexT cloud = row / rows_per_cloud;
+            pad[u] = L && row - cloud * rows_per_cloud >= (IndexT)cloud_length(lengths, (int)cloud, (int)rows_per_cloud);
+            if (L && pad[u]) {
+                i1[u] = i2[u] = i3[u] = 0;
+                w1[u] = w2[u] = w3[u] = 0.f;
+                pb[u] = points;
+                continue;
+            }
             i1[u] = __ldg(idx + (size_t)row * 3 + 0);
             i2[u] = __ldg(idx + (size_t)row * 3 + 1);
             i3[u] = __ldg(idx + (size_t)row * 3 + 2);
@@ -201,7 +226,7 @@ three_interp_vec4_kernel(int m, int c4, IndexT rows_per_cloud, IndexT total_vec,
         float4 a[U], b[U], c[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-            if (ok[u]) {
+            if (ok[u] && !(L && pad[u])) {
                 a[u] = unpack4(__ldg(pb[u] + (size_t)i1[u] * c4), T());
                 b[u] = unpack4(__ldg(pb[u] + (size_t)i2[u] * c4), T());
                 c[u] = unpack4(__ldg(pb[u] + (size_t)i3[u] * c4), T());
@@ -209,7 +234,9 @@ three_interp_vec4_kernel(int m, int c4, IndexT rows_per_cloud, IndexT total_vec,
         }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-            if (ok[u]) {
+            if (L && ok[u] && pad[u]) {
+                __stcs(out + v0 + (IndexT)u * stride, pack4(make_float4(0.f, 0.f, 0.f, 0.f), T()));
+            } else if (ok[u]) {
                 float4 o;
                 o.x = interp3(a[u].x, b[u].x, c[u].x, w1[u], w2[u], w3[u]);
                 o.y = interp3(a[u].y, b[u].y, c[u].y, w1[u], w2[u], w3[u]);
@@ -221,15 +248,20 @@ three_interp_vec4_kernel(int m, int c4, IndexT rows_per_cloud, IndexT total_vec,
     }
 }
 
-template <typename IndexT, typename T>
+template <typename IndexT, typename T, bool L = false>
 __global__ void __launch_bounds__(kItThreads)
 three_interp_scalar_kernel(int m, int c, IndexT rows_per_cloud, IndexT total, const T* __restrict__ points,
-                           const int* __restrict__ idx, const float* __restrict__ weight, T* __restrict__ out) {
+                           const int* __restrict__ idx, const float* __restrict__ weight, T* __restrict__ out,
+                           const int* __restrict__ lengths) {
     const IndexT stride = (IndexT)gridDim.x * kItThreads;
     for (IndexT e = (IndexT)blockIdx.x * kItThreads + threadIdx.x; e < total; e += stride) {
         const IndexT row = e / (IndexT)c;
         const int l = (int)(e - row * (IndexT)c);
         const IndexT cloud = row / rows_per_cloud;
+        if (L && row - cloud * rows_per_cloud >= (IndexT)cloud_length(lengths, (int)cloud, (int)rows_per_cloud)) {
+            out[e] = from_f32<T>(0.f);
+            continue;
+        }
         const int* ii = idx + (size_t)row * 3;
         const float* w = weight + (size_t)row * 3;
         const T* pb = points + (size_t)cloud * m * c + l;
@@ -239,16 +271,19 @@ three_interp_scalar_kernel(int m, int c, IndexT rows_per_cloud, IndexT total, co
 }
 
 // grad_points[b, idx[b,j,t], l] += grad_out[b,j,l] * weight[b,j,t]
-template <typename IndexT>
+// L: rows j >= the cloud's length (lengths, as in three_interp_vec4_kernel) are skipped.
+template <typename IndexT, bool L = false>
 __global__ void __launch_bounds__(kItThreads)
 three_interp_grad_vec4_kernel(int m, int c4, IndexT rows_per_cloud, IndexT total_vec,
                               const float4* __restrict__ grad_out, const int* __restrict__ idx,
-                              const float* __restrict__ weight, float4* __restrict__ grad_points) {
+                              const float* __restrict__ weight, float4* __restrict__ grad_points,
+                              const int* __restrict__ lengths) {
     const IndexT stride = (IndexT)gridDim.x * kItThreads;
     for (IndexT v = (IndexT)blockIdx.x * kItThreads + threadIdx.x; v < total_vec; v += stride) {
         const IndexT row = v / (IndexT)c4;
         const int l = (int)(v - row * (IndexT)c4);
         const IndexT cloud = row / rows_per_cloud;
+        if (L && row - cloud * rows_per_cloud >= (IndexT)cloud_length(lengths, (int)cloud, (int)rows_per_cloud)) continue;
         const float4 g = __ldcs(grad_out + v);
         float4* gb = grad_points + (size_t)cloud * m * c4 + l;
 #pragma unroll
@@ -261,16 +296,17 @@ three_interp_grad_vec4_kernel(int m, int c4, IndexT rows_per_cloud, IndexT total
     }
 }
 
-template <typename IndexT>
+template <typename IndexT, bool L = false>
 __global__ void __launch_bounds__(kItThreads)
 three_interp_grad_scalar_kernel(int m, int c, IndexT rows_per_cloud, IndexT total, const float* __restrict__ grad_out,
                                 const int* __restrict__ idx, const float* __restrict__ weight,
-                                float* __restrict__ grad_points) {
+                                float* __restrict__ grad_points, const int* __restrict__ lengths) {
     const IndexT stride = (IndexT)gridDim.x * kItThreads;
     for (IndexT e = (IndexT)blockIdx.x * kItThreads + threadIdx.x; e < total; e += stride) {
         const IndexT row = e / (IndexT)c;
         const int l = (int)(e - row * (IndexT)c);
         const IndexT cloud = row / rows_per_cloud;
+        if (L && row - cloud * rows_per_cloud >= (IndexT)cloud_length(lengths, (int)cloud, (int)rows_per_cloud)) continue;
         const float g = __ldcs(grad_out + e);
         float* gb = grad_points + (size_t)cloud * m * c + l;
 #pragma unroll
@@ -325,11 +361,15 @@ __device__ __forceinline__ void scan_tile_strided(Top3& t, const KnownTile& tile
 // T: element type of points1 / points2 / out: float, or unsigned short for both 2-byte formats, f16 choosing float16 or
 // bfloat16 at run time (the 3-NN phase is most of the code: one 2-byte instance per G instead of two).  Phase 2 upcasts,
 // interpolates in float32 and rounds once; points1 is copied.
-template <int G, typename T>
+// L (ragged unknown side, as in three_nn_kernel): padding rows get dist +inf, idx 0, weight 0 and an all-zero output row
+// (points1 is not read there).  A CTA made only of padding writes that and leaves before the known-point loop; in a
+// partly filled one every lane still takes part in the merge, and `valid` gates only loads and stores.
+template <int G, typename T, bool L>
 __global__ void __launch_bounds__(kNnThreads)
 fp_front_kernel(int n, int m, int c2, int c1, const float* __restrict__ xyz1, const float* __restrict__ xyz2,
                 const T* __restrict__ points1, const T* __restrict__ points2, T* __restrict__ out,
-                float* __restrict__ dist_o, int* __restrict__ idx_o, float* __restrict__ weight_o, int f16) {
+                float* __restrict__ dist_o, int* __restrict__ idx_o, float* __restrict__ weight_o, int f16,
+                const int* __restrict__ lengths) {
     constexpr int PPB = kNnThreads / G;  // unknown points per CTA
     __shared__ KnownTile s_tile;
     __shared__ int s_i[PPB][3];
@@ -339,7 +379,22 @@ fp_front_kernel(int n, int m, int c2, int c1, const float* __restrict__ xyz1, co
     const int cloud = blockIdx.y;
     const int j0 = blockIdx.x * PPB;
     const int j = j0 + slot;
-    const bool valid = j < n;
+    const int len = L ? cloud_length(lengths, cloud, n) : n;
+    const bool valid = j < len;
+    if (L && j0 >= len) {
+        if (g == 0 && j < n) {
+            const size_t o = ((size_t)cloud * n + j) * 3;
+            if (dist_o) { dist_o[o] = INFINITY; dist_o[o + 1] = INFINITY; dist_o[o + 2] = INFINITY; }
+            if (idx_o) { idx_o[o] = 0; idx_o[o + 1] = 0; idx_o[o + 2] = 0; }
+            if (weight_o) { weight_o[o] = 0.f; weight_o[o + 1] = 0.f; weight_o[o + 2] = 0.f; }
+        }
+        if (out) {
+            const int cw = c2 + c1;
+            T* __restrict__ ob = out + ((size_t)cloud * n + j0) * cw;
+            for (int e = tid; e < min(PPB, n - j0) * cw; e += kNnThreads) ob[e] = of_f32<T>(0.f, f16);
+        }
+        return;
+    }
     const float* __restrict__ known = xyz2 + (size_t)cloud * m * 3;
     float ux = 0.f, uy = 0.f, uz = 0.f;
     if (valid) {
@@ -384,11 +439,17 @@ fp_front_kernel(int n, int m, int c2, int c1, const float* __restrict__ xyz1, co
             if (dist_o) { dist_o[o] = t.d1; dist_o[o + 1] = t.d2; dist_o[o + 2] = t.d3; }
             if (idx_o) { idx_o[o] = t.i1; idx_o[o + 1] = t.i2; idx_o[o + 2] = t.i3; }
             if (weight_o) { weight_o[o] = w1; weight_o[o + 1] = w2; weight_o[o + 2] = w3; }
+        } else if (L && j < n) {  // a padding row of a partly filled CTA
+            const size_t o = ((size_t)cloud * n + j) * 3;
+            if (dist_o) { dist_o[o] = INFINITY; dist_o[o + 1] = INFINITY; dist_o[o + 2] = INFINITY; }
+            if (idx_o) { idx_o[o] = 0; idx_o[o + 1] = 0; idx_o[o + 2] = 0; }
+            if (weight_o) { weight_o[o] = 0.f; weight_o[o + 1] = 0.f; weight_o[o + 2] = 0.f; }
         }
     }
     __syncthreads();
     if (!out) return;
     const int rows = min(PPB, n - j0);
+    const int real_rows = L ? min(PPB, len - j0) : rows;  // rows from real_rows on are padding: zeros
     const int cw = c2 + c1;  // output row width
     const T* __restrict__ pb = points2 + (size_t)cloud * m * c2;
     const T* __restrict__ p1 = points1 ? points1 + ((size_t)cloud * n + j0) * c1 : nullptr;
@@ -404,7 +465,9 @@ fp_front_kernel(int n, int m, int c2, int c1, const float* __restrict__ xyz1, co
         for (int e = tid; e < rows * cw4; e += kNnThreads) {
             const int r = e / cw4, l = e - r * cw4;
             P o;
-            if (l < c24) {
+            if (L && r >= real_rows) {
+                o = pack4_of(make_float4(0.f, 0.f, 0.f, 0.f), T(), f16);
+            } else if (l < c24) {
                 const float4 a = unpack4_of(__ldg(pb4 + (size_t)s_i[r][0] * c24 + l), f16),
                              b = unpack4_of(__ldg(pb4 + (size_t)s_i[r][1] * c24 + l), f16),
                              cc = unpack4_of(__ldg(pb4 + (size_t)s_i[r][2] * c24 + l), f16);
@@ -424,7 +487,9 @@ fp_front_kernel(int n, int m, int c2, int c1, const float* __restrict__ xyz1, co
         for (int e = tid; e < rows * cw; e += kNnThreads) {
             const int r = e / cw, l = e - r * cw;
             T o;
-            if (l < c2)
+            if (L && r >= real_rows)
+                o = of_f32<T>(0.f, f16);
+            else if (l < c2)
                 o = of_f32<T>(interp3(f32_of(__ldg(pb + (size_t)s_i[r][0] * c2 + l), f16), f32_of(__ldg(pb + (size_t)s_i[r][1] * c2 + l), f16),
                                       f32_of(__ldg(pb + (size_t)s_i[r][2] * c2 + l), f16), s_w[r][0], s_w[r][1], s_w[r][2]), f16);
             else
@@ -435,30 +500,41 @@ fp_front_kernel(int n, int m, int c2, int c1, const float* __restrict__ xyz1, co
 }
 
 template <int G, typename T>
-static int launch_fp_front(int b, int n, int m, int c2, int c1, const float* xyz1, const float* xyz2, const T* points1,
-                           const T* points2, T* out, float* dist, int* idx, float* weight, int f16, cudaStream_t st) {
+static int launch_fp_front(int b, int n, int m, int c2, int c1, const float* xyz1, const int* lengths, const float* xyz2,
+                           const T* points1, const T* points2, T* out, float* dist, int* idx, float* weight, int f16,
+                           cudaStream_t st) {
     constexpr int PPB = kNnThreads / G;
     dim3 grid((n + PPB - 1) / PPB, b, 1);
-    fp_front_kernel<G, T><<<grid, kNnThreads, 0, st>>>(n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16);
+    if (lengths)
+        fp_front_kernel<G, T, true><<<grid, kNnThreads, 0, st>>>(n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16,
+                                                                 lengths);
+    else
+        fp_front_kernel<G, T, false><<<grid, kNnThreads, 0, st>>>(n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight,
+                                                                  f16, nullptr);
     return finish_launch();
 }
 
+// lengths (b,) device int32 of xyz1 / points1 / out, or NULL
 template <typename T>
-static int fp_front_dispatch(int b, int n, int m, int c2, int c1, const float* xyz1, const float* xyz2, const T* points1,
-                             const T* points2, T* out, float* dist, int* idx, float* weight, int f16, cudaStream_t st) {
+static int fp_front_dispatch(int b, int n, int m, int c2, int c1, const float* xyz1, const int* lengths, const float* xyz2,
+                             const T* points1, const T* points2, T* out, float* dist, int* idx, float* weight, int f16,
+                             cudaStream_t st) {
     // lanes per unknown point: as many as it takes to put ~2 CTAs on every SM (a CTA covers 128/G points),
-    // but never more lanes than there are pairs of known points to share
+    // but never more lanes than there are pairs of known points to share.  Chosen from b*n with or without lengths.
     const long long pts = (long long)b * n;
     int G = 1;
     while (G < 32 && pts * G < 2LL * num_sms() * kNnThreads && 2 * G <= (m + 1) / 2) G *= 2;
+#define PN2_FP_FRONT(GG) \
+    launch_fp_front<GG, T>(b, n, m, c2, c1, xyz1, lengths, xyz2, points1, points2, out, dist, idx, weight, f16, st)
     switch (G) {
-        case 1: return launch_fp_front<1, T>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16, st);
-        case 2: return launch_fp_front<2, T>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16, st);
-        case 4: return launch_fp_front<4, T>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16, st);
-        case 8: return launch_fp_front<8, T>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16, st);
-        case 16: return launch_fp_front<16, T>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16, st);
-        default: return launch_fp_front<32, T>(b, n, m, c2, c1, xyz1, xyz2, points1, points2, out, dist, idx, weight, f16, st);
+        case 1: return PN2_FP_FRONT(1);
+        case 2: return PN2_FP_FRONT(2);
+        case 4: return PN2_FP_FRONT(4);
+        case 8: return PN2_FP_FRONT(8);
+        case 16: return PN2_FP_FRONT(16);
+        default: return PN2_FP_FRONT(32);
     }
+#undef PN2_FP_FRONT
 }
 
 // ---- scatter-add without atomics: an inverse index, then one warp per target row ----------------------
@@ -474,13 +550,24 @@ static int fp_front_dispatch(int b, int n, int m, int c2, int c1, const float* x
 // is arbitrary), then every warp sorts its own list (<= 256 entries: bitonic sort in registers).  Longer lists are
 // queued: inv_long_kernel (weighted) and inv_long_seq_kernel (unweighted) serve them with an index-ordered scan of
 // the cloud's entries.
+// L (three_interpolate's gradient on a ragged unknown side): a cloud of length len has the real entries e < 3*len (the
+// prefix, since e = 3j+t); the build and the long-list kernels stop there, so off[nt] = 3*len and the padding's idx is
+// never counted.  lengths (b,) holds the lengths of the ne / 3 rows per cloud.  A template flag, so that the instances
+// without lengths, which also serve the unweighted sums, compile to the code they always did.
 constexpr int kInvThreads = 256;
 constexpr int kInvSortCap = 256;
 
+__device__ __forceinline__ int real_entries(const int* __restrict__ lengths, int cloud, int ne) {
+    return 3 * cloud_length(lengths, cloud, ne / 3);
+}
+
+template <bool L>
 __global__ void __launch_bounds__(kInvThreads)
-inv_count_kernel(int ne, int nt, long long total, const int* __restrict__ idx, int* __restrict__ cnt) {
+inv_count_kernel(int ne, int nt, long long total, const int* __restrict__ idx, int* __restrict__ cnt,
+                 const int* __restrict__ lengths) {
     for (long long e = (long long)blockIdx.x * kInvThreads + threadIdx.x; e < total; e += (long long)gridDim.x * kInvThreads) {
         const long long cloud = e / ne;
+        if (L && e - cloud * ne >= real_entries(lengths, (int)cloud, ne)) continue;
         atomicAdd(cnt + cloud * (nt + 1) + __ldg(idx + e), 1);
     }
 }
@@ -522,10 +609,13 @@ inv_scan_kernel(int nt, int* __restrict__ cnt_off, int* __restrict__ cur) {
     }
 }
 
+template <bool L>
 __global__ void __launch_bounds__(kInvThreads)
-inv_fill_kernel(int ne, int nt, long long total, const int* __restrict__ idx, int* __restrict__ cur, int* __restrict__ entries) {
+inv_fill_kernel(int ne, int nt, long long total, const int* __restrict__ idx, int* __restrict__ cur, int* __restrict__ entries,
+                const int* __restrict__ lengths) {
     for (long long e = (long long)blockIdx.x * kInvThreads + threadIdx.x; e < total; e += (long long)gridDim.x * kInvThreads) {
         const long long cloud = e / ne;
+        if (L && e - cloud * ne >= real_entries(lengths, (int)cloud, ne)) continue;
         const int pos = atomicAdd(cur + cloud * nt + __ldg(idx + e), 1);
         entries[cloud * ne + pos] = (int)(e - cloud * ne);
     }
@@ -534,22 +624,24 @@ inv_fill_kernel(int ne, int nt, long long total, const int* __restrict__ idx, in
 // count + scan + fill of one cloud in ONE CTA, with the counters and cursors in shared memory (nt <= 16000): the
 // inverse index of a layer costs one launch instead of two memsets and three kernels.
 constexpr int kInvBuildMaxM = 16000;
+template <bool L>
 __global__ void __launch_bounds__(1024)
 inv_build_kernel(int ne, int nt, const int* __restrict__ idx, int* __restrict__ off, int* __restrict__ entries,
-                 int* __restrict__ long_queue) {
+                 int* __restrict__ long_queue, const int* __restrict__ lengths) {
     extern __shared__ int s_c[];  // [nt + 1]: counts -> exclusive offsets (kept as the fill cursors)
     __shared__ int s_w[32];
     __shared__ int s_carry;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const long long cloud = blockIdx.x;
     const int* __restrict__ cidx = idx + cloud * ne;
+    const int ne_c = L ? real_entries(lengths, (int)cloud, ne) : ne;  // entries of this cloud; ne stays the stride
     for (int i = tid; i <= nt; i += 1024) s_c[i] = 0;
     if (tid == 0) {
         s_carry = 0;
         if (cloud == 0) long_queue[0] = 0;
     }
     __syncthreads();
-    for (int e = tid; e < ne; e += 1024) atomicAdd(&s_c[__ldg(cidx + e)], 1);
+    for (int e = tid; e < ne_c; e += 1024) atomicAdd(&s_c[__ldg(cidx + e)], 1);
     __syncthreads();
     int* __restrict__ o = off + cloud * (nt + 1);
     for (int base = 0; base <= nt; base += 1024) {
@@ -579,7 +671,7 @@ inv_build_kernel(int ne, int nt, const int* __restrict__ idx, int* __restrict__ 
         __syncthreads();
     }
     int* __restrict__ ent = entries + cloud * ne;
-    for (int e = tid; e < ne; e += 1024) ent[atomicAdd(&s_c[__ldg(cidx + e)], 1)] = e;
+    for (int e = tid; e < ne_c; e += 1024) ent[atomicAdd(&s_c[__ldg(cidx + e)], 1)] = e;
 }
 
 // one warp per target row (b, i); lanes over channels (float4 when VEC).  Lists longer than kInvSortCap are
@@ -775,10 +867,12 @@ inv_long_seq_kernel(int ne, int c, int m, const T* __restrict__ grad_out, const 
 // (coalesced index loads + ballot), adds the entries that point at i in that order, and the 8 partial sums are
 // combined in piece order — a fixed association, hence deterministic (it differs from one long sequential sum
 // only in rounding; short lists, the normal case, are bit-identical to the reference's loop).
-template <bool VEC, typename T>
+// L: the cloud's 3*len real entries are cut into the 8 pieces, as the call on the truncated cloud cuts them.
+template <bool VEC, typename T, bool L = false>
 __global__ void __launch_bounds__(kInvThreads)
 inv_long_kernel(int n, int c, int m, const T* __restrict__ grad_out, const int* __restrict__ idx,
-                const float* __restrict__ weight, const int* __restrict__ long_queue, T* __restrict__ grad_points, int f16) {
+                const float* __restrict__ weight, const int* __restrict__ long_queue, T* __restrict__ grad_points, int f16,
+                const int* __restrict__ lengths) {
     constexpr int NW = kInvThreads / 32;
     constexpr int W = VEC ? 4 : 1;
     __shared__ float s_part[NW][32 * W];
@@ -794,7 +888,9 @@ inv_long_kernel(int n, int c, int m, const T* __restrict__ grad_out, const int* 
         const float* __restrict__ wt = weight + (size_t)cloud * n3;
         const int* __restrict__ cidx = idx + cloud * n3;
         T* __restrict__ gp = grad_points + ((size_t)cloud * m + i) * c;
-        const int e_lo = warp * piece, e_hi = min(n3, e_lo + piece);
+        const int n3_c = L ? real_entries(lengths, (int)cloud, n3) : n3;
+        const int piece_c = L ? (n3_c + NW - 1) / NW : piece;
+        const int e_lo = warp * piece_c, e_hi = min(n3_c, e_lo + piece_c);
         for (int l0 = 0; l0 < c; l0 += 32 * W) {
             const int l = l0 + lane * W;
             const bool act = l < c;
@@ -875,25 +971,33 @@ static unsigned it_grid(unsigned long long work_items, unsigned per_block) {
 
 static bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-template <typename T>
-static int three_interpolate_impl(int b, int m, int c, int n, const T* points, const int* idx, const float* weight, T* out,
-                                  cudaStream_t st) {
+template <typename T, bool L>
+static void three_interpolate_launch(int b, int m, int c, int n, const T* points, const int* idx, const float* weight,
+                                     const int* lengths, T* out, cudaStream_t st) {
     using P = typename Pack4<T>::type;
     const unsigned long long total = (unsigned long long)b * n * c;
     if (c % 4 == 0 && aligned_to(points, sizeof(P)) && aligned_to(out, sizeof(P))) {
         const unsigned long long tv = total / 4;
         const unsigned grid = it_grid(tv, kItThreads);
         if (tv < (1ull << 31))
-            three_interp_vec4_kernel<unsigned, 1, T><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned)n, (unsigned)tv, (const P*)points, idx, weight, (P*)out);
+            three_interp_vec4_kernel<unsigned, 1, T, L><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned)n, (unsigned)tv, (const P*)points, idx, weight, (P*)out, lengths);
         else
-            three_interp_vec4_kernel<unsigned long long, 1, T><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned long long)n, tv, (const P*)points, idx, weight, (P*)out);
+            three_interp_vec4_kernel<unsigned long long, 1, T, L><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned long long)n, tv, (const P*)points, idx, weight, (P*)out, lengths);
     } else {
         const unsigned grid = it_grid(total, kItThreads);
         if (total < (1ull << 31))
-            three_interp_scalar_kernel<unsigned, T><<<grid, kItThreads, 0, st>>>(m, c, (unsigned)n, (unsigned)total, points, idx, weight, out);
+            three_interp_scalar_kernel<unsigned, T, L><<<grid, kItThreads, 0, st>>>(m, c, (unsigned)n, (unsigned)total, points, idx, weight, out, lengths);
         else
-            three_interp_scalar_kernel<unsigned long long, T><<<grid, kItThreads, 0, st>>>(m, c, (unsigned long long)n, total, points, idx, weight, out);
+            three_interp_scalar_kernel<unsigned long long, T, L><<<grid, kItThreads, 0, st>>>(m, c, (unsigned long long)n, total, points, idx, weight, out, lengths);
     }
+}
+
+// lengths (b,) device int32 of the n unknown rows, or NULL
+template <typename T>
+static int three_interpolate_impl(int b, int m, int c, int n, const T* points, const int* idx, const float* weight,
+                                  const int* lengths, T* out, cudaStream_t st) {
+    if (lengths) three_interpolate_launch<T, true>(b, m, c, n, points, idx, weight, lengths, out, st);
+    else three_interpolate_launch<T, false>(b, m, c, n, points, idx, weight, nullptr, out, st);
     return finish_launch();
 }
 
@@ -905,9 +1009,10 @@ size_t inv_workspace_bytes(int b, long long ne, int nt) {
 
 // Inverse index of the b clouds' entries over nt targets, built in `workspace` (inv_workspace_bytes), then the ordered
 // sums.  Weighted: source rows n = ne / 3 (three_interpolate); unweighted: n = ne.  The arguments are checked by the caller.
+// lengths (weighted only): (b,) device int32 of the n source rows, or NULL.
 template <bool WEIGHTED, typename T>
 static int inv_scatter_det(int b, int n, int ne, int c, int nt, const T* grad_out, const int* idx, const float* weight,
-                           T* grad_points, void* workspace, int f16, cudaStream_t st) {
+                           const int* lengths, T* grad_points, void* workspace, int f16, cudaStream_t st) {
     const long long warps = (long long)b * nt;
     const unsigned long long blocks = ((unsigned long long)warps * 32 + kInvThreads - 1) / kInvThreads;
     if (blocks > 0x7fffffffull) return (int)cudaErrorInvalidValue;
@@ -922,11 +1027,16 @@ static int inv_scatter_det(int b, int n, int ne, int c, int nt, const T* grad_ou
         cudaError_t e = cudaGetDevice(&dev);
         if (e != cudaSuccess) return (int)e;
         if (dev >= 64 || !(attr_done.load(std::memory_order_acquire) & (1ull << dev))) {
-            e = cudaFuncSetAttribute(inv_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(int) * (kInvBuildMaxM + 1));
+            e = cudaFuncSetAttribute(inv_build_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(int) * (kInvBuildMaxM + 1));
+            if (e == cudaSuccess && WEIGHTED)
+                e = cudaFuncSetAttribute(inv_build_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(int) * (kInvBuildMaxM + 1));
             if (e != cudaSuccess) return (int)e;
             if (dev < 64) attr_done.fetch_or(1ull << dev, std::memory_order_release);
         }
-        inv_build_kernel<<<b, 1024, sizeof(int) * (size_t)(nt + 1), st>>>(ne, nt, idx, off, entries, long_queue);
+        if (lengths)
+            inv_build_kernel<true><<<b, 1024, sizeof(int) * (size_t)(nt + 1), st>>>(ne, nt, idx, off, entries, long_queue, lengths);
+        else
+            inv_build_kernel<false><<<b, 1024, sizeof(int) * (size_t)(nt + 1), st>>>(ne, nt, idx, off, entries, long_queue, nullptr);
         launches += 1;
     } else {
         cudaError_t e = cudaMemsetAsync(off, 0, sizeof(int) * (size_t)b * (nt + 1), st);
@@ -934,9 +1044,11 @@ static int inv_scatter_det(int b, int n, int ne, int c, int nt, const T* grad_ou
         if (e != cudaSuccess) return (int)e;
         const long long total = (long long)b * ne;
         const unsigned g1 = it_grid((unsigned long long)total, kInvThreads);
-        inv_count_kernel<<<g1, kInvThreads, 0, st>>>(ne, nt, total, idx, off);
+        if (lengths) inv_count_kernel<true><<<g1, kInvThreads, 0, st>>>(ne, nt, total, idx, off, lengths);
+        else inv_count_kernel<false><<<g1, kInvThreads, 0, st>>>(ne, nt, total, idx, off, nullptr);
         inv_scan_kernel<<<b, 1024, 0, st>>>(nt, off, cur);
-        inv_fill_kernel<<<g1, kInvThreads, 0, st>>>(ne, nt, total, idx, cur, entries);
+        if (lengths) inv_fill_kernel<true><<<g1, kInvThreads, 0, st>>>(ne, nt, total, idx, cur, entries, lengths);
+        else inv_fill_kernel<false><<<g1, kInvThreads, 0, st>>>(ne, nt, total, idx, cur, entries, nullptr);
         launches += 3;
     }
     // long lists: a fixed grid walks the queue (usually empty: the CTAs read one word and leave)
@@ -945,9 +1057,14 @@ static int inv_scatter_det(int b, int n, int ne, int c, int nt, const T* grad_ou
 #define PN2_INV_SUMS(VEC)                                                                                                     \
     inv_gather_kernel<VEC, WEIGHTED, T><<<(unsigned)blocks, kInvThreads, 0, st>>>(n, c, nt, warps, grad_out, weight, off, entries, \
                                                                                   grad_points, long_queue, f16);            \
-    if constexpr (WEIGHTED)                                                                                                   \
-        inv_long_kernel<VEC, T><<<long_grid, kInvThreads, 0, st>>>(n, c, nt, grad_out, idx, weight, long_queue, grad_points, f16); \
-    else                                                                                                                      \
+    if constexpr (WEIGHTED) {                                                                                                 \
+        if (lengths)                                                                                                          \
+            inv_long_kernel<VEC, T, true><<<long_grid, kInvThreads, 0, st>>>(n, c, nt, grad_out, idx, weight, long_queue,       \
+                                                                             grad_points, f16, lengths);                      \
+        else                                                                                                                  \
+            inv_long_kernel<VEC, T, false><<<long_grid, kInvThreads, 0, st>>>(n, c, nt, grad_out, idx, weight, long_queue,      \
+                                                                              grad_points, f16, nullptr);                     \
+    } else                                                                                                                    \
         inv_long_seq_kernel<VEC, T><<<long_grid, kInvThreads, 0, st>>>(ne, c, nt, grad_out, idx, long_queue, grad_points, f16)
     if (vec) {
         PN2_INV_SUMS(true);
@@ -961,7 +1078,8 @@ static int inv_scatter_det(int b, int n, int ne, int c, int nt, const T* grad_ou
 
 template <typename T>
 static int three_interpolate_grad_det_impl(int b, int n, int c, int m, const T* grad_out, const int* idx, const float* weight,
-                                           T* grad_points, void* workspace, size_t workspace_bytes, int f16, void* stream) {
+                                           const int* lengths, T* grad_points, void* workspace, size_t workspace_bytes, int f16,
+                                           void* stream) {
     if (b < 0 || m <= 0 || c < 0 || n < 0) return (int)cudaErrorInvalidValue;
     if ((unsigned long long)b * m * c == 0) return 0;
     if (!grad_points) return (int)cudaErrorInvalidValue;
@@ -970,14 +1088,14 @@ static int three_interpolate_grad_det_impl(int b, int n, int c, int m, const T* 
     if (!grad_out || !idx || !weight || !workspace) return (int)cudaErrorInvalidValue;
     if (workspace_bytes < ::pn2_three_interpolate_grad_det_workspace_bytes(b, n, m) || (long long)n * 3 > 0x7fffffffLL)
         return (int)cudaErrorInvalidValue;
-    return inv_scatter_det<true, T>(b, n, 3 * n, c, m, grad_out, idx, weight, grad_points, workspace, f16, st);
+    return inv_scatter_det<true, T>(b, n, 3 * n, c, m, grad_out, idx, weight, lengths, grad_points, workspace, f16, st);
 }
 
 // explicit instances for the group_point / gather_point gradients (group.cu)
 template <typename T>
 int inv_sum_rows_det(int b, int ne, int c, int nt, const T* src, const int* idx, T* dst, void* workspace, int f16,
                      cudaStream_t st) {
-    return inv_scatter_det<false, T>(b, ne, ne, c, nt, src, idx, nullptr, dst, workspace, f16, st);
+    return inv_scatter_det<false, T>(b, ne, ne, c, nt, src, idx, nullptr, nullptr, dst, workspace, f16, st);
 }
 template int inv_sum_rows_det<float>(int, int, int, int, const float*, const int*, float*, void*, int, cudaStream_t);
 template int inv_sum_rows_det<unsigned short>(int, int, int, int, const unsigned short*, const int*, unsigned short*, void*, int,
@@ -987,121 +1105,152 @@ template int inv_sum_rows_det<unsigned short>(int, int, int, int, const unsigned
 
 extern "C" {
 
-int pn2_three_nn(int b, int n, int m, const float* xyz1, const float* xyz2, float* dist, int* idx, void* stream) {
+// Every entry without lengths forwards to its *_ragged twin with lengths1 = NULL.
+
+int pn2_three_nn_ragged(int b, int n, int m, const float* xyz1, const int* lengths1, const float* xyz2, float* dist, int* idx,
+                        void* stream) {
     using namespace pn2;
     if (b < 0 || n < 0 || m < 0) return (int)cudaErrorInvalidValue;
     if (b == 0 || n == 0) return 0;
     if (!xyz1 || (m > 0 && !xyz2) || !dist || !idx) return (int)cudaErrorInvalidValue;
     if (b > 65535) return (int)cudaErrorInvalidValue;
     dim3 grid((n + kNnThreads - 1) / kNnThreads, b, 1);
-    three_nn_kernel<<<grid, kNnThreads, 0, as_stream(stream)>>>(n, m, xyz1, xyz2, dist, idx);
+    if (lengths1)
+        three_nn_kernel<true><<<grid, kNnThreads, 0, as_stream(stream)>>>(n, m, xyz1, xyz2, dist, idx, lengths1);
+    else
+        three_nn_kernel<false><<<grid, kNnThreads, 0, as_stream(stream)>>>(n, m, xyz1, xyz2, dist, idx, nullptr);
     return finish_launch();
+}
+
+int pn2_three_nn(int b, int n, int m, const float* xyz1, const float* xyz2, float* dist, int* idx, void* stream) {
+    return pn2_three_nn_ragged(b, n, m, xyz1, nullptr, xyz2, dist, idx, stream);
+}
+
+int pn2_three_interpolate_ragged_typed(int dtype, int b, int m, int c, int n, const void* points, const int* idx,
+                                       const float* weight, const int* lengths1, void* out, void* stream) {
+    using namespace pn2;
+    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
+    if (b < 0 || m <= 0 || c < 0 || n < 0) return (int)cudaErrorInvalidValue;
+    if ((unsigned long long)b * n * c == 0) return 0;
+    if (!points || !idx || !weight || !out) return (int)cudaErrorInvalidValue;
+    if (dtype == PN2_F32)
+        return three_interpolate_impl<float>(b, m, c, n, static_cast<const float*>(points), idx, weight, lengths1,
+                                             static_cast<float*>(out), as_stream(stream));
+    if (dtype == PN2_BF16)
+        return three_interpolate_impl<__nv_bfloat16>(b, m, c, n, static_cast<const __nv_bfloat16*>(points), idx, weight, lengths1,
+                                                     static_cast<__nv_bfloat16*>(out), as_stream(stream));
+    return three_interpolate_impl<__half>(b, m, c, n, static_cast<const __half*>(points), idx, weight, lengths1,
+                                          static_cast<__half*>(out), as_stream(stream));
 }
 
 int pn2_three_interpolate(int b, int m, int c, int n, const float* points, const int* idx, const float* weight,
                           float* out, void* stream) {
-    using namespace pn2;
-    if (b < 0 || m <= 0 || c < 0 || n < 0) return (int)cudaErrorInvalidValue;
-    const unsigned long long total = (unsigned long long)b * n * c;
-    if (total == 0) return 0;
-    if (!points || !idx || !weight || !out) return (int)cudaErrorInvalidValue;
-    return three_interpolate_impl<float>(b, m, c, n, points, idx, weight, out, as_stream(stream));
+    return pn2_three_interpolate_ragged_typed(PN2_F32, b, m, c, n, points, idx, weight, nullptr, out, stream);
 }
 
 int pn2_three_interpolate_typed(int dtype, int b, int m, int c, int n, const void* points, const int* idx,
                                 const float* weight, void* out, void* stream) {
-    using namespace pn2;
-    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
-    if (dtype == PN2_F32) return pn2_three_interpolate(b, m, c, n, static_cast<const float*>(points), idx, weight, static_cast<float*>(out), stream);
-    if (b < 0 || m <= 0 || c < 0 || n < 0) return (int)cudaErrorInvalidValue;
-    if ((unsigned long long)b * n * c == 0) return 0;
-    if (!points || !idx || !weight || !out) return (int)cudaErrorInvalidValue;
-    if (dtype == PN2_BF16)
-        return three_interpolate_impl<__nv_bfloat16>(b, m, c, n, static_cast<const __nv_bfloat16*>(points), idx, weight,
-                                                     static_cast<__nv_bfloat16*>(out), as_stream(stream));
-    return three_interpolate_impl<__half>(b, m, c, n, static_cast<const __half*>(points), idx, weight, static_cast<__half*>(out),
-                                          as_stream(stream));
+    return pn2_three_interpolate_ragged_typed(dtype, b, m, c, n, points, idx, weight, nullptr, out, stream);
 }
 
-int pn2_three_interpolate_grad(int b, int n, int c, int m, const float* grad_out, const int* idx, const float* weight,
-                               float* grad_points, void* stream) {
+int pn2_three_interpolate_grad_ragged(int b, int n, int c, int m, const float* grad_out, const int* idx, const float* weight,
+                                      const int* lengths1, float* grad_points, void* stream) {
     using namespace pn2;
     if (b < 0 || m <= 0 || c < 0 || n < 0) return (int)cudaErrorInvalidValue;
     const unsigned long long total = (unsigned long long)b * n * c;
     if (total == 0) return 0;
     if (!grad_out || !idx || !weight || !grad_points) return (int)cudaErrorInvalidValue;
     cudaStream_t st = as_stream(stream);
-    if (c % 4 == 0 && al16(grad_out) && al16(grad_points)) {
-        const unsigned long long tv = total / 4;
-        const unsigned grid = it_grid(tv, kItThreads);
-        if (tv < (1ull << 31))
-            three_interp_grad_vec4_kernel<unsigned><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned)n, (unsigned)tv, (const float4*)grad_out, idx, weight, (float4*)grad_points);
-        else
-            three_interp_grad_vec4_kernel<unsigned long long><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned long long)n, tv, (const float4*)grad_out, idx, weight, (float4*)grad_points);
-    } else {
-        const unsigned grid = it_grid(total, kItThreads);
-        if (total < (1ull << 31))
-            three_interp_grad_scalar_kernel<unsigned><<<grid, kItThreads, 0, st>>>(m, c, (unsigned)n, (unsigned)total, grad_out, idx, weight, grad_points);
-        else
-            three_interp_grad_scalar_kernel<unsigned long long><<<grid, kItThreads, 0, st>>>(m, c, (unsigned long long)n, total, grad_out, idx, weight, grad_points);
+#define PN2_GRAD_ATOMIC(L, LEN)                                                                                                \
+    if (c % 4 == 0 && al16(grad_out) && al16(grad_points)) {                                                                   \
+        const unsigned long long tv = total / 4;                                                                               \
+        const unsigned grid = it_grid(tv, kItThreads);                                                                         \
+        if (tv < (1ull << 31))                                                                                                 \
+            three_interp_grad_vec4_kernel<unsigned, L><<<grid, kItThreads, 0, st>>>(m, c / 4, (unsigned)n, (unsigned)tv,         \
+                                                                                    (const float4*)grad_out, idx, weight,        \
+                                                                                    (float4*)grad_points, LEN);                  \
+        else                                                                                                                   \
+            three_interp_grad_vec4_kernel<unsigned long long, L><<<grid, kItThreads, 0, st>>>(                                  \
+                m, c / 4, (unsigned long long)n, tv, (const float4*)grad_out, idx, weight, (float4*)grad_points, LEN);          \
+    } else {                                                                                                                   \
+        const unsigned grid = it_grid(total, kItThreads);                                                                      \
+        if (total < (1ull << 31))                                                                                              \
+            three_interp_grad_scalar_kernel<unsigned, L><<<grid, kItThreads, 0, st>>>(m, c, (unsigned)n, (unsigned)total,        \
+                                                                                      grad_out, idx, weight, grad_points, LEN);  \
+        else                                                                                                                   \
+            three_interp_grad_scalar_kernel<unsigned long long, L><<<grid, kItThreads, 0, st>>>(                                \
+                m, c, (unsigned long long)n, total, grad_out, idx, weight, grad_points, LEN);                                   \
     }
+    if (lengths1) {
+        PN2_GRAD_ATOMIC(true, lengths1)
+    } else {
+        PN2_GRAD_ATOMIC(false, nullptr)
+    }
+#undef PN2_GRAD_ATOMIC
     return finish_launch();
 }
 
-int pn2_three_nn_interpolate(int b, int n, int m, int c, const float* xyz1, const float* xyz2, const float* points2,
-                             float* out, float* dist, int* idx, float* weight, void* stream) {
+int pn2_three_interpolate_grad(int b, int n, int c, int m, const float* grad_out, const int* idx, const float* weight,
+                               float* grad_points, void* stream) {
+    return pn2_three_interpolate_grad_ragged(b, n, c, m, grad_out, idx, weight, nullptr, grad_points, stream);
+}
+
+int pn2_three_nn_interpolate_ragged_typed(int dtype, int b, int n, int m, int c, const float* xyz1, const int* lengths1,
+                                          const float* xyz2, const void* points2, void* out, float* dist, int* idx,
+                                          float* weight, void* stream) {
     using namespace pn2;
+    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
     if (b < 0 || n < 0 || m <= 0 || c < 0) return (int)cudaErrorInvalidValue;
     if (b == 0 || n == 0) return 0;
     if (!xyz1 || !xyz2 || (c > 0 && (!points2 || !out))) return (int)cudaErrorInvalidValue;
     if (b > 65535) return (int)cudaErrorInvalidValue;
-    return fp_front_dispatch<float>(b, n, m, c, 0, xyz1, xyz2, nullptr, points2, c > 0 ? out : nullptr, dist, idx, weight, 0, as_stream(stream));
+    if (dtype == PN2_F32)
+        return fp_front_dispatch<float>(b, n, m, c, 0, xyz1, lengths1, xyz2, nullptr, static_cast<const float*>(points2),
+                                        c > 0 ? static_cast<float*>(out) : nullptr, dist, idx, weight, 0, as_stream(stream));
+    using U16 = unsigned short;  // bfloat16 and float16 share one instance: dtype == PN2_F16 selects the format
+    return fp_front_dispatch<U16>(b, n, m, c, 0, xyz1, lengths1, xyz2, nullptr, static_cast<const U16*>(points2),
+                                  c > 0 ? static_cast<U16*>(out) : nullptr, dist, idx, weight, dtype == PN2_F16, as_stream(stream));
+}
+
+int pn2_three_nn_interpolate(int b, int n, int m, int c, const float* xyz1, const float* xyz2, const float* points2,
+                             float* out, float* dist, int* idx, float* weight, void* stream) {
+    return pn2_three_nn_interpolate_ragged_typed(PN2_F32, b, n, m, c, xyz1, nullptr, xyz2, points2, out, dist, idx, weight, stream);
 }
 
 int pn2_three_nn_interpolate_typed(int dtype, int b, int n, int m, int c, const float* xyz1, const float* xyz2,
                                    const void* points2, void* out, float* dist, int* idx, float* weight,
                                    void* stream) {
-    using namespace pn2;
-    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
-    if (dtype == PN2_F32)
-        return pn2_three_nn_interpolate(b, n, m, c, xyz1, xyz2, static_cast<const float*>(points2), static_cast<float*>(out), dist, idx,
-                                        weight, stream);
-    if (b < 0 || n < 0 || m <= 0 || c < 0) return (int)cudaErrorInvalidValue;
-    if (b == 0 || n == 0) return 0;
-    if (!xyz1 || !xyz2 || (c > 0 && (!points2 || !out))) return (int)cudaErrorInvalidValue;
-    if (b > 65535) return (int)cudaErrorInvalidValue;
-    using U16 = unsigned short;  // bfloat16 and float16 share one instance: dtype == PN2_F16 selects the format
-    return fp_front_dispatch<U16>(b, n, m, c, 0, xyz1, xyz2, nullptr, static_cast<const U16*>(points2),
-                                  c > 0 ? static_cast<U16*>(out) : nullptr, dist, idx, weight, dtype == PN2_F16, as_stream(stream));
+    return pn2_three_nn_interpolate_ragged_typed(dtype, b, n, m, c, xyz1, nullptr, xyz2, points2, out, dist, idx, weight, stream);
 }
 
-int pn2_fp_interpolate_concat(int b, int n, int m, int c2, int c1, const float* xyz1, const float* xyz2, const float* points1,
-                              const float* points2, float* out, void* stream) {
+int pn2_fp_interpolate_concat_ragged_typed(int dtype, int b, int n, int m, int c2, int c1, const float* xyz1,
+                                           const int* lengths1, const float* xyz2, const void* points1, const void* points2,
+                                           void* out, void* stream) {
     using namespace pn2;
+    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
     if (b < 0 || n < 0 || m <= 0 || c2 <= 0 || c1 < 0) return (int)cudaErrorInvalidValue;
     if (b == 0 || n == 0) return 0;
     if (!xyz1 || !xyz2 || !points2 || !out || (c1 > 0 && !points1)) return (int)cudaErrorInvalidValue;
     if (b > 65535) return (int)cudaErrorInvalidValue;
-    return fp_front_dispatch<float>(b, n, m, c2, c1, xyz1, xyz2, c1 > 0 ? points1 : nullptr, points2, out, nullptr, nullptr, nullptr,
-                                    0, as_stream(stream));
+    if (dtype == PN2_F32)
+        return fp_front_dispatch<float>(b, n, m, c2, c1, xyz1, lengths1, xyz2, c1 > 0 ? static_cast<const float*>(points1) : nullptr,
+                                        static_cast<const float*>(points2), static_cast<float*>(out), nullptr, nullptr, nullptr, 0,
+                                        as_stream(stream));
+    using U16 = unsigned short;  // bfloat16 and float16 share one instance: dtype == PN2_F16 selects the format
+    return fp_front_dispatch<U16>(b, n, m, c2, c1, xyz1, lengths1, xyz2, c1 > 0 ? static_cast<const U16*>(points1) : nullptr,
+                                  static_cast<const U16*>(points2), static_cast<U16*>(out), nullptr, nullptr, nullptr, dtype == PN2_F16,
+                                  as_stream(stream));
+}
+
+int pn2_fp_interpolate_concat(int b, int n, int m, int c2, int c1, const float* xyz1, const float* xyz2, const float* points1,
+                              const float* points2, float* out, void* stream) {
+    return pn2_fp_interpolate_concat_ragged_typed(PN2_F32, b, n, m, c2, c1, xyz1, nullptr, xyz2, points1, points2, out, stream);
 }
 
 int pn2_fp_interpolate_concat_typed(int dtype, int b, int n, int m, int c2, int c1, const float* xyz1,
                                     const float* xyz2, const void* points1, const void* points2, void* out,
                                     void* stream) {
-    using namespace pn2;
-    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
-    if (dtype == PN2_F32)
-        return pn2_fp_interpolate_concat(b, n, m, c2, c1, xyz1, xyz2, static_cast<const float*>(points1), static_cast<const float*>(points2),
-                                         static_cast<float*>(out), stream);
-    if (b < 0 || n < 0 || m <= 0 || c2 <= 0 || c1 < 0) return (int)cudaErrorInvalidValue;
-    if (b == 0 || n == 0) return 0;
-    if (!xyz1 || !xyz2 || !points2 || !out || (c1 > 0 && !points1)) return (int)cudaErrorInvalidValue;
-    if (b > 65535) return (int)cudaErrorInvalidValue;
-    using U16 = unsigned short;  // bfloat16 and float16 share one instance: dtype == PN2_F16 selects the format
-    return fp_front_dispatch<U16>(b, n, m, c2, c1, xyz1, xyz2, c1 > 0 ? static_cast<const U16*>(points1) : nullptr,
-                                  static_cast<const U16*>(points2), static_cast<U16*>(out), nullptr, nullptr, nullptr, dtype == PN2_F16,
-                                  as_stream(stream));
+    return pn2_fp_interpolate_concat_ragged_typed(dtype, b, n, m, c2, c1, xyz1, nullptr, xyz2, points1, points2, out, stream);
 }
 
 size_t pn2_three_interpolate_grad_det_workspace_bytes(int b, int n, int m) {
@@ -1109,22 +1258,30 @@ size_t pn2_three_interpolate_grad_det_workspace_bytes(int b, int n, int m) {
     return pn2::inv_workspace_bytes(b, 3 * (long long)n, m);
 }
 
+int pn2_three_interpolate_grad_det_ragged_typed(int dtype, int b, int n, int c, int m, const void* grad_out, const int* idx,
+                                                const float* weight, const int* lengths1, void* grad_points, void* workspace,
+                                                size_t workspace_bytes, void* stream) {
+    using namespace pn2;
+    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
+    if (dtype == PN2_F32)
+        return three_interpolate_grad_det_impl<float>(b, n, c, m, static_cast<const float*>(grad_out), idx, weight, lengths1,
+                                                      static_cast<float*>(grad_points), workspace, workspace_bytes, 0, stream);
+    using U16 = unsigned short;  // bfloat16 and float16 share one instance: dtype == PN2_F16 selects the format
+    return three_interpolate_grad_det_impl<U16>(b, n, c, m, static_cast<const U16*>(grad_out), idx, weight, lengths1,
+                                                static_cast<U16*>(grad_points), workspace, workspace_bytes, dtype == PN2_F16, stream);
+}
+
 int pn2_three_interpolate_grad_det(int b, int n, int c, int m, const float* grad_out, const int* idx, const float* weight,
                                    float* grad_points, void* workspace, size_t workspace_bytes, void* stream) {
-    return pn2::three_interpolate_grad_det_impl<float>(b, n, c, m, grad_out, idx, weight, grad_points, workspace, workspace_bytes, 0, stream);
+    return pn2_three_interpolate_grad_det_ragged_typed(PN2_F32, b, n, c, m, grad_out, idx, weight, nullptr, grad_points, workspace,
+                                                       workspace_bytes, stream);
 }
 
 int pn2_three_interpolate_grad_det_typed(int dtype, int b, int n, int c, int m, const void* grad_out,
                                          const int* idx, const float* weight, void* grad_points, void* workspace,
                                          size_t workspace_bytes, void* stream) {
-    using namespace pn2;
-    if (!valid_dtype(dtype)) return (int)cudaErrorInvalidValue;
-    if (dtype == PN2_F32)
-        return pn2_three_interpolate_grad_det(b, n, c, m, static_cast<const float*>(grad_out), idx, weight, static_cast<float*>(grad_points),
-                                              workspace, workspace_bytes, stream);
-    using U16 = unsigned short;  // bfloat16 and float16 share one instance: dtype == PN2_F16 selects the format
-    return three_interpolate_grad_det_impl<U16>(b, n, c, m, static_cast<const U16*>(grad_out), idx, weight, static_cast<U16*>(grad_points),
-                                                workspace, workspace_bytes, dtype == PN2_F16, stream);
+    return pn2_three_interpolate_grad_det_ragged_typed(dtype, b, n, c, m, grad_out, idx, weight, nullptr, grad_points, workspace,
+                                                       workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -44,9 +44,62 @@ class SharedMLP(nn.Module):
         self.body = nn.Sequential(*layers)
         self.in_channels, self.out_channels = int(in_channels), c
 
-    def forward(self, t: torch.Tensor) -> torch.Tensor:
+    def forward(self, t: torch.Tensor, mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``mask``: optional bool tensor of t.shape[:-1] (or as many elements), True on the real rows of a padded batch
+        (see row_mask).  Batch norm then takes its training statistics from the real rows only, and the padding rows of
+        every layer's output are 0 (whatever t holds there, NaN included).  Without a mask: the plain stack."""
         lead = t.shape[:-1]
-        return self.body(t.reshape(-1, t.shape[-1])).reshape(*lead, self.out_channels)
+        if mask is None:
+            return self.body(t.reshape(-1, t.shape[-1])).reshape(*lead, self.out_channels)
+        keep = mask.reshape(-1, 1)
+        # torch.where, not a multiply: NaN * 0 is NaN
+        x = torch.where(keep, t.reshape(-1, t.shape[-1]), 0)
+        for mod in self.body:
+            if isinstance(mod, nn.BatchNorm1d):
+                x = torch.where(keep, masked_batch_norm(mod, x, keep), 0)
+            elif isinstance(mod, nn.Linear):
+                x = torch.where(keep, mod(x), 0)
+            else:
+                x = mod(x)  # ReLU keeps the zeros
+        return x.reshape(*lead, self.out_channels)
+
+
+def row_mask(lengths: torch.Tensor, n: int) -> torch.Tensor:
+    """(b, n) bool, True on rows j < lengths[i] of a padded batch.  The lengths are clamped to [1, n], as the kernels
+    clamp them, and never leave the device."""
+    return torch.arange(n, device=lengths.device).unsqueeze(0) < lengths.clamp(1, n).unsqueeze(1)
+
+
+def masked_batch_norm(bn: nn.BatchNorm1d, x: torch.Tensor, keep: torch.Tensor) -> torch.Tensor:
+    """``bn`` on the rows of x (R, C) where keep (R, 1) is True.  Training mode: normalised with the mean and (biased)
+    variance of those rows, and the running statistics are updated from them as BatchNorm1d would from a batch made of
+    them alone (unbiased variance, momentum or the cumulative average, num_batches_tracked).  Eval mode: the running
+    statistics, as bn itself.  The statistics are float32 whatever x's dtype (as torch's batch norm keeps them under
+    autocast); the result has x's dtype, and its padding rows are left for the caller to zero.  The padding rows of x
+    must be 0 (the caller zeroes them), so the mean is a plain sum over every row.  The variance is a second pass over
+    the centred real rows, not E[x^2] - mean^2, which cancels catastrophically once |mean| is large against the
+    standard deviation.  The row count stays on the device: nothing synchronises with the host."""
+    if not bn.training and bn.running_mean is not None:
+        return bn(x)
+    xf = x.float()
+    cnt = keep.sum(dtype=torch.float32)
+    mean = xf.sum(0) / cnt
+    centred = xf - mean
+    d = torch.where(keep, centred, 0)
+    var = (d * d).sum(0) / cnt
+    scale = torch.rsqrt(var + bn.eps)
+    if bn.affine:
+        y = torch.addcmul(bn.bias, centred, scale * bn.weight)
+    else:
+        y = centred * scale
+    if bn.track_running_stats and bn.running_mean is not None:
+        with torch.no_grad():
+            bn.num_batches_tracked.add_(1)
+            f = 1.0 / bn.num_batches_tracked if bn.momentum is None else bn.momentum
+            unbiased = var * cnt / torch.clamp(cnt - 1, min=1)
+            bn.running_mean.mul_(1 - f).add_(mean * f)
+            bn.running_var.mul_(1 - f).add_(unbiased * f)
+    return y.to(x.dtype)
 
 
 def set_bn_momentum(model: nn.Module, bn_decay: float) -> None:

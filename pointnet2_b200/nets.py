@@ -19,7 +19,8 @@ from typing import Optional, Sequence
 import torch
 from torch import nn
 
-from .layers import SharedMLP, set_bn_momentum  # noqa: F401
+from ._tensor import device_lengths
+from .layers import SharedMLP, row_mask, set_bn_momentum  # noqa: F401
 from .pointnet_util import pointnet_fp_module, pointnet_sa_module, pointnet_sa_module_msg
 
 
@@ -68,8 +69,8 @@ class FeaturePropagation(nn.Module):
         self.mlp = SharedMLP(in_channels, mlp, bn)
         self.out_channels = self.mlp.out_channels
 
-    def forward(self, xyz1, xyz2, points1, points2):
-        return pointnet_fp_module(xyz1, xyz2, points1, points2, self.mlp)
+    def forward(self, xyz1, xyz2, points1, points2, lengths=None):
+        return pointnet_fp_module(xyz1, xyz2, points1, points2, self.mlp, lengths=lengths)
 
 
 class _ClsHead(nn.Module):
@@ -125,7 +126,11 @@ class PointNet2ClsMSG(nn.Module):
 
 
 class PointNet2SemSeg(nn.Module):
-    """Semantic segmentation net, input (B,N,3) -> logits (B,N,num_class). models/pointnet2_sem_seg.py:20-46."""
+    """Semantic segmentation net, input (B,N,3) -> logits (B,N,num_class). models/pointnet2_sem_seg.py:20-46.
+    ``lengths`` (B,), optional: cloud i is ``point_cloud[i, :lengths[i]]`` (variable-size clouds padded to N).  Only the
+    first and the last levels see the padding: sa1 samples 1024 centroids per cloud from the real points (every deeper
+    level is dense), and fp4 interpolates onto the real points only.  The batch norms of fp4 and fc1 take their
+    statistics from the real rows, and the padding rows of the logits are 0 (sem_seg_loss(..., lengths=) ignores them)."""
 
     def __init__(self, num_class: int = 21):
         super().__init__()
@@ -141,18 +146,23 @@ class PointNet2SemSeg(nn.Module):
         self.dp1 = nn.Dropout(0.5)
         self.fc2 = SharedMLP(128, [num_class], bn=False, last_activation=False)
 
-    def forward(self, point_cloud):
+    def forward(self, point_cloud, lengths=None):
         l0_xyz = point_cloud
-        l1_xyz, l1_points, _ = self.sa1(l0_xyz, None)
+        mask = None
+        if lengths is not None:
+            b, n = point_cloud.shape[0], point_cloud.shape[1]
+            lengths = device_lengths(lengths, b, n, point_cloud.device, "PointNet2SemSeg")
+            mask = row_mask(lengths, n)
+        l1_xyz, l1_points, _ = self.sa1(l0_xyz, None, lengths)
         l2_xyz, l2_points, _ = self.sa2(l1_xyz, l1_points)
         l3_xyz, l3_points, _ = self.sa3(l2_xyz, l2_points)
         l4_xyz, l4_points, _ = self.sa4(l3_xyz, l3_points)
         l3_points = self.fp1(l3_xyz, l4_xyz, l3_points, l4_points)
         l2_points = self.fp2(l2_xyz, l3_xyz, l2_points, l3_points)
         l1_points = self.fp3(l1_xyz, l2_xyz, l1_points, l2_points)
-        l0_points = self.fp4(l0_xyz, l1_xyz, None, l1_points)
-        feats = self.fc1(l0_points)
-        return self.fc2(self.dp1(feats)), {"feats": feats}
+        l0_points = self.fp4(l0_xyz, l1_xyz, None, l1_points, lengths)
+        feats = self.fc1(l0_points, mask)
+        return self.fc2(self.dp1(feats), mask), {"feats": feats}
 
 
 def cls_loss(pred: torch.Tensor, label: torch.Tensor) -> torch.Tensor:
@@ -160,9 +170,21 @@ def cls_loss(pred: torch.Tensor, label: torch.Tensor) -> torch.Tensor:
     return nn.functional.cross_entropy(pred, label.long())
 
 
-def sem_seg_loss(pred: torch.Tensor, label: torch.Tensor, smpw: torch.Tensor) -> torch.Tensor:
+def sem_seg_loss(pred: torch.Tensor, label: torch.Tensor, smpw: torch.Tensor, lengths=None) -> torch.Tensor:
     """sample-weighted cross entropy — models/pointnet2_sem_seg.py:49-56 (tf.losses default reduction:
-    sum of weighted losses / number of non-zero weights)."""
-    per = nn.functional.cross_entropy(pred.reshape(-1, pred.shape[-1]), label.reshape(-1).long(), reduction="none")
+    sum of weighted losses / number of non-zero weights).  ``lengths`` (B,), optional: the padding rows j >= lengths[i]
+    count as weight 0, whatever smpw, label and pred hold there."""
+    label = label.reshape(-1).long()
+    keep = None
+    logits = pred.reshape(-1, pred.shape[-1])
+    if lengths is not None:
+        b, n = pred.shape[0], pred.shape[1]
+        keep = row_mask(device_lengths(lengths, b, n, pred.device, "sem_seg_loss"), n).reshape(-1)
+        label = torch.where(keep, label, 0)  # any class: the row's weight is 0
+        # select before the softmax, not after: its backward would turn a zero gradient times NaN logits into NaN
+        logits = torch.where(keep.unsqueeze(1), logits, 0)
+    per = nn.functional.cross_entropy(logits, label, reduction="none")
     w = smpw.reshape(-1).to(per.dtype)
+    if keep is not None:
+        w = torch.where(keep, w, 0)
     return (per * w).sum() / torch.clamp((w != 0).sum(), min=1)

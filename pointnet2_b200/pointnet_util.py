@@ -20,7 +20,7 @@ from typing import Callable, Optional, Sequence
 import torch
 
 from . import _lib, layers
-from ._tensor import DTYPE_CODES, FEATURE_DTYPES, on_device, ptr, require_cuda, same_device, stream_ptr
+from ._tensor import DTYPE_CODES, FEATURE_DTYPES, device_lengths, on_device, ptr, require_cuda, same_device, stream_ptr
 from .tf_grouping import group_point, group_point_grad, knn_point, query_ball_point
 from .tf_interpolate import fp_interpolate_concat, three_interpolate, three_nn, three_nn_interpolate
 from .sa_layer import sample_group, sample_group_msg
@@ -180,17 +180,19 @@ def sample_and_group_all(xyz, points, use_xyz=True):
     return new_xyz, new_points, idx, grouped_xyz
 
 
-def _apply_mlp(mlp, t: torch.Tensor, scope=None, name="mlp", bn=True, is_training=None, bn_decay=None) -> torch.Tensor:
+def _apply_mlp(mlp, t: torch.Tensor, scope=None, name="mlp", bn=True, is_training=None, bn_decay=None, mask=None) -> torch.Tensor:
     """``mlp`` is None (identity), a callable on a (..., channel) tensor, or — the reference's form — a list of
-    output widths, resolved to the SharedMLP registered under ``scope/name`` (layers.scoped_mlp)."""
+    output widths, resolved to the SharedMLP registered under ``scope/name`` (layers.scoped_mlp).  ``mask`` (rows of a
+    padded batch, see layers.SharedMLP.forward) is passed on to a SharedMLP; the caller has refused other callables."""
     if mlp is None:
         return t
     if callable(mlp):
-        return mlp(t)
+        return mlp(t) if mask is None else mlp(t, mask)
     widths = [int(w) for w in mlp]
     if not widths:
         return t
-    return layers.scoped_mlp(scope, name, t.shape[-1], widths, bn, t.device, is_training, bn_decay)(t)
+    mod = layers.scoped_mlp(scope, name, t.shape[-1], widths, bn, t.device, is_training, bn_decay)
+    return mod(t) if mask is None else mod(t, mask)
 
 
 def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp=None, mlp2=None, group_all=False, is_training=None,
@@ -277,31 +279,49 @@ def pointnet_sa_module_msg(xyz, points, npoint, radius_list: Sequence[float], ns
     return new_xyz, torch.cat(new_points_list, dim=-1)
 
 
-def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp=None, is_training=None, bn_decay=None, scope=None, bn=True, fused=True):
+def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp=None, is_training=None, bn_decay=None, scope=None, bn=True, fused=True,
+                       lengths=None):
     ''' PointNet Feature Propogation (FP) Module — same positional arguments as the reference
         (utils/pointnet_util.py:199-229).
         xyz1 (b,n1,3) dense, xyz2 (b,n2,3) sparser, points1 (b,n1,c1) or None, points2 (b,n2,c2);
         mlp: list of output widths (scope registry), a callable on a (b,n1,1,channel) tensor, or None.
+        lengths: optional (b,) integers: cloud i of the dense level is xyz1[i, :lengths[i]] (and points1[i, :lengths[i]]),
+        padded to n1; xyz2 / points2 stay dense.  Real rows are what the call without lengths computes for them (the
+        batch norm statistics of the mlp come from the real rows only); padding rows are never read and come out 0.
+        With lengths, mlp must be a list of widths or a layers.SharedMLP (it takes the row mask); another callable
+        raises ValueError.
         Return: new_points (b,n1,mlp[-1]) (or (b,n1,c2+c1) when mlp is None)
     '''
+    mask = None
+    if lengths is not None:
+        if mlp is not None and callable(mlp) and not isinstance(mlp, layers.SharedMLP):
+            raise ValueError("pointnet_fp_module with lengths needs mlp as a list of widths or a layers.SharedMLP "
+                             "(the batch norm must see the row mask)")
+        b, n = xyz1.shape[0], xyz1.shape[1]
+        lengths = device_lengths(lengths, b, n, xyz1.device, "pointnet_fp_module")
+        mask = layers.row_mask(lengths, n)
     no_grad = not points2.requires_grad and (points1 is None or not points1.requires_grad)
     same_dtype = points1 is None or points1.dtype == points2.dtype
     if fused and no_grad and same_dtype and points2.shape[2] > 0:
         # one kernel: 3-NN, weights, interpolation and the concat of :219
-        new_points1 = fp_interpolate_concat(xyz1, xyz2, points1, points2)
+        new_points1 = fp_interpolate_concat(xyz1, xyz2, points1, points2, lengths=lengths)
     else:
         if fused and not points2.requires_grad:
-            interpolated_points = three_nn_interpolate(xyz1, xyz2, points2)
+            interpolated_points = three_nn_interpolate(xyz1, xyz2, points2, lengths=lengths)
         else:
-            dist, idx = three_nn(xyz1, xyz2)
+            dist, idx = three_nn(xyz1, xyz2, lengths=lengths)
             dist = torch.clamp(dist, min=1e-10)
             norm = (1.0 / dist).sum(dim=2, keepdim=True)
+            # with lengths, the padding rows' weights are NaN (1/inf = 0, then 0/0): three_interpolate never reads them
             weight = (1.0 / dist) / norm
-            interpolated_points = three_interpolate(points2, idx, weight)
+            interpolated_points = three_interpolate(points2, idx, weight, lengths=lengths)
         if points1 is not None:
+            if mask is not None:
+                points1 = torch.where(mask.unsqueeze(2), points1, 0)  # padding rows are 0, as the fused kernel writes them
             new_points1 = torch.cat([interpolated_points, points1], dim=2)  # B,ndataset1,nchannel1+nchannel2
         else:
             new_points1 = interpolated_points
     if mlp is not None:
-        new_points1 = _apply_mlp(mlp, new_points1.unsqueeze(2), scope, "conv", bn, is_training, bn_decay).squeeze(2)
+        new_points1 = _apply_mlp(mlp, new_points1.unsqueeze(2), scope, "conv", bn, is_training, bn_decay,
+                                 mask=None if mask is None else mask.unsqueeze(2)).squeeze(2)
     return new_points1

@@ -11,15 +11,18 @@ from __future__ import annotations
 import torch
 
 from . import _lib
-from ._tensor import DTYPE_CODES, FEATURE_DTYPES, on_device, ptr, require_cuda, same_device, stream_ptr
+from ._tensor import DTYPE_CODES, FEATURE_DTYPES, device_lengths, on_device, ptr, require_cuda, same_device, stream_ptr
 
 
-def three_nn(xyz1: torch.Tensor, xyz2: torch.Tensor):
+def three_nn(xyz1: torch.Tensor, xyz2: torch.Tensor, *, lengths=None):
     """The three nearest known points of every unknown point.
 
     ``xyz1`` float32 (B, n, 3): the points that need values; ``xyz2`` float32 (B, m, 3): the points that carry them.
     Returns ``dist`` float32 (B, n, 3) — SQUARED distances, ascending — and ``idx`` int32 (B, n, 3), positions in
     ``xyz2``.
+    ``lengths``: optional (B,) integers: cloud i's unknown points are ``xyz1[i, :lengths[i]]`` (a padded batch, see
+    pointnet2_b200._tensor.device_lengths).  Real rows are what the call without lengths gives; padding rows are never
+    read and hold dist +inf, idx 0.
     Reference: tf_interpolate.py:8-17 -> ThreeNNOp (tf_interpolate.cpp:157-187) -> threenn_cpu (:60-103).
     """
     xyz1 = require_cuda(xyz1, "xyz1", torch.float32)
@@ -31,11 +34,16 @@ def three_nn(xyz1: torch.Tensor, xyz2: torch.Tensor):
         raise ValueError(f"ThreeNN expects (b,m,3) xyz2 shape, got {tuple(xyz2.shape)}")
     b, n, _ = xyz1.shape
     m = xyz2.shape[1]
+    lengths = device_lengths(lengths, b, n, xyz1.device, "ThreeNN")
     dist = torch.empty((b, n, 3), dtype=torch.float32, device=xyz1.device)
     idx = torch.empty((b, n, 3), dtype=torch.int32, device=xyz1.device)
     if b * n:
         with on_device(xyz1):
-            rc = _lib.load().pn2_three_nn(b, n, m, ptr(xyz1), ptr(xyz2), ptr(dist), ptr(idx), stream_ptr(xyz1.device))
+            if lengths is None:
+                rc = _lib.load().pn2_three_nn(b, n, m, ptr(xyz1), ptr(xyz2), ptr(dist), ptr(idx), stream_ptr(xyz1.device))
+            else:
+                rc = _lib.load().pn2_three_nn_ragged(b, n, m, ptr(xyz1), ptr(lengths), ptr(xyz2), ptr(dist), ptr(idx),
+                                                     stream_ptr(xyz1.device))
         _lib.check(rc, "pn2_three_nn")
     return dist, idx
 
@@ -51,27 +59,32 @@ DETERMINISTIC_GRAD = True
 
 class _ThreeInterpolate(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, points, idx, weight):
+    def forward(ctx, points, idx, weight, lengths):
         b, m, c = points.shape
         n = idx.shape[1]
         out = torch.empty((b, n, c), dtype=points.dtype, device=points.device)
         if out.numel():
             with on_device(points):
-                if points.dtype == torch.float32:
+                if lengths is not None:
+                    rc = _lib.load().pn2_three_interpolate_ragged_typed(DTYPE_CODES[points.dtype], b, m, c, n, ptr(points), ptr(idx),
+                                                                        ptr(weight), ptr(lengths), ptr(out), stream_ptr(points.device))
+                elif points.dtype == torch.float32:
                     rc = _lib.load().pn2_three_interpolate(b, m, c, n, ptr(points), ptr(idx), ptr(weight), ptr(out),
                                                            stream_ptr(points.device))
                 else:
                     rc = _lib.load().pn2_three_interpolate_typed(DTYPE_CODES[points.dtype], b, m, c, n, ptr(points), ptr(idx),
                                                                  ptr(weight), ptr(out), stream_ptr(points.device))
             _lib.check(rc, "pn2_three_interpolate")
-        ctx.save_for_backward(idx, weight)
+        ctx.save_for_backward(*((idx, weight) if lengths is None else (idx, weight, lengths)))
         ctx.shape = (b, m, c)
         ctx.dtype = points.dtype
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        idx, weight = ctx.saved_tensors
+        saved = ctx.saved_tensors
+        idx, weight = saved[:2]
+        lengths = saved[2] if len(saved) > 2 else None
         b, m, c = ctx.shape
         n = idx.shape[1]
         grad_out = grad_out.to(ctx.dtype).contiguous()
@@ -83,10 +96,15 @@ class _ThreeInterpolate(torch.autograd.Function):
                 with on_device(grad_out):
                     wsb = int(lib.pn2_three_interpolate_grad_det_workspace_bytes(b, max(n, 1), m))
                     ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-                    rc = lib.pn2_three_interpolate_grad_det_typed(DTYPE_CODES[ctx.dtype], b, n, c, m, ptr(grad_out), ptr(idx),
-                                                                  ptr(weight), ptr(grad_points), ptr(ws), wsb, stream_ptr(dev))
+                    if lengths is None:
+                        rc = lib.pn2_three_interpolate_grad_det_typed(DTYPE_CODES[ctx.dtype], b, n, c, m, ptr(grad_out), ptr(idx),
+                                                                      ptr(weight), ptr(grad_points), ptr(ws), wsb, stream_ptr(dev))
+                    else:
+                        rc = lib.pn2_three_interpolate_grad_det_ragged_typed(DTYPE_CODES[ctx.dtype], b, n, c, m, ptr(grad_out),
+                                                                             ptr(idx), ptr(weight), ptr(lengths), ptr(grad_points),
+                                                                             ptr(ws), wsb, stream_ptr(dev))
                 _lib.check(rc, "pn2_three_interpolate_grad_det")
-            return grad_points, None, None
+            return grad_points, None, None, None
         if (DETERMINISTIC_GRAD or torch.are_deterministic_algorithms_enabled()) and b * m * c:
             # inverse index + ordered accumulation: deterministic, bit-identical to threeinterpolate_grad_cpu
             # (tf_interpolate.cpp:131-153), and ~3x faster than the atomics at the sem-seg sizes
@@ -94,26 +112,38 @@ class _ThreeInterpolate(torch.autograd.Function):
             with on_device(grad_out):
                 wsb = int(lib.pn2_three_interpolate_grad_det_workspace_bytes(b, max(n, 1), m))
                 ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-                rc = lib.pn2_three_interpolate_grad_det(b, n, c, m, ptr(grad_out), ptr(idx), ptr(weight), ptr(grad_points),
-                                                        ptr(ws), wsb, stream_ptr(dev))
+                if lengths is None:
+                    rc = lib.pn2_three_interpolate_grad_det(b, n, c, m, ptr(grad_out), ptr(idx), ptr(weight), ptr(grad_points),
+                                                            ptr(ws), wsb, stream_ptr(dev))
+                else:
+                    rc = lib.pn2_three_interpolate_grad_det_ragged_typed(DTYPE_CODES[torch.float32], b, n, c, m, ptr(grad_out),
+                                                                         ptr(idx), ptr(weight), ptr(lengths), ptr(grad_points),
+                                                                         ptr(ws), wsb, stream_ptr(dev))
             _lib.check(rc, "pn2_three_interpolate_grad_det")
-            return grad_points, None, None
+            return grad_points, None, None, None
         # zero-filled by the caller, as ThreeInterpolateGradOp does (tf_interpolate.cpp:258)
         grad_points = torch.zeros((b, m, c), dtype=torch.float32, device=dev)
         if grad_out.numel():
             with on_device(grad_out):
-                rc = lib.pn2_three_interpolate_grad(b, n, c, m, ptr(grad_out), ptr(idx), ptr(weight),
-                                                    ptr(grad_points), stream_ptr(dev))
+                if lengths is None:
+                    rc = lib.pn2_three_interpolate_grad(b, n, c, m, ptr(grad_out), ptr(idx), ptr(weight),
+                                                        ptr(grad_points), stream_ptr(dev))
+                else:
+                    rc = lib.pn2_three_interpolate_grad_ragged(b, n, c, m, ptr(grad_out), ptr(idx), ptr(weight), ptr(lengths),
+                                                               ptr(grad_points), stream_ptr(dev))
             _lib.check(rc, "pn2_three_interpolate_grad")
-        return grad_points, None, None
+        return grad_points, None, None, None
 
 
-def three_interpolate(points: torch.Tensor, idx: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+def three_interpolate(points: torch.Tensor, idx: torch.Tensor, weight: torch.Tensor, *, lengths=None) -> torch.Tensor:
     """Weighted sum of three feature rows: ``out[b, i, :] = sum_t weight[b, i, t] * points[b, idx[b, i, t], :]``.
 
     ``points`` float32, bfloat16 or float16 (B, m, c): features of the known points; ``idx`` int32 and ``weight``
     float32, both (B, n, 3), as produced from three_nn.  Returns (B, n, c) in the dtype of ``points``: the float32
     result of the upcast features, rounded once.  Differentiable in ``points``.
+    ``lengths``: optional (B,) integers, the real rows of each cloud's n (as for three_nn).  Padding rows of the output
+    are 0 and their idx / weight are never read (they may be NaN); the gradient into ``points`` is that of the call on
+    the truncated clouds, and the padding rows of the incoming gradient are never read either.
     Reference: tf_interpolate.py:19-28 -> threeinterpolate_cpu (tf_interpolate.cpp:107-127);
     gradient :29-34 -> threeinterpolate_grad_cpu (:131-153).
     """
@@ -130,15 +160,19 @@ def three_interpolate(points: torch.Tensor, idx: torch.Tensor, weight: torch.Ten
         raise ValueError(f"ThreeInterpolate expects (b,n,3) weight shape, got {tuple(weight.shape)}")
     if points.shape[1] <= 0 and idx.numel():
         raise ValueError("ThreeInterpolate expects a non-empty points tensor")
-    return _ThreeInterpolate.apply(points, idx, weight.detach())
+    lengths = device_lengths(lengths, b, idx.shape[1], points.device, "ThreeInterpolate")
+    return _ThreeInterpolate.apply(points, idx, weight.detach(), lengths)
 
 
-def three_nn_interpolate(xyz1: torch.Tensor, xyz2: torch.Tensor, points2: torch.Tensor, return_aux: bool = False):
+def three_nn_interpolate(xyz1: torch.Tensor, xyz2: torch.Tensor, points2: torch.Tensor, return_aux: bool = False, *,
+                         lengths=None):
     """Fused feature-propagation front end (utils/pointnet_util.py:211-216): three_nn, the
     inverse-distance weights (dist=max(dist,1e-10); w=(1/dist)/sum(1/dist)) and three_interpolate
     in one kernel; dist/idx/weight stay on chip unless ``return_aux``.  Forward only (use the
     unfused ops when ``points2`` needs a gradient).  ``points2`` may be float32, bfloat16 or float16; ``out`` has its
     dtype, dist/idx/weight stay float32/int32.
+    ``lengths``: optional (b,) integers, the real rows of each cloud of ``xyz1`` (as for three_nn); padding rows of out
+    are 0, with dist +inf, idx 0 and weight 0.
     Returns out (b,n,c) [, dist (b,n,3), idx (b,n,3), weight (b,n,3)]."""
     xyz1 = require_cuda(xyz1, "xyz1", torch.float32)
     xyz2 = require_cuda(xyz2, "xyz2", torch.float32)
@@ -154,13 +188,18 @@ def three_nn_interpolate(xyz1: torch.Tensor, xyz2: torch.Tensor, points2: torch.
     if m <= 0:
         raise ValueError("three_nn_interpolate expects at least one known point")
     dev = xyz1.device
+    lengths = device_lengths(lengths, b, n, dev, "three_nn_interpolate")
     out = torch.empty((b, n, c), dtype=points2.dtype, device=dev)
     dist = torch.empty((b, n, 3), dtype=torch.float32, device=dev) if return_aux else None
     idx = torch.empty((b, n, 3), dtype=torch.int32, device=dev) if return_aux else None
     weight = torch.empty((b, n, 3), dtype=torch.float32, device=dev) if return_aux else None
     if b * n:
         with on_device(xyz1):
-            if points2.dtype == torch.float32:
+            if lengths is not None:
+                rc = _lib.load().pn2_three_nn_interpolate_ragged_typed(DTYPE_CODES[points2.dtype], b, n, m, c, ptr(xyz1),
+                                                                       ptr(lengths), ptr(xyz2), ptr(points2.detach()), ptr(out),
+                                                                       ptr(dist), ptr(idx), ptr(weight), stream_ptr(dev))
+            elif points2.dtype == torch.float32:
                 rc = _lib.load().pn2_three_nn_interpolate(b, n, m, c, ptr(xyz1), ptr(xyz2), ptr(points2.detach()), ptr(out),
                                                           ptr(dist), ptr(idx), ptr(weight), stream_ptr(dev))
             else:
@@ -173,11 +212,13 @@ def three_nn_interpolate(xyz1: torch.Tensor, xyz2: torch.Tensor, points2: torch.
     return out
 
 
-def fp_interpolate_concat(xyz1: torch.Tensor, xyz2: torch.Tensor, points1, points2: torch.Tensor) -> torch.Tensor:
+def fp_interpolate_concat(xyz1: torch.Tensor, xyz2: torch.Tensor, points1, points2: torch.Tensor, *, lengths=None) -> torch.Tensor:
     """The front end of pointnet_fp_module in one kernel (utils/pointnet_util.py:211-219): three_nn, the
     inverse-distance weights, three_interpolate AND the concat with ``points1``:
     returns (b, n, c2 + c1) = [interpolated points2 | points1] (c1 = 0 when ``points1`` is None).  Forward only.
-    ``points2`` and ``points1`` may be float32, bfloat16 or float16, the same dtype for both; the output has it."""
+    ``points2`` and ``points1`` may be float32, bfloat16 or float16, the same dtype for both; the output has it.
+    ``lengths``: optional (b,) integers, the real rows of each cloud of ``xyz1`` and ``points1`` (as for three_nn);
+    padding rows of the output, its points1 half included, are 0 and the padding of points1 is never read."""
     if isinstance(points1, torch.Tensor) and isinstance(points2, torch.Tensor) and points1.dtype != points2.dtype:
         raise TypeError(f"points1 and points2 must have the same dtype, got {points1.dtype} and {points2.dtype}")
     xyz1 = require_cuda(xyz1, "xyz1", torch.float32)
@@ -199,10 +240,16 @@ def fp_interpolate_concat(xyz1: torch.Tensor, xyz2: torch.Tensor, points1, point
         c1 = points1.shape[2]
     if m <= 0 or c2 <= 0:
         raise ValueError("fp_interpolate_concat expects at least one known point and one channel")
+    lengths = device_lengths(lengths, b, n, xyz1.device, "fp_interpolate_concat")
     out = torch.empty((b, n, c2 + c1), dtype=points2.dtype, device=xyz1.device)
     if b * n:
         with on_device(xyz1):
-            if points2.dtype == torch.float32:
+            if lengths is not None:
+                rc = _lib.load().pn2_fp_interpolate_concat_ragged_typed(DTYPE_CODES[points2.dtype], b, n, m, c2, c1, ptr(xyz1),
+                                                                        ptr(lengths), ptr(xyz2),
+                                                                        ptr(points1.detach()) if c1 else None,
+                                                                        ptr(points2.detach()), ptr(out), stream_ptr(xyz1.device))
+            elif points2.dtype == torch.float32:
                 rc = _lib.load().pn2_fp_interpolate_concat(b, n, m, c2, c1, ptr(xyz1), ptr(xyz2),
                                                            ptr(points1.detach()) if c1 else None, ptr(points2.detach()), ptr(out),
                                                            stream_ptr(xyz1.device))
