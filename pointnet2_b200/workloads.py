@@ -75,6 +75,48 @@ def features(b: int, n: int, c: int, seed: int) -> np.ndarray:
     return np.random.RandomState(seed).standard_normal((b, n, c)).astype(F32)
 
 
+def part_shapes(b: int, n: int, seed: int, offsets):
+    """A synthetic part-segmentation batch (the reference's ShapeNet part data is not shipped): (b, n, 6) float32
+    points (xyz, then unit normals), (b,) int64 categories and (b, n) int64 part labels.  Category k of the
+    len(offsets) - 1 is a sphere, a cylinder side or a box surface (k mod 3), taller with k // 3, with analytic normals,
+    rotated about the up axis, scaled and centred into the unit sphere.  Its parts offsets[k] .. offsets[k + 1] - 1
+    are equal height bands, bottom to top."""
+    rs = np.random.RandomState(seed)
+    cls = rs.randint(0, len(offsets) - 1, b)
+    pts = np.empty((b, n, 6), F32)
+    label = np.empty((b, n), np.int64)
+    rows = np.arange(n)
+    for i, k in enumerate(cls):
+        th, z = 2 * np.pi * rs.rand(n), 2 * rs.rand(n) - 1
+        kind = k % 3
+        if kind == 0:    # sphere
+            r = np.sqrt(1 - z * z)
+            p = np.stack([r * np.cos(th), r * np.sin(th), z], 1)
+            nrm = p.copy()
+        elif kind == 1:  # cylinder side
+            p = np.stack([np.cos(th), np.sin(th), z], 1)
+            nrm = np.stack([np.cos(th), np.sin(th), np.zeros(n)], 1)
+        else:            # box surface
+            p = rs.uniform(-1, 1, (n, 3))
+            ax, sg = rs.randint(0, 3, n), rs.choice([-1.0, 1.0], n)
+            p[rows, ax] = sg
+            nrm = np.zeros((n, 3))
+            nrm[rows, ax] = sg
+        h = 1.0 + 0.25 * (k // 3)  # stretch z by h: the normals scale by 1 / h there
+        p[:, 2] *= h
+        nrm[:, 2] /= h
+        nrm /= np.linalg.norm(nrm, axis=1, keepdims=True)
+        a = rs.uniform(0, 2 * np.pi)
+        rot = np.array([[np.cos(a), -np.sin(a), 0], [np.sin(a), np.cos(a), 0], [0, 0, 1]])
+        p, nrm = p @ rot.T, nrm @ rot.T
+        parts = offsets[k + 1] - offsets[k]
+        zq = (p[:, 2] - p[:, 2].min()) / max(np.ptp(p[:, 2]), 1e-12)
+        label[i] = offsets[k] + np.minimum((zq * parts).astype(np.int64), parts - 1)
+        pts[i, :, :3] = pc_normalize(p * rs.uniform(0.8, 1.25))
+        pts[i, :, 3:] = nrm
+    return pts, cls.astype(np.int64), label
+
+
 # ---- BASELINE.json configs ---------------------------------------------------------------------
 CFG2_SSG_SA = dict(name="cfg2_ssg_sa_layer", b=32, n=4096, npoint=1024, nsample=32, radius=0.1, dist="U", seed=100)
 CFG1_FPS_CPU = dict(name="cfg1_fps_plumbing", b=8, n=1024, npoint=512, dist="U", seed=100)

@@ -11,12 +11,16 @@ min(0.99, 1 - 0.5 * 0.5^(samples/200000)).
     python tools/train_ddp_demo.py --steps 20                                   # one GPU
     python tools/train_ddp_demo.py --steps 30 --amp bf16                        # bf16 autocast
     python tools/train_ddp_demo.py --steps 5 --deterministic                    # reproducible: prints a weights hash
+    python tools/train_ddp_demo.py --model part_seg_msg --ragged --steps 30     # part segmentation, variable sizes
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 \
         tools/train_ddp_demo.py --steps 20                                      # one rank per GPU
 
 Data is synthetic (no dataset in this image): each cloud is one of `num_class` parametric shapes
 (sphere, box, cylinder, cone, torus ... scaled/rotated/jittered like utils/provider.py), so the
-loss has something to learn and the demo can assert that it goes down.
+loss has something to learn and the demo can assert that it goes down.  The part segmentation models
+(part_seg, part_seg_msg) train on workloads.part_shapes instead: (B, N, 6) points with normals, one
+of the 16 ShapeNet categories each, its parts the height bands of the shape.  --ragged (segmentation
+models) draws each cloud's length from U[N/2, N], fills the padding rows with NaN and passes lengths=.
 """
 from __future__ import annotations
 
@@ -32,7 +36,7 @@ import torch
 import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from pointnet2_b200 import nets  # noqa: E402
+from pointnet2_b200 import nets, workloads as W  # noqa: E402
 from pointnet2_b200.parallel import shard_batch  # noqa: E402
 
 
@@ -71,7 +75,7 @@ def synthetic_shapes(batch: int, num_point: int, num_class: int, rs: np.random.R
 
 def main() -> None:
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=["cls_ssg", "cls_msg", "sem_seg"], default="cls_ssg")
+    ap.add_argument("--model", choices=["cls_ssg", "cls_msg", "sem_seg", "part_seg", "part_seg_msg"], default="cls_ssg")
     ap.add_argument("--batch", type=int, default=32, help="GLOBAL batch (split across ranks)")
     ap.add_argument("--num-point", type=int, default=1024)
     ap.add_argument("--num-class", type=int, default=10)
@@ -83,7 +87,9 @@ def main() -> None:
                     help="mixed precision: torch.autocast in bfloat16, or float16 with a GradScaler")
     ap.add_argument("--deterministic", action="store_true",
                     help="torch.use_deterministic_algorithms(True): run-to-run identical weights; prints their SHA-256")
+    ap.add_argument("--ragged", action="store_true", help="cloud lengths from U[N/2, N], NaN padding, passed as lengths=")
     args = ap.parse_args()
+    part = args.model in ("part_seg", "part_seg_msg")
     if args.deterministic:
         os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")  # read when cuBLAS starts: before the first matmul
         torch.use_deterministic_algorithms(True)
@@ -105,6 +111,10 @@ def main() -> None:
         model = nets.PointNet2ClsSSG(args.num_class)
     elif args.model == "cls_msg":
         model = nets.PointNet2ClsMSG(args.num_class)
+    elif args.model == "part_seg":  # 50 ShapeNet parts: --num-class does not apply
+        model = nets.PointNet2PartSeg()
+    elif args.model == "part_seg_msg":
+        model = nets.PointNet2PartSegMSG()
     else:
         model = nets.PointNet2SemSeg(args.num_class)
     model = model.to(dev)
@@ -121,17 +131,33 @@ def main() -> None:
         for g in opt.param_groups:
             g["lr"] = lr
         nets.set_bn_momentum(model, min(0.99, 1 - 0.5 * 0.5 ** (seen // args.decay_step)))
-        xyz_np, lab_np = synthetic_shapes(args.batch, args.num_point, args.num_class, rs)
+        if part:  # (B, N, 6) points with normals, per-point part labels, and the category
+            xyz_np, lab_np, part_np = W.part_shapes(args.batch, args.num_point, int(rs.randint(1 << 30)), nets.PART_OFFSETS)
+        else:
+            xyz_np, lab_np = synthetic_shapes(args.batch, args.num_point, args.num_class, rs)
+        lengths = None
+        if args.ragged:
+            len_np = rs.randint(args.num_point // 2, args.num_point + 1, args.batch)
+            for i, l in enumerate(len_np):
+                xyz_np[i, l:] = np.nan  # never read: only the first lengths[i] rows of cloud i are real
+            lengths = shard_batch(torch.from_numpy(len_np.astype(np.int32)), world, rank).to(dev, non_blocking=True)
         xyz = shard_batch(torch.from_numpy(xyz_np), world, rank).to(dev, non_blocking=True).contiguous()
         lab = shard_batch(torch.from_numpy(lab_np), world, rank).to(dev, non_blocking=True)
+        if part:
+            lab_part = shard_batch(torch.from_numpy(part_np), world, rank).to(dev, non_blocking=True)
         torch.cuda.synchronize(dev)
         t0 = time.perf_counter()
         net.train()
         with torch.autocast(device_type="cuda", dtype=amp_dtype, enabled=amp_dtype is not None):
-            pred, _ = net(xyz)
-            if args.model == "sem_seg":  # per-point labels: the cloud's class everywhere, unit weights
+            if args.model == "part_seg_msg":
+                pred, _ = net(xyz, lab, lengths=lengths)
+            else:
+                pred, _ = net(xyz, lengths=lengths)
+            if part:
+                loss = nets.part_seg_loss(pred, lab_part, lengths=lengths)
+            elif args.model == "sem_seg":  # per-point labels: the cloud's class everywhere, unit weights
                 lab_pt = lab[:, None].expand(-1, args.num_point)
-                loss = nets.sem_seg_loss(pred, lab_pt, torch.ones_like(lab_pt, dtype=torch.float32))
+                loss = nets.sem_seg_loss(pred, lab_pt, torch.ones_like(lab_pt, dtype=torch.float32), lengths=lengths)
             else:
                 loss = nets.cls_loss(pred, lab)
         opt.zero_grad(set_to_none=True)
@@ -167,8 +193,9 @@ def main() -> None:
         out = {"model": args.model, "amp": args.amp, "world": world, "global_batch": args.batch, "num_point": args.num_point,
                "steps": args.steps, "loss_first": first, "loss_last": last, "loss_decreased": last < first,
                "weights_identical_across_ranks": same, "ms_per_step_wallclock": 1e3 * float(np.median(steady)),
-               "clouds_per_s": args.batch / float(np.median(steady)), "data": "synthetic parametric shapes",
-               "deterministic": args.deterministic}
+               "clouds_per_s": args.batch / float(np.median(steady)),
+               "data": "synthetic part shapes" if part else "synthetic parametric shapes",
+               "deterministic": args.deterministic, "ragged": args.ragged}
         if args.deterministic:
             h = hashlib.sha256()
             for p in model.parameters():
