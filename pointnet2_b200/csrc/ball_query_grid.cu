@@ -311,7 +311,8 @@ static int ball_grid_build(int b, int n, float radius, int nsample, const float*
                            size_t workspace_bytes, cudaStream_t st) {
     if (b <= 0 || n <= 0 || nsample <= 0 || !(radius > 0.0f) || !xyz1 || !workspace) return (int)cudaErrorInvalidValue;
     const size_t need = pn2_query_ball_point_workspace_bytes(b, n);
-    if (need == 0 || workspace_bytes < need || b > 65535) return (int)cudaErrorInvalidValue;
+    // radius <= 1e-20: no distance passes the reference's max(d, 1e-20) < radius test, and the query half refuses it
+    if (need == 0 || workspace_bytes < need || b > 65535 || pn2_ball_threshold(radius) < 0.0f) return (int)cudaErrorInvalidValue;
     bq_grid_build_kernel<<<b, kGbThreads, 0, st>>>(n, radius, nsample, xyz1, static_cast<int*>(workspace),
                                                    grid_ws_ints_per_cloud(n), lengths);
     return finish_launch();

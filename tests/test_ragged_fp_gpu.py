@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 import torch
 
+import numerics as NUM
 from oracle import oracle as O
 from pointnet2_b200 import _lib, tf_interpolate, workloads as W
 from pointnet2_b200.layers import SharedMLP, row_mask
@@ -24,6 +25,7 @@ pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FAR = np.float32(50.0)
+FMT = {torch.float32: "f32", torch.bfloat16: "bf16", torch.float16: "f16"}
 
 
 def pad(x, lengths, kind):
@@ -168,7 +170,7 @@ GRAD_CASES = [
 ]
 
 
-@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16])
+@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16, torch.float16])
 @pytest.mark.parametrize("b,n,m,c,lengths", GRAD_CASES)
 def test_three_interpolate_and_its_deterministic_gradient(dev, b, n, m, c, lengths, dtype):
     idx, weight = interp_inputs(b, n, m, lengths, 21, dev)
@@ -188,18 +190,23 @@ def test_three_interpolate_and_its_deterministic_gradient(dev, b, n, m, c, lengt
     want = three_interpolate(T(pts, dev).to(dtype), T(idx, dev), T(weight, dev))
     assert torch.equal(bits(out[mask]), bits(want[mask]))
     assert_filler(out, mask, 0)
-    # the gradient of the call on each truncated cloud, and the oracle's ordered sum
-    long_lists = m < 16
+    # the gradient of the call on each truncated cloud, and the oracle's ordered sum of the upcast gradient, rounded
+    # once: bit for bit on lists of up to 256 entries, within the float64 bound on longer ones (summed in 8 pieces)
+    fmt = FMT[dtype]
+    gq = NUM.quantize(gout, fmt)
     for k, l in enumerate(lengths):
         p = T(pts[k:k + 1], dev).to(dtype).requires_grad_(True)
         three_interpolate(p, T(idx[k:k + 1, :l], dev), T(weight[k:k + 1, :l], dev)).backward(T(gout[k:k + 1, :l], dev).to(dtype))
         assert torch.equal(bits(grad[k:k + 1]), bits(p.grad)), f"length {l}"
-        if dtype == torch.float32:
-            o = O.oracle_three_interpolate_grad((1, m, c), idx[k:k + 1, :l], weight[k:k + 1, :l], gout[k:k + 1, :l])
-            if long_lists:  # summed in 8 pieces: deterministic, equal to the sequential sum up to rounding
-                np.testing.assert_allclose(grad[k:k + 1].cpu().numpy(), o, rtol=1e-5, atol=1e-4)
-            else:
-                np.testing.assert_array_equal(grad[k:k + 1].cpu().numpy().view(np.int32), o.view(np.int32), err_msg=f"length {l}")
+        o = O.oracle_three_interpolate_grad((1, m, c), idx[k:k + 1, :l], weight[k:k + 1, :l], gq[k:k + 1, :l])[0]
+        terms = weight[k, :l].astype(np.float64).reshape(-1, 1) * np.repeat(gq[k, :l].astype(np.float64), 3, axis=0)
+        ref, mass, count = NUM.scatter64(m, idx[k, :l], terms)
+        got = grad[k].float().cpu().numpy()
+        short = count <= 256
+        assert (m < 16) == (not short.all()), "the cases with m < 16 are the ones with lists longer than 256 entries"
+        want = NUM.quantize(o, fmt)
+        np.testing.assert_array_equal(got[short].view(np.int32), want[short].view(np.int32), err_msg=f"length {l}")
+        assert NUM.within_bound(got, ref, mass, np.maximum(count, 1)[:, None], fmt).all(), f"length {l}"
 
 
 @pytest.mark.parametrize("b,n,m,c,lengths", [GRAD_CASES[0], GRAD_CASES[3]])
@@ -210,9 +217,11 @@ def test_three_interpolate_atomic_gradient(dev, monkeypatch, b, n, m, c, lengths
     ii, ww = poison_rows(idx, weight, lengths, "poison", m)
     p = T(pts, dev).requires_grad_(True)
     three_interpolate(p, T(ii, dev), T(ww, dev), lengths=lengths).backward(T(pad(gout, lengths, "poison"), dev))
-    for k, l in enumerate(lengths):
-        o = O.oracle_three_interpolate_grad((1, m, c), idx[k:k + 1, :l], weight[k:k + 1, :l], gout[k:k + 1, :l])
-        np.testing.assert_allclose(p.grad[k:k + 1].cpu().numpy(), o, rtol=1e-5, atol=1e-5)
+    got = p.grad.cpu().numpy()
+    for k, l in enumerate(lengths):  # float atomics: any order of the float32 sum, within the float64 bound
+        terms = weight[k, :l].astype(np.float64).reshape(-1, 1) * np.repeat(gout[k, :l].astype(np.float64), 3, axis=0)
+        ref, mass, count = NUM.scatter64(m, idx[k, :l], terms)
+        assert NUM.within_bound(got[k], ref, mass, np.maximum(count, 1)[:, None], "f32").all(), f"length {l}"
 
 
 def test_deterministic_gradient_of_full_lengths_equals_todays(dev):
