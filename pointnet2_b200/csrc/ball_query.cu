@@ -22,6 +22,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <atomic>
+
 #include "pn2_common.cuh"
 
 namespace pn2 {
@@ -30,37 +32,6 @@ constexpr int kBqThreads = 256;
 constexpr int kBqTile = 2048;             // data points per shared-memory tile
 constexpr int kBqPairs = kBqTile / 2;     // stored as pairs: (x0,x1,y0,y1) + (z0,z1)
 constexpr int kBqUnroll = 2;              // pairs per lane per step (4 points)
-
-// FP32 pair arithmetic: two points per helper call, IEEE round-to-nearest per half, i.e.
-// bit-identical to the scalar contraction pattern (sm_90 has no packed FP32x2 instructions: each
-// helper issues two scalar operations)
-__device__ __forceinline__ unsigned long long bq_pack(float a, float b) {
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-    return r;
-}
-__device__ __forceinline__ void bq_unpack(unsigned long long v, float& a, float& b) {
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
-}
-__device__ __forceinline__ unsigned long long bq_sub2(unsigned long long a, unsigned long long b) {
-    float a0, a1, b0, b1;
-    bq_unpack(a, a0, a1);
-    bq_unpack(b, b0, b1);
-    return bq_pack(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
-}
-__device__ __forceinline__ unsigned long long bq_mul2(unsigned long long a, unsigned long long b) {
-    float a0, a1, b0, b1;
-    bq_unpack(a, a0, a1);
-    bq_unpack(b, b0, b1);
-    return bq_pack(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
-}
-__device__ __forceinline__ unsigned long long bq_fma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-    float a0, a1, b0, b1, c0, c1;
-    bq_unpack(a, a0, a1);
-    bq_unpack(b, b0, b1);
-    bq_unpack(c, c0, c1);
-    return bq_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
-}
 
 template <int G>
 __global__ void __launch_bounds__(kBqThreads)
@@ -95,7 +66,7 @@ ball_query_kernel(int n, int m, float thr, int nsample, const float* __restrict_
         qy = qp[1];
         qz = qp[2];
     }
-    const unsigned long long QX = bq_pack(qx, qx), QY = bq_pack(qy, qy), QZ = bq_pack(qz, qz);
+    const unsigned long long QX = f2_pack(qx, qx), QY = f2_pack(qy, qy), QZ = f2_pack(qz, qz);
     int* __restrict__ row = idx + ((size_t)cloud * m + (valid ? q : 0)) * nsample;
 
     int cnt = valid ? 0 : nsample;  // out-of-range groups count as already full
@@ -131,10 +102,10 @@ ball_query_kernel(int n, int m, float thr, int nsample, const float* __restrict_
             for (int u = 0; u < kBqUnroll; ++u) {
                 const ulonglong2 xy = s_xy[p + u * G + g];
                 const unsigned long long zz = s_z[p + u * G + g];
-                const unsigned long long dx = bq_sub2(QX, xy.x), dy = bq_sub2(QY, xy.y), dz = bq_sub2(QZ, zz);
-                const unsigned long long d = bq_fma2(dz, dz, bq_fma2(dx, dx, bq_mul2(dy, dy)));
+                const unsigned long long dx = f2_sub(QX, xy.x), dy = f2_sub(QY, xy.y), dz = f2_sub(QZ, zz);
+                const unsigned long long d = f2_fma(dz, dz, f2_fma(dx, dx, f2_mul(dy, dy)));
                 float d0, d1;
-                bq_unpack(d, d0, d1);
+                f2_unpack(d, d0, d1);
                 h[u][0] = !(d0 > thr);
                 h[u][1] = !(d1 > thr);
                 any |= h[u][0] | h[u][1];
@@ -180,16 +151,17 @@ static int launch_bq(int b, int n, int m, float thr, int nsample, const float* x
     return finish_launch();
 }
 
-static int g_bq_group = 0;  // experiment override (pn2_set_bq_group, or PN2_BQ_GROUP env read once)
+// experiment override of the lanes per query (0: automatic): pn2_set_bq_group, or PN2_BQ_GROUP, applied at the first query
+static std::atomic<int> g_bq_group{0};
 
 static int pick_group(int b, int m) {
-    static bool init = false;
-    if (!init) {
-        const char* e = getenv("PN2_BQ_GROUP");
-        if (e) g_bq_group = atoi(e);
-        init = true;
-    }
-    if (g_bq_group > 0) return g_bq_group;
+    static const bool env_applied = [] {  // thread-safe: runs once
+        if (const char* e = getenv("PN2_BQ_GROUP")) g_bq_group.store(atoi(e), std::memory_order_relaxed);
+        return true;
+    }();
+    (void)env_applied;
+    const int forced = g_bq_group.load(std::memory_order_relaxed);
+    if (forced > 0) return forced;
     // enough lanes to fill every SM's 2048 thread slots (more, smaller groups win until the machine
     // is full)
     const long long queries = (long long)b * m;
@@ -248,7 +220,7 @@ float pn2_ball_threshold(float radius) {
     return f;
 }
 
-void pn2_set_bq_group(int lanes_per_query) { pn2::g_bq_group = lanes_per_query; }
+void pn2_set_bq_group(int lanes_per_query) { pn2::g_bq_group.store(lanes_per_query, std::memory_order_relaxed); }
 
 int pn2_query_ball_point(int b, int n, int m, float radius, int nsample, const float* xyz1, const float* xyz2,
                          int* idx, int* pts_cnt, void* stream) {

@@ -15,13 +15,14 @@
 // the build kernel and served by the brute-force kernel instead.
 #include <math.h>
 
+#include <atomic>
+
 #include "pn2_common.cuh"
 
 namespace pn2 {
 
 constexpr int kGbThreads = 1024;   // build: one CTA per cloud
 constexpr int kGqThreads = 256;    // query: 8 warps, one query per warp
-constexpr int kGridMaxDim = 16;    // cells per axis
 constexpr int kGridMaxN = 1 << 20;   // workspace sizing only: larger clouds take the brute-force path
 constexpr int kGridMinN = 2048;      // below this the brute-force kernel is already latency-bound
 constexpr float kGridDenseFrac = 0.9f;  // local-density estimate of points per ball above this fraction of nsample: early-exit scan wins
@@ -33,28 +34,10 @@ __host__ __device__ inline size_t grid_ws_ints_per_cloud(int n) {
     return (size_t)kGridParamInts + (size_t)n + (size_t)kGridMaxDim * kGridMaxDim * kGridMaxDim + 1;
 }
 
-__device__ __forceinline__ int cell_coord(float x, float origin, float inv_h, int dim) {
-    // monotone in x; clamped so that out-of-box queries map to the border cells +-1
-    float f = floorf(__fmul_rn(__fsub_rn(x, origin), inv_h));
-    f = fminf(fmaxf(f, -1.0f), (float)dim);
-    return (int)f;
-}
-
-__device__ __forceinline__ float wmin(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fminf(v, __shfl_xor_sync(kFullMask, v, o));
-    return v;
-}
-__device__ __forceinline__ float wmax(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(kFullMask, v, o));
-    return v;
-}
-
 __global__ void __launch_bounds__(kGbThreads, 1)
 bq_grid_build_kernel(int n, float radius, int nsample, const float* __restrict__ xyz1, int* __restrict__ ws, size_t ws_stride,
                      const int* __restrict__ lengths) {
-    constexpr int T = kGbThreads, NW = T / 32;
+    constexpr int T = kGbThreads;
     constexpr int MAXC = kGridMaxDim * kGridMaxDim * kGridMaxDim;
     __shared__ float s_red[6][32];
     __shared__ int s_cnt[MAXC];     // per-cell count, then the scatter cursor
@@ -68,71 +51,29 @@ bq_grid_build_kernel(int n, float radius, int nsample, const float* __restrict__
     int* __restrict__ cell_start = sorted_idx + n;
     n = cloud_length(lengths, cloud, n);  // the layout above is sized for the stride; from here on n is the cloud's length
 
-    float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
-    for (int k = tid; k < n; k += T) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            const float v = __ldg(pts + 3 * (size_t)k + c);
-            mn[c] = fminf(mn[c], v);
-            // a NaN coordinate (fminf/fmaxf would ignore it) must disable the grid: the reference
-            // counts a NaN point as a hit in EVERY ball (fmaxf(NaN,1e-20f) < radius), which only the
-            // brute-force scan reproduces; an infinite box does that (finite_box below)
-            mx[c] = (v == v) ? fmaxf(mx[c], v) : INFINITY;
-        }
-    }
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        const float a = wmin(mn[c]), b = wmax(mx[c]);
-        if (lane == 0) {
-            s_red[c][warp] = a;
-            s_red[3 + c][warp] = b;
-        }
-    }
-    for (int c = tid; c < MAXC; c += T) s_cnt[c] = 0;
-    if (tid == 0) s_heavy = 0;
-    __syncthreads();
-    float ext[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        mn[c] = wmin(lane < NW ? s_red[c][lane] : INFINITY);
-        mx[c] = wmax(lane < NW ? s_red[3 + c][lane] : -INFINITY);
-        ext[c] = mx[c] - mn[c];
-    }
-    const float emax = fmaxf(fmaxf(ext[0], ext[1]), ext[2]);
-    // cell edge: at least 1.01 * radius (any point within the radius of a query is then at most
-    // one cell away on every axis, with margin for the rounding of the cell function), and
-    // large enough for kGridMaxDim cells to span the box
-    float h = fmaxf(1.01f * radius, emax / (float)(kGridMaxDim - 1));
-    const bool finite_box = (emax >= 0.f) && (emax < 1e30f) && (h > 0.f) && (h < 1e30f);
-    if (!finite_box) h = 1.0f;
-    const float inv_h = 1.0f / h;
-    int dims[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-        int d = finite_box ? (int)floorf(ext[c] * inv_h) + 1 : 1;
-        dims[c] = min(max(d, 1), kGridMaxDim);
-    }
-    const int ncell = dims[0] * dims[1] * dims[2];
-    // neighbourhood / grid volume: use the grid only when it prunes at least ~70 % of the cloud
-    const int nb = min(dims[0], 3) * min(dims[1], 3) * min(dims[2], 3);
+    const GridGeometry geo = grid_geometry(pts, n, radius, s_red, [&] {
+        for (int c = tid; c < MAXC; c += T) s_cnt[c] = 0;
+        if (tid == 0) s_heavy = 0;
+    });
     // expected points per ball if the cloud were uniform in its box: when that reaches nsample the
     // ordered scan of the brute-force kernel exits early and beats the neighbourhood search
-    const float vol = fmaxf(ext[0], h) * fmaxf(ext[1], h) * fmaxf(ext[2], h);
+    const float vol = fmaxf(geo.ext[0], geo.h) * fmaxf(geo.ext[1], geo.h) * fmaxf(geo.ext[2], geo.h);
     const float expect = (float)n * 4.18879f * radius * radius * radius / vol;
-    bool use_grid = finite_box && n >= kGridMinN && 10 * nb <= 3 * ncell && expect < 0.75f * (float)nsample;
+    // neighbourhood / grid volume: use the grid only when it prunes at least ~70 % of the cloud
+    bool use_grid = geo.finite_box && n >= kGridMinN && 10 * geo.nb <= 3 * geo.ncell && expect < 0.75f * (float)nsample;
     if (use_grid) {  // CTA-uniform
         // pass 1: histogram
         for (int k = tid; k < n; k += T) {
             int cc[3];
 #pragma unroll
             for (int c = 0; c < 3; ++c)
-                cc[c] = min(max(cell_coord(__ldg(pts + 3 * (size_t)k + c), mn[c], inv_h, dims[c]), 0), dims[c] - 1);
-            atomicAdd(&s_cnt[(cc[2] * dims[1] + cc[1]) * dims[0] + cc[0]], 1);
+                cc[c] = min(max(grid_cell(__ldg(pts + 3 * (size_t)k + c), geo.mn[c], geo.inv_h, geo.dims[c]), 0), geo.dims[c] - 1);
+            atomicAdd(&s_cnt[(cc[2] * geo.dims[1] + cc[1]) * geo.dims[0] + cc[0]], 1);
         }
         __syncthreads();
         // exclusive scan over the cells: each thread owns a contiguous run of cells
-        const int per = (ncell + T - 1) / T;
-        const int c0 = min(tid * per, ncell), c1 = min(c0 + per, ncell);
+        const int per = (geo.ncell + T - 1) / T;
+        const int c0 = min(tid * per, geo.ncell), c1 = min(c0 + per, geo.ncell);
         int local = 0, heavy = 0;
         float sq = 0.f;
         for (int c = c0; c < c1; ++c) {
@@ -149,35 +90,19 @@ bq_grid_build_kernel(int n, float radius, int nsample, const float* __restrict__
         for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(kFullMask, sq, o);
         if (lane == 0) s_red[0][warp] = sq;
         if (heavy) s_heavy = 1;
-        int incl = local;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int v = __shfl_up_sync(kFullMask, incl, o);
-            if (lane >= o) incl += v;
-        }
-        if (lane == 31) s_wsum[warp] = incl;
-        __syncthreads();
-        // exclusive prefix over the warp totals (every warp scans the 32 totals with shuffles)
-        int wv = (lane < NW) ? s_wsum[lane] : 0, winc = wv;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int v = __shfl_up_sync(kFullMask, winc, o);
-            if (lane >= o) winc += v;
-        }
-        const int wprefix = __shfl_sync(kFullMask, winc - wv, warp);
-        int run = wprefix + incl - local;
+        int run = cta_exclusive_sum_1024(local, s_wsum);
         for (int c = c0; c < c1; ++c) {
             const int cntc = s_cnt[c];
             cell_start[c] = run;
             s_cnt[c] = run;  // becomes the scatter cursor
             run += cntc;
         }
-        if (tid == 0) cell_start[ncell] = n;
+        if (tid == 0) cell_start[geo.ncell] = n;
         __syncthreads();
-        float sqsum = (lane < NW) ? s_red[0][lane] : 0.f;
+        float sqsum = s_red[0][lane];
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) sqsum += __shfl_xor_sync(kFullMask, sqsum, o);
-        const float rh = radius * inv_h;
+        const float rh = radius * geo.inv_h;
         const float expect_local = 4.18879f * rh * rh * rh * sqsum / (float)n;
         use_grid = (s_heavy == 0) && (expect_local < kGridDenseFrac * (float)nsample);
         if (use_grid) {
@@ -186,17 +111,17 @@ bq_grid_build_kernel(int n, float radius, int nsample, const float* __restrict__
                 int cc[3];
 #pragma unroll
                 for (int c = 0; c < 3; ++c)
-                    cc[c] = min(max(cell_coord(__ldg(pts + 3 * (size_t)k + c), mn[c], inv_h, dims[c]), 0), dims[c] - 1);
-                const int pos = atomicAdd(&s_cnt[(cc[2] * dims[1] + cc[1]) * dims[0] + cc[0]], 1);
+                    cc[c] = min(max(grid_cell(__ldg(pts + 3 * (size_t)k + c), geo.mn[c], geo.inv_h, geo.dims[c]), 0), geo.dims[c] - 1);
+                const int pos = atomicAdd(&s_cnt[(cc[2] * geo.dims[1] + cc[1]) * geo.dims[0] + cc[0]], 1);
                 sorted_idx[pos] = k;
             }
         }
     }
     if (tid == 0) {
         params[0] = use_grid ? 1 : 0;
-        params[1] = dims[0]; params[2] = dims[1]; params[3] = dims[2];
-        params[4] = __float_as_int(mn[0]); params[5] = __float_as_int(mn[1]); params[6] = __float_as_int(mn[2]);
-        params[7] = __float_as_int(inv_h);
+        params[1] = geo.dims[0]; params[2] = geo.dims[1]; params[3] = geo.dims[2];
+        params[4] = __float_as_int(geo.mn[0]); params[5] = __float_as_int(geo.mn[1]); params[6] = __float_as_int(geo.mn[2]);
+        params[7] = __float_as_int(geo.inv_h);
     }
 }
 
@@ -225,7 +150,7 @@ bq_grid_query_kernel(int n, int m, float thr, int nsample, const float* __restri
     int* __restrict__ row = idx + ((size_t)cloud * m + q) * nsample;
     const unsigned lt_mask = (1u << lane) - 1u;
 
-    const int cx = cell_coord(qx, ox, inv_h, dx), cy = cell_coord(qy, oy, inv_h, dy), cz = cell_coord(qz, oz, inv_h, dz);
+    const int cx = grid_cell(qx, ox, inv_h, dx), cy = grid_cell(qy, oy, inv_h, dy), cz = grid_cell(qz, oz, inv_h, dz);
     const int x0 = max(cx - 1, 0), x1 = min(cx + 1, dx - 1);
     // the neighbourhood is 9 rows (dy, dz in {-1,0,1}) of up to 3 x-adjacent cells, i.e. 9 contiguous
     // candidate ranges; lanes 3r..3r+2 walk range r with stride 3
@@ -304,7 +229,7 @@ bq_grid_query_kernel(int n, int m, float thr, int nsample, const float* __restri
     if (lane == 0) pts_cnt[(size_t)cloud * m + q] = cnt;
 }
 
-static int g_bq_mode = 0;  // 0 auto (shared-memory grid kernel when the cloud fits it), 1 brute force only, 2 the global-memory grid path
+static std::atomic<int> g_bq_mode{0};  // 0 auto (shared-memory grid kernel when the cloud fits it), 1 brute force only, 2 the global-memory grid path
 
 // The grid build / query / whole-path entries below, on the clouds' first lengths[b] points (lengths == NULL: all n).
 static int ball_grid_build(int b, int n, float radius, int nsample, const float* xyz1, const int* lengths, void* workspace,
@@ -347,14 +272,15 @@ int query_ball_point_ws(int b, int n, int m, float radius, int nsample, const fl
     // clouds that fit the shared-memory grid of sa_fused.cu (n <= 9700): one launch that builds the grid in shared
     // memory and serves the queries from it — one launch instead of build + query + brute-force back to back from
     // n = 2048 up; no workspace needed
-    if (g_bq_mode == 0 && n >= kGridMinN && pn2_ball_group_fits(n) && thr >= 0.0f) {
+    const int mode = g_bq_mode.load(std::memory_order_relaxed);
+    if (mode == 0 && n >= kGridMinN && pn2_ball_group_fits(n) && thr >= 0.0f) {
         // ... when there are queries enough to pay for the grids (every CTA builds its own): below ~4096 queries the
         // packed brute-force kernel is ahead (r2_report.json, cfg4 SA1024 at B = 2: 2048 queries x 8192 points,
         // 0.0246 ms against 0.0287)
         if ((long long)b * m >= 4096) return ball_group(b, n, m, radius, nsample, xyz1, lengths, xyz2, idx, pts_cnt, nullptr, 0, st);
         return query_ball_point_brute(b, n, m, radius, nsample, xyz1, lengths, xyz2, idx, pts_cnt, st);
     }
-    if (g_bq_mode == 1 || !workspace || need == 0 || workspace_bytes < need || thr < 0.0f || b > 65535)
+    if (mode == 1 || !workspace || need == 0 || workspace_bytes < need || thr < 0.0f || b > 65535)
         return query_ball_point_brute(b, n, m, radius, nsample, xyz1, lengths, xyz2, idx, pts_cnt, st);
     int rc = ball_grid_build(b, n, radius, nsample, xyz1, lengths, workspace, workspace_bytes, st);
     if (rc) return rc;
@@ -365,7 +291,7 @@ int query_ball_point_ws(int b, int n, int m, float radius, int nsample, const fl
 
 extern "C" {
 
-void pn2_set_bq_mode(int mode) { pn2::g_bq_mode = mode; }
+void pn2_set_bq_mode(int mode) { pn2::g_bq_mode.store(mode, std::memory_order_relaxed); }
 
 size_t pn2_query_ball_point_workspace_bytes(int b, int n) {
     if (b <= 0 || n < pn2::kGridMinN || n > pn2::kGridMaxN) return 0;

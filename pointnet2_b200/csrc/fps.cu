@@ -120,37 +120,6 @@ __device__ __forceinline__ void fps_step(const float (&px)[P], const float (&py)
 // as soon as every CTA of this grid has got here (SASS: PREEXIT).  A no-op for ordinary launches.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-// ---- FP32 pairs: two points per helper call, each half rounded to nearest on its own, so bit-identical
-// to d2_fma_pattern on either half.  sm_90 has no packed FP32x2 instructions: every helper issues two
-// scalar FADD / FMUL / FFMA (the explicit .rn operations are never contracted) ------------------------
-__device__ __forceinline__ unsigned long long f2_pack(float a, float b) {
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-    return r;
-}
-__device__ __forceinline__ void f2_unpack(unsigned long long v, float& a, float& b) {
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
-}
-__device__ __forceinline__ unsigned long long f2_sub(unsigned long long a, unsigned long long b) {
-    float a0, a1, b0, b1;
-    f2_unpack(a, a0, a1);
-    f2_unpack(b, b0, b1);
-    return f2_pack(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
-}
-__device__ __forceinline__ unsigned long long f2_mul(unsigned long long a, unsigned long long b) {
-    float a0, a1, b0, b1;
-    f2_unpack(a, a0, a1);
-    f2_unpack(b, b0, b1);
-    return f2_pack(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
-}
-__device__ __forceinline__ unsigned long long f2_fma(unsigned long long a, unsigned long long b, unsigned long long c) {
-    float a0, a1, b0, b1, c0, c1;
-    f2_unpack(a, a0, a1);
-    f2_unpack(b, b0, b1);
-    f2_unpack(c, c0, c1);
-    return f2_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
-}
-
 // Packed pair update: the running minima of the H register-resident pairs (X, Y, Z)[h] = points 2h, 2h + 1 against
 // the last pick (x1, y1, z1), d2_fma_pattern on both halves.
 template <int H, int P>
@@ -1004,29 +973,6 @@ static int override_chain(int threads, int builtin) {
 static unsigned long long pack_cfg(int threads, int ppt, int cluster) {
     if (threads <= 0) return 0ull;
     return ((unsigned long long)threads << 40) | ((unsigned long long)(ppt & 0xfffff) << 20) | (unsigned long long)(cluster + 64);
-}
-
-// cudaFuncSetAttribute once per (kernel instantiation, device), not on every launch
-struct AttrOnce {
-    std::atomic<unsigned long long> done{0ull};  // bit d: attributes set on device d (< 64)
-};
-template <typename K>
-static cudaError_t ensure_attrs(AttrOnce& once, K kern, size_t dyn, bool nonportable_cluster) {
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    const unsigned long long bit = 1ull << (dev & 63);
-    if (dev < 64 && (once.done.load(std::memory_order_acquire) & bit)) return cudaSuccess;
-    if (dyn > 40 * 1024) {  // static + dynamic beyond the 48 KB default needs the opt-in
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
-        if (e != cudaSuccess) return e;
-    }
-    if (nonportable_cluster) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-        if (e != cudaSuccess) return e;
-    }
-    if (dev < 64) once.done.fetch_or(bit, std::memory_order_release);
-    return cudaSuccess;
 }
 
 template <int P, int T, int V>

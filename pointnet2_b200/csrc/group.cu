@@ -22,8 +22,6 @@ namespace pn2 {
 
 constexpr int kCopyThreads = 256;
 
-static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
 // ---- gather_point: out[b,j,:] = inp[b,idx[b,j],:] (3 floats) -----------------------------------
 __global__ void __launch_bounds__(kCopyThreads)
 gather_point_kernel(int n, int m, long long total, const float* __restrict__ inp, const int* __restrict__ idx,
@@ -55,30 +53,17 @@ gather_point_grad_kernel(int n, int m, long long total, const float* __restrict_
 
 // ---- group_point, vector path: c % 4 == 0, 16-byte aligned bases -------------------------------
 // One thread per output float4.  rows = b*m*nsample flat rows, rows_per_cloud = m*nsample.
-template <typename IndexT, int U>
+template <typename IndexT>
 __global__ void __launch_bounds__(kCopyThreads)
 group_point_vec4_kernel(int n, int c4, IndexT rows_per_cloud, IndexT total_vec, const float4* __restrict__ points,
                         const int* __restrict__ idx, float4* __restrict__ out) {
-    // U independent 16-byte gathers in flight per thread (all loads first, then the streaming stores)
     const IndexT stride = (IndexT)gridDim.x * kCopyThreads;
-    for (IndexT v0 = (IndexT)blockIdx.x * kCopyThreads + threadIdx.x; v0 < total_vec; v0 += stride * U) {
-        float4 val[U];
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const IndexT v = v0 + (IndexT)u * stride;
-            if (v < total_vec) {
-                const IndexT row = v / (IndexT)c4;
-                const int l = (int)(v - row * (IndexT)c4);
-                const IndexT cloud = row / rows_per_cloud;
-                const int a = __ldg(idx + row);
-                val[u] = __ldg(points + ((size_t)cloud * n + a) * c4 + l);
-            }
-        }
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-            const IndexT v = v0 + (IndexT)u * stride;
-            if (v < total_vec) st_stream_f4(out + v, val[u]);
-        }
+    for (IndexT v = (IndexT)blockIdx.x * kCopyThreads + threadIdx.x; v < total_vec; v += stride) {
+        const IndexT row = v / (IndexT)c4;
+        const int l = (int)(v - row * (IndexT)c4);
+        const IndexT cloud = row / rows_per_cloud;
+        const int a = __ldg(idx + row);
+        st_stream_f4(out + v, __ldg(points + ((size_t)cloud * n + a) * c4 + l));
     }
 }
 
@@ -344,7 +329,7 @@ static int launch_group_rows(int b, int n, int c, int m, int nsample, const floa
                                                                                 grouped_xyz, f16);
         return finish_launch();
     }
-    if (std::is_same<T, float>::value && HAS_XYZ && c >= 8 && c <= 64 && c % 4 == 0 && aligned16(points) && aligned16(out)) {
+    if (std::is_same<T, float>::value && HAS_XYZ && c >= 8 && c <= 64 && c % 4 == 0 && aligned_to(points, 16) && aligned_to(out, 16)) {
         // vectorised tail (see group_concat_vec_kernel).  Measured: it wins at C = 64 (30.7 against 35.6 us, cfg4 SA256) and
         // loses to the row kernel below from C = 128 up (C = 320 + 3, S = 64: 125 against 94 us), so only narrow rows take it
         const int c4 = c / 4;
@@ -474,14 +459,19 @@ selection_sort_kernel(int n, int k, long long rows, const float* __restrict__ di
     }
 }
 
-static unsigned grid_for(unsigned long long work_items, unsigned per_block) {
-    unsigned long long blocks = (work_items + per_block - 1) / per_block;
-    const unsigned long long cap = (unsigned long long)num_sms() * 64;  // grid-stride beyond this
-    if (blocks > cap) blocks = cap;
-    if (blocks < 1) blocks = 1;
-    return (unsigned)blocks;
+// Tuning hooks of group_point's 16-byte path, read from the environment once: PN2_GROUP_MODE 0 = row-batched (default),
+// 1 = flat one-vector-per-thread; PN2_GROUP_CTAS = CTAs per SM (default 16).
+struct GroupTuning {
+    int mode, ctas_per_sm;
+};
+static const GroupTuning& group_tuning() {
+    static const GroupTuning t = [] {  // thread-safe: runs once
+        const char* e = getenv("PN2_GROUP_MODE");
+        const char* gq = getenv("PN2_GROUP_CTAS");
+        return GroupTuning{e ? atoi(e) : 0, gq ? atoi(gq) : 16};
+    }();
+    return t;
 }
-
 
 // ---- entry bodies, one per element type T (float, __nv_bfloat16, __half) ----------------------------
 // The 16-byte vector kernels copy bytes, so they serve every T: a row of c elements is c * sizeof(T) / 16 vectors
@@ -491,24 +481,18 @@ static int group_point_impl(int b, int n, int c, int m, int nsample, const T* po
                             cudaStream_t st) {
     const unsigned long long rows = (unsigned long long)b * m * nsample;
     const unsigned long long rpc = (unsigned long long)m * nsample;
-    if (((size_t)c * sizeof(T)) % 16 == 0 && aligned16(points) && aligned16(out)) {
+    if (((size_t)c * sizeof(T)) % 16 == 0 && aligned_to(points, 16) && aligned_to(out, 16)) {
         const int c4 = (int)((size_t)c * sizeof(T) / 16);  // 16-byte vectors per row
         const unsigned long long tv = rows * c4;
-        static int mode = -1, ctas_per_sm = 0;
-        if (mode < 0) {  // tuning hooks: PN2_GROUP_MODE 0 = row-batched (default), 1 = flat one-vector-per-thread
-            const char* e = getenv("PN2_GROUP_MODE");
-            mode = e ? atoi(e) : 0;
-            const char* gq = getenv("PN2_GROUP_CTAS");
-            ctas_per_sm = gq ? atoi(gq) : 16;
-        }
+        const GroupTuning& tune = group_tuning();
         const float4* p4 = reinterpret_cast<const float4*>(points);
         float4* o4 = reinterpret_cast<float4*>(out);
-        if (mode == 0 && rpc < (1ull << 32) && b <= 65535) {
+        if (tune.mode == 0 && rpc < (1ull << 32) && b <= 65535) {
             const int lpr = c4 <= 4 ? 4 : (c4 <= 8 ? 8 : (c4 <= 16 ? 16 : 32));
             constexpr int R = 4;
             const unsigned rows_per_block = (kCopyThreads / 32) * (32 / lpr) * R;
             unsigned gx = (unsigned)((rpc + rows_per_block - 1) / rows_per_block);
-            const unsigned cap = ((unsigned)num_sms() * (unsigned)ctas_per_sm + b - 1) / b;
+            const unsigned cap = ((unsigned)num_sms() * (unsigned)tune.ctas_per_sm + b - 1) / b;
             if (gx > cap) gx = cap;
             if (gx < 1) gx = 1;
             dim3 grid(gx, b, 1);
@@ -519,12 +503,12 @@ static int group_point_impl(int b, int n, int c, int m, int nsample, const T* po
             return finish_launch();
         }
         unsigned long long blocks = (tv + kCopyThreads - 1) / kCopyThreads;
-        const unsigned long long cap = (unsigned long long)num_sms() * (unsigned long long)ctas_per_sm;
+        const unsigned long long cap = (unsigned long long)num_sms() * (unsigned long long)tune.ctas_per_sm;
         const unsigned grid = (unsigned)(blocks > cap ? cap : (blocks < 1 ? 1 : blocks));
         if (tv < (1ull << 31))
-            group_point_vec4_kernel<unsigned, 1><<<grid, kCopyThreads, 0, st>>>(n, c4, (unsigned)rpc, (unsigned)tv, p4, idx, o4);
+            group_point_vec4_kernel<unsigned><<<grid, kCopyThreads, 0, st>>>(n, c4, (unsigned)rpc, (unsigned)tv, p4, idx, o4);
         else
-            group_point_vec4_kernel<unsigned long long, 1><<<grid, kCopyThreads, 0, st>>>(n, c4, rpc, tv, p4, idx, o4);
+            group_point_vec4_kernel<unsigned long long><<<grid, kCopyThreads, 0, st>>>(n, c4, rpc, tv, p4, idx, o4);
     } else {
         if (rpc >= (1ull << 32) || b > 65535) return (int)cudaErrorInvalidValue;
         return launch_group_rows<false, T>(b, n, c, m, nsample, nullptr, nullptr, points, idx, 0, 0, out, nullptr, 0, st);
@@ -538,7 +522,7 @@ static int group_point_grad_impl(int b, int n, int c, int m, int nsample, const 
                                  float* accum, cudaStream_t st) {
     const unsigned long long total = (unsigned long long)b * m * nsample * c;
     const unsigned long long rpc = (unsigned long long)m * nsample;
-    if (c % 4 == 0 && aligned_to(grad_out, 4 * sizeof(T)) && aligned16(accum)) {
+    if (c % 4 == 0 && aligned_to(grad_out, 4 * sizeof(T)) && aligned_to(accum, 16)) {
         const unsigned long long tv = total / 4;
         const unsigned grid = grid_for(tv, kCopyThreads);
         if (tv < (1ull << 31))
@@ -578,7 +562,7 @@ static int group_point_grad_det_impl(int b, int n, int c, int m, int nsample, co
     if (ne == 0) return (int)cudaMemsetAsync(grad_points, 0, sizeof(T) * (size_t)b * n * c, st);
     if (!grad_out || !idx || !workspace) return (int)cudaErrorInvalidValue;
     if (ne > 0x7fffffffLL || workspace_bytes < inv_workspace_bytes(b, ne, n)) return (int)cudaErrorInvalidValue;
-    return inv_sum_rows_det<T>(b, (int)ne, c, n, grad_out, idx, grad_points, workspace, f16, st);
+    return inv_scatter_det<false, T>(b, (int)ne, (int)ne, c, n, grad_out, idx, nullptr, nullptr, grad_points, workspace, f16, st);
 }
 
 template <typename T>

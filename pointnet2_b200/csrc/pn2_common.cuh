@@ -3,6 +3,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 
 #include <atomic>
@@ -46,6 +47,39 @@ inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s
 
 inline unsigned ceil_div_u(unsigned long long a, unsigned long long b) { return (unsigned)((a + b - 1) / b); }
 
+// CTAs for a grid-stride kernel over work_items items, per_block per CTA: one item per thread up to 64 CTAs per SM,
+// then grid-stride.
+inline unsigned grid_for(unsigned long long work_items, unsigned per_block) {
+    unsigned long long blocks = (work_items + per_block - 1) / per_block;
+    const unsigned long long cap = (unsigned long long)num_sms() * 64;
+    if (blocks > cap) blocks = cap;
+    if (blocks < 1) blocks = 1;
+    return (unsigned)blocks;
+}
+
+// cudaFuncSetAttribute once per (kernel instantiation, device), not on every launch
+struct AttrOnce {
+    std::atomic<unsigned long long> done{0ull};  // bit d: attributes set on device d (< 64)
+};
+template <typename K>
+cudaError_t ensure_attrs(AttrOnce& once, K kern, size_t dyn, bool nonportable_cluster) {
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    const unsigned long long bit = 1ull << (dev & 63);
+    if (dev < 64 && (once.done.load(std::memory_order_acquire) & bit)) return cudaSuccess;
+    if (dyn > 40 * 1024) {  // static + dynamic beyond the 48 KB default needs the opt-in
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
+        if (e != cudaSuccess) return e;
+    }
+    if (nonportable_cluster) {
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+        if (e != cudaSuccess) return e;
+    }
+    if (dev < 64) once.done.fetch_or(bit, std::memory_order_release);
+    return cudaSuccess;
+}
+
 // ---- arithmetic contracts --------------------------------------------------------------------
 // Squared distance exactly as nvcc contracts the reference's FPS and ball-query source
 // (tf_sampling_g.cu:142, tf_grouping_g.cu:24; SASS: FMUL dy*dy, FFMA dx, FFMA dz).  Written with
@@ -60,6 +94,37 @@ __device__ __forceinline__ float d2_fma_pattern(float ax, float ay, float az, fl
 __device__ __forceinline__ float d2_nofma(float ax, float ay, float az, float bx, float by, float bz) {
     const float dx = __fsub_rn(ax, bx), dy = __fsub_rn(ay, by), dz = __fsub_rn(az, bz);
     return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+}
+
+// ---- FP32 pairs: two points per helper call, each half rounded to nearest on its own, so bit-identical to the scalar
+// expressions on either half.  sm_90 has no packed FP32x2 instructions: every helper issues two scalar FADD / FMUL /
+// FFMA (the explicit .rn operations are never contracted) ---------------------------------------------------------
+__device__ __forceinline__ unsigned long long f2_pack(float a, float b) {
+    unsigned long long r;
+    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
+    return r;
+}
+__device__ __forceinline__ void f2_unpack(unsigned long long v, float& a, float& b) {
+    asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v));
+}
+__device__ __forceinline__ unsigned long long f2_sub(unsigned long long a, unsigned long long b) {
+    float a0, a1, b0, b1;
+    f2_unpack(a, a0, a1);
+    f2_unpack(b, b0, b1);
+    return f2_pack(__fsub_rn(a0, b0), __fsub_rn(a1, b1));
+}
+__device__ __forceinline__ unsigned long long f2_mul(unsigned long long a, unsigned long long b) {
+    float a0, a1, b0, b1;
+    f2_unpack(a, a0, a1);
+    f2_unpack(b, b0, b1);
+    return f2_pack(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
+}
+__device__ __forceinline__ unsigned long long f2_fma(unsigned long long a, unsigned long long b, unsigned long long c) {
+    float a0, a1, b0, b1, c0, c1;
+    f2_unpack(a, a0, a1);
+    f2_unpack(b, b0, b1);
+    f2_unpack(c, c0, c1);
+    return f2_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 
 // ---- per-cloud lengths -----------------------------------------------------------------------
@@ -94,6 +159,115 @@ __device__ __forceinline__ void warp_max_pair(unsigned& hi, unsigned& lo) {
     const unsigned ml = warp_max_u32(hi == mh ? lo : 0u);
     hi = mh;
     lo = ml;
+}
+
+// float min / max over the warp; every lane gets the result
+__device__ __forceinline__ float warp_min_f32(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fminf(v, __shfl_xor_sync(kFullMask, v, o));
+    return v;
+}
+__device__ __forceinline__ float warp_max_f32(float v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(kFullMask, v, o));
+    return v;
+}
+
+// Exclusive prefix sum over a 1024-thread CTA: thread t gets the sum of v over threads 0..t-1.  Every thread must
+// call it; s_w is 32 ints of shared scratch, written before the one __syncthreads inside and read after it, so a
+// second call needs a barrier in between.
+__device__ __forceinline__ int cta_exclusive_sum_1024(int v, int* s_w) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int incl = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(kFullMask, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) s_w[warp] = incl;
+    __syncthreads();
+    // exclusive prefix over the warp totals (every warp scans the 32 totals with shuffles)
+    const int wv = s_w[lane];
+    int winc = wv;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(kFullMask, winc, o);
+        if (lane >= o) winc += t;
+    }
+    return __shfl_sync(kFullMask, winc - wv, warp) + incl - v;
+}
+
+// ---- uniform grid over one cloud, for the ball query (ball_query_grid.cu, sa_fused.cu) ---------------------------
+constexpr int kGridMaxDim = 16;  // cells per axis
+
+// Cell of coordinate x: monotone in x; clamped so that out-of-box (and NaN) queries map to the border cells -1, dim.
+__device__ __forceinline__ int grid_cell(float x, float origin, float inv_h, int dim) {
+    float f = floorf(__fmul_rn(__fsub_rn(x, origin), inv_h));
+    f = fminf(fmaxf(f, -1.0f), (float)dim);
+    return (int)f;
+}
+
+struct GridGeometry {
+    float mn[3];    // origin: the box's minimum corner
+    float ext[3];   // box extent per axis
+    float h, inv_h; // cell edge
+    bool finite_box;
+    int dims[3], ncell;
+    int nb;  // cells of the 3x3x3 neighbourhood that fit in the grid
+};
+
+// Bounding box of the n points pts[0 .. 3n) and the grid over it, computed by a 1024-thread CTA; every thread gets
+// the result.  Every thread must call it; it contains one __syncthreads, and s_red (6 x 32 floats of shared scratch)
+// must not be written again before another barrier.  before_barrier() runs just before that barrier (the caller zeroes
+// its cell counters there, behind the latency of the box loads).
+template <typename F>
+__device__ __forceinline__ GridGeometry grid_geometry(const float* __restrict__ pts, int n, float radius, float (&s_red)[6][32],
+                                                      F&& before_barrier) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    GridGeometry g;
+    float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
+    for (int k = tid; k < n; k += 1024) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            const float v = __ldg(pts + 3 * (size_t)k + c);
+            mn[c] = fminf(mn[c], v);
+            // a NaN coordinate (fminf/fmaxf would ignore it) must disable the grid: the reference counts a NaN point
+            // as a hit in EVERY ball (fmaxf(NaN,1e-20f) < radius, tf_grouping_g.cu:24-25), which only an index-ordered
+            // scan reproduces; an infinite box does that (finite_box below)
+            mx[c] = (v == v) ? fmaxf(mx[c], v) : INFINITY;
+        }
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const float a = warp_min_f32(mn[c]), b = warp_max_f32(mx[c]);
+        if (lane == 0) {
+            s_red[c][warp] = a;
+            s_red[3 + c][warp] = b;
+        }
+    }
+    before_barrier();
+    __syncthreads();
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        g.mn[c] = warp_min_f32(s_red[c][lane]);
+        g.ext[c] = warp_max_f32(s_red[3 + c][lane]) - g.mn[c];
+    }
+    const float emax = fmaxf(fmaxf(g.ext[0], g.ext[1]), g.ext[2]);
+    // cell edge: at least 1.01 * radius (any point within the radius of a query is then at most one cell away on
+    // every axis, with margin for the rounding of the cell function), and large enough for kGridMaxDim cells to span
+    // the box
+    g.h = fmaxf(1.01f * radius, emax / (float)(kGridMaxDim - 1));
+    g.finite_box = (emax >= 0.f) && (emax < 1e30f) && (g.h > 0.f) && (g.h < 1e30f);
+    if (!g.finite_box) g.h = 1.0f;
+    g.inv_h = 1.0f / g.h;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        const int d = g.finite_box ? (int)floorf(g.ext[c] * g.inv_h) + 1 : 1;
+        g.dims[c] = min(max(d, 1), kGridMaxDim);
+    }
+    g.ncell = g.dims[0] * g.dims[1] * g.dims[2];
+    g.nb = min(g.dims[0], 3) * min(g.dims[1], 3) * min(g.dims[2], 3);
+    return g;
 }
 
 // Ascending bitonic sort of 32*K ints held K per lane (element i = register i/32 of lane i%32; K <= KMAX, a power of 2).
@@ -152,13 +326,18 @@ int fps_dispatch(int b, int n, int m, const float* inp, const int* lengths, floa
 bool fps_single_cta(int b, int n);
 size_t fps_scratch_bytes(int b, int n);
 
-// ordered-sum scatter through an inverse index (interpolate.cu), shared by three_interpolate's gradient and the
-// group_point / gather_point gradients: dst[b, i, :] = sum of the rows src[b, e, :] with idx[b, e] == i, e ascending, in
-// float32, rounded once to T (unsigned short: f16 != 0 float16, else bfloat16).  Every dst row is written (0 if no entry
-// points at it).  b clouds of ne entries over nt targets; workspace of inv_workspace_bytes(b, ne, nt) bytes.
+// ordered-sum scatter through an inverse index (scatter_det.cu), shared by three_interpolate's gradient and the
+// group_point / gather_point gradients: dst[b, i, :] = sum over the entries e with idx[b, e] == i, e ascending, of
+//   WEIGHTED:  src[b, e / 3, :] * weight[b, e]   (ne = 3n: three_interpolate, n source rows)
+//   otherwise: src[b, e, :]                      (ne = n)
+// in float32, rounded once to T (float; unsigned short: f16 != 0 float16, else bfloat16).  Every dst row is written (0
+// if no entry points at it).  b clouds of ne entries over nt targets; workspace of inv_workspace_bytes(b, ne, nt)
+// bytes; lengths (WEIGHTED only): (b,) device int32 of the n source rows, or NULL.  The arguments are checked by the
+// caller.
 size_t inv_workspace_bytes(int b, long long ne, int nt);
-template <typename T>
-int inv_sum_rows_det(int b, int ne, int c, int nt, const T* src, const int* idx, T* dst, void* workspace, int f16, cudaStream_t st);
+template <bool WEIGHTED, typename T>
+int inv_scatter_det(int b, int n, int ne, int c, int nt, const T* src, const int* idx, const float* weight, const int* lengths,
+                    T* dst, void* workspace, int f16, cudaStream_t st);
 
 // ---- streaming memory ops ---------------------------------------------------------------------
 __device__ __forceinline__ void st_stream_f4(float4* p, float4 v) { __stcs(p, v); }

@@ -22,7 +22,7 @@ SHOW = ["fps_cta_kernel<16, 256, 0, false>", "fps_cta_kernel<16, 256, 1, false>"
         "ball_group_kernel", "knn_kernel", "ball_query_kernel<16>", "bq_grid_build_kernel", "bq_grid_query_kernel",
         "group_rows_vec4_kernel<32, 4>", "group_narrow_kernel<false, float>", "group_rows_kernel<32, true, float>", "group_concat_vec_kernel<16, 2>",
         "group_point_grad_vec4_kernel<unsigned int, float>", "group_point_grad_vec4_kernel<unsigned int, __nv_bfloat16>", "three_nn_kernel", "fp_front_kernel<1, float>", "fp_front_kernel<8, float>", "fp_front_kernel<8, unsigned short>", "group_rows_kernel<32, true, unsigned short>",
-        "three_interp_vec4_kernel<unsigned int, 1, float, float4>", "three_interp_vec4_kernel<unsigned int, 1, __nv_bfloat16, uint2>", "three_interp_grad_vec4_kernel<unsigned int>", "inv_build_kernel",
+        "three_interp_vec4_kernel<unsigned int, float, false, float4>", "three_interp_vec4_kernel<unsigned int, __nv_bfloat16, false, uint2>", "three_interp_grad_vec4_kernel<unsigned int>", "inv_build_kernel",
         "inv_gather_kernel<true, float>", "inv_long_kernel<true, float>", "inv_gather_kernel<true, unsigned short>", "inv_long_kernel<true, unsigned short>", "selection_sort_kernel", "prob_cumsum_kernel", "prob_search_kernel"]
 
 
