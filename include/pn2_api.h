@@ -286,6 +286,35 @@ int pn2_three_interpolate_grad_det_ragged_typed(int dtype, int b, int n, int c, 
                                                 void* grad_points, void* workspace, size_t workspace_bytes,
                                                 void* stream);
 
+/* ---- learned layers: masked batch norm + ReLU (the ragged rows of the segmentation nets) ---------------------------
+ * x (rows, c) in `dtype`, keep (rows,) uint8 (a torch bool mask viewed as bytes): batch norm whose training statistics
+ * come from the rows with keep[r] != 0 only, followed by ReLU:
+ *   y = keep ? max(0, (x - mean) * (invstd * gamma) + beta) : 0,   invstd = rsqrt(var + eps), var biased.
+ * Padding rows (keep[r] == 0) of x and dy are never read (they may hold NaN or inf); those of y and dx are written 0.
+ * Statistics, gamma, beta, dgamma, dbeta and the running buffers are float32 whatever `dtype` is; arithmetic is float32.
+ * The mean and variance are an exact two-pass over register-held groups of rows merged with Chan's formula, never
+ * E[x^2] - mean^2.  The row partition depends on (rows, c) only and every sum has a fixed order, with no float atomics:
+ * results are bit-identical from run to run and device to device.  Nothing is read back to the host.
+ * Forward: writes save_mean / save_invstd (c floats each); when running_mean / running_var are given (both or neither)
+ * updates them from the real rows as torch's BatchNorm1d would from a batch of them alone: unbiased variance
+ * var * cnt / max(cnt - 1, 1), weight `momentum`, or 1 / *num_batches_tracked (read on the device, already incremented by
+ * the caller) when momentum < 0.  gamma / beta may be NULL (affine = False).
+ * Backward (y and the saved statistics from the forward): g = keep ? dy * [y > 0] : 0, xhat = (x - mean) * invstd,
+ *   dx = keep ? gamma * invstd * (g - sum(g) / cnt - xhat * sum(g * xhat) / cnt) : 0,  dgamma = sum(g * xhat),
+ *   dbeta = sum(g)   (sums over the real rows; dgamma / dbeta may be NULL, gamma NULL means 1).
+ * Both take a device workspace of pn2_masked_bn_workspace_bytes(rows, c) bytes (16-byte aligned).  rows == 0 launches
+ * nothing.  An unknown dtype, a NULL required tensor, c <= 0, rows < 0 or a short workspace return cudaErrorInvalidValue
+ * without a launch. */
+size_t pn2_masked_bn_workspace_bytes(int rows, int c);
+int pn2_masked_bn_relu_forward_typed(int dtype, int rows, int c, const void* x, const unsigned char* keep, const float* gamma,
+                                     const float* beta, float eps, float momentum, const long long* num_batches_tracked,
+                                     float* running_mean, float* running_var, void* y, float* save_mean, float* save_invstd,
+                                     void* workspace, size_t workspace_bytes, void* stream);
+int pn2_masked_bn_relu_backward_typed(int dtype, int rows, int c, const void* dy, const void* x, const void* y,
+                                      const unsigned char* keep, const float* gamma, const float* save_mean,
+                                      const float* save_invstd, void* dx, float* dgamma, float* dbeta, void* workspace,
+                                      size_t workspace_bytes, void* stream);
+
 /* ---- the sampling+grouping half of a set-abstraction layer, device-resident ------------------ */
 
 /* query_ball_point + group_point(xyz) in ONE launch (tf_grouping_g.cu:3-57 back to back, as

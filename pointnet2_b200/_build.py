@@ -17,7 +17,7 @@ INCLUDE = os.path.join(REPO_ROOT, "include")
 BUILD_DIR = os.path.join(PKG_DIR, "build")
 LIB_PATH = os.path.join(PKG_DIR, "libpn2_b200.so")
 
-SOURCES = ["api.cu", "fps.cu", "ball_query.cu", "ball_query_grid.cu", "sa_fused.cu", "knn.cu", "group.cu", "interpolate.cu", "scatter_det.cu", "prob_sample.cu"]
+SOURCES = ["api.cu", "fps.cu", "ball_query.cu", "ball_query_grid.cu", "sa_fused.cu", "knn.cu", "group.cu", "interpolate.cu", "scatter_det.cu", "prob_sample.cu", "masked_bn.cu"]
 HEADERS = [os.path.join(CSRC, "pn2_common.cuh"), os.path.join(INCLUDE, "pn2_api.h")]
 
 NVCC_FLAGS = [

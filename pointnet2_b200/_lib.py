@@ -68,6 +68,11 @@ _SIGNATURES = {
     "pn2_three_interpolate_ragged_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     "pn2_three_interpolate_grad_ragged": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     "pn2_three_interpolate_grad_det_ragged_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    # masked batch norm + ReLU over the real rows of a padded (rows, c) tensor
+    "pn2_masked_bn_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "pn2_masked_bn_relu_forward_typed": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, c_float, c_float, _P, _P, _P, _P, _P, _P, _P,
+                                                 c_size_t, _P]),
+    "pn2_masked_bn_relu_backward_typed": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_sa_layer_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "pn2_sa_layer_host": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_api_version": (c_int, []),

@@ -21,6 +21,10 @@ from typing import Dict, Optional, Sequence
 
 import torch
 from torch import nn
+from torch.autograd.function import once_differentiable
+
+from . import _lib
+from ._tensor import DTYPE_CODES, FEATURE_DTYPES, on_device, ptr, stream_ptr
 
 
 class SharedMLP(nn.Module):
@@ -52,15 +56,27 @@ class SharedMLP(nn.Module):
         if mask is None:
             return self.body(t.reshape(-1, t.shape[-1])).reshape(*lead, self.out_channels)
         keep = mask.reshape(-1, 1)
-        # torch.where, not a multiply: NaN * 0 is NaN
+        # torch.where, not a multiply: NaN * 0 is NaN.  This one stays even before the fused op: NaN input rows would
+        # reach the Linear's weight gradient through x^T dy.
         x = torch.where(keep, t.reshape(-1, t.shape[-1]), 0)
-        for mod in self.body:
+        mods = list(self.body)
+        i = 0
+        while i < len(mods):
+            mod = mods[i]
             if isinstance(mod, nn.BatchNorm1d):
+                if _fuses_at(mods, i, x):
+                    # BatchNorm1d + the ReLU after it in the CUDA op, which reads no padding row and writes 0 there
+                    x = masked_batch_norm_relu(mod, x, keep.reshape(-1))
+                    i += 2
+                    continue
                 x = torch.where(keep, masked_batch_norm(mod, x, keep), 0)
             elif isinstance(mod, nn.Linear):
-                x = torch.where(keep, mod(x), 0)
+                x = mod(x)
+                if not _fuses_at(mods, i + 1, x):
+                    x = torch.where(keep, x, 0)
             else:
                 x = mod(x)  # ReLU keeps the zeros
+            i += 1
         return x.reshape(*lead, self.out_channels)
 
 
@@ -100,6 +116,116 @@ def masked_batch_norm(bn: nn.BatchNorm1d, x: torch.Tensor, keep: torch.Tensor) -
             bn.running_mean.mul_(1 - f).add_(mean * f)
             bn.running_var.mul_(1 - f).add_(unbiased * f)
     return y.to(x.dtype)
+
+
+def _bn_tensors_misfit(bn: nn.BatchNorm1d, device) -> Optional[Exception]:
+    """Why the kernels cannot take ``bn``'s own tensors (TypeError: dtype or layout, RuntimeError: device), or None: they
+    read weight / bias and update the running statistics as contiguous float32 on x's device (num_batches_tracked
+    int64), so a module converted with .half() or .to(torch.bfloat16), or left on another device, keeps the torch
+    path."""
+    tensors = [("weight", bn.weight, torch.float32), ("bias", bn.bias, torch.float32)] if bn.affine else []
+    if bn.track_running_stats and bn.running_mean is not None:
+        tensors += [("running_mean", bn.running_mean, torch.float32), ("running_var", bn.running_var, torch.float32),
+                    ("num_batches_tracked", bn.num_batches_tracked, torch.int64)]
+    for name, t, dtype in tensors:
+        if t is None or t.dtype != dtype or not t.is_contiguous():
+            got = "None" if t is None else f"{t.dtype}{'' if t.is_contiguous() else ' (not contiguous)'}"
+            return TypeError(f"batch norm {name} must be a contiguous {dtype} tensor, got {got}")
+        if t.device != device:
+            return RuntimeError(f"batch norm {name} must be on x's device {device}, got device {t.device}")
+    return None
+
+
+def fused_bn_applies(bn: nn.BatchNorm1d, x: torch.Tensor) -> bool:
+    """Whether SharedMLP(t, mask) runs ``bn`` + the ReLU after it through masked_batch_norm_relu: on CUDA, for float32 /
+    bfloat16 / float16 x, wherever the torch path would compute batch statistics (training mode, or no running
+    statistics), on a non-empty batch, with the module's parameters and buffers float32 on x's device.  Everything else
+    (CPU, float64, eval with running statistics, a module converted to 16 bits) keeps masked_batch_norm."""
+    return (x.is_cuda and x.dtype in FEATURE_DTYPES and x.shape[0] > 0
+            and (bn.training or bn.running_mean is None) and _bn_tensors_misfit(bn, x.device) is None)
+
+
+def _fuses_at(mods, i: int, x: torch.Tensor) -> bool:
+    """mods[i] is a BatchNorm1d followed by a ReLU, and the pair runs through masked_batch_norm_relu"""
+    return (i + 1 < len(mods) and isinstance(mods[i], nn.BatchNorm1d) and isinstance(mods[i + 1], nn.ReLU)
+            and fused_bn_applies(mods[i], x))
+
+
+class _MaskedBatchNormReLU(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, keep, bn):
+        rows, c = x.shape
+        dev = x.device
+        tracking = bn.track_running_stats and bn.running_mean is not None
+        momentum = -1.0 if bn.momentum is None else float(bn.momentum)
+        y = torch.empty_like(x)
+        save_mean = torch.empty(c, dtype=torch.float32, device=dev)
+        save_invstd = torch.empty(c, dtype=torch.float32, device=dev)
+        lib = _lib.load()
+        with on_device(x):
+            if tracking:
+                bn.num_batches_tracked.add_(1)  # on the device; the kernel reads it for the cumulative average
+            wsb = int(lib.pn2_masked_bn_workspace_bytes(rows, c))
+            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+            rc = lib.pn2_masked_bn_relu_forward_typed(
+                DTYPE_CODES[x.dtype], rows, c, ptr(x), ptr(keep), ptr(weight), ptr(bias), float(bn.eps), momentum,
+                ptr(bn.num_batches_tracked if tracking else None), ptr(bn.running_mean if tracking else None),
+                ptr(bn.running_var if tracking else None), ptr(y), ptr(save_mean), ptr(save_invstd), ptr(ws), wsb,
+                stream_ptr(dev))
+        _lib.check(rc, "pn2_masked_bn_relu_forward_typed")
+        ctx.save_for_backward(x, y, keep, weight, save_mean, save_invstd)
+        ctx.affine = weight is not None
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        x, y, keep, weight, save_mean, save_invstd = ctx.saved_tensors
+        rows, c = x.shape
+        dev = x.device
+        dy = dy.to(x.dtype).contiguous()
+        dx = torch.empty_like(x)
+        dgamma = torch.empty(c, dtype=torch.float32, device=dev) if ctx.affine else None
+        dbeta = torch.empty(c, dtype=torch.float32, device=dev) if ctx.affine else None
+        lib = _lib.load()
+        with on_device(x):
+            wsb = int(lib.pn2_masked_bn_workspace_bytes(rows, c))
+            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+            rc = lib.pn2_masked_bn_relu_backward_typed(
+                DTYPE_CODES[x.dtype], rows, c, ptr(dy), ptr(x), ptr(y), ptr(keep), ptr(weight), ptr(save_mean),
+                ptr(save_invstd), ptr(dx), ptr(dgamma), ptr(dbeta), ptr(ws), wsb, stream_ptr(dev))
+        _lib.check(rc, "pn2_masked_bn_relu_backward_typed")
+        return dx, dgamma, dbeta, None, None
+
+
+def masked_batch_norm_relu(bn: nn.BatchNorm1d, x: torch.Tensor, keep: torch.Tensor) -> torch.Tensor:
+    """relu(masked_batch_norm(bn, x, keep)) with its padding rows 0, as one CUDA op (csrc/masked_bn.cu) forward and
+    backward.  ``x`` (R, C) float32 / bfloat16 / float16 on CUDA; ``keep`` (R,) bool, True on the real rows.  The
+    statistics come from the real rows only (a two-pass per row group, merged with Chan's formula in a fixed order, in
+    float32), the running statistics are updated as masked_batch_norm updates them, and the padding rows of x and of the
+    incoming gradient are never read (they may be NaN).  Results are bit-identical from run to run; against the torch
+    composition they differ by float32 rounding (the sums are ordered differently).  Nothing is read back to the host.
+    For batch statistics only: in eval mode with running statistics it raises (that is ``bn(x)``).  ``bn``'s weight,
+    bias and running buffers must be float32 on x's device."""
+    if not (x.is_cuda and x.dtype in FEATURE_DTYPES):
+        raise RuntimeError(f"masked_batch_norm_relu needs a float32/bfloat16/float16 CUDA tensor, got {x.dtype} on {x.device}")
+    if x.dim() != 2 or x.shape[1] != bn.num_features:
+        raise ValueError(f"masked_batch_norm_relu expects (rows, {bn.num_features}) x, got {tuple(x.shape)}")
+    if not isinstance(keep, torch.Tensor) or keep.dtype != torch.bool or keep.numel() != x.shape[0]:
+        raise ValueError(f"masked_batch_norm_relu expects a bool keep of {x.shape[0]} rows, got "
+                         f"{getattr(keep, 'dtype', type(keep).__name__)} {tuple(getattr(keep, 'shape', ()))}")
+    if keep.device != x.device:
+        raise RuntimeError(f"keep must be on x's device ({x.device}), got {keep.device}")
+    if not bn.training and bn.running_mean is not None:
+        raise ValueError("masked_batch_norm_relu computes batch statistics; in eval mode with running statistics use bn(x)")
+    misfit = _bn_tensors_misfit(bn, x.device)
+    if misfit is not None:
+        raise misfit
+    x = x.contiguous()
+    keep = keep.reshape(-1).contiguous().view(torch.uint8)  # the bool mask as bytes, no copy
+    weight = bn.weight if bn.affine else None
+    bias = bn.bias if bn.affine else None
+    return _MaskedBatchNormReLU.apply(x, weight, bias, keep, bn)
 
 
 def set_bn_momentum(model: nn.Module, bn_decay: float) -> None:

@@ -23,7 +23,10 @@ SHOW = ["fps_cta_kernel<16, 256, 0, false>", "fps_cta_kernel<16, 256, 1, false>"
         "group_rows_vec4_kernel<32, 4>", "group_narrow_kernel<false, float>", "group_rows_kernel<32, true, float>", "group_concat_vec_kernel<16, 2>",
         "group_point_grad_vec4_kernel<unsigned int, float>", "group_point_grad_vec4_kernel<unsigned int, __nv_bfloat16>", "three_nn_kernel", "fp_front_kernel<1, float>", "fp_front_kernel<8, float>", "fp_front_kernel<8, unsigned short>", "group_rows_kernel<32, true, unsigned short>",
         "three_interp_vec4_kernel<unsigned int, float, false, float4>", "three_interp_vec4_kernel<unsigned int, __nv_bfloat16, false, uint2>", "three_interp_grad_vec4_kernel<unsigned int>", "inv_build_kernel",
-        "inv_gather_kernel<true, float>", "inv_long_kernel<true, float>", "inv_gather_kernel<true, unsigned short>", "inv_long_kernel<true, unsigned short>", "selection_sort_kernel", "prob_cumsum_kernel", "prob_search_kernel"]
+        "inv_gather_kernel<true, float>", "inv_long_kernel<true, float>", "inv_gather_kernel<true, unsigned short>", "inv_long_kernel<true, unsigned short>", "selection_sort_kernel", "prob_cumsum_kernel", "prob_search_kernel",
+        "mbn_stats_kernel<float, 4, true>", "mbn_stats_kernel<__nv_bfloat16, 4, true>", "mbn_stats_kernel<float, 1, false>", "mbn_finalize_kernel",
+        "mbn_norm_relu_kernel<float, 4, true>", "mbn_norm_relu_kernel<__nv_bfloat16, 4, true>", "mbn_bwd_sums_kernel<float, 4, true>",
+        "mbn_bwd_sums_kernel<__nv_bfloat16, 4, true>", "mbn_bwd_finalize_kernel", "mbn_bwd_dx_kernel<float, 4, true>", "mbn_bwd_dx_kernel<__nv_bfloat16, 4, true>"]
 
 
 def demangle(names):
