@@ -366,6 +366,41 @@ int pn2_sa_layer_msg_device_ragged(int b, int n, int m, int nscales, const float
                                    int* const* idx, int* const* pts_cnt, float* const* grouped_xyz, int center,
                                    void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- whole-scene segmentation (scannet/scannet_dataset.py:83-118, scannet/train.py:326-427; DESIGN.md §6.9) --------
+ * A scene xyz (p,3) f32 (finite) is cut into nx x ny xy blocks, i-major: block (i,j) spans bmin = (lo_x + i*stride,
+ * lo_y + j*stride), bmax = bmin + block_size.  Every test is in double on the float32 coordinate, each operation rounded:
+ * context member: bmin - padding <= x,y <= bmax + padding; core member: a context member with
+ * bmin - 0.001 <= x,y <= bmax + 0.001.  z is not tested.  The caller plans the grid (lo = the scene's minimum, nx the
+ * smallest k >= 1 with lo_x + (k-1)*stride + block_size >= the maximum; ny alike), needs 0 < stride <= block_size,
+ * padding >= 0 and nx * ny <= 16384.
+ *
+ * Two calls on one workspace of pn2_scene_blocks_workspace_bytes(p, nx, ny) bytes (256-byte aligned; 0 = invalid grid):
+ *   pn2_scene_blocks_count: counts (2*nx*ny) int32 receives the context member count of every block, then the core
+ *     member count of every block.  The caller reads them back and plans the batch: a block without core members is
+ *     dropped, a block of c members becomes k = ceil(c / max_points) sub-blocks, and sub_begin / sub_count (nx*ny) int32
+ *     give each block's first sub-block and k (0 = dropped).
+ *   pn2_scene_blocks_fill: writes the padded (b, n) batch.  Member r (in ascending scene index) of a block goes to
+ *     sub-block sub_begin + r mod k, row r div k: out_xyz (b,n,3) its coordinates, point_idx (b,n) its scene index,
+ *     core (b,n) 1 for a core member; padding rows are 0 / -1 / 0.  occ_off (p+1) and occ_row (occ_off[p] entries) are
+ *     the CSR of every point's core rows b*n_row + row, ascending.  b*n*3 < 2^31.
+ * Results are the same bits on every run (no atomic order reaches them).  Invalid arguments return cudaErrorInvalidValue
+ * without a launch. */
+size_t pn2_scene_blocks_workspace_bytes(int p, int nx, int ny);
+int pn2_scene_blocks_count(int p, const float* xyz, double lo_x, double lo_y, double block_size, double stride, double padding,
+                           int nx, int ny, int* counts, void* workspace, size_t workspace_bytes, void* stream);
+int pn2_scene_blocks_fill(int p, const float* xyz, double lo_x, double lo_y, double block_size, double stride, double padding,
+                          int nx, int ny, const int* sub_begin, const int* sub_count, int b, int n, float* out_xyz,
+                          int* point_idx, unsigned char* core, int* occ_off, int* occ_row, void* workspace,
+                          size_t workspace_bytes, void* stream);
+/* Ordered merge of block logits: logits (row_end - row_begin, c) in `dtype` hold the rows [row_begin, row_end) of the
+ * (b, n) batch pn2_scene_blocks_fill wrote (point_idx, core, occ_off, occ_row as it wrote them).  For every point, its
+ * core rows inside the range are added one at a time, in ascending row order, onto accum (p,c) float32:
+ * accum = accum + logit, each add rounded.  Merging a batch chunk by chunk gives the bits of one merge over all of it.
+ * No atomics, no read-back. */
+int pn2_scene_merge_typed(int dtype, int p, int c, int b, int n, int row_begin, int row_end, const void* logits,
+                          const int* point_idx, const unsigned char* core, const int* occ_off, const int* occ_row,
+                          float* accum, void* stream);
+
 /* ---- host-buffer entry point (the reference feeds numpy through feed_dict) ----------------- */
 
 /* One SSG set-abstraction sampling+grouping layer (farthest_point_sample + gather_point +

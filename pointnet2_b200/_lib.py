@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import c_float, c_int, c_size_t, c_ulonglong, c_void_p
+from ctypes import c_double, c_float, c_int, c_size_t, c_ulonglong, c_void_p
 
 from . import _build
 
@@ -73,6 +73,13 @@ _SIGNATURES = {
     "pn2_masked_bn_relu_forward_typed": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, c_float, c_float, _P, _P, _P, _P, _P, _P, _P,
                                                  c_size_t, _P]),
     "pn2_masked_bn_relu_backward_typed": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    # whole-scene segmentation: block partition of a scene and the ordered merge of block logits
+    "pn2_scene_blocks_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "pn2_scene_blocks_count": (c_int, [c_int, _P, c_double, c_double, c_double, c_double, c_double, c_int, c_int, _P, _P,
+                                       c_size_t, _P]),
+    "pn2_scene_blocks_fill": (c_int, [c_int, _P, c_double, c_double, c_double, c_double, c_double, c_int, c_int, _P, _P,
+                                      c_int, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    "pn2_scene_merge_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P]),
     "pn2_sa_layer_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "pn2_sa_layer_host": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_api_version": (c_int, []),

@@ -117,6 +117,45 @@ def part_shapes(b: int, n: int, seed: int, offsets):
     return pts, cls.astype(np.int64), label
 
 
+def scene_room(p: int, seed: int):
+    """A synthetic indoor scene (the reference's ScanNet data is not shipped): (p, 3) float32 points in metres and (p,)
+    int64 labels in 0..20.  A rectangular room whose floor area grows with p (about 5000 points per square metre of floor,
+    a 1.5e5-point room is about 5.5 m across): floor (label 2), four 2.5 m walls (1), box furniture on the floor, each
+    box's surface carrying one label of 3..20, 3 % unlabelled clutter (0) anywhere in the room, and 2 % of the rows
+    exact duplicates of other rows.  Rows are shuffled."""
+    rs = np.random.RandomState(seed)
+    side = 5.5 * np.sqrt(max(p, 1) / 1.5e5)
+    w, d, h = side * rs.uniform(0.9, 1.1), side * rs.uniform(0.8, 1.0), 2.5
+    n_floor, n_wall, n_clutter = int(0.35 * p), int(0.30 * p), int(0.03 * p)
+    n_dup = int(0.02 * p)
+    n_furn = p - n_floor - n_wall - n_clutter - n_dup
+    floor = np.stack([rs.uniform(0, w, n_floor), rs.uniform(0, d, n_floor), np.zeros(n_floor)], 1)
+    # walls: perimeter parameter t in [0, 2(w + d)), height uniform
+    t = rs.uniform(0, 2 * (w + d), n_wall)
+    wx = np.select([t < w, t < w + d, t < 2 * w + d], [t, w, 2 * w + d - t], 0.0)
+    wy = np.select([t < w, t < w + d, t < 2 * w + d], [0.0, t - w, d], 2 * (w + d) - t)
+    wall = np.stack([wx, wy, rs.uniform(0, h, n_wall)], 1)
+    # furniture: boxes resting on the floor, points on their five visible faces
+    nbox = max(1, int(round(w * d / 4)))
+    size = rs.uniform([0.4, 0.4, 0.4], [2.0, 1.2, 1.8], (nbox, 3))
+    corner = rs.uniform(0, 1, (nbox, 2)) * np.maximum(np.array([w, d]) - size[:, :2], 0)
+    box_label = rs.randint(3, 21, nbox)
+    which = rs.randint(0, nbox, n_furn)
+    fp = rs.uniform(0, 1, (n_furn, 3))
+    face = rs.randint(0, 5, n_furn)  # 0..3: side faces, 4: top
+    ax = np.where(face < 2, 0, np.where(face < 4, 1, 2))
+    fp[np.arange(n_furn), ax] = np.where(face == 4, 1.0, (face % 2).astype(np.float64))
+    furn = fp * size[which]
+    furn[:, :2] += corner[which]
+    clutter = rs.uniform(0, 1, (n_clutter, 3)) * np.array([w, d, h])
+    pts = np.concatenate([floor, wall, furn, clutter], 0)
+    lab = np.concatenate([np.full(n_floor, 2), np.full(n_wall, 1), box_label[which], np.zeros(n_clutter, np.int64)])
+    dup = rs.randint(0, len(pts), n_dup) if len(pts) else np.zeros(0, np.int64)
+    pts, lab = np.concatenate([pts, pts[dup]], 0), np.concatenate([lab, lab[dup]])
+    order = rs.permutation(len(pts))
+    return pts[order].astype(F32), lab[order].astype(np.int64)
+
+
 # ---- BASELINE.json configs ---------------------------------------------------------------------
 CFG2_SSG_SA = dict(name="cfg2_ssg_sa_layer", b=32, n=4096, npoint=1024, nsample=32, radius=0.1, dist="U", seed=100)
 CFG1_FPS_CPU = dict(name="cfg1_fps_plumbing", b=8, n=1024, npoint=512, dist="U", seed=100)

@@ -26,7 +26,9 @@ SHOW = ["fps_cta_kernel<16, 256, 0, false>", "fps_cta_kernel<16, 256, 1, false>"
         "inv_gather_kernel<true, float>", "inv_long_kernel<true, float>", "inv_gather_kernel<true, unsigned short>", "inv_long_kernel<true, unsigned short>", "selection_sort_kernel", "prob_cumsum_kernel", "prob_search_kernel",
         "mbn_stats_kernel<float, 4, true>", "mbn_stats_kernel<__nv_bfloat16, 4, true>", "mbn_stats_kernel<float, 1, false>", "mbn_finalize_kernel",
         "mbn_norm_relu_kernel<float, 4, true>", "mbn_norm_relu_kernel<__nv_bfloat16, 4, true>", "mbn_bwd_sums_kernel<float, 4, true>",
-        "mbn_bwd_sums_kernel<__nv_bfloat16, 4, true>", "mbn_bwd_finalize_kernel", "mbn_bwd_dx_kernel<float, 4, true>", "mbn_bwd_dx_kernel<__nv_bfloat16, 4, true>"]
+        "mbn_bwd_sums_kernel<__nv_bfloat16, 4, true>", "mbn_bwd_finalize_kernel", "mbn_bwd_dx_kernel<float, 4, true>", "mbn_bwd_dx_kernel<__nv_bfloat16, 4, true>",
+        "scene_count_kernel", "scene_scan_kernel", "scene_fill_kernel", "scene_merge_kernel<float>", "scene_merge_kernel<__nv_bfloat16>",
+        "scene_merge_kernel<__half>"]
 
 
 def demangle(names):
