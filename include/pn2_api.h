@@ -401,6 +401,28 @@ int pn2_scene_merge_typed(int dtype, int p, int c, int b, int n, int row_begin, 
                           const int* point_idx, const unsigned char* core, const int* occ_off, const int* occ_row,
                           float* accum, void* stream);
 
+/* ---- training crops (scannet/scannet_dataset.py:27-60, scannet/train.py:181-197, utils/provider.py:52-70; DESIGN.md
+ * §6.10) ----------------------------------------------------------------------------------------------------------
+ * A scene set: s scenes packed into xyz (p,3) f32 (finite), label (p) int32 in [0, num_class), offsets (s+1) int64
+ * (scene k holds rows offsets[k] .. offsets[k+1]-1, none empty; max_scene = the largest scene), lo / hi (s,3) f32 the
+ * per-scene extrema (hi_z > lo_z), label_weights (num_class) f32.  Crop i of b is drawn from scene crop_scene[i]
+ * (int64, device) with the counter-based draws of DESIGN.md §6.10 keyed by the seed (*seed_dev when seed_dev is not
+ * NULL, read on the device, else `seed`): ten attempted columns, the first valid one taken (else the last), its m =
+ * min(c, npoints) context members of smallest (hash key, scene-local index) in that order, rows r >= 1 dropped with
+ * probability u * max_dropout, x/y rotated about the origin by a random angle when `rotate`.  Outputs (b, npoints):
+ * out_xyz (x3) f32, out_label int64, out_weight f32 (label_weights[label] on core rows), point_idx int32 (row of the
+ * scene set, -1 on padding), core u8; per crop lengths int32 (>= 1), attempt int32, valid u8.  Padding rows are 0 / -1.
+ * A crop_scene value outside [0, s) gives lengths 0 and attempt -1.  npoints <= 16384, b <= 65535, b*npoints*3 < 2^31,
+ * 0 <= max_dropout <= 1.  The workspace is pn2_scene_crops_workspace_bytes(b, npoints) bytes, 256-byte aligned
+ * (0 = invalid shape).  Same bits on every run; nothing is read back, so the call can be captured in a CUDA graph.
+ * Invalid arguments return cudaErrorInvalidValue without a launch. */
+size_t pn2_scene_crops_workspace_bytes(int b, int npoints);
+int pn2_scene_crops(int s, int p, int max_scene, const float* xyz, const int* label, const long long* offsets, const float* lo,
+                    const float* hi, int num_class, const float* label_weights, int b, const long long* crop_scene,
+                    long long seed, const long long* seed_dev, int npoints, double max_dropout, int rotate, float* out_xyz,
+                    long long* out_label, float* out_weight, int* lengths, int* point_idx, unsigned char* core, int* attempt,
+                    unsigned char* valid, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- host-buffer entry point (the reference feeds numpy through feed_dict) ----------------- */
 
 /* One SSG set-abstraction sampling+grouping layer (farthest_point_sample + gather_point +

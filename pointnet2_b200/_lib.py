@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import c_double, c_float, c_int, c_size_t, c_ulonglong, c_void_p
+from ctypes import c_double, c_float, c_int, c_longlong, c_size_t, c_ulonglong, c_void_p
 
 from . import _build
 
@@ -80,6 +80,10 @@ _SIGNATURES = {
     "pn2_scene_blocks_fill": (c_int, [c_int, _P, c_double, c_double, c_double, c_double, c_double, c_int, c_int, _P, _P,
                                       c_int, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_scene_merge_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P]),
+    # training crops of a scene set: seeded, validity-checked columns as a padded ragged batch
+    "pn2_scene_crops_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "pn2_scene_crops": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, c_int, _P, c_int, _P, c_longlong, _P, c_int, c_double,
+                                c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_sa_layer_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "pn2_sa_layer_host": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_api_version": (c_int, []),

@@ -1,0 +1,430 @@
+// crops.cu — ScanNet training crops: B seeded, validity-checked xy columns drawn from a set of scenes, as a padded
+// ragged batch with point dropout and a rotation about z (scannet/scannet_dataset.py:27-60, scannet/train.py:181-197,
+// utils/provider.py:52-70, without the resampling; DESIGN.md §6.10).
+//
+// Two kernels per call, nothing read back:
+//   attempt: CTA (chunk, crop) reads a chunk of the crop's scene once and tests the boxes of all ten attempts: integer
+//            context / labelled counts and the core voxel-key bitmap in shared memory, merged into the crop's workspace
+//            with integer atomicAdd / atomicOr (order-free);
+//   select:  one CTA per crop takes the first valid attempt (else attempt 9), radix-selects the m smallest
+//            (key, scene index) pairs of its members, recomputing every key from the hash on each pass, sorts them in
+//            shared memory and writes the rows (dropout compaction, rotation, labels, weights, padding).
+// Every membership test is the double test of the definition, done exactly in float32: for a float p and a double t,
+// (double)p >= t <=> p >= (t rounded up to float), and (double)p <= t <=> p <= (t rounded down to float).
+#include "pn2_common.cuh"
+
+namespace pn2 {
+namespace {
+
+constexpr int kAttempts = 10;            // scannet_dataset.py:37
+constexpr int kKeyWords = 1986;          // keys 0 .. 32*31*62 + 32*62 + 62 = 63550 -> 63551 bits
+constexpr int kCropWsWords = kAttempts * 2 + kAttempts * kKeyWords;  // per crop: (context, labelled) x 10, 10 bitmaps
+constexpr int kCropMaxPoints = 16384;    // sort buffer: 16384 x 8 B of shared memory
+constexpr int kAttemptThreads = 512;
+constexpr int kAttemptChunk = 8192;      // scene points per CTA of the attempt pass
+constexpr int kSelectThreads = 1024;
+constexpr int kRadixBins = 2048;
+constexpr unsigned long long kGolden = 0x9E3779B97F4A7C15ull;
+
+struct CropArgs {
+    const float* xyz;
+    const int* label;
+    const long long* offsets;
+    const float* lo;
+    const float* hi;
+    const long long* crop_scene;
+    const long long* seed_dev;  // non-null: the seed is read here, on the device
+    unsigned long long seed;
+    int s;
+};
+
+__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
+    x ^= x >> 30;
+    x *= 0xBF58476D1CE4E5B9ull;
+    x ^= x >> 27;
+    x *= 0x94D049BB133111EBull;
+    x ^= x >> 31;
+    return x;
+}
+
+__device__ __forceinline__ unsigned long long crop_draw(unsigned long long seed, unsigned long long stream,
+                                                        unsigned long long b, unsigned long long i) {
+    return mix64(mix64(mix64(seed + stream * kGolden) + b * kGolden) + i * kGolden);
+}
+
+__device__ __forceinline__ double crop_u(unsigned long long d) { return (double)(d >> 11) * 0x1.0p-53; }
+
+__device__ __forceinline__ unsigned long long crop_seed(const CropArgs& a) {
+    return a.seed_dev ? (unsigned long long)__ldg(a.seed_dev) : a.seed;
+}
+
+// One attempt's box: context and core bounds as exact float thresholds, and curmin / curmax - curmin for the keys.
+struct CropBox {
+    float c0[3], c1[3];  // context: c0 <= p <= c1
+    float k0[3], k1[3];  // core
+    double mn[3], ext[3];
+};
+
+__device__ __forceinline__ void crop_box(const CropArgs& a, unsigned long long seed, int b, int att, long long off, long long ps,
+                                         int sc, CropBox& B) {
+    const long long ci = off + (long long)(crop_draw(seed, 1, (unsigned long long)b, (unsigned long long)att) % (unsigned long long)ps);
+    double mn[3], mx[3];
+    for (int d = 0; d < 2; ++d) {
+        const double c = (double)__ldg(a.xyz + 3 * ci + d);
+        mn[d] = __dsub_rn(c, 0.75);
+        mx[d] = __dadd_rn(c, 0.75);
+    }
+    mn[2] = (double)__ldg(a.lo + 3 * sc + 2);
+    mx[2] = (double)__ldg(a.hi + 3 * sc + 2);
+    for (int d = 0; d < 3; ++d) {
+        B.c0[d] = __double2float_ru(__dsub_rn(mn[d], 0.2));
+        B.c1[d] = __double2float_rd(__dadd_rn(mx[d], 0.2));
+        B.k0[d] = __double2float_ru(__dsub_rn(mn[d], 0.01));
+        B.k1[d] = __double2float_rd(__dadd_rn(mx[d], 0.01));
+        B.mn[d] = mn[d];
+        B.ext[d] = __dsub_rn(mx[d], mn[d]);
+    }
+}
+
+__device__ __forceinline__ bool in_ctx(const CropBox& B, float x, float y, float z) {
+    return x >= B.c0[0] && x <= B.c1[0] && y >= B.c0[1] && y <= B.c1[1] && z >= B.c0[2] && z <= B.c1[2];
+}
+__device__ __forceinline__ bool in_core(const CropBox& B, float x, float y, float z) {
+    return x >= B.k0[0] && x <= B.k1[0] && y >= B.k0[1] && y <= B.k1[1] && z >= B.k0[2] && z <= B.k1[2];
+}
+
+// ceil((p - curmin) / (curmax - curmin) * (31, 31, 62)), then vx*31*62 + vy*62 + vz (scannet_dataset.py:49-50).  The
+// clamp only guards the bitmap: for a core member the key is always in [0, 63550].
+__device__ __forceinline__ int voxel_key(const CropBox& B, float x, float y, float z) {
+    const double vx = ceil(__dmul_rn(__ddiv_rn(__dsub_rn((double)x, B.mn[0]), B.ext[0]), 31.0));
+    const double vy = ceil(__dmul_rn(__ddiv_rn(__dsub_rn((double)y, B.mn[1]), B.ext[1]), 31.0));
+    const double vz = ceil(__dmul_rn(__ddiv_rn(__dsub_rn((double)z, B.mn[2]), B.ext[2]), 62.0));
+    const int k = (int)vx * (31 * 62) + (int)vy * 62 + (int)vz;
+    return min(max(k, 0), kKeyWords * 32 - 1);
+}
+
+__device__ __forceinline__ bool crop_scene_of(const CropArgs& a, int b, int& sc, long long& off, long long& ps) {
+    const long long v = __ldg(a.crop_scene + b);
+    if (v < 0 || v >= a.s) return false;
+    sc = (int)v;
+    off = __ldg(a.offsets + sc);
+    ps = __ldg(a.offsets + sc + 1) - off;
+    return ps > 0;
+}
+
+// grid (chunks, B).  ws: per crop, counts[10][2] then bitmap[10][kKeyWords], zeroed by the caller.
+__global__ void __launch_bounds__(kAttemptThreads) crop_attempt_kernel(CropArgs a, unsigned* __restrict__ ws) {
+    extern __shared__ unsigned s_bits[];  // [kAttempts][kKeyWords]
+    __shared__ CropBox s_box[kAttempts];
+    __shared__ int s_cnt[kAttempts][2];
+    __shared__ int s_any[kAttempts];
+    const int b = blockIdx.y;
+    int sc;
+    long long off, ps;
+    if (!crop_scene_of(a, b, sc, off, ps)) return;
+    const long long q0 = (long long)blockIdx.x * kAttemptChunk;
+    if (q0 >= ps) return;
+    const long long q1 = min(ps, q0 + kAttemptChunk);
+    if (threadIdx.x < kAttempts) {
+        crop_box(a, crop_seed(a), b, threadIdx.x, off, ps, sc, s_box[threadIdx.x]);
+        s_cnt[threadIdx.x][0] = s_cnt[threadIdx.x][1] = 0;
+        s_any[threadIdx.x] = 0;
+    }
+    for (int k = threadIdx.x; k < kAttempts * kKeyWords; k += blockDim.x) s_bits[k] = 0u;
+    __syncthreads();
+    int ctx[kAttempts], lab[kAttempts];
+#pragma unroll
+    for (int t = 0; t < kAttempts; ++t) ctx[t] = lab[t] = 0;
+    for (long long q = q0 + threadIdx.x; q < q1; q += blockDim.x) {
+        const long long g = off + q;
+        const float x = __ldg(a.xyz + 3 * g), y = __ldg(a.xyz + 3 * g + 1), z = __ldg(a.xyz + 3 * g + 2);
+        const int labelled = __ldg(a.label + g) > 0;
+#pragma unroll
+        for (int t = 0; t < kAttempts; ++t) {
+            const CropBox& B = s_box[t];
+            if (!in_ctx(B, x, y, z)) continue;
+            ++ctx[t];
+            lab[t] += labelled;
+            if (in_core(B, x, y, z)) {
+                const int key = voxel_key(B, x, y, z);
+                atomicOr(&s_bits[t * kKeyWords + (key >> 5)], 1u << (key & 31));
+                s_any[t] = 1;
+            }
+        }
+    }
+#pragma unroll
+    for (int t = 0; t < kAttempts; ++t) {
+        const int c = __reduce_add_sync(kFullMask, ctx[t]), l = __reduce_add_sync(kFullMask, lab[t]);
+        if ((threadIdx.x & 31) == 0 && c) {
+            atomicAdd(&s_cnt[t][0], c);
+            atomicAdd(&s_cnt[t][1], l);
+        }
+    }
+    __syncthreads();
+    unsigned* w = ws + (size_t)b * kCropWsWords;
+    if (threadIdx.x < kAttempts && s_cnt[threadIdx.x][0]) {
+        atomicAdd(reinterpret_cast<int*>(w) + 2 * threadIdx.x, s_cnt[threadIdx.x][0]);
+        atomicAdd(reinterpret_cast<int*>(w) + 2 * threadIdx.x + 1, s_cnt[threadIdx.x][1]);
+    }
+    for (int k = threadIdx.x; k < kAttempts * kKeyWords; k += blockDim.x) {
+        if (!s_any[k / kKeyWords]) continue;
+        const unsigned v = s_bits[k];
+        if (v) atomicOr(w + 2 * kAttempts + k, v);
+    }
+}
+
+struct CropOut {
+    float* xyz;
+    long long* label;
+    float* weight;
+    int* lengths;
+    int* point_idx;
+    unsigned char* core;
+    int* attempt;
+    unsigned char* valid;
+};
+
+// (key, scene-local index) of member j, as one 64-bit value: the row order.
+__device__ __forceinline__ unsigned long long member_order(unsigned long long seed, int b, long long j) {
+    return (crop_draw(seed, 2, (unsigned long long)b, (unsigned long long)j) >> 32 << 32) | (unsigned long long)j;
+}
+
+// One CTA per crop.  Dynamic shared memory: the sort buffer, pow2 >= npoints 64-bit values.
+__global__ void __launch_bounds__(kSelectThreads) crop_select_kernel(CropArgs a, const unsigned* __restrict__ ws, int num_class,
+                                                                     const float* __restrict__ label_weights, int npoints,
+                                                                     double max_dropout, int rotate, CropOut o) {
+    extern __shared__ unsigned long long s_keys[];
+    __shared__ int s_hist[kRadixBins];
+    __shared__ int s_w[32];
+    __shared__ int s_vox[kAttempts];
+    __shared__ CropBox s_box;
+    __shared__ int s_c, s_n, s_carry, s_digit, s_before, s_cnt;
+    __shared__ double s_cos, s_sin;
+    const int b = blockIdx.x, tid = threadIdx.x;
+    const size_t row0 = (size_t)b * npoints;
+    int sc;
+    long long off, ps;
+    if (!crop_scene_of(a, b, sc, off, ps)) {  // a scene index outside [0, S): an empty crop, attempt -1
+        for (int r = tid; r < npoints; r += blockDim.x) {
+            o.xyz[3 * (row0 + r)] = o.xyz[3 * (row0 + r) + 1] = o.xyz[3 * (row0 + r) + 2] = 0.f;
+            o.label[row0 + r] = 0;
+            o.weight[row0 + r] = 0.f;
+            o.point_idx[row0 + r] = -1;
+            o.core[row0 + r] = 0;
+        }
+        if (tid == 0) {
+            o.lengths[b] = 0;
+            o.attempt[b] = -1;
+            o.valid[b] = 0;
+        }
+        return;
+    }
+    const unsigned long long seed = crop_seed(a);
+    const unsigned* w = ws + (size_t)b * kCropWsWords;
+    // distinct voxel keys of every attempt
+    if (tid < kAttempts) s_vox[tid] = 0;
+    __syncthreads();
+    for (int t = 0; t < kAttempts; ++t) {
+        int v = 0;
+        for (int k = tid; k < kKeyWords; k += blockDim.x) v += __popc(__ldg(w + 2 * kAttempts + t * kKeyWords + k));
+        v = __reduce_add_sync(kFullMask, v);
+        if ((tid & 31) == 0 && v) atomicAdd(&s_vox[t], v);
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int att = kAttempts - 1, ok = 0;
+        for (int t = 0; t < kAttempts; ++t) {
+            const int c = (int)__ldg(w + 2 * t), l = (int)__ldg(w + 2 * t + 1);
+            const bool lab_ok = __ddiv_rn((double)l, (double)c) >= 0.7;
+            const bool vox_ok = __ddiv_rn(__ddiv_rn(__ddiv_rn((double)s_vox[t], 31.0), 31.0), 62.0) >= 0.02;
+            if (lab_ok && vox_ok) {
+                att = t;
+                ok = 1;
+                break;
+            }
+        }
+        s_c = (int)__ldg(w + 2 * att);
+        crop_box(a, seed, b, att, off, ps, sc, s_box);
+        o.attempt[b] = att;
+        o.valid[b] = (unsigned char)ok;
+        if (rotate) {
+            // theta = u * 2 pi: sincospi(2u) needs no argument reduction (2u is exact) and agrees with cos / sin of
+            // the rounded theta to within a double ulp, far below the float32 result's rounding
+            double sn, cs;
+            sincospi(__dmul_rn(crop_u(crop_draw(seed, 5, (unsigned long long)b, 0)), 2.0), &sn, &cs);
+            s_cos = cs;
+            s_sin = sn;
+        }
+        s_n = 0;
+    }
+    __syncthreads();
+    const CropBox B = s_box;
+    const int c = s_c, m = min(c, npoints);
+    // Radix select: the m smallest member orders are those whose top `bits` bits are <= prefix.  Digits of 11, 11, 10
+    // bits over the key half, then over the index half; stop as soon as the whole boundary bucket is taken.
+    unsigned long long prefix = ~0ull;
+    int bits = 0;
+    if (c > npoints) {
+        prefix = 0;
+        int need = m;
+        for (int pass = 0; pass < 6; ++pass) {
+            const int wd = pass % 3 == 2 ? 10 : 11, shift = 64 - bits - wd;
+            for (int k = tid; k < kRadixBins; k += blockDim.x) s_hist[k] = 0;
+            __syncthreads();
+            for (long long j = tid; j < ps; j += blockDim.x) {
+                const long long g = off + j;
+                if (!in_ctx(B, __ldg(a.xyz + 3 * g), __ldg(a.xyz + 3 * g + 1), __ldg(a.xyz + 3 * g + 2))) continue;
+                const unsigned long long v = member_order(seed, b, j);
+                if (bits && (v >> (64 - bits)) != prefix) continue;
+                atomicAdd(&s_hist[(int)((v >> shift) & ((1ull << wd) - 1))], 1);
+            }
+            __syncthreads();
+            const int h0 = s_hist[2 * tid], h1 = s_hist[2 * tid + 1];
+            const int ex = cta_exclusive_sum_1024(h0 + h1, s_w);
+            if (ex < need && need <= ex + h0) {
+                s_digit = 2 * tid;
+                s_before = ex;
+                s_cnt = h0;
+            } else if (ex + h0 < need && need <= ex + h0 + h1) {
+                s_digit = 2 * tid + 1;
+                s_before = ex + h0;
+                s_cnt = h1;
+            }
+            __syncthreads();
+            need -= s_before;
+            prefix = (prefix << wd) | (unsigned long long)s_digit;
+            bits += wd;
+            const bool done = s_cnt == need;
+            __syncthreads();  // s_digit / s_before / s_cnt and s_hist are rewritten by the next pass
+            if (done) break;
+        }
+    }
+    // gather the m selected member orders (in any order: the sort below fixes it) and sort them ascending
+    for (long long j = tid; j < ps; j += blockDim.x) {
+        const long long g = off + j;
+        if (!in_ctx(B, __ldg(a.xyz + 3 * g), __ldg(a.xyz + 3 * g + 1), __ldg(a.xyz + 3 * g + 2))) continue;
+        const unsigned long long v = member_order(seed, b, j);
+        if (bits && (v >> (64 - bits)) > prefix) continue;
+        s_keys[atomicAdd(&s_n, 1)] = v;
+    }
+    __syncthreads();
+    int sort_n = 1;
+    while (sort_n < m) sort_n <<= 1;
+    for (int k = m + tid; k < sort_n; k += blockDim.x) s_keys[k] = ~0ull;
+    __syncthreads();
+    for (int k = 2; k <= sort_n; k <<= 1) {
+        for (int h = k >> 1; h > 0; h >>= 1) {
+            for (int i = tid; i < sort_n; i += blockDim.x) {
+                const int p = i ^ h;
+                if (p > i) {
+                    const unsigned long long x = s_keys[i], y = s_keys[p];
+                    if ((x > y) == ((i & k) == 0)) {
+                        s_keys[i] = y;
+                        s_keys[p] = x;
+                    }
+                }
+            }
+            __syncthreads();
+        }
+    }
+    // rows: dropout compaction (row 0 always stays), then each survivor written in row order
+    const double ratio = __dmul_rn(crop_u(crop_draw(seed, 3, (unsigned long long)b, 0)), max_dropout);
+    int carry = 0;
+    for (int base = 0; base < m; base += blockDim.x) {
+        const int r = base + tid;
+        const bool dropped = r < m && crop_u(crop_draw(seed, 4, (unsigned long long)b, (unsigned long long)r)) <= ratio;
+        const int keep = r < m && (r == 0 || !dropped);
+        const int ex = cta_exclusive_sum_1024(keep, s_w);
+        if (keep) {
+            const size_t row = row0 + carry + ex;
+            const long long j = (long long)(s_keys[r] & 0xffffffffull), g = off + j;
+            const float x = __ldg(a.xyz + 3 * g), y = __ldg(a.xyz + 3 * g + 1), z = __ldg(a.xyz + 3 * g + 2);
+            const int l = __ldg(a.label + g);
+            const bool is_core = in_core(B, x, y, z);
+            float wt = (is_core && l >= 0 && l < num_class) ? __ldg(label_weights + l) : 0.f;
+            if (dropped) wt = 0.f;  // row 0 whose own draw drops it: its point stays, unweighted
+            float ox = x, oy = y;
+            if (rotate) {
+                ox = __double2float_rn(__dsub_rn(__dmul_rn((double)x, s_cos), __dmul_rn((double)y, s_sin)));
+                oy = __double2float_rn(__dadd_rn(__dmul_rn((double)x, s_sin), __dmul_rn((double)y, s_cos)));
+            }
+            o.xyz[3 * row] = ox;
+            o.xyz[3 * row + 1] = oy;
+            o.xyz[3 * row + 2] = z;
+            o.label[row] = l;
+            o.weight[row] = wt;
+            o.point_idx[row] = (int)g;
+            o.core[row] = is_core ? 1 : 0;
+        }
+        if (tid == blockDim.x - 1) s_carry = ex + keep;
+        __syncthreads();
+        carry += s_carry;
+        __syncthreads();
+    }
+    for (int r = carry + tid; r < npoints; r += blockDim.x) {
+        const size_t row = row0 + r;
+        o.xyz[3 * row] = o.xyz[3 * row + 1] = o.xyz[3 * row + 2] = 0.f;
+        o.label[row] = 0;
+        o.weight[row] = 0.f;
+        o.point_idx[row] = -1;
+        o.core[row] = 0;
+    }
+    if (tid == 0) o.lengths[b] = carry;
+}
+
+size_t crop_ws_bytes(int b) { return ((size_t)b * kCropWsWords * sizeof(unsigned) + 255) / 256 * 256; }
+int crop_sort_n(int npoints) {
+    int n = 1;
+    while (n < npoints) n <<= 1;
+    return n;
+}
+bool crop_shape_ok(int b, int npoints) {
+    return b >= 1 && b <= 65535 && npoints >= 1 && npoints <= kCropMaxPoints && (long long)b * npoints * 3 < (1ll << 31);
+}
+
+AttrOnce g_attempt_attr, g_select_attr;
+
+}  // namespace
+}  // namespace pn2
+
+extern "C" {
+
+size_t pn2_scene_crops_workspace_bytes(int b, int npoints) {
+    if (!pn2::crop_shape_ok(b, npoints)) return 0;
+    return pn2::crop_ws_bytes(b);
+}
+
+int pn2_scene_crops(int s, int p, int max_scene, const float* xyz, const int* label, const long long* offsets, const float* lo,
+                    const float* hi, int num_class, const float* label_weights, int b, const long long* crop_scene,
+                    long long seed, const long long* seed_dev, int npoints, double max_dropout, int rotate, float* out_xyz,
+                    long long* out_label, float* out_weight, int* lengths, int* point_idx, unsigned char* core, int* attempt,
+                    unsigned char* valid, void* workspace, size_t workspace_bytes, void* stream) {
+    using namespace pn2;
+    if (s < 1 || p < 1 || p >= 0x7fffffff || max_scene < 1 || max_scene > p || num_class < 1 || !crop_shape_ok(b, npoints))
+        return (int)cudaErrorInvalidValue;
+    if (!(max_dropout >= 0.0 && max_dropout <= 1.0)) return (int)cudaErrorInvalidValue;
+    if (!xyz || !label || !offsets || !lo || !hi || !label_weights || !crop_scene || !out_xyz || !out_label || !out_weight ||
+        !lengths || !point_idx || !core || !attempt || !valid || !workspace)
+        return (int)cudaErrorInvalidValue;
+    if (workspace_bytes < crop_ws_bytes(b) || !aligned_to(workspace, 256)) return (int)cudaErrorInvalidValue;
+    cudaStream_t st = as_stream(stream);
+    const size_t attempt_smem = sizeof(unsigned) * kAttempts * kKeyWords;
+    const int sort_n = crop_sort_n(npoints);
+    cudaError_t e = ensure_attrs(g_attempt_attr, crop_attempt_kernel, attempt_smem, false);
+    if (e != cudaSuccess) return (int)e;
+    e = ensure_attrs(g_select_attr, crop_select_kernel, sizeof(unsigned long long) * kCropMaxPoints, false);
+    if (e != cudaSuccess) return (int)e;
+    if ((e = cudaMemsetAsync(workspace, 0, crop_ws_bytes(b), st)) != cudaSuccess) return (int)e;
+    const CropArgs a{xyz, label, offsets, lo, hi, crop_scene, seed_dev, (unsigned long long)seed, s};
+    const dim3 grid((unsigned)((max_scene + kAttemptChunk - 1) / kAttemptChunk), (unsigned)b);
+    unsigned* ws = static_cast<unsigned*>(workspace);
+    crop_attempt_kernel<<<grid, kAttemptThreads, attempt_smem, st>>>(a, ws);
+    int rc = finish_launch();
+    if (rc) return rc;
+    const CropOut o{out_xyz, out_label, out_weight, lengths, point_idx, core, attempt, valid};
+    crop_select_kernel<<<b, kSelectThreads, sizeof(unsigned long long) * sort_n, st>>>(a, ws, num_class, label_weights, npoints,
+                                                                                      max_dropout, rotate, o);
+    return finish_launch();
+}
+
+}  // extern "C"

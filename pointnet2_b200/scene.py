@@ -278,3 +278,188 @@ class VoxelAccuracy:
                 "class_accuracy": float(per_class.mean()),
                 "calibrated_accuracy": float(np.average(per_class, weights=w)),
                 "per_class": per_class}
+
+
+# ---- training crops (scannet/scannet_dataset.py:27-60, scannet/train.py:181-197, utils/provider.py:52-70) ----------
+CROP_MAX_POINTS = 16384   # npoints cap of sample_crops: its sort buffer is npoints x 8 bytes of shared memory
+CROP_MAX_BATCH = 65535    # crops per call
+_U64 = 2 ** 64
+
+
+class SceneSet:
+    """S scenes packed into one set on the device, the training side's counterpart of a list of scene arrays.
+
+    xyz (P, 3) float32, label (P,) int32, offsets (S + 1,) int64 (scene k holds rows offsets[k] .. offsets[k + 1] - 1),
+    lo / hi (S, 3) float32, each scene's per-axis minimum and maximum as np.min / np.max give them.  ``sizes`` (numpy
+    int64) and ``label_hist`` (numpy int64, (num_class,)) stay on the host.  Construction validates everything on the
+    host and is the only place anything is read back.  ``device`` defaults to the current CUDA device; sample_crops
+    needs one."""
+
+    def __init__(self, xyz_list, label_list, num_class: int = 21, device=None):
+        if isinstance(num_class, bool) or not isinstance(num_class, int) or num_class < 1:
+            raise ValueError(f"SceneSet expects a positive integer num_class, got {num_class!r}")
+        xyz_list, label_list = list(xyz_list), list(label_list)
+        if not xyz_list:
+            raise ValueError("SceneSet expects at least one scene")
+        if len(xyz_list) != len(label_list):
+            raise ValueError(f"SceneSet expects one label array per scene, got {len(xyz_list)} scenes and "
+                             f"{len(label_list)} label arrays")
+        xyz_list, label_list = [_host(x) for x in xyz_list], [_host(lab) for lab in label_list]
+        for k, (x, lab) in enumerate(zip(xyz_list, label_list)):
+            if x.ndim != 2 or x.shape[1] != 3:
+                raise ValueError(f"SceneSet: scene {k} must be (num_points, 3), got {x.shape}")
+            if len(x) == 0:
+                raise ValueError(f"SceneSet: scene {k} is empty")
+            if lab.shape != (len(x),):
+                raise ValueError(f"SceneSet: scene {k} has {len(x)} points but labels of shape {lab.shape}")
+            if not np.issubdtype(lab.dtype, np.integer):
+                raise TypeError(f"SceneSet: scene {k} has {lab.dtype} labels, expected integers")
+        self.sizes = np.array([len(x) for x in xyz_list], np.int64)
+        if int(self.sizes.sum()) >= _I31 - 1:
+            raise ValueError(f"SceneSet takes fewer than 2^31 - 1 points in all, got {int(self.sizes.sum())}")
+        pts, labs, lo, hi = [], [], [], []
+        hist = np.zeros(num_class, np.int64)
+        for k, (x, lab) in enumerate(zip(xyz_list, label_list)):
+            x = x.astype(np.float32)
+            if not np.isfinite(x).all():
+                raise ValueError(f"SceneSet: scene {k} holds NaN or inf coordinates")
+            if np.abs(x).max() > 1e9:  # DESIGN.md §6.10: keeps the crop box's double arithmetic away from its collapse
+                raise ValueError(f"SceneSet: scene {k} has coordinates beyond 1e9 in magnitude (sample_crops' limit)")
+            mn, mx = np.min(x, axis=0), np.max(x, axis=0)
+            if not mx[2] > mn[2]:
+                raise ValueError(f"SceneSet: scene {k} has zero z extent (the voxel test divides by it)")
+            if lab.min() < 0 or lab.max() >= num_class:
+                raise ValueError(f"SceneSet: scene {k} has labels outside [0, {num_class})")
+            hist += np.bincount(lab.astype(np.int64), minlength=num_class)
+            pts.append(x)
+            labs.append(lab.astype(np.int32))
+            lo.append(mn)
+            hi.append(mx)
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.num_class = num_class
+        self.label_hist = hist
+        self.xyz = torch.from_numpy(np.concatenate(pts)).to(dev)
+        self.device = self.xyz.device  # "cuda" resolves to the current index here: compared against in sample_crops
+        self.label = torch.from_numpy(np.concatenate(labs)).to(dev)
+        self.offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(self.sizes)]).astype(np.int64)).to(dev)
+        self.lo = torch.from_numpy(np.stack(lo)).to(dev)
+        self.hi = torch.from_numpy(np.stack(hi)).to(dev)
+
+    def __len__(self) -> int:
+        return len(self.sizes)
+
+    def train_label_weights(self) -> torch.Tensor:
+        """scannet_dataset.py:17-24 over the set's labels: 1 / log(1.2 + freq), with the reference's dtypes (float64
+        counts, then float32 throughout), as a (num_class,) float32 tensor on the set's device.  The test split uses
+        torch.ones(num_class) instead (:25-26)."""
+        w = self.label_hist.astype(np.float64).astype(np.float32)
+        w = w / np.sum(w)
+        w = 1 / np.log(1.2 + w)
+        return torch.from_numpy(np.asarray(w, np.float32)).to(self.device)
+
+
+def _host(a) -> np.ndarray:
+    if isinstance(a, torch.Tensor):
+        return a.detach().cpu().numpy()
+    return np.asarray(a)
+
+
+class SceneCrops(NamedTuple):
+    """B training crops as a padded ragged batch of ``npoints`` rows, every field on the scene set's device.
+
+    xyz (B, npoints, 3) float32; label (B, npoints) int64; weight (B, npoints) float32, label_weights[label] on core
+    rows; lengths (B,) int32, >= 1 for every crop whose crop_scene value is in [0, S) and 0 for one outside it (the
+    only way a bad index can show without a read-back); point_idx (B, npoints) int32, the row of the scene set, -1 on padding; core
+    (B, npoints) bool; attempt (B,) int32, the attempt taken; valid (B,) bool, whether it passed the test.  Padding
+    rows are 0 (-1 in point_idx)."""
+    xyz: torch.Tensor
+    label: torch.Tensor
+    weight: torch.Tensor
+    lengths: torch.Tensor
+    point_idx: torch.Tensor
+    core: torch.Tensor
+    attempt: torch.Tensor
+    valid: torch.Tensor
+
+
+def sample_crops(scenes: SceneSet, crop_scene: torch.Tensor, seed, label_weights: torch.Tensor, npoints: int = 8192,
+                 max_dropout: float = 0.875, rotate: bool = True) -> SceneCrops:
+    """B random training crops of ``scenes`` on the GPU (DESIGN.md §6.10): crop i is a 1.5 m column of scene
+    crop_scene[i] with 0.2 m of context, taken from ten seeded attempts as ScannetDataset.__getitem__ takes it; its
+    rows are up to ``npoints`` of the column's points in a seeded random order, without replacement; rows after the
+    first are dropped with probability U[0, 1) * max_dropout (get_batch_wdp; max_dropout=0 is get_batch); x and y are
+    rotated about the origin by a U[0, 2 pi) angle when ``rotate`` (rotate_point_cloud_z).
+
+    ``crop_scene`` (B,) integer CUDA tensor: the scene of each crop.  ``seed``: a Python int, or a (1,) int64 CUDA tensor
+    read on the device (rewrite it in place to draw new crops from a captured CUDA graph).  Give every step and rank its
+    own seed.  ``label_weights`` (num_class,) float32 CUDA tensor, e.g. scenes.train_label_weights().  Nothing is read
+    back and the same seed gives the same bits.  A crop_scene value outside [0, S) gives an empty crop (lengths 0,
+    attempt -1): it cannot be reported without a read-back."""
+    if not isinstance(scenes, SceneSet):
+        raise TypeError(f"sample_crops expects a SceneSet, got {type(scenes).__name__}")
+    if isinstance(npoints, bool) or not isinstance(npoints, int):
+        raise TypeError(f"sample_crops expects an integer npoints, got {type(npoints).__name__}")
+    if not 1 <= npoints <= CROP_MAX_POINTS:
+        raise ValueError(f"sample_crops expects 1 <= npoints <= {CROP_MAX_POINTS} (the shared-memory sort), got {npoints}")
+    if isinstance(max_dropout, bool) or not isinstance(max_dropout, (int, float)):
+        raise TypeError(f"sample_crops expects a number for max_dropout, got {type(max_dropout).__name__}")
+    if not 0.0 <= max_dropout <= 1.0:
+        raise ValueError(f"sample_crops expects 0 <= max_dropout <= 1, got {max_dropout}")
+    if not isinstance(rotate, bool):
+        raise TypeError(f"sample_crops expects a bool rotate, got {type(rotate).__name__}")
+    dev = scenes.device
+    if dev.type != "cuda":
+        raise RuntimeError(f"sample_crops needs a SceneSet on a CUDA device: pointnet2_b200 has no CPU path (got {dev})")
+    if not isinstance(crop_scene, torch.Tensor):
+        raise TypeError(f"crop_scene must be a torch.Tensor, got {type(crop_scene).__name__}")
+    if crop_scene.dtype.is_floating_point or crop_scene.dtype.is_complex or crop_scene.dtype == torch.bool:
+        raise TypeError(f"crop_scene must be an integer tensor, got {crop_scene.dtype}")
+    if crop_scene.dim() != 1 or not 1 <= crop_scene.shape[0] <= CROP_MAX_BATCH:
+        raise ValueError(f"sample_crops expects a (B,) crop_scene with 1 <= B <= {CROP_MAX_BATCH}, got {tuple(crop_scene.shape)}")
+    if not crop_scene.is_cuda:
+        raise RuntimeError(f"crop_scene must be a CUDA tensor: pointnet2_b200 has no CPU path (got device {crop_scene.device})")
+    b = crop_scene.shape[0]
+    if b * npoints * 3 >= _I31:
+        raise ValueError(f"sample_crops: {b} crops of {npoints} rows pass 2^31 elements")
+    seed_val, seed_dev = 0, None
+    if isinstance(seed, torch.Tensor):
+        if seed.dtype != torch.int64 or tuple(seed.shape) != (1,):
+            raise TypeError(f"a tensor seed must be a (1,) int64 tensor, got {seed.dtype} {tuple(seed.shape)}")
+        if not seed.is_cuda:
+            raise RuntimeError(f"a tensor seed must be a CUDA tensor (got device {seed.device})")
+        seed_dev = seed
+    elif isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
+        raise TypeError(f"sample_crops expects an int or a (1,) int64 CUDA tensor seed, got {type(seed).__name__}")
+    else:
+        seed = int(seed)
+        if not -2 ** 63 <= seed < _U64:
+            raise ValueError(f"sample_crops expects a 64-bit seed, got {seed}")
+        seed_val = seed - _U64 if seed >= 2 ** 63 else seed   # the same 64 bits, as a signed value
+    label_weights = require_cuda(label_weights, "label_weights", torch.float32)
+    if tuple(label_weights.shape) != (scenes.num_class,):
+        raise ValueError(f"sample_crops expects ({scenes.num_class},) label_weights, got {tuple(label_weights.shape)}")
+    for name, t in (("crop_scene", crop_scene), ("label_weights", label_weights), ("seed", seed_dev)):
+        if t is not None and t.device != dev:
+            raise RuntimeError(f"{name} must be on the scene set's device {dev}, got {t.device}")
+    crop_scene = crop_scene.to(torch.int64).contiguous()
+    lib = _lib.load()
+    with on_device(scenes.xyz):
+        wsb = int(lib.pn2_scene_crops_workspace_bytes(b, npoints))
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+        out = SceneCrops(
+            xyz=torch.empty(b, npoints, 3, dtype=torch.float32, device=dev),
+            label=torch.empty(b, npoints, dtype=torch.int64, device=dev),
+            weight=torch.empty(b, npoints, dtype=torch.float32, device=dev),
+            lengths=torch.empty(b, dtype=torch.int32, device=dev),
+            point_idx=torch.empty(b, npoints, dtype=torch.int32, device=dev),
+            core=torch.empty(b, npoints, dtype=torch.bool, device=dev),
+            attempt=torch.empty(b, dtype=torch.int32, device=dev),
+            valid=torch.empty(b, dtype=torch.bool, device=dev))
+        rc = lib.pn2_scene_crops(len(scenes), int(scenes.sizes.sum()), int(scenes.sizes.max()), ptr(scenes.xyz),
+                                 ptr(scenes.label), ptr(scenes.offsets), ptr(scenes.lo), ptr(scenes.hi), scenes.num_class,
+                                 ptr(label_weights), b, ptr(crop_scene), seed_val, ptr(seed_dev), npoints,
+                                 float(max_dropout), int(rotate), ptr(out.xyz), ptr(out.label), ptr(out.weight),
+                                 ptr(out.lengths), ptr(out.point_idx), ptr(out.core), ptr(out.attempt), ptr(out.valid),
+                                 ptr(ws), wsb, stream_ptr(dev))
+    _lib.check(rc, "pn2_scene_crops")
+    return out

@@ -12,6 +12,7 @@ min(0.99, 1 - 0.5 * 0.5^(samples/200000)).
     python tools/train_ddp_demo.py --steps 30 --amp bf16                        # bf16 autocast
     python tools/train_ddp_demo.py --steps 5 --deterministic                    # reproducible: prints a weights hash
     python tools/train_ddp_demo.py --model part_seg_msg --ragged --steps 30     # part segmentation, variable sizes
+    python tools/train_ddp_demo.py --model sem_seg --scene-crops --steps 30     # training crops of synthetic rooms
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 \
         tools/train_ddp_demo.py --steps 20                                      # one rank per GPU
 
@@ -21,6 +22,9 @@ loss has something to learn and the demo can assert that it goes down.  The part
 (part_seg, part_seg_msg) train on workloads.part_shapes instead: (B, N, 6) points with normals, one
 of the 16 ShapeNet categories each, its parts the height bands of the shape.  --ragged (segmentation
 models) draws each cloud's length from U[N/2, N], fills the padding rows with NaN and passes lengths=.
+--scene-crops (sem_seg) trains on scene.sample_crops of a SceneSet of synthetic rooms (workloads.scene_room, 21
+classes): each step's scenes come from a seeded permutation of the set, each rank draws its crops on its own GPU with a
+seed derived from (step, rank), with dropout and rotation, and passes the crops' lengths and sample weights.
 """
 from __future__ import annotations
 
@@ -36,7 +40,7 @@ import torch
 import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from pointnet2_b200 import nets, workloads as W  # noqa: E402
+from pointnet2_b200 import nets, scene, workloads as W  # noqa: E402
 from pointnet2_b200.parallel import shard_batch  # noqa: E402
 
 
@@ -88,7 +92,14 @@ def main() -> None:
     ap.add_argument("--deterministic", action="store_true",
                     help="torch.use_deterministic_algorithms(True): run-to-run identical weights; prints their SHA-256")
     ap.add_argument("--ragged", action="store_true", help="cloud lengths from U[N/2, N], NaN padding, passed as lengths=")
+    ap.add_argument("--scene-crops", action="store_true",
+                    help="sem_seg only: train on seeded crops of synthetic rooms drawn on the GPU by scene.sample_crops")
+    ap.add_argument("--rooms", type=int, default=6, help="rooms in the --scene-crops set")
     args = ap.parse_args()
+    if args.scene_crops and (args.model != "sem_seg" or args.ragged):
+        raise SystemExit("--scene-crops trains the sem_seg model on its own ragged crops (no --ragged)")
+    if args.scene_crops:
+        args.num_class = 21  # the rooms' labels
     part = args.model in ("part_seg", "part_seg_msg")
     if args.deterministic:
         os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")  # read when cuBLAS starts: before the first matmul
@@ -124,6 +135,11 @@ def main() -> None:
     scaler = torch.amp.GradScaler("cuda") if args.amp == "fp16" else None
 
     rs = np.random.RandomState(1234)  # the same global batch stream on every rank; each takes its slice
+    if args.scene_crops:  # every rank builds the same set; only the crops' seeds differ between ranks
+        rooms = [W.scene_room(60000 + 20000 * k, 500 + k) for k in range(args.rooms)]
+        scenes = scene.SceneSet([r[0] for r in rooms], [r[1] for r in rooms], num_class=21, device=dev)
+        label_w = scenes.train_label_weights()
+        order = np.zeros(0, np.int64)
     losses, t_steps = [], []
     for step in range(args.steps):
         seen = step * args.batch
@@ -131,18 +147,27 @@ def main() -> None:
         for g in opt.param_groups:
             g["lr"] = lr
         nets.set_bn_momentum(model, min(0.99, 1 - 0.5 * 0.5 ** (seen // args.decay_step)))
-        if part:  # (B, N, 6) points with normals, per-point part labels, and the category
+        if args.scene_crops:
+            while len(order) < args.batch:  # the scenes of the global batch: a seeded permutation per epoch of the set
+                order = np.concatenate([order, rs.permutation(len(scenes))])
+            crop_scene = shard_batch(torch.from_numpy(order[:args.batch]), world, rank).to(dev, non_blocking=True)
+            order = order[args.batch:]
+            crops = scene.sample_crops(scenes, crop_scene, step * 65536 + rank, label_w, npoints=args.num_point)
+            xyz, lab, lengths = crops.xyz, crops.label, crops.lengths
+        elif part:  # (B, N, 6) points with normals, per-point part labels, and the category
             xyz_np, lab_np, part_np = W.part_shapes(args.batch, args.num_point, int(rs.randint(1 << 30)), nets.PART_OFFSETS)
         else:
             xyz_np, lab_np = synthetic_shapes(args.batch, args.num_point, args.num_class, rs)
-        lengths = None
+        if not args.scene_crops:
+            lengths = None
         if args.ragged:
             len_np = rs.randint(args.num_point // 2, args.num_point + 1, args.batch)
             for i, l in enumerate(len_np):
                 xyz_np[i, l:] = np.nan  # never read: only the first lengths[i] rows of cloud i are real
             lengths = shard_batch(torch.from_numpy(len_np.astype(np.int32)), world, rank).to(dev, non_blocking=True)
-        xyz = shard_batch(torch.from_numpy(xyz_np), world, rank).to(dev, non_blocking=True).contiguous()
-        lab = shard_batch(torch.from_numpy(lab_np), world, rank).to(dev, non_blocking=True)
+        if not args.scene_crops:
+            xyz = shard_batch(torch.from_numpy(xyz_np), world, rank).to(dev, non_blocking=True).contiguous()
+            lab = shard_batch(torch.from_numpy(lab_np), world, rank).to(dev, non_blocking=True)
         if part:
             lab_part = shard_batch(torch.from_numpy(part_np), world, rank).to(dev, non_blocking=True)
         torch.cuda.synchronize(dev)
@@ -155,6 +180,8 @@ def main() -> None:
                 pred, _ = net(xyz, lengths=lengths)
             if part:
                 loss = nets.part_seg_loss(pred, lab_part, lengths=lengths)
+            elif args.scene_crops:  # the crops' labels and sample weights (label weight on core rows)
+                loss = nets.sem_seg_loss(pred, lab, crops.weight, lengths=lengths)
             elif args.model == "sem_seg":  # per-point labels: the cloud's class everywhere, unit weights
                 lab_pt = lab[:, None].expand(-1, args.num_point)
                 loss = nets.sem_seg_loss(pred, lab_pt, torch.ones_like(lab_pt, dtype=torch.float32), lengths=lengths)
@@ -194,8 +221,9 @@ def main() -> None:
                "steps": args.steps, "loss_first": first, "loss_last": last, "loss_decreased": last < first,
                "weights_identical_across_ranks": same, "ms_per_step_wallclock": 1e3 * float(np.median(steady)),
                "clouds_per_s": args.batch / float(np.median(steady)),
-               "data": "synthetic part shapes" if part else "synthetic parametric shapes",
-               "deterministic": args.deterministic, "ragged": args.ragged}
+               "data": ("synthetic room crops" if args.scene_crops else
+                        "synthetic part shapes" if part else "synthetic parametric shapes"),
+               "deterministic": args.deterministic, "ragged": args.ragged, "scene_crops": args.scene_crops}
         if args.deterministic:
             h = hashlib.sha256()
             for p in model.parameters():
