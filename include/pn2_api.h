@@ -423,6 +423,30 @@ int pn2_scene_crops(int s, int p, int max_scene, const float* xyz, const int* la
                     long long* out_label, float* out_weight, int* lengths, int* point_idx, unsigned char* core, int* attempt,
                     unsigned char* valid, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- shape batches (modelnet_dataset.py:60-84, modelnet_h5_dataset.py:72-114, utils/provider.py:40-234,
+ * part_seg/part_dataset_all_normal.py:83-112, evaluate.py:117-158; DESIGN.md §6.11) -------------------------------
+ * A shape set: s shapes packed into xyz (p,3) f32, normals (p,3) f32 or NULL, part (p) int32 or NULL, label (s) int32,
+ * offsets (s+1) int64 (shape k holds rows offsets[k] .. offsets[k+1]-1, none empty; max_shape = the largest shape,
+ * <= 16384).  Entry e is drawn from shape shape_idx[e] (int64, device; b entries) with the counter-based draws of
+ * DESIGN.md §6.11 keyed by the seed (*seed_dev when seed_dev is not NULL, read on the device, else `seed`): the m
+ * smallest (hash key, row) pairs of its pool (rows 0 .. min(P, npoints)-1, or all P rows when subset_random), rows
+ * r >= 1 dropped with probability u * max_dropout, then xyz' = (p M) s + t + j and n' = n M in double, rounded once:
+ * M = Ry(theta) Rp (rotate, perturb), s in [scale_lo, scale_hi) (scale_on), t in [-shift, shift), j = clip(jitter_sigma
+ * N(0,1), +-jitter_clip) per coordinate (jitter_on); a step that is off is the identity.  votes > 0: b * votes entries,
+ * entry e = v*b + i the vote v of shape_idx[i], rotated by v / votes of a turn about y, its first npoints rows in a
+ * seeded order; every other step must then be off.  Outputs (E, npoints), E the entries: out_points (x3, or x6 with
+ * with_normals) f32, out_part int64 (NULL: not written; needs part), point_idx int32 (row of the set, -1 on padding);
+ * per entry out_label int64, lengths int32.  Padding rows are 0 / -1.  A shape_idx value outside [0, s) gives lengths 0.
+ * npoints <= 16384, E * npoints * channels < 2^31, 0 <= max_dropout <= 1, shift >= 0, jitter_clip > 0.  No workspace.
+ * Same bits on every run; nothing is read back, so the call can be captured in a CUDA graph.  Invalid arguments return
+ * cudaErrorInvalidValue without a launch. */
+int pn2_shape_batch(int s, int p, int max_shape, const float* xyz, const float* normals, const int* label, const int* part,
+                    const long long* offsets, int b, const long long* shape_idx, long long seed, const long long* seed_dev,
+                    int votes, int npoints, int subset_random, int rotate, int perturb, int scale_on, double scale_lo,
+                    double scale_hi, double shift, int jitter_on, double jitter_sigma, double jitter_clip,
+                    double max_dropout, int with_normals, float* out_points, long long* out_label, long long* out_part,
+                    int* lengths, int* point_idx, void* stream);
+
 /* ---- host-buffer entry point (the reference feeds numpy through feed_dict) ----------------- */
 
 /* One SSG set-abstraction sampling+grouping layer (farthest_point_sample + gather_point +

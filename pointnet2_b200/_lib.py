@@ -84,6 +84,10 @@ _SIGNATURES = {
     "pn2_scene_crops_workspace_bytes": (c_size_t, [c_int, c_int]),
     "pn2_scene_crops": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, c_int, _P, c_int, _P, c_longlong, _P, c_int, c_double,
                                 c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    # shape batches of a shape set: seeded rows, dropout and augmentation, or rotated votes
+    "pn2_shape_batch": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, c_int, _P, c_longlong, _P, c_int, c_int, c_int,
+                                c_int, c_int, c_int, c_double, c_double, c_double, c_int, c_double, c_double, c_double,
+                                c_int, _P, _P, _P, _P, _P, _P]),
     "pn2_sa_layer_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "pn2_sa_layer_host": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_api_version": (c_int, []),

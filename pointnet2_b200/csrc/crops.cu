@@ -24,7 +24,6 @@ constexpr int kAttemptThreads = 512;
 constexpr int kAttemptChunk = 8192;      // scene points per CTA of the attempt pass
 constexpr int kSelectThreads = 1024;
 constexpr int kRadixBins = 2048;
-constexpr unsigned long long kGolden = 0x9E3779B97F4A7C15ull;
 
 struct CropArgs {
     const float* xyz;
@@ -37,22 +36,6 @@ struct CropArgs {
     unsigned long long seed;
     int s;
 };
-
-__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
-    x ^= x >> 30;
-    x *= 0xBF58476D1CE4E5B9ull;
-    x ^= x >> 27;
-    x *= 0x94D049BB133111EBull;
-    x ^= x >> 31;
-    return x;
-}
-
-__device__ __forceinline__ unsigned long long crop_draw(unsigned long long seed, unsigned long long stream,
-                                                        unsigned long long b, unsigned long long i) {
-    return mix64(mix64(mix64(seed + stream * kGolden) + b * kGolden) + i * kGolden);
-}
-
-__device__ __forceinline__ double crop_u(unsigned long long d) { return (double)(d >> 11) * 0x1.0p-53; }
 
 __device__ __forceinline__ unsigned long long crop_seed(const CropArgs& a) {
     return a.seed_dev ? (unsigned long long)__ldg(a.seed_dev) : a.seed;
@@ -67,7 +50,7 @@ struct CropBox {
 
 __device__ __forceinline__ void crop_box(const CropArgs& a, unsigned long long seed, int b, int att, long long off, long long ps,
                                          int sc, CropBox& B) {
-    const long long ci = off + (long long)(crop_draw(seed, 1, (unsigned long long)b, (unsigned long long)att) % (unsigned long long)ps);
+    const long long ci = off + (long long)(rng_draw(seed, 1, (unsigned long long)b, (unsigned long long)att) % (unsigned long long)ps);
     double mn[3], mx[3];
     for (int d = 0; d < 2; ++d) {
         const double c = (double)__ldg(a.xyz + 3 * ci + d);
@@ -186,7 +169,7 @@ struct CropOut {
 
 // (key, scene-local index) of member j, as one 64-bit value: the row order.
 __device__ __forceinline__ unsigned long long member_order(unsigned long long seed, int b, long long j) {
-    return (crop_draw(seed, 2, (unsigned long long)b, (unsigned long long)j) >> 32 << 32) | (unsigned long long)j;
+    return (rng_draw(seed, 2, (unsigned long long)b, (unsigned long long)j) >> 32 << 32) | (unsigned long long)j;
 }
 
 // One CTA per crop.  Dynamic shared memory: the sort buffer, pow2 >= npoints 64-bit values.
@@ -251,7 +234,7 @@ __global__ void __launch_bounds__(kSelectThreads) crop_select_kernel(CropArgs a,
             // theta = u * 2 pi: sincospi(2u) needs no argument reduction (2u is exact) and agrees with cos / sin of
             // the rounded theta to within a double ulp, far below the float32 result's rounding
             double sn, cs;
-            sincospi(__dmul_rn(crop_u(crop_draw(seed, 5, (unsigned long long)b, 0)), 2.0), &sn, &cs);
+            sincospi(__dmul_rn(rng_unit(rng_draw(seed, 5, (unsigned long long)b, 0)), 2.0), &sn, &cs);
             s_cos = cs;
             s_sin = sn;
         }
@@ -328,11 +311,11 @@ __global__ void __launch_bounds__(kSelectThreads) crop_select_kernel(CropArgs a,
         }
     }
     // rows: dropout compaction (row 0 always stays), then each survivor written in row order
-    const double ratio = __dmul_rn(crop_u(crop_draw(seed, 3, (unsigned long long)b, 0)), max_dropout);
+    const double ratio = __dmul_rn(rng_unit(rng_draw(seed, 3, (unsigned long long)b, 0)), max_dropout);
     int carry = 0;
     for (int base = 0; base < m; base += blockDim.x) {
         const int r = base + tid;
-        const bool dropped = r < m && crop_u(crop_draw(seed, 4, (unsigned long long)b, (unsigned long long)r)) <= ratio;
+        const bool dropped = r < m && rng_unit(rng_draw(seed, 4, (unsigned long long)b, (unsigned long long)r)) <= ratio;
         const int keep = r < m && (r == 0 || !dropped);
         const int ex = cta_exclusive_sum_1024(keep, s_w);
         if (keep) {

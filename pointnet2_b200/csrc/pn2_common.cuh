@@ -197,6 +197,27 @@ __device__ __forceinline__ int cta_exclusive_sum_1024(int v, int* s_w) {
     return __shfl_sync(kFullMask, winc - wv, warp) + incl - v;
 }
 
+// ---- counter-based random draws (DESIGN.md §6.10; crops.cu, shapes.cu) --------------------------------------------
+// rng_draw(seed, stream, e, i) = mix(mix(mix(seed + stream*G) + e*G) + i*G) with mix = SplitMix64's finaliser, in
+// uint64 wrap-around arithmetic; rng_unit maps a draw to a double in [0, 1).  tests/crop_oracle.py restates both.
+constexpr unsigned long long kRngGolden = 0x9E3779B97F4A7C15ull;
+
+__device__ __forceinline__ unsigned long long rng_mix64(unsigned long long x) {
+    x ^= x >> 30;
+    x *= 0xBF58476D1CE4E5B9ull;
+    x ^= x >> 27;
+    x *= 0x94D049BB133111EBull;
+    x ^= x >> 31;
+    return x;
+}
+
+__device__ __forceinline__ unsigned long long rng_draw(unsigned long long seed, unsigned long long stream,
+                                                       unsigned long long e, unsigned long long i) {
+    return rng_mix64(rng_mix64(rng_mix64(seed + stream * kRngGolden) + e * kRngGolden) + i * kRngGolden);
+}
+
+__device__ __forceinline__ double rng_unit(unsigned long long d) { return (double)(d >> 11) * 0x1.0p-53; }
+
 // ---- uniform grid over one cloud, for the ball query (ball_query_grid.cu, sa_fused.cu) ---------------------------
 constexpr int kGridMaxDim = 16;  // cells per axis
 

@@ -13,6 +13,7 @@ min(0.99, 1 - 0.5 * 0.5^(samples/200000)).
     python tools/train_ddp_demo.py --steps 5 --deterministic                    # reproducible: prints a weights hash
     python tools/train_ddp_demo.py --model part_seg_msg --ragged --steps 30     # part segmentation, variable sizes
     python tools/train_ddp_demo.py --model sem_seg --scene-crops --steps 30     # training crops of synthetic rooms
+    python tools/train_ddp_demo.py --shape-set --votes 12 --steps 30            # augmented shape batches, voted accuracy
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 \
         tools/train_ddp_demo.py --steps 20                                      # one rank per GPU
 
@@ -25,6 +26,11 @@ models) draws each cloud's length from U[N/2, N], fills the padding rows with Na
 --scene-crops (sem_seg) trains on scene.sample_crops of a SceneSet of synthetic rooms (workloads.scene_room, 21
 classes): each step's scenes come from a seeded permutation of the set, each rank draws its crops on its own GPU with a
 seed derived from (step, rank), with dropout and rotation, and passes the crops' lengths and sample weights.
+--shape-set (cls_ssg, cls_msg, part_seg, part_seg_msg) builds one shapes.ShapeSet of synthetic shapes (--set-shapes of
+--set-points points: the parametric shapes above, or workloads.part_shapes for the part models) and trains on
+shapes.sample_shapes batches drawn on the GPU with a seed derived from (step, rank): ModelNet's augmentation for the
+classification nets, the ShapeNet part recipe (random rows, jitter, normals) for the part nets.  --votes V then prints
+the accuracy of shapes.classify_votes with V rotated votes on a held-out synthetic set (classification nets).
 """
 from __future__ import annotations
 
@@ -40,7 +46,7 @@ import torch
 import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from pointnet2_b200 import nets, scene, workloads as W  # noqa: E402
+from pointnet2_b200 import nets, scene, shapes, workloads as W  # noqa: E402
 from pointnet2_b200.parallel import shard_batch  # noqa: E402
 
 
@@ -95,7 +101,17 @@ def main() -> None:
     ap.add_argument("--scene-crops", action="store_true",
                     help="sem_seg only: train on seeded crops of synthetic rooms drawn on the GPU by scene.sample_crops")
     ap.add_argument("--rooms", type=int, default=6, help="rooms in the --scene-crops set")
+    ap.add_argument("--shape-set", action="store_true",
+                    help="cls / part models: train on augmented batches of a synthetic ShapeSet drawn by shapes.sample_shapes")
+    ap.add_argument("--set-shapes", type=int, default=256, help="shapes in the --shape-set set (and in its held-out set)")
+    ap.add_argument("--set-points", type=int, default=2048, help="points per shape of the --shape-set sets")
+    ap.add_argument("--votes", type=int, default=0,
+                    help="with --shape-set (cls models): accuracy of shapes.classify_votes with this many votes")
     args = ap.parse_args()
+    if args.shape_set and (args.model == "sem_seg" or args.ragged or args.scene_crops):
+        raise SystemExit("--shape-set trains the cls / part models on their own ragged batches (no --ragged)")
+    if args.votes and (not args.shape_set or args.model not in ("cls_ssg", "cls_msg")):
+        raise SystemExit("--votes scores a classification model trained with --shape-set")
     if args.scene_crops and (args.model != "sem_seg" or args.ragged):
         raise SystemExit("--scene-crops trains the sem_seg model on its own ragged crops (no --ragged)")
     if args.scene_crops:
@@ -140,6 +156,18 @@ def main() -> None:
         scenes = scene.SceneSet([r[0] for r in rooms], [r[1] for r in rooms], num_class=21, device=dev)
         label_w = scenes.train_label_weights()
         order = np.zeros(0, np.int64)
+    if args.shape_set:  # every rank builds the same set; only the batches' seeds differ between ranks
+        if part:
+            pts6, cat, parts = W.part_shapes(args.set_shapes, args.set_points, 77, nets.PART_OFFSETS)
+            shape_set = shapes.ShapeSet(list(pts6[:, :, :3]), cat, list(pts6[:, :, 3:]), list(parts), num_class=16,
+                                        normalize=False, device=dev)
+            recipe = dict(subset="random", rotate=False, perturb=False, scale=None, shift=0, with_normals=True)
+        else:
+            pts, cat = synthetic_shapes(args.set_shapes, args.set_points, args.num_class, np.random.RandomState(77))
+            shape_set = shapes.ShapeSet(list(pts), cat, num_class=args.num_class, device=dev)
+            recipe = {}
+        order = np.zeros(0, np.int64)
+    device_data = args.scene_crops or args.shape_set
     losses, t_steps = [], []
     for step in range(args.steps):
         seen = step * args.batch
@@ -154,21 +182,30 @@ def main() -> None:
             order = order[args.batch:]
             crops = scene.sample_crops(scenes, crop_scene, step * 65536 + rank, label_w, npoints=args.num_point)
             xyz, lab, lengths = crops.xyz, crops.label, crops.lengths
+        elif args.shape_set:
+            while len(order) < args.batch:  # the shapes of the global batch: a seeded permutation per epoch of the set
+                order = np.concatenate([order, rs.permutation(len(shape_set))])
+            shape_idx = shard_batch(torch.from_numpy(order[:args.batch]), world, rank).to(dev, non_blocking=True)
+            order = order[args.batch:]
+            batch = shapes.sample_shapes(shape_set, shape_idx, step * 65536 + rank, npoints=args.num_point, **recipe)
+            xyz, lab, lengths = batch.points, batch.label, batch.lengths
+            if part:
+                lab_part = batch.part
         elif part:  # (B, N, 6) points with normals, per-point part labels, and the category
             xyz_np, lab_np, part_np = W.part_shapes(args.batch, args.num_point, int(rs.randint(1 << 30)), nets.PART_OFFSETS)
         else:
             xyz_np, lab_np = synthetic_shapes(args.batch, args.num_point, args.num_class, rs)
-        if not args.scene_crops:
+        if not device_data:
             lengths = None
         if args.ragged:
             len_np = rs.randint(args.num_point // 2, args.num_point + 1, args.batch)
             for i, l in enumerate(len_np):
                 xyz_np[i, l:] = np.nan  # never read: only the first lengths[i] rows of cloud i are real
             lengths = shard_batch(torch.from_numpy(len_np.astype(np.int32)), world, rank).to(dev, non_blocking=True)
-        if not args.scene_crops:
+        if not device_data:
             xyz = shard_batch(torch.from_numpy(xyz_np), world, rank).to(dev, non_blocking=True).contiguous()
             lab = shard_batch(torch.from_numpy(lab_np), world, rank).to(dev, non_blocking=True)
-        if part:
+        if part and not args.shape_set:
             lab_part = shard_batch(torch.from_numpy(part_np), world, rank).to(dev, non_blocking=True)
         torch.cuda.synchronize(dev)
         t0 = time.perf_counter()
@@ -204,6 +241,21 @@ def main() -> None:
         if rank == 0:
             print(f"step {step:3d}  loss {losses[-1]:.4f}  lr {lr:.2e}  {t_steps[-1] * 1e3:7.1f} ms", flush=True)
 
+    voted = None
+    if args.votes:  # a held-out set of the same kinds of shapes, 16 shapes per call as evaluate.py's BATCH_SIZE
+        pts, cat = synthetic_shapes(args.set_shapes, args.set_points, args.num_class, np.random.RandomState(99))
+        test_set = shapes.ShapeSet(list(pts), cat, num_class=args.num_class, device=dev)
+        model.eval()
+        preds = []
+        for b0 in range(0, len(test_set), 16):
+            idx = torch.arange(b0, min(len(test_set), b0 + 16), device=dev)
+            preds.append(shapes.classify_votes(model, test_set, idx, args.votes, 1 << 40, npoints=args.num_point).argmax(1))
+        acc, class_acc = shapes.cls_accuracy(torch.cat(preds), test_set.label.long(), args.num_class)
+        voted = {"votes": args.votes, "shapes": len(test_set), "accuracy": float(acc), "class_accuracy": float(class_acc)}
+        if rank == 0:
+            print(f"voted accuracy ({args.votes} votes, {len(test_set)} held-out shapes): {voted['accuracy']:.4f}  "
+                  f"mean class accuracy {voted['class_accuracy']:.4f}", flush=True)
+
     # weights must be identical on every rank after data-parallel training
     flat = torch.cat([p.detach().reshape(-1) for p in model.parameters()])
     checksum = flat.double().sum()
@@ -223,7 +275,10 @@ def main() -> None:
                "clouds_per_s": args.batch / float(np.median(steady)),
                "data": ("synthetic room crops" if args.scene_crops else
                         "synthetic part shapes" if part else "synthetic parametric shapes"),
-               "deterministic": args.deterministic, "ragged": args.ragged, "scene_crops": args.scene_crops}
+               "deterministic": args.deterministic, "ragged": args.ragged, "scene_crops": args.scene_crops,
+               "shape_set": args.shape_set}
+        if voted is not None:
+            out["voted"] = voted
         if args.deterministic:
             h = hashlib.sha256()
             for p in model.parameters():
