@@ -447,6 +447,29 @@ int pn2_shape_batch(int s, int p, int max_shape, const float* xyz, const float* 
                     double max_dropout, int with_normals, float* out_points, long long* out_label, long long* out_part,
                     int* lengths, int* point_idx, void* stream);
 
+/* ---- virtual scans (scannet/scene_util.py virtual_scan, scannet/scannet_dataset.py:122-166; DESIGN.md §6.12) -------
+ * A scene set as for pn2_scene_crops, plus mean (s,3) f64, each scene's mean in float64.  Entry i of b scans scene
+ * scan_scene[i] (int64, device) from the view scan_mode[i] (int64, device): -1 a random view from the counter-based
+ * draws of DESIGN.md §6.12 keyed by the seed (*seed_dev when seed_dev is not NULL, read on the device, else `seed`),
+ * any other m the fixed view at azimuth pi/4 m.  200 x 150 rays; a point is near when its nearest ray in (azimuth,
+ * elevation) is within 0.01 (ties: the lower ray), and visible when it is near, at least 100 points are near, and its
+ * range is the minimum over the near points of its ray.  The rows are the m = min(visible, npoints) visible points of
+ * smallest (hash key, scene-local index), in that order.  Outputs (b, npoints): out_xyz (x3) f32 (the scene's own
+ * coordinates), out_label int64, out_weight f32 (label_weights[label], 0 on every row of an invalid entry), point_idx
+ * int32 (row of the scene set, -1 on padding); per entry lengths int32 (m), visible int32 (the visible points; 0 when
+ * fewer than 100 are near; -1 for a scan_scene value outside [0, s), with lengths 0), valid u8 (visible >= min_points).
+ * Padding rows are 0 / -1.  npoints <= 16384, b <= 4096, b*npoints*3 < 2^31, min_points >= 0.  The workspace is
+ * pn2_virtual_scans_workspace_bytes(b, max_scene, npoints) bytes, 256-byte aligned (0 = invalid shape); it holds
+ * per-entry ray tables, cell offsets and z-buffers and a bitmap of max_scene bits per entry.  Same bits on every run;
+ * nothing is read back, so the call can be captured in a CUDA graph.  Invalid arguments return cudaErrorInvalidValue
+ * without a launch. */
+size_t pn2_virtual_scans_workspace_bytes(int b, int max_scene, int npoints);
+int pn2_virtual_scans(int s, int p, int max_scene, const float* xyz, const int* label, const long long* offsets,
+                      const double* mean, int num_class, const float* label_weights, int b, const long long* scan_scene,
+                      const long long* scan_mode, long long seed, const long long* seed_dev, int npoints, int min_points,
+                      float* out_xyz, long long* out_label, float* out_weight, int* lengths, int* point_idx, int* visible,
+                      unsigned char* valid, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- host-buffer entry point (the reference feeds numpy through feed_dict) ----------------- */
 
 /* One SSG set-abstraction sampling+grouping layer (farthest_point_sample + gather_point +

@@ -88,6 +88,10 @@ _SIGNATURES = {
     "pn2_shape_batch": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, c_int, _P, c_longlong, _P, c_int, c_int, c_int,
                                 c_int, c_int, c_int, c_double, c_double, c_double, c_int, c_double, c_double, c_double,
                                 c_int, _P, _P, _P, _P, _P, _P]),
+    # virtual scans of a scene set: the points a camera sees from one view, as a padded ragged batch
+    "pn2_virtual_scans_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "pn2_virtual_scans": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, c_int, _P, c_int, _P, _P, c_longlong, _P, c_int, c_int,
+                                  _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_sa_layer_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "pn2_sa_layer_host": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_api_version": (c_int, []),

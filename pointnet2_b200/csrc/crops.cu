@@ -6,9 +6,9 @@
 //   attempt: CTA (chunk, crop) reads a chunk of the crop's scene once and tests the boxes of all ten attempts: integer
 //            context / labelled counts and the core voxel-key bitmap in shared memory, merged into the crop's workspace
 //            with integer atomicAdd / atomicOr (order-free);
-//   select:  one CTA per crop takes the first valid attempt (else attempt 9), radix-selects the m smallest
-//            (key, scene index) pairs of its members, recomputing every key from the hash on each pass, sorts them in
-//            shared memory and writes the rows (dropout compaction, rotation, labels, weights, padding).
+//   select:  one CTA per crop takes the first valid attempt (else attempt 9), takes the m smallest (key, scene index)
+//            pairs of its members in order (cta_select_sorted) and writes the rows (dropout compaction, rotation,
+//            labels, weights, padding).
 // Every membership test is the double test of the definition, done exactly in float32: for a float p and a double t,
 // (double)p >= t <=> p >= (t rounded up to float), and (double)p <= t <=> p <= (t rounded down to float).
 #include "pn2_common.cuh"
@@ -23,7 +23,6 @@ constexpr int kCropMaxPoints = 16384;    // sort buffer: 16384 x 8 B of shared m
 constexpr int kAttemptThreads = 512;
 constexpr int kAttemptChunk = 8192;      // scene points per CTA of the attempt pass
 constexpr int kSelectThreads = 1024;
-constexpr int kRadixBins = 2048;
 
 struct CropArgs {
     const float* xyz;
@@ -177,11 +176,10 @@ __global__ void __launch_bounds__(kSelectThreads) crop_select_kernel(CropArgs a,
                                                                      const float* __restrict__ label_weights, int npoints,
                                                                      double max_dropout, int rotate, CropOut o) {
     extern __shared__ unsigned long long s_keys[];
-    __shared__ int s_hist[kRadixBins];
-    __shared__ int s_w[32];
+    __shared__ SelectScratch s_sel;
     __shared__ int s_vox[kAttempts];
     __shared__ CropBox s_box;
-    __shared__ int s_c, s_n, s_carry, s_digit, s_before, s_cnt;
+    __shared__ int s_c, s_carry;
     __shared__ double s_cos, s_sin;
     const int b = blockIdx.x, tid = threadIdx.x;
     const size_t row0 = (size_t)b * npoints;
@@ -238,78 +236,18 @@ __global__ void __launch_bounds__(kSelectThreads) crop_select_kernel(CropArgs a,
             s_cos = cs;
             s_sin = sn;
         }
-        s_n = 0;
     }
     __syncthreads();
     const CropBox B = s_box;
     const int c = s_c, m = min(c, npoints);
-    // Radix select: the m smallest member orders are those whose top `bits` bits are <= prefix.  Digits of 11, 11, 10
-    // bits over the key half, then over the index half; stop as soon as the whole boundary bucket is taken.
-    unsigned long long prefix = ~0ull;
-    int bits = 0;
-    if (c > npoints) {
-        prefix = 0;
-        int need = m;
-        for (int pass = 0; pass < 6; ++pass) {
-            const int wd = pass % 3 == 2 ? 10 : 11, shift = 64 - bits - wd;
-            for (int k = tid; k < kRadixBins; k += blockDim.x) s_hist[k] = 0;
-            __syncthreads();
-            for (long long j = tid; j < ps; j += blockDim.x) {
-                const long long g = off + j;
-                if (!in_ctx(B, __ldg(a.xyz + 3 * g), __ldg(a.xyz + 3 * g + 1), __ldg(a.xyz + 3 * g + 2))) continue;
-                const unsigned long long v = member_order(seed, b, j);
-                if (bits && (v >> (64 - bits)) != prefix) continue;
-                atomicAdd(&s_hist[(int)((v >> shift) & ((1ull << wd) - 1))], 1);
-            }
-            __syncthreads();
-            const int h0 = s_hist[2 * tid], h1 = s_hist[2 * tid + 1];
-            const int ex = cta_exclusive_sum_1024(h0 + h1, s_w);
-            if (ex < need && need <= ex + h0) {
-                s_digit = 2 * tid;
-                s_before = ex;
-                s_cnt = h0;
-            } else if (ex + h0 < need && need <= ex + h0 + h1) {
-                s_digit = 2 * tid + 1;
-                s_before = ex + h0;
-                s_cnt = h1;
-            }
-            __syncthreads();
-            need -= s_before;
-            prefix = (prefix << wd) | (unsigned long long)s_digit;
-            bits += wd;
-            const bool done = s_cnt == need;
-            __syncthreads();  // s_digit / s_before / s_cnt and s_hist are rewritten by the next pass
-            if (done) break;
-        }
-    }
-    // gather the m selected member orders (in any order: the sort below fixes it) and sort them ascending
-    for (long long j = tid; j < ps; j += blockDim.x) {
-        const long long g = off + j;
-        if (!in_ctx(B, __ldg(a.xyz + 3 * g), __ldg(a.xyz + 3 * g + 1), __ldg(a.xyz + 3 * g + 2))) continue;
-        const unsigned long long v = member_order(seed, b, j);
-        if (bits && (v >> (64 - bits)) > prefix) continue;
-        s_keys[atomicAdd(&s_n, 1)] = v;
-    }
-    __syncthreads();
-    int sort_n = 1;
-    while (sort_n < m) sort_n <<= 1;
-    for (int k = m + tid; k < sort_n; k += blockDim.x) s_keys[k] = ~0ull;
-    __syncthreads();
-    for (int k = 2; k <= sort_n; k <<= 1) {
-        for (int h = k >> 1; h > 0; h >>= 1) {
-            for (int i = tid; i < sort_n; i += blockDim.x) {
-                const int p = i ^ h;
-                if (p > i) {
-                    const unsigned long long x = s_keys[i], y = s_keys[p];
-                    if ((x > y) == ((i & k) == 0)) {
-                        s_keys[i] = y;
-                        s_keys[p] = x;
-                    }
-                }
-            }
-            __syncthreads();
-        }
-    }
+    // the m smallest member orders, sorted
+    cta_select_sorted(
+        ps, c, m,
+        [&](long long j) {
+            const long long g = off + j;
+            return in_ctx(B, __ldg(a.xyz + 3 * g), __ldg(a.xyz + 3 * g + 1), __ldg(a.xyz + 3 * g + 2));
+        },
+        [&](long long j) { return member_order(seed, b, j); }, s_keys, s_sel);
     // rows: dropout compaction (row 0 always stays), then each survivor written in row order
     const double ratio = __dmul_rn(rng_unit(rng_draw(seed, 3, (unsigned long long)b, 0)), max_dropout);
     int carry = 0;
@@ -317,7 +255,7 @@ __global__ void __launch_bounds__(kSelectThreads) crop_select_kernel(CropArgs a,
         const int r = base + tid;
         const bool dropped = r < m && rng_unit(rng_draw(seed, 4, (unsigned long long)b, (unsigned long long)r)) <= ratio;
         const int keep = r < m && (r == 0 || !dropped);
-        const int ex = cta_exclusive_sum_1024(keep, s_w);
+        const int ex = cta_exclusive_sum_1024(keep, s_sel.w);
         if (keep) {
             const size_t row = row0 + carry + ex;
             const long long j = (long long)(s_keys[r] & 0xffffffffull), g = off + j;

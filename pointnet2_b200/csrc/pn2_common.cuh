@@ -197,7 +197,7 @@ __device__ __forceinline__ int cta_exclusive_sum_1024(int v, int* s_w) {
     return __shfl_sync(kFullMask, winc - wv, warp) + incl - v;
 }
 
-// ---- counter-based random draws (DESIGN.md §6.10; crops.cu, shapes.cu) --------------------------------------------
+// ---- counter-based random draws (DESIGN.md §6.10; crops.cu, shapes.cu, vscan.cu) ----------------------------------
 // rng_draw(seed, stream, e, i) = mix(mix(mix(seed + stream*G) + e*G) + i*G) with mix = SplitMix64's finaliser, in
 // uint64 wrap-around arithmetic; rng_unit maps a draw to a double in [0, 1).  tests/crop_oracle.py restates both.
 constexpr unsigned long long kRngGolden = 0x9E3779B97F4A7C15ull;
@@ -217,6 +217,92 @@ __device__ __forceinline__ unsigned long long rng_draw(unsigned long long seed, 
 }
 
 __device__ __forceinline__ double rng_unit(unsigned long long d) { return (double)(d >> 11) * 0x1.0p-53; }
+
+// ---- seeded row selection (crops.cu, shapes.cu, vscan.cu) ----------------------------------------------------------
+constexpr int kSelectRadixBins = 2048;
+
+struct SelectScratch {  // shared memory of cta_select_sorted
+    int hist[kSelectRadixBins];
+    int w[32];
+    int digit, before, cnt, n;
+};
+
+// The m smallest orders among the members of [0, n), sorted ascending into s_keys[0 .. m), by a 1024-thread CTA.
+// member(j) says whether j is a member and order(j) gives its distinct 64-bit order; c is the number of members and
+// c >= m.  s_keys holds pow2 >= m values.  When c > m a radix select first finds the m smallest: they are those whose
+// top `bits` bits are <= prefix, found with digits of 11, 11, 10 bits over the high half of the orders, then over the
+// low half, stopping as soon as the whole boundary bucket is taken.  Every order is recomputed on each pass, so
+// nothing per member is stored.  Every thread must call it; it ends with a barrier.
+template <typename Member, typename Order>
+__device__ __forceinline__ void cta_select_sorted(long long n, int c, int m, Member&& member, Order&& order,
+                                                  unsigned long long* s_keys, SelectScratch& s) {
+    const int tid = threadIdx.x;
+    unsigned long long prefix = ~0ull;
+    int bits = 0;
+    if (c > m) {
+        prefix = 0;
+        int need = m;
+        for (int pass = 0; pass < 6; ++pass) {
+            const int wd = pass % 3 == 2 ? 10 : 11, shift = 64 - bits - wd;
+            for (int k = tid; k < kSelectRadixBins; k += blockDim.x) s.hist[k] = 0;
+            __syncthreads();
+            for (long long j = tid; j < n; j += blockDim.x) {
+                if (!member(j)) continue;
+                const unsigned long long v = order(j);
+                if (bits && (v >> (64 - bits)) != prefix) continue;
+                atomicAdd(&s.hist[(int)((v >> shift) & ((1ull << wd) - 1))], 1);
+            }
+            __syncthreads();
+            const int h0 = s.hist[2 * tid], h1 = s.hist[2 * tid + 1];
+            const int ex = cta_exclusive_sum_1024(h0 + h1, s.w);
+            if (ex < need && need <= ex + h0) {
+                s.digit = 2 * tid;
+                s.before = ex;
+                s.cnt = h0;
+            } else if (ex + h0 < need && need <= ex + h0 + h1) {
+                s.digit = 2 * tid + 1;
+                s.before = ex + h0;
+                s.cnt = h1;
+            }
+            __syncthreads();
+            need -= s.before;
+            prefix = (prefix << wd) | (unsigned long long)s.digit;
+            bits += wd;
+            const bool done = s.cnt == need;
+            __syncthreads();  // digit / before / cnt and hist are rewritten by the next pass
+            if (done) break;
+        }
+    }
+    // gather the m selected orders (in any order: the sort below fixes it) and sort them ascending
+    if (tid == 0) s.n = 0;
+    __syncthreads();
+    for (long long j = tid; j < n; j += blockDim.x) {
+        if (!member(j)) continue;
+        const unsigned long long v = order(j);
+        if (bits && (v >> (64 - bits)) > prefix) continue;
+        s_keys[atomicAdd(&s.n, 1)] = v;
+    }
+    __syncthreads();
+    int sort_n = 1;
+    while (sort_n < m) sort_n <<= 1;
+    for (int k = m + tid; k < sort_n; k += blockDim.x) s_keys[k] = ~0ull;
+    __syncthreads();
+    for (int k = 2; k <= sort_n; k <<= 1) {
+        for (int h = k >> 1; h > 0; h >>= 1) {
+            for (int i = tid; i < sort_n; i += blockDim.x) {
+                const int p = i ^ h;
+                if (p > i) {
+                    const unsigned long long x = s_keys[i], y = s_keys[p];
+                    if ((x > y) == ((i & k) == 0)) {
+                        s_keys[i] = y;
+                        s_keys[p] = x;
+                    }
+                }
+            }
+            __syncthreads();
+        }
+    }
+}
 
 // ---- uniform grid over one cloud, for the ball query (ball_query_grid.cu, sa_fused.cu) ---------------------------
 constexpr int kGridMaxDim = 16;  // cells per axis

@@ -2,16 +2,14 @@
 // augmentation steps of utils/provider.py (modelnet_dataset.py:60-72, part_seg/part_dataset_all_normal.py:83-112), and
 // the rotated votes of evaluate.py:117-158, as a padded ragged batch (DESIGN.md §6.11).
 //
-// One kernel, one 1024-thread CTA per entry, nothing read back: the CTA draws the entry's transform, radix-selects the
-// m smallest (key, row) pairs of its pool when the pool is larger than npoints (recomputing every key from the hash on
-// each pass), sorts them in shared memory, and writes the rows with the dropout compaction.
+// One kernel, one 1024-thread CTA per entry, nothing read back: the CTA draws the entry's transform, takes the m
+// smallest (key, row) pairs of its pool in order (cta_select_sorted), and writes the rows with the dropout compaction.
 #include "pn2_common.cuh"
 
 namespace pn2 {
 namespace {
 
 constexpr int kShapeMaxPoints = 16384;  // sort buffer: 16384 x 8 B of shared memory
-constexpr int kShapeRadixBins = 2048;
 constexpr int kShapeThreads = 1024;
 constexpr double kPi = 3.141592653589793;
 // random streams of DESIGN.md §6.11
@@ -80,9 +78,8 @@ struct EntryXform {
 // One CTA per entry.  Dynamic shared memory: the sort buffer, pow2 >= m 64-bit values.
 __global__ void __launch_bounds__(kShapeThreads) shape_batch_kernel(ShapeArgs a, ShapeOut o) {
     extern __shared__ unsigned long long s_keys[];
-    __shared__ int s_hist[kShapeRadixBins];
-    __shared__ int s_w[32];
-    __shared__ int s_carry, s_digit, s_before, s_cnt;
+    __shared__ SelectScratch s_sel;
+    __shared__ int s_carry;
     __shared__ EntryXform s_x;
     const int tid = threadIdx.x;
     const unsigned long long e = blockIdx.x;
@@ -152,72 +149,8 @@ __global__ void __launch_bounds__(kShapeThreads) shape_batch_kernel(ShapeArgs a,
     // the pool: rows 0 .. q-1 of the shape; its m smallest row orders are the entry's rows
     const int q = (a.subset_random && !a.votes) ? (int)ps : (int)min(ps, (long long)npoints);
     const int m = min(q, npoints);
-    unsigned long long prefix = ~0ull;
-    int bits = 0;
-    if (q > m) {
-        // Radix select, as crop_select_kernel: the m smallest orders are those whose top `bits` bits are <= prefix.
-        // Digits of 11, 11, 10 bits over the key half, then over the row half; stop as soon as the whole boundary bucket
-        // is taken.
-        prefix = 0;
-        int need = m;
-        for (int pass = 0; pass < 6; ++pass) {
-            const int wd = pass % 3 == 2 ? 10 : 11, shift = 64 - bits - wd;
-            for (int k = tid; k < kShapeRadixBins; k += blockDim.x) s_hist[k] = 0;
-            __syncthreads();
-            for (int j = tid; j < q; j += blockDim.x) {
-                const unsigned long long val = row_order(seed, e, j);
-                if (bits && (val >> (64 - bits)) != prefix) continue;
-                atomicAdd(&s_hist[(int)((val >> shift) & ((1ull << wd) - 1))], 1);
-            }
-            __syncthreads();
-            const int h0 = s_hist[2 * tid], h1 = s_hist[2 * tid + 1];
-            const int ex = cta_exclusive_sum_1024(h0 + h1, s_w);
-            if (ex < need && need <= ex + h0) {
-                s_digit = 2 * tid;
-                s_before = ex;
-                s_cnt = h0;
-            } else if (ex + h0 < need && need <= ex + h0 + h1) {
-                s_digit = 2 * tid + 1;
-                s_before = ex + h0;
-                s_cnt = h1;
-            }
-            __syncthreads();
-            need -= s_before;
-            prefix = (prefix << wd) | (unsigned long long)s_digit;
-            bits += wd;
-            const bool done = s_cnt == need;
-            __syncthreads();  // s_digit / s_before / s_cnt and s_hist are rewritten by the next pass
-            if (done) break;
-        }
-    }
-    // gather the m selected orders (in any order: the sort below fixes it) and sort them ascending
-    if (tid == 0) s_cnt = 0;
-    __syncthreads();
-    for (int j = tid; j < q; j += blockDim.x) {
-        const unsigned long long val = row_order(seed, e, j);
-        if (bits && (val >> (64 - bits)) > prefix) continue;
-        s_keys[atomicAdd(&s_cnt, 1)] = val;
-    }
-    __syncthreads();
-    int sort_n = 1;
-    while (sort_n < m) sort_n <<= 1;
-    for (int k = m + tid; k < sort_n; k += blockDim.x) s_keys[k] = ~0ull;
-    __syncthreads();
-    for (int k = 2; k <= sort_n; k <<= 1) {
-        for (int h = k >> 1; h > 0; h >>= 1) {
-            for (int i = tid; i < sort_n; i += blockDim.x) {
-                const int p = i ^ h;
-                if (p > i) {
-                    const unsigned long long x = s_keys[i], y = s_keys[p];
-                    if ((x > y) == ((i & k) == 0)) {
-                        s_keys[i] = y;
-                        s_keys[p] = x;
-                    }
-                }
-            }
-            __syncthreads();
-        }
-    }
+    cta_select_sorted(
+        q, q, m, [](long long) { return true; }, [&](long long j) { return row_order(seed, e, (int)j); }, s_keys, s_sel);
     // rows: dropout compaction (row 0 always stays), then each survivor transformed and written in row order
     const EntryXform& X = s_x;
     const bool drop_on = !a.votes && a.max_dropout > 0.0, shift_on = !a.votes && a.shift > 0.0;
@@ -228,7 +161,7 @@ __global__ void __launch_bounds__(kShapeThreads) shape_batch_kernel(ShapeArgs a,
         const bool dropped = drop_on && r >= 1 && r < m &&
                              rng_unit(rng_draw(seed, kStreamDrop, e, (unsigned long long)r)) <= X.ratio;
         const int keep = r < m && !dropped;
-        const int ex = cta_exclusive_sum_1024(keep, s_w);
+        const int ex = cta_exclusive_sum_1024(keep, s_sel.w);
         if (keep) {
             const size_t row = row0 + carry + ex;
             const int j = (int)(s_keys[r] & 0xffffffffull);

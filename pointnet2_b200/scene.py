@@ -290,7 +290,8 @@ class SceneSet:
     """S scenes packed into one set on the device, the training side's counterpart of a list of scene arrays.
 
     xyz (P, 3) float32, label (P,) int32, offsets (S + 1,) int64 (scene k holds rows offsets[k] .. offsets[k + 1] - 1),
-    lo / hi (S, 3) float32, each scene's per-axis minimum and maximum as np.min / np.max give them.  ``sizes`` (numpy
+    lo / hi (S, 3) float32, each scene's per-axis minimum and maximum as np.min / np.max give them, mean (S, 3) float64,
+    each scene's np.mean(x.astype(np.float64), axis=0) (the virtual scans' room centre).  ``sizes`` (numpy
     int64) and ``label_hist`` (numpy int64, (num_class,)) stay on the host.  Construction validates everything on the
     host and is the only place anything is read back.  ``device`` defaults to the current CUDA device; sample_crops
     needs one."""
@@ -317,7 +318,7 @@ class SceneSet:
         self.sizes = np.array([len(x) for x in xyz_list], np.int64)
         if int(self.sizes.sum()) >= _I31 - 1:
             raise ValueError(f"SceneSet takes fewer than 2^31 - 1 points in all, got {int(self.sizes.sum())}")
-        pts, labs, lo, hi = [], [], [], []
+        pts, labs, lo, hi, mean = [], [], [], [], []
         hist = np.zeros(num_class, np.int64)
         for k, (x, lab) in enumerate(zip(xyz_list, label_list)):
             x = x.astype(np.float32)
@@ -335,6 +336,7 @@ class SceneSet:
             labs.append(lab.astype(np.int32))
             lo.append(mn)
             hi.append(mx)
+            mean.append(np.mean(x.astype(np.float64), axis=0))
         dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
         self.num_class = num_class
         self.label_hist = hist
@@ -344,6 +346,7 @@ class SceneSet:
         self.offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(self.sizes)]).astype(np.int64)).to(dev)
         self.lo = torch.from_numpy(np.stack(lo)).to(dev)
         self.hi = torch.from_numpy(np.stack(hi)).to(dev)
+        self.mean = torch.from_numpy(np.stack(mean)).to(dev)
 
     def __len__(self) -> int:
         return len(self.sizes)
@@ -462,4 +465,118 @@ def sample_crops(scenes: SceneSet, crop_scene: torch.Tensor, seed, label_weights
                                  ptr(out.lengths), ptr(out.point_idx), ptr(out.core), ptr(out.attempt), ptr(out.valid),
                                  ptr(ws), wsb, stream_ptr(dev))
     _lib.check(rc, "pn2_scene_crops")
+    return out
+
+
+# ---- virtual scans (scannet/scene_util.py virtual_scan, scannet/scannet_dataset.py:122-166) ------------------------
+SCAN_MAX_BATCH = 4096     # entries per call of sample_virtual_scans: its workspace is about 1.7 MB per entry
+SCAN_VIEWS = 8            # the dataset's fixed views: azimuth pi/4 m for m = 0..7
+
+
+class SceneScans(NamedTuple):
+    """B virtual scans as a padded ragged batch of ``npoints`` rows, every field on the scene set's device.
+
+    xyz (B, npoints, 3) float32, the scene's own coordinates (not centred or rotated); label (B, npoints) int64; weight
+    (B, npoints) float32, label_weights[label], 0 on every row of an invalid entry; lengths (B,) int32, min(visible,
+    npoints); point_idx (B, npoints) int32, the row of the scene set, -1 on padding; visible (B,) int32, the number of
+    points the scan sees (0 when fewer than 100 points are near a ray, -1 for a scan_scene value outside [0, S), the only
+    way a bad index can show without a read-back); valid (B,) bool, visible >= min_points.  Padding rows are 0 (-1 in
+    point_idx)."""
+    xyz: torch.Tensor
+    label: torch.Tensor
+    weight: torch.Tensor
+    lengths: torch.Tensor
+    point_idx: torch.Tensor
+    visible: torch.Tensor
+    valid: torch.Tensor
+
+
+def _index_tensor(t, name: str, what: str, max_batch: int) -> torch.Tensor:
+    if not isinstance(t, torch.Tensor):
+        raise TypeError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
+    if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+        raise TypeError(f"{name} must be an integer tensor, got {t.dtype}")
+    if t.dim() != 1 or not 1 <= t.shape[0] <= max_batch:
+        raise ValueError(f"{what} expects a (B,) {name} with 1 <= B <= {max_batch}, got {tuple(t.shape)}")
+
+
+def sample_virtual_scans(scenes: SceneSet, scan_scene: torch.Tensor, scan_mode: torch.Tensor, seed,
+                         label_weights: torch.Tensor, npoints: int = 8192, min_points: int = 300) -> SceneScans:
+    """B virtual scans of ``scenes`` on the GPU (DESIGN.md §6.12): entry i is what a camera 1.5 m high, behind the
+    centre of scene scan_scene[i], sees through a 200 x 150 grid of rays, as scene_util.virtual_scan computes it; its
+    rows are up to ``npoints`` of the visible points in a seeded random order, without replacement.
+
+    ``scan_scene`` (B,) integer CUDA tensor: the scene of each entry.  ``scan_mode`` (B,) integer CUDA tensor: -1 draws
+    a random view from the seed (virtual_scan(mode=-1)); any other m is the fixed view at azimuth pi/4 m (the dataset
+    uses m = 0..7).  ``seed``: a Python int, or a (1,) int64 CUDA tensor read on the device (rewrite it in place to draw
+    new scans from a captured CUDA graph).  ``label_weights`` (num_class,) float32 CUDA tensor:
+    scenes.train_label_weights() for the train split, torch.ones(num_class) for the test split.  An entry with fewer
+    than ``min_points`` visible points stays in the batch, flagged invalid with weight 0 (the reference drops it).
+    Nothing is read back and the same seed gives the same bits."""
+    what = "sample_virtual_scans"
+    if not isinstance(scenes, SceneSet):
+        raise TypeError(f"{what} expects a SceneSet, got {type(scenes).__name__}")
+    if isinstance(npoints, bool) or not isinstance(npoints, int):
+        raise TypeError(f"{what} expects an integer npoints, got {type(npoints).__name__}")
+    if not 1 <= npoints <= CROP_MAX_POINTS:
+        raise ValueError(f"{what} expects 1 <= npoints <= {CROP_MAX_POINTS} (the shared-memory sort), got {npoints}")
+    if isinstance(min_points, bool) or not isinstance(min_points, int):
+        raise TypeError(f"{what} expects an integer min_points, got {type(min_points).__name__}")
+    if not 0 <= min_points < _I31:
+        raise ValueError(f"{what} expects 0 <= min_points < 2^31, got {min_points}")
+    dev = scenes.device
+    if dev.type != "cuda":
+        raise RuntimeError(f"{what} needs a SceneSet on a CUDA device: pointnet2_b200 has no CPU path (got {dev})")
+    _index_tensor(scan_scene, "scan_scene", what, SCAN_MAX_BATCH)
+    _index_tensor(scan_mode, "scan_mode", what, SCAN_MAX_BATCH)
+    b = scan_scene.shape[0]
+    if scan_mode.shape[0] != b:
+        raise ValueError(f"{what} expects one scan_mode per scan_scene, got {scan_mode.shape[0]} and {b}")
+    for name, t in (("scan_scene", scan_scene), ("scan_mode", scan_mode)):
+        if not t.is_cuda:
+            raise RuntimeError(f"{name} must be a CUDA tensor: pointnet2_b200 has no CPU path (got device {t.device})")
+    if b * npoints * 3 >= _I31:
+        raise ValueError(f"{what}: {b} scans of {npoints} rows pass 2^31 elements")
+    seed_val, seed_dev = 0, None
+    if isinstance(seed, torch.Tensor):
+        if seed.dtype != torch.int64 or tuple(seed.shape) != (1,):
+            raise TypeError(f"a tensor seed must be a (1,) int64 tensor, got {seed.dtype} {tuple(seed.shape)}")
+        if not seed.is_cuda:
+            raise RuntimeError(f"a tensor seed must be a CUDA tensor (got device {seed.device})")
+        seed_dev = seed
+    elif isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
+        raise TypeError(f"{what} expects an int or a (1,) int64 CUDA tensor seed, got {type(seed).__name__}")
+    else:
+        seed = int(seed)
+        if not -2 ** 63 <= seed < _U64:
+            raise ValueError(f"{what} expects a 64-bit seed, got {seed}")
+        seed_val = seed - _U64 if seed >= 2 ** 63 else seed   # the same 64 bits, as a signed value
+    label_weights = require_cuda(label_weights, "label_weights", torch.float32)
+    if tuple(label_weights.shape) != (scenes.num_class,):
+        raise ValueError(f"{what} expects ({scenes.num_class},) label_weights, got {tuple(label_weights.shape)}")
+    for name, t in (("scan_scene", scan_scene), ("scan_mode", scan_mode), ("label_weights", label_weights),
+                    ("seed", seed_dev)):
+        if t is not None and t.device != dev:
+            raise RuntimeError(f"{name} must be on the scene set's device {dev}, got {t.device}")
+    scan_scene = scan_scene.to(torch.int64).contiguous()
+    scan_mode = scan_mode.to(torch.int64).contiguous()
+    lib = _lib.load()
+    max_scene = int(scenes.sizes.max())
+    with on_device(scenes.xyz):
+        wsb = int(lib.pn2_virtual_scans_workspace_bytes(b, max_scene, npoints))
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+        out = SceneScans(
+            xyz=torch.empty(b, npoints, 3, dtype=torch.float32, device=dev),
+            label=torch.empty(b, npoints, dtype=torch.int64, device=dev),
+            weight=torch.empty(b, npoints, dtype=torch.float32, device=dev),
+            lengths=torch.empty(b, dtype=torch.int32, device=dev),
+            point_idx=torch.empty(b, npoints, dtype=torch.int32, device=dev),
+            visible=torch.empty(b, dtype=torch.int32, device=dev),
+            valid=torch.empty(b, dtype=torch.bool, device=dev))
+        rc = lib.pn2_virtual_scans(len(scenes), int(scenes.sizes.sum()), max_scene, ptr(scenes.xyz), ptr(scenes.label),
+                                   ptr(scenes.offsets), ptr(scenes.mean), scenes.num_class, ptr(label_weights), b,
+                                   ptr(scan_scene), ptr(scan_mode), seed_val, ptr(seed_dev), npoints, min_points,
+                                   ptr(out.xyz), ptr(out.label), ptr(out.weight), ptr(out.lengths), ptr(out.point_idx),
+                                   ptr(out.visible), ptr(out.valid), ptr(ws), wsb, stream_ptr(dev))
+    _lib.check(rc, "pn2_virtual_scans")
     return out

@@ -28,7 +28,8 @@ SHOW = ["fps_cta_kernel<16, 256, 0, false>", "fps_cta_kernel<16, 256, 1, false>"
         "mbn_norm_relu_kernel<float, 4, true>", "mbn_norm_relu_kernel<__nv_bfloat16, 4, true>", "mbn_bwd_sums_kernel<float, 4, true>",
         "mbn_bwd_sums_kernel<__nv_bfloat16, 4, true>", "mbn_bwd_finalize_kernel", "mbn_bwd_dx_kernel<float, 4, true>", "mbn_bwd_dx_kernel<__nv_bfloat16, 4, true>",
         "scene_count_kernel", "scene_scan_kernel", "scene_fill_kernel", "scene_merge_kernel<float>", "scene_merge_kernel<__nv_bfloat16>",
-        "scene_merge_kernel<__half>", "crop_attempt_kernel", "crop_select_kernel", "shape_batch_kernel"]
+        "scene_merge_kernel<__half>", "crop_attempt_kernel", "crop_select_kernel", "shape_batch_kernel",
+        "vscan_ray_kernel", "vscan_cell_kernel", "vscan_point_kernel", "vscan_select_kernel"]
 
 
 def demangle(names):

@@ -101,6 +101,9 @@ def main() -> None:
     ap.add_argument("--scene-crops", action="store_true",
                     help="sem_seg only: train on seeded crops of synthetic rooms drawn on the GPU by scene.sample_crops")
     ap.add_argument("--rooms", type=int, default=6, help="rooms in the --scene-crops set")
+    ap.add_argument("--scan-eval", action="store_true",
+                    help="with --scene-crops: after training, the voxel accuracy on the valid fixed-view virtual scans "
+                         "(scene.sample_virtual_scans) of held-out synthetic rooms")
     ap.add_argument("--shape-set", action="store_true",
                     help="cls / part models: train on augmented batches of a synthetic ShapeSet drawn by shapes.sample_shapes")
     ap.add_argument("--set-shapes", type=int, default=256, help="shapes in the --shape-set set (and in its held-out set)")
@@ -114,6 +117,8 @@ def main() -> None:
         raise SystemExit("--votes scores a classification model trained with --shape-set")
     if args.scene_crops and (args.model != "sem_seg" or args.ragged):
         raise SystemExit("--scene-crops trains the sem_seg model on its own ragged crops (no --ragged)")
+    if args.scan_eval and not args.scene_crops:
+        raise SystemExit("--scan-eval scores a sem_seg model trained with --scene-crops")
     if args.scene_crops:
         args.num_class = 21  # the rooms' labels
     part = args.model in ("part_seg", "part_seg_msg")
@@ -256,6 +261,33 @@ def main() -> None:
             print(f"voted accuracy ({args.votes} votes, {len(test_set)} held-out shapes): {voted['accuracy']:.4f}  "
                   f"mean class accuracy {voted['class_accuracy']:.4f}", flush=True)
 
+    scanned = None
+    if args.scan_eval:  # train on crops of whole rooms, test on virtual scans (the paper's ScanNet robustness check)
+        held = [W.scene_room(60000 + 20000 * k, 900 + k) for k in range(3)]
+        test_scenes = scene.SceneSet([r[0] for r in held], [r[1] for r in held], num_class=21, device=dev)
+        views = scene.SCAN_VIEWS
+        scans = scene.sample_virtual_scans(test_scenes, torch.arange(len(held) * views, device=dev) // views,
+                                           torch.arange(views, device=dev).repeat(len(held)), 1 << 41,
+                                           torch.ones(21, device=dev), npoints=args.num_point)
+        model.eval()
+        metric = scene.VoxelAccuracy(21, device=dev)
+        valid = scans.valid.cpu().tolist()
+        lengths_h = scans.lengths.cpu().tolist()
+        with torch.no_grad():
+            for b0 in range(0, len(valid), 8):
+                pred, _ = model(scans.xyz[b0:b0 + 8], scans.lengths[b0:b0 + 8])
+                for i in range(b0, min(b0 + 8, len(valid))):
+                    if valid[i]:
+                        n = lengths_h[i]
+                        metric.update(scans.xyz[i, :n], scans.label[i, :n], pred[i - b0, :n].argmax(-1))
+        r = metric.results()
+        scanned = {"rooms": len(held), "scans": len(valid), "valid_scans": int(sum(valid)),
+                   "accuracy": r["accuracy"], "class_accuracy": r["class_accuracy"],
+                   "calibrated_accuracy": r["calibrated_accuracy"]}
+        if rank == 0:
+            print(f"virtual-scan voxel accuracy ({scanned['valid_scans']} valid scans of {len(held)} held-out rooms): "
+                  f"{scanned['accuracy']:.4f}  mean class accuracy {scanned['class_accuracy']:.4f}", flush=True)
+
     # weights must be identical on every rank after data-parallel training
     flat = torch.cat([p.detach().reshape(-1) for p in model.parameters()])
     checksum = flat.double().sum()
@@ -279,6 +311,8 @@ def main() -> None:
                "shape_set": args.shape_set}
         if voted is not None:
             out["voted"] = voted
+        if scanned is not None:
+            out["virtual_scans"] = scanned
         if args.deterministic:
             h = hashlib.sha256()
             for p in model.parameters():
