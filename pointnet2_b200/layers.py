@@ -27,8 +27,15 @@ from . import _lib
 from ._tensor import DTYPE_CODES, FEATURE_DTYPES, on_device, ptr, stream_ptr
 
 
+# tf_util.batch_norm_template calls tf.contrib.layers.batch_norm without an epsilon, so the reference normalises with
+# its default 1e-3, not torch's 1e-5.  It matters where the pre-BN variance is small: at sa1 of the sem-seg net (radius
+# 0.1) it is a few 1e-4 at init.
+BN_EPS = 1e-3
+
+
 class SharedMLP(nn.Module):
-    """conv2d(1x1)+BN+ReLU stack on (..., C) tensors — tf_util.conv2d with xavier weights, zero bias."""
+    """conv2d(1x1)+BN+ReLU stack on (..., C) tensors — tf_util.conv2d with xavier weights, zero bias, and the
+    reference's batch-norm epsilon (BN_EPS)."""
 
     def __init__(self, in_channels: int, widths: Sequence[int], bn: bool = True, last_activation: bool = True):
         super().__init__()
@@ -41,7 +48,7 @@ class SharedMLP(nn.Module):
             layers.append(lin)
             act = last_activation or i + 1 < len(widths)
             if bn and act:
-                layers.append(nn.BatchNorm1d(int(w)))
+                layers.append(nn.BatchNorm1d(int(w), eps=BN_EPS))
             if act:
                 layers.append(nn.ReLU(inplace=True))
             c = int(w)
@@ -90,15 +97,15 @@ def masked_batch_norm(bn: nn.BatchNorm1d, x: torch.Tensor, keep: torch.Tensor) -
     """``bn`` on the rows of x (R, C) where keep (R, 1) is True.  Training mode: normalised with the mean and (biased)
     variance of those rows, and the running statistics are updated from them as BatchNorm1d would from a batch made of
     them alone (unbiased variance, momentum or the cumulative average, num_batches_tracked).  Eval mode: the running
-    statistics, as bn itself.  The statistics are float32 whatever x's dtype (as torch's batch norm keeps them under
-    autocast); the result has x's dtype, and its padding rows are left for the caller to zero.  The padding rows of x
+    statistics, as bn itself.  The statistics are float32 for float32 and 16-bit x (as torch's batch norm keeps them
+    under autocast) and float64 for float64 x; the result has x's dtype, and its padding rows are left for the caller to zero.  The padding rows of x
     must be 0 (the caller zeroes them), so the mean is a plain sum over every row.  The variance is a second pass over
     the centred real rows, not E[x^2] - mean^2, which cancels catastrophically once |mean| is large against the
     standard deviation.  The row count stays on the device: nothing synchronises with the host."""
     if not bn.training and bn.running_mean is not None:
         return bn(x)
-    xf = x.float()
-    cnt = keep.sum(dtype=torch.float32)
+    xf = x.to(torch.promote_types(x.dtype, torch.float32))  # float64 keeps float64
+    cnt = keep.sum(dtype=xf.dtype)
     mean = xf.sum(0) / cnt
     centred = xf - mean
     d = torch.where(keep, centred, 0)
