@@ -3,13 +3,15 @@
 Mirrors the reference OpKernels' OP_REQUIRES checks (tf_ops/sampling/tf_sampling.cpp:99,105,131,135;
 tf_ops/grouping/tf_grouping.cpp:71-84,90,96; tf_ops/3d_interpolation/tf_interpolate.cpp:163-168,
 197-206): shape / attribute violations raise ValueError (TensorFlow: InvalidArgument), wrong dtypes
-raise TypeError.  Tensors must live on a CUDA device: there is no CPU path.
+raise TypeError.  Tensors must live on a CUDA device: there is no CPU path.  The seeded samplers (scene.py, shapes.py)
+share their set packing and their seed, index and npoints checks here.
 """
 from __future__ import annotations
 
 import ctypes
 from contextlib import contextmanager
 
+import numpy as np
 import torch
 
 
@@ -61,7 +63,6 @@ def device_lengths(lengths, b: int, n: int, device: torch.device, op: str):
             raise TypeError(f"{op} expects integer lengths, got {lengths.dtype}")
         host = lengths.detach().to(torch.int64)
     else:
-        import numpy as np
         arr = np.asarray(lengths)
         if arr.size and not np.issubdtype(arr.dtype, np.integer):
             raise TypeError(f"{op} expects integer lengths, got {arr.dtype}")
@@ -71,6 +72,87 @@ def device_lengths(lengths, b: int, n: int, device: torch.device, op: str):
     if b and (int(host.min()) < 1 or int(host.max()) > n):
         raise ValueError(f"{op} expects 1 <= lengths <= {n} (the padded number of points), got {host.tolist()}")
     return host.to(torch.int32).to(device)
+
+
+I31 = 2 ** 31
+SELECT_MAX_ROWS = 16384  # npoints cap of the samplers: their row sort is npoints x 8 bytes of shared memory
+
+
+def to_host(a) -> np.ndarray:
+    if isinstance(a, torch.Tensor):
+        return a.detach().cpu().numpy()
+    return np.asarray(a)
+
+
+def pack_offsets(arrays, owner: str, device):
+    """(sizes, offsets) of a set packed from ``arrays``: sizes (S,) numpy int64, kept on the host, and offsets (S + 1,)
+    int64 on ``device`` (default: the current CUDA device), member k holding rows offsets[k] .. offsets[k + 1] - 1.
+    Refuses 2^31 - 1 rows or more in all: rows and their ends are int32 in the kernels."""
+    sizes = np.array([len(a) for a in arrays], np.int64)
+    if int(sizes.sum()) >= I31 - 1:
+        raise ValueError(f"{owner} takes fewer than 2^31 - 1 points in all, got {int(sizes.sum())}")
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    return sizes, torch.from_numpy(np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)).to(dev)
+
+
+def on_set_device(t: torch.Tensor, name: str, dev: torch.device) -> None:
+    if t.device != dev:
+        raise RuntimeError(f"{name} must be on the set's device {dev}, got {t.device}")
+
+
+def check_npoints(npoints, op: str) -> None:
+    if isinstance(npoints, bool) or not isinstance(npoints, int):
+        raise TypeError(f"{op} expects an integer npoints, got {type(npoints).__name__}")
+    if not 1 <= npoints <= SELECT_MAX_ROWS:
+        raise ValueError(f"{op} expects 1 <= npoints <= {SELECT_MAX_ROWS} (the shared-memory sort), got {npoints}")
+
+
+def check_dropout(max_dropout, op: str) -> None:
+    if isinstance(max_dropout, bool) or not isinstance(max_dropout, (int, float)):
+        raise TypeError(f"{op} expects a number for max_dropout, got {type(max_dropout).__name__}")
+    if not 0.0 <= max_dropout <= 1.0:
+        raise ValueError(f"{op} expects 0 <= max_dropout <= 1, got {max_dropout}")
+
+
+def index_tensors(op: str, dev: torch.device, max_batch=None, **named) -> tuple:
+    """The (B,) integer CUDA tensors that give each of a call's B entries its set member (and mode), 1 <= B (<=
+    max_batch), on the set's device ``dev``, as the contiguous int64 tensors the kernels read.  Their values are not read
+    back: the kernels turn a member index outside the set into an empty entry."""
+    for name, t in named.items():
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
+        if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
+            raise TypeError(f"{name} must be an integer tensor, got {t.dtype}")
+        if t.dim() != 1 or t.shape[0] < 1 or (max_batch is not None and t.shape[0] > max_batch):
+            bound = "B >= 1" if max_batch is None else f"1 <= B <= {max_batch}"
+            raise ValueError(f"{op} expects a (B,) {name} with {bound}, got {tuple(t.shape)}")
+    (first, t0), *rest = named.items()
+    for name, t in rest:
+        if t.shape[0] != t0.shape[0]:
+            raise ValueError(f"{op} expects one {name} per {first}, got {t.shape[0]} and {t0.shape[0]}")
+    for name, t in named.items():
+        if not t.is_cuda:
+            raise RuntimeError(f"{name} must be a CUDA tensor: pointnet2_b200 has no CPU path (got device {t.device})")
+        on_set_device(t, name, dev)
+    return tuple(t.to(torch.int64).contiguous() for t in named.values())
+
+
+def seed_args(seed, op: str, dev: torch.device):
+    """(value, tensor or None) of a sampler's seed: a Python int as its 64 bits (signed), or a (1,) int64 CUDA tensor
+    on the set's device ``dev``, which the kernels read on the device."""
+    if isinstance(seed, torch.Tensor):
+        if seed.dtype != torch.int64 or tuple(seed.shape) != (1,):
+            raise TypeError(f"a tensor seed must be a (1,) int64 tensor, got {seed.dtype} {tuple(seed.shape)}")
+        if not seed.is_cuda:
+            raise RuntimeError(f"a tensor seed must be a CUDA tensor (got device {seed.device})")
+        on_set_device(seed, "seed", dev)
+        return 0, seed
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
+        raise TypeError(f"{op} expects an int or a (1,) int64 CUDA tensor seed, got {type(seed).__name__}")
+    seed = int(seed)
+    if not -2 ** 63 <= seed < 2 ** 64:
+        raise ValueError(f"{op} expects a 64-bit seed, got {seed}")
+    return (seed - 2 ** 64 if seed >= 2 ** 63 else seed), None
 
 
 def same_device(*ts: torch.Tensor) -> None:

@@ -19,7 +19,6 @@ namespace {
 constexpr int kAttempts = 10;            // scannet_dataset.py:37
 constexpr int kKeyWords = 1986;          // keys 0 .. 32*31*62 + 32*62 + 62 = 63550 -> 63551 bits
 constexpr int kCropWsWords = kAttempts * 2 + kAttempts * kKeyWords;  // per crop: (context, labelled) x 10, 10 bitmaps
-constexpr int kCropMaxPoints = 16384;    // sort buffer: 16384 x 8 B of shared memory
 constexpr int kAttemptThreads = 512;
 constexpr int kAttemptChunk = 8192;      // scene points per CTA of the attempt pass
 constexpr int kSelectThreads = 1024;
@@ -35,10 +34,6 @@ struct CropArgs {
     unsigned long long seed;
     int s;
 };
-
-__device__ __forceinline__ unsigned long long crop_seed(const CropArgs& a) {
-    return a.seed_dev ? (unsigned long long)__ldg(a.seed_dev) : a.seed;
-}
 
 // One attempt's box: context and core bounds as exact float thresholds, and curmin / curmax - curmin for the keys.
 struct CropBox {
@@ -85,15 +80,6 @@ __device__ __forceinline__ int voxel_key(const CropBox& B, float x, float y, flo
     return min(max(k, 0), kKeyWords * 32 - 1);
 }
 
-__device__ __forceinline__ bool crop_scene_of(const CropArgs& a, int b, int& sc, long long& off, long long& ps) {
-    const long long v = __ldg(a.crop_scene + b);
-    if (v < 0 || v >= a.s) return false;
-    sc = (int)v;
-    off = __ldg(a.offsets + sc);
-    ps = __ldg(a.offsets + sc + 1) - off;
-    return ps > 0;
-}
-
 // grid (chunks, B).  ws: per crop, counts[10][2] then bitmap[10][kKeyWords], zeroed by the caller.
 __global__ void __launch_bounds__(kAttemptThreads) crop_attempt_kernel(CropArgs a, unsigned* __restrict__ ws) {
     extern __shared__ unsigned s_bits[];  // [kAttempts][kKeyWords]
@@ -103,12 +89,12 @@ __global__ void __launch_bounds__(kAttemptThreads) crop_attempt_kernel(CropArgs 
     const int b = blockIdx.y;
     int sc;
     long long off, ps;
-    if (!crop_scene_of(a, b, sc, off, ps)) return;
+    if (!set_entry(a.crop_scene, b, a.s, a.offsets, sc, off, ps)) return;
     const long long q0 = (long long)blockIdx.x * kAttemptChunk;
     if (q0 >= ps) return;
     const long long q1 = min(ps, q0 + kAttemptChunk);
     if (threadIdx.x < kAttempts) {
-        crop_box(a, crop_seed(a), b, threadIdx.x, off, ps, sc, s_box[threadIdx.x]);
+        crop_box(a, rng_seed(a.seed_dev, a.seed), b, threadIdx.x, off, ps, sc, s_box[threadIdx.x]);
         s_cnt[threadIdx.x][0] = s_cnt[threadIdx.x][1] = 0;
         s_any[threadIdx.x] = 0;
     }
@@ -166,11 +152,6 @@ struct CropOut {
     unsigned char* valid;
 };
 
-// (key, scene-local index) of member j, as one 64-bit value: the row order.
-__device__ __forceinline__ unsigned long long member_order(unsigned long long seed, int b, long long j) {
-    return (rng_draw(seed, 2, (unsigned long long)b, (unsigned long long)j) >> 32 << 32) | (unsigned long long)j;
-}
-
 // One CTA per crop.  Dynamic shared memory: the sort buffer, pow2 >= npoints 64-bit values.
 __global__ void __launch_bounds__(kSelectThreads) crop_select_kernel(CropArgs a, const unsigned* __restrict__ ws, int num_class,
                                                                      const float* __restrict__ label_weights, int npoints,
@@ -179,110 +160,95 @@ __global__ void __launch_bounds__(kSelectThreads) crop_select_kernel(CropArgs a,
     __shared__ SelectScratch s_sel;
     __shared__ int s_vox[kAttempts];
     __shared__ CropBox s_box;
-    __shared__ int s_c, s_carry;
+    __shared__ int s_c;
     __shared__ double s_cos, s_sin;
     const int b = blockIdx.x, tid = threadIdx.x;
     const size_t row0 = (size_t)b * npoints;
-    int sc;
+    int sc, kept = 0;
     long long off, ps;
-    if (!crop_scene_of(a, b, sc, off, ps)) {  // a scene index outside [0, S): an empty crop, attempt -1
-        for (int r = tid; r < npoints; r += blockDim.x) {
-            o.xyz[3 * (row0 + r)] = o.xyz[3 * (row0 + r) + 1] = o.xyz[3 * (row0 + r) + 2] = 0.f;
-            o.label[row0 + r] = 0;
-            o.weight[row0 + r] = 0.f;
-            o.point_idx[row0 + r] = -1;
-            o.core[row0 + r] = 0;
-        }
-        if (tid == 0) {
-            o.lengths[b] = 0;
-            o.attempt[b] = -1;
-            o.valid[b] = 0;
-        }
-        return;
-    }
-    const unsigned long long seed = crop_seed(a);
-    const unsigned* w = ws + (size_t)b * kCropWsWords;
-    // distinct voxel keys of every attempt
-    if (tid < kAttempts) s_vox[tid] = 0;
-    __syncthreads();
-    for (int t = 0; t < kAttempts; ++t) {
-        int v = 0;
-        for (int k = tid; k < kKeyWords; k += blockDim.x) v += __popc(__ldg(w + 2 * kAttempts + t * kKeyWords + k));
-        v = __reduce_add_sync(kFullMask, v);
-        if ((tid & 31) == 0 && v) atomicAdd(&s_vox[t], v);
-    }
-    __syncthreads();
-    if (tid == 0) {
-        int att = kAttempts - 1, ok = 0;
+    if (set_entry(a.crop_scene, b, a.s, a.offsets, sc, off, ps)) {
+        const unsigned long long seed = rng_seed(a.seed_dev, a.seed);
+        const unsigned* w = ws + (size_t)b * kCropWsWords;
+        // distinct voxel keys of every attempt
+        if (tid < kAttempts) s_vox[tid] = 0;
+        __syncthreads();
         for (int t = 0; t < kAttempts; ++t) {
-            const int c = (int)__ldg(w + 2 * t), l = (int)__ldg(w + 2 * t + 1);
-            const bool lab_ok = __ddiv_rn((double)l, (double)c) >= 0.7;
-            const bool vox_ok = __ddiv_rn(__ddiv_rn(__ddiv_rn((double)s_vox[t], 31.0), 31.0), 62.0) >= 0.02;
-            if (lab_ok && vox_ok) {
-                att = t;
-                ok = 1;
-                break;
+            int v = 0;
+            for (int k = tid; k < kKeyWords; k += blockDim.x) v += __popc(__ldg(w + 2 * kAttempts + t * kKeyWords + k));
+            v = __reduce_add_sync(kFullMask, v);
+            if ((tid & 31) == 0 && v) atomicAdd(&s_vox[t], v);
+        }
+        __syncthreads();
+        if (tid == 0) {
+            int att = kAttempts - 1, ok = 0;
+            for (int t = 0; t < kAttempts; ++t) {
+                const int c = (int)__ldg(w + 2 * t), l = (int)__ldg(w + 2 * t + 1);
+                const bool lab_ok = __ddiv_rn((double)l, (double)c) >= 0.7;
+                const bool vox_ok = __ddiv_rn(__ddiv_rn(__ddiv_rn((double)s_vox[t], 31.0), 31.0), 62.0) >= 0.02;
+                if (lab_ok && vox_ok) {
+                    att = t;
+                    ok = 1;
+                    break;
+                }
             }
-        }
-        s_c = (int)__ldg(w + 2 * att);
-        crop_box(a, seed, b, att, off, ps, sc, s_box);
-        o.attempt[b] = att;
-        o.valid[b] = (unsigned char)ok;
-        if (rotate) {
-            // theta = u * 2 pi: sincospi(2u) needs no argument reduction (2u is exact) and agrees with cos / sin of
-            // the rounded theta to within a double ulp, far below the float32 result's rounding
-            double sn, cs;
-            sincospi(__dmul_rn(rng_unit(rng_draw(seed, 5, (unsigned long long)b, 0)), 2.0), &sn, &cs);
-            s_cos = cs;
-            s_sin = sn;
-        }
-    }
-    __syncthreads();
-    const CropBox B = s_box;
-    const int c = s_c, m = min(c, npoints);
-    // the m smallest member orders, sorted
-    cta_select_sorted(
-        ps, c, m,
-        [&](long long j) {
-            const long long g = off + j;
-            return in_ctx(B, __ldg(a.xyz + 3 * g), __ldg(a.xyz + 3 * g + 1), __ldg(a.xyz + 3 * g + 2));
-        },
-        [&](long long j) { return member_order(seed, b, j); }, s_keys, s_sel);
-    // rows: dropout compaction (row 0 always stays), then each survivor written in row order
-    const double ratio = __dmul_rn(rng_unit(rng_draw(seed, 3, (unsigned long long)b, 0)), max_dropout);
-    int carry = 0;
-    for (int base = 0; base < m; base += blockDim.x) {
-        const int r = base + tid;
-        const bool dropped = r < m && rng_unit(rng_draw(seed, 4, (unsigned long long)b, (unsigned long long)r)) <= ratio;
-        const int keep = r < m && (r == 0 || !dropped);
-        const int ex = cta_exclusive_sum_1024(keep, s_sel.w);
-        if (keep) {
-            const size_t row = row0 + carry + ex;
-            const long long j = (long long)(s_keys[r] & 0xffffffffull), g = off + j;
-            const float x = __ldg(a.xyz + 3 * g), y = __ldg(a.xyz + 3 * g + 1), z = __ldg(a.xyz + 3 * g + 2);
-            const int l = __ldg(a.label + g);
-            const bool is_core = in_core(B, x, y, z);
-            float wt = (is_core && l >= 0 && l < num_class) ? __ldg(label_weights + l) : 0.f;
-            if (dropped) wt = 0.f;  // row 0 whose own draw drops it: its point stays, unweighted
-            float ox = x, oy = y;
+            s_c = (int)__ldg(w + 2 * att);
+            crop_box(a, seed, b, att, off, ps, sc, s_box);
+            o.attempt[b] = att;
+            o.valid[b] = (unsigned char)ok;
             if (rotate) {
-                ox = __double2float_rn(__dsub_rn(__dmul_rn((double)x, s_cos), __dmul_rn((double)y, s_sin)));
-                oy = __double2float_rn(__dadd_rn(__dmul_rn((double)x, s_sin), __dmul_rn((double)y, s_cos)));
+                // theta = u * 2 pi: sincospi(2u) needs no argument reduction (2u is exact) and agrees with cos / sin
+                // of the rounded theta to within a double ulp, far below the float32 result's rounding
+                double sn, cs;
+                sincospi(__dmul_rn(rng_unit(rng_draw(seed, 5, (unsigned long long)b, 0)), 2.0), &sn, &cs);
+                s_cos = cs;
+                s_sin = sn;
             }
-            o.xyz[3 * row] = ox;
-            o.xyz[3 * row + 1] = oy;
-            o.xyz[3 * row + 2] = z;
-            o.label[row] = l;
-            o.weight[row] = wt;
-            o.point_idx[row] = (int)g;
-            o.core[row] = is_core ? 1 : 0;
         }
-        if (tid == blockDim.x - 1) s_carry = ex + keep;
         __syncthreads();
-        carry += s_carry;
-        __syncthreads();
+        const CropBox B = s_box;
+        const int c = s_c, m = min(c, npoints);
+        // the m smallest member orders, sorted
+        cta_select_sorted(
+            ps, c, m,
+            [&](long long j) {
+                const long long g = off + j;
+                return in_ctx(B, __ldg(a.xyz + 3 * g), __ldg(a.xyz + 3 * g + 1), __ldg(a.xyz + 3 * g + 2));
+            },
+            [&](long long j) { return rng_row_key(seed, 2, (unsigned long long)b, j); }, s_keys, s_sel);
+        // rows: dropout compaction (row 0 always stays), then each survivor written in row order
+        const double ratio = __dmul_rn(rng_unit(rng_draw(seed, 3, (unsigned long long)b, 0)), max_dropout);
+        const auto dropped = [&](int r) {
+            return rng_unit(rng_draw(seed, 4, (unsigned long long)b, (unsigned long long)r)) <= ratio;
+        };
+        kept = cta_compact(
+            m, [&](int r) { return r == 0 || !dropped(r); },
+            [&](int r, int at) {
+                const size_t row = row0 + at;
+                const long long j = (long long)(s_keys[r] & 0xffffffffull), g = off + j;
+                const float x = __ldg(a.xyz + 3 * g), y = __ldg(a.xyz + 3 * g + 1), z = __ldg(a.xyz + 3 * g + 2);
+                const int l = __ldg(a.label + g);
+                const bool is_core = in_core(B, x, y, z);
+                float wt = (is_core && l >= 0 && l < num_class) ? __ldg(label_weights + l) : 0.f;
+                if (r == 0 && dropped(0)) wt = 0.f;  // row 0 whose own draw drops it: its point stays, unweighted
+                float ox = x, oy = y;
+                if (rotate) {
+                    ox = __double2float_rn(__dsub_rn(__dmul_rn((double)x, s_cos), __dmul_rn((double)y, s_sin)));
+                    oy = __double2float_rn(__dadd_rn(__dmul_rn((double)x, s_sin), __dmul_rn((double)y, s_cos)));
+                }
+                o.xyz[3 * row] = ox;
+                o.xyz[3 * row + 1] = oy;
+                o.xyz[3 * row + 2] = z;
+                o.label[row] = l;
+                o.weight[row] = wt;
+                o.point_idx[row] = (int)g;
+                o.core[row] = is_core ? 1 : 0;
+            },
+            s_sel.w);
+    } else if (tid == 0) {  // a scene index outside [0, S): an empty crop, attempt -1
+        o.attempt[b] = -1;
+        o.valid[b] = 0;
     }
-    for (int r = carry + tid; r < npoints; r += blockDim.x) {
+    for (int r = kept + tid; r < npoints; r += blockDim.x) {
         const size_t row = row0 + r;
         o.xyz[3 * row] = o.xyz[3 * row + 1] = o.xyz[3 * row + 2] = 0.f;
         o.label[row] = 0;
@@ -290,17 +256,12 @@ __global__ void __launch_bounds__(kSelectThreads) crop_select_kernel(CropArgs a,
         o.point_idx[row] = -1;
         o.core[row] = 0;
     }
-    if (tid == 0) o.lengths[b] = carry;
+    if (tid == 0) o.lengths[b] = kept;
 }
 
 size_t crop_ws_bytes(int b) { return ((size_t)b * kCropWsWords * sizeof(unsigned) + 255) / 256 * 256; }
-int crop_sort_n(int npoints) {
-    int n = 1;
-    while (n < npoints) n <<= 1;
-    return n;
-}
 bool crop_shape_ok(int b, int npoints) {
-    return b >= 1 && b <= 65535 && npoints >= 1 && npoints <= kCropMaxPoints && (long long)b * npoints * 3 < (1ll << 31);
+    return b >= 1 && b <= 65535 && npoints >= 1 && npoints <= kSelectMaxRows && (long long)b * npoints * 3 < (1ll << 31);
 }
 
 AttrOnce g_attempt_attr, g_select_attr;
@@ -330,10 +291,9 @@ int pn2_scene_crops(int s, int p, int max_scene, const float* xyz, const int* la
     if (workspace_bytes < crop_ws_bytes(b) || !aligned_to(workspace, 256)) return (int)cudaErrorInvalidValue;
     cudaStream_t st = as_stream(stream);
     const size_t attempt_smem = sizeof(unsigned) * kAttempts * kKeyWords;
-    const int sort_n = crop_sort_n(npoints);
     cudaError_t e = ensure_attrs(g_attempt_attr, crop_attempt_kernel, attempt_smem, false);
     if (e != cudaSuccess) return (int)e;
-    e = ensure_attrs(g_select_attr, crop_select_kernel, sizeof(unsigned long long) * kCropMaxPoints, false);
+    e = ensure_attrs(g_select_attr, crop_select_kernel, sizeof(unsigned long long) * kSelectMaxRows, false);
     if (e != cudaSuccess) return (int)e;
     if ((e = cudaMemsetAsync(workspace, 0, crop_ws_bytes(b), st)) != cudaSuccess) return (int)e;
     const CropArgs a{xyz, label, offsets, lo, hi, crop_scene, seed_dev, (unsigned long long)seed, s};
@@ -343,8 +303,8 @@ int pn2_scene_crops(int s, int p, int max_scene, const float* xyz, const int* la
     int rc = finish_launch();
     if (rc) return rc;
     const CropOut o{out_xyz, out_label, out_weight, lengths, point_idx, core, attempt, valid};
-    crop_select_kernel<<<b, kSelectThreads, sizeof(unsigned long long) * sort_n, st>>>(a, ws, num_class, label_weights, npoints,
-                                                                                      max_dropout, rotate, o);
+    crop_select_kernel<<<b, kSelectThreads, sizeof(unsigned long long) * pow2_at_least(npoints), st>>>(
+        a, ws, num_class, label_weights, npoints, max_dropout, rotate, o);
     return finish_launch();
 }
 

@@ -218,8 +218,40 @@ __device__ __forceinline__ unsigned long long rng_draw(unsigned long long seed, 
 
 __device__ __forceinline__ double rng_unit(unsigned long long d) { return (double)(d >> 11) * 0x1.0p-53; }
 
+// A sampler call's seed: read on the device when seed_dev is non-null (a (1,) tensor rewritten between replays of a
+// captured graph), else the launch argument.
+__device__ __forceinline__ unsigned long long rng_seed(const long long* seed_dev, unsigned long long seed) {
+    return seed_dev ? (unsigned long long)__ldg(seed_dev) : seed;
+}
+
+// (key, local row) of row j of entry e as one 64-bit value: the high half of its draw, then j.  Distinct for distinct
+// j < 2^32, so sorting them is the entry's seeded row order.
+__device__ __forceinline__ unsigned long long rng_row_key(unsigned long long seed, unsigned long long stream,
+                                                          unsigned long long e, long long j) {
+    return (rng_draw(seed, stream, e, (unsigned long long)j) >> 32 << 32) | (unsigned long long)j;
+}
+
 // ---- seeded row selection (crops.cu, shapes.cu, vscan.cu) ----------------------------------------------------------
+// Entry b of a packed set: k = index[b] and its rows off .. off + ps - 1 (offsets[k] .. offsets[k + 1] - 1).  False for
+// an index outside [0, s) or an empty member; the kernels turn that into an empty entry.
+__device__ __forceinline__ bool set_entry(const long long* __restrict__ index, int b, int s,
+                                          const long long* __restrict__ offsets, int& k, long long& off, long long& ps) {
+    const long long v = __ldg(index + b);
+    if (v < 0 || v >= s) return false;
+    k = (int)v;
+    off = __ldg(offsets + k);
+    ps = __ldg(offsets + k + 1) - off;
+    return ps > 0;
+}
+
+constexpr __host__ __device__ int pow2_at_least(int n) {
+    int p = 1;
+    while (p < n) p <<= 1;
+    return p;
+}
+
 constexpr int kSelectRadixBins = 2048;
+constexpr int kSelectMaxRows = 16384;  // m of cta_select_sorted: its sort buffer is pow2 >= m x 8 B of shared memory
 
 struct SelectScratch {  // shared memory of cta_select_sorted
     int hist[kSelectRadixBins];
@@ -283,8 +315,7 @@ __device__ __forceinline__ void cta_select_sorted(long long n, int c, int m, Mem
         s_keys[atomicAdd(&s.n, 1)] = v;
     }
     __syncthreads();
-    int sort_n = 1;
-    while (sort_n < m) sort_n <<= 1;
+    const int sort_n = pow2_at_least(m);
     for (int k = m + tid; k < sort_n; k += blockDim.x) s_keys[k] = ~0ull;
     __syncthreads();
     for (int k = 2; k <= sort_n; k <<= 1) {
@@ -302,6 +333,23 @@ __device__ __forceinline__ void cta_select_sorted(long long n, int c, int m, Mem
             __syncthreads();
         }
     }
+}
+
+// Ordered compaction of rows 0 .. m-1 by a 1024-thread CTA: write(r, q) for every row r with keep(r), q being the
+// number of kept rows before r.  Returns the number kept, to every thread.  Every thread must call it with the same
+// m; s_w is 32 ints of shared scratch (SelectScratch::w), free again on return.
+template <typename Keep, typename Write>
+__device__ __forceinline__ int cta_compact(int m, Keep&& keep, Write&& write, int* s_w) {
+    int kept = 0;
+    for (int base = 0; base < m; base += blockDim.x) {
+        const int r = base + threadIdx.x;
+        const int k = r < m && keep(r);
+        const int ex = cta_exclusive_sum_1024(k, s_w);
+        if (k) write(r, kept + ex);
+        kept += __reduce_add_sync(kFullMask, s_w[threadIdx.x & 31]);  // the 32 warp totals: this pass's count
+        __syncthreads();  // s_w is rewritten by the next pass
+    }
+    return kept;
 }
 
 // ---- uniform grid over one cloud, for the ball query (ball_query_grid.cu, sa_fused.cu) ---------------------------

@@ -9,7 +9,6 @@
 namespace pn2 {
 namespace {
 
-constexpr int kShapeMaxPoints = 16384;  // sort buffer: 16384 x 8 B of shared memory
 constexpr int kShapeThreads = 1024;
 constexpr double kPi = 3.141592653589793;
 // random streams of DESIGN.md §6.11
@@ -62,11 +61,6 @@ __device__ __forceinline__ void rot_y(double c, double s, double (&r)[9]) {
     r[6] = -s; r[7] = 0.0; r[8] = c;
 }
 
-// (key, shape-local row) of pool row j, as one 64-bit value: the row order
-__device__ __forceinline__ unsigned long long row_order(unsigned long long seed, unsigned long long e, int j) {
-    return (rng_draw(seed, kStreamKey, e, (unsigned long long)j) >> 32 << 32) | (unsigned long long)j;
-}
-
 struct EntryXform {
     double m[9];       // p' = p M (row vectors)
     double scale;
@@ -79,32 +73,17 @@ struct EntryXform {
 __global__ void __launch_bounds__(kShapeThreads) shape_batch_kernel(ShapeArgs a, ShapeOut o) {
     extern __shared__ unsigned long long s_keys[];
     __shared__ SelectScratch s_sel;
-    __shared__ int s_carry;
     __shared__ EntryXform s_x;
     const int tid = threadIdx.x;
     const unsigned long long e = blockIdx.x;
     const int npoints = a.npoints, ch = a.with_normals ? 6 : 3;
     const size_t row0 = (size_t)e * npoints;
     const int v = a.votes ? (int)(e / a.b) : 0, bi = a.votes ? (int)(e % a.b) : (int)e;
-    const long long sv = __ldg(a.shape_idx + bi);
+    int sv = 0;
     long long off = 0, ps = 0;
-    if (sv >= 0 && sv < a.s) {
-        off = __ldg(a.offsets + sv);
-        ps = __ldg(a.offsets + sv + 1) - off;
-    }
-    if (ps <= 0) {  // a shape index outside [0, S): an empty entry
-        for (int r = tid; r < npoints; r += blockDim.x) {
-            for (int c = 0; c < ch; ++c) o.points[ch * (row0 + r) + c] = 0.f;
-            if (o.part) o.part[row0 + r] = 0;
-            o.point_idx[row0 + r] = -1;
-        }
-        if (tid == 0) {
-            o.label[e] = 0;
-            o.lengths[e] = 0;
-        }
-        return;
-    }
-    const unsigned long long seed = a.seed_dev ? (unsigned long long)__ldg(a.seed_dev) : a.seed;
+    // a shape index outside [0, S): an empty entry, zero rows and label 0
+    const bool in_range = set_entry(a.shape_idx, bi, a.s, a.offsets, sv, off, ps);
+    const unsigned long long seed = rng_seed(a.seed_dev, a.seed);
     if (tid == 0) {
         EntryXform x;
         double r[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0};
@@ -144,26 +123,25 @@ __global__ void __launch_bounds__(kShapeThreads) shape_batch_kernel(ShapeArgs a,
             x.shift[d] = __dadd_rn(-a.shift, __dmul_rn(2.0 * a.shift, rng_unit(rng_draw(seed, kStreamShift, e, d))));
         x.ratio = __dmul_rn(rng_unit(rng_draw(seed, kStreamRatio, e, 0)), a.max_dropout);
         s_x = x;
-        o.label[e] = __ldg(a.label + sv);
+        o.label[e] = in_range ? __ldg(a.label + sv) : 0;
     }
     // the pool: rows 0 .. q-1 of the shape; its m smallest row orders are the entry's rows
-    const int q = (a.subset_random && !a.votes) ? (int)ps : (int)min(ps, (long long)npoints);
+    const int q = !in_range ? 0 : (a.subset_random && !a.votes) ? (int)ps : (int)min(ps, (long long)npoints);
     const int m = min(q, npoints);
     cta_select_sorted(
-        q, q, m, [](long long) { return true; }, [&](long long j) { return row_order(seed, e, (int)j); }, s_keys, s_sel);
+        q, q, m, [](long long) { return true; }, [&](long long j) { return rng_row_key(seed, kStreamKey, e, j); },
+        s_keys, s_sel);
     // rows: dropout compaction (row 0 always stays), then each survivor transformed and written in row order
     const EntryXform& X = s_x;
     const bool drop_on = !a.votes && a.max_dropout > 0.0, shift_on = !a.votes && a.shift > 0.0;
     const bool scale_on = !a.votes && a.scale_on, jitter_on = !a.votes && a.jitter_on;
-    int carry = 0;
-    for (int base = 0; base < m; base += blockDim.x) {
-        const int r = base + tid;
-        const bool dropped = drop_on && r >= 1 && r < m &&
-                             rng_unit(rng_draw(seed, kStreamDrop, e, (unsigned long long)r)) <= X.ratio;
-        const int keep = r < m && !dropped;
-        const int ex = cta_exclusive_sum_1024(keep, s_sel.w);
-        if (keep) {
-            const size_t row = row0 + carry + ex;
+    const int kept = cta_compact(
+        m,
+        [&](int r) {
+            return !(drop_on && r >= 1 && rng_unit(rng_draw(seed, kStreamDrop, e, (unsigned long long)r)) <= X.ratio);
+        },
+        [&](int r, int at) {
+            const size_t row = row0 + at;
             const int j = (int)(s_keys[r] & 0xffffffffull);
             const long long g = off + j;
             double p[3], out[3];
@@ -193,25 +171,15 @@ __global__ void __launch_bounds__(kShapeThreads) shape_batch_kernel(ShapeArgs a,
             }
             if (o.part) o.part[row] = __ldg(a.part + g);
             o.point_idx[row] = (int)g;
-        }
-        if (tid == blockDim.x - 1) s_carry = ex + keep;
-        __syncthreads();
-        carry += s_carry;
-        __syncthreads();
-    }
-    for (int r = carry + tid; r < npoints; r += blockDim.x) {
+        },
+        s_sel.w);
+    for (int r = kept + tid; r < npoints; r += blockDim.x) {
         const size_t row = row0 + r;
         for (int c = 0; c < ch; ++c) o.points[ch * row + c] = 0.f;
         if (o.part) o.part[row] = 0;
         o.point_idx[row] = -1;
     }
-    if (tid == 0) o.lengths[e] = carry;
-}
-
-int shape_sort_n(int m) {
-    int n = 1;
-    while (n < m) n <<= 1;
-    return n;
+    if (tid == 0) o.lengths[e] = kept;
 }
 
 bool finite_d(double x) { return x == x && x - x == 0.0; }
@@ -230,8 +198,8 @@ int pn2_shape_batch(int s, int p, int max_shape, const float* xyz, const float* 
                     double max_dropout, int with_normals, float* out_points, long long* out_label, long long* out_part,
                     int* lengths, int* point_idx, void* stream) {
     using namespace pn2;
-    if (s < 1 || p < 1 || p >= 0x7fffffff || max_shape < 1 || max_shape > p || max_shape > kShapeMaxPoints || b < 1 ||
-        votes < 0 || npoints < 1 || npoints > kShapeMaxPoints)
+    if (s < 1 || p < 1 || p >= 0x7fffffff || max_shape < 1 || max_shape > p || max_shape > kSelectMaxRows || b < 1 ||
+        votes < 0 || npoints < 1 || npoints > kSelectMaxRows)
         return (int)cudaErrorInvalidValue;
     const long long ent = votes ? (long long)votes * b : (long long)b;
     const int ch = with_normals ? 6 : 3;
@@ -251,8 +219,8 @@ int pn2_shape_batch(int s, int p, int max_shape, const float* xyz, const float* 
         return (int)cudaErrorInvalidValue;
     if ((with_normals && !normals) || (out_part && !part)) return (int)cudaErrorInvalidValue;
     const int pool = subset_random ? max_shape : (max_shape < npoints ? max_shape : npoints);
-    const size_t smem = sizeof(unsigned long long) * shape_sort_n(pool < npoints ? pool : npoints);
-    cudaError_t e = ensure_attrs(g_shape_attr, shape_batch_kernel, sizeof(unsigned long long) * kShapeMaxPoints, false);
+    const size_t smem = sizeof(unsigned long long) * pow2_at_least(pool < npoints ? pool : npoints);
+    cudaError_t e = ensure_attrs(g_shape_attr, shape_batch_kernel, sizeof(unsigned long long) * kSelectMaxRows, false);
     if (e != cudaSuccess) return (int)e;
     const ShapeArgs a{xyz, with_normals ? normals : nullptr, label, out_part ? part : nullptr, offsets, shape_idx, seed_dev,
                       (unsigned long long)seed, s, b, votes, npoints, subset_random, with_normals, rotate, perturb,

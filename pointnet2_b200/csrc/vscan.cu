@@ -30,7 +30,6 @@ constexpr int kMinNear = 100;                                      // scene_util
 // el in [-0.8, 0.8059): every ray's |el| is at most |theta| + atan(0.45) < 0.66.
 constexpr double kCellH = 0.0101, kAz0 = -3.2, kEl0 = -0.8;
 constexpr int kCellsAz = 634, kCellsEl = 159, kCells = kCellsAz * kCellsEl;
-constexpr int kScanMaxPoints = 16384;  // sort buffer: 16384 x 8 B of shared memory
 constexpr int kScanMaxBatch = 4096;    // entries per call: the workspace is ~1.7 MB per entry
 constexpr int kRayThreads = 256;
 constexpr int kPointThreads = 256;
@@ -98,19 +97,6 @@ ScanWs scan_ws(void* base, int b, int max_scene) {
     return w;
 }
 
-__device__ __forceinline__ unsigned long long scan_seed(const ScanArgs& a) {
-    return a.seed_dev ? (unsigned long long)__ldg(a.seed_dev) : a.seed;
-}
-
-__device__ __forceinline__ bool scan_scene_of(const ScanArgs& a, int b, int& sc, long long& off, long long& ps) {
-    const long long v = __ldg(a.scan_scene + b);
-    if (v < 0 || v >= a.s) return false;
-    sc = (int)v;
-    off = __ldg(a.offsets + sc);
-    ps = __ldg(a.offsets + sc + 1) - off;
-    return ps > 0;
-}
-
 struct ScanView {
     double ct[3], hr[3], vt[3];  // view direction and the image plane's unit axes
     double cam[3];               // camera location
@@ -131,7 +117,7 @@ __device__ __forceinline__ void normalise3(double (&v)[3]) {
 // scene_util.py:21-33.  Random view: phi = 2 pi u1, theta = pi/10 (u2 - 0.75), the camera (0.8 + 0.7 u3) behind the
 // centre; fixed view m: phi = pi/4 m, theta = 0, the camera 1 behind.  sin / cos as sincospi of phi / pi and theta / pi.
 __device__ void scan_view(const ScanArgs& a, int b, int sc, ScanView& v) {
-    const unsigned long long seed = scan_seed(a), e = (unsigned long long)b;
+    const unsigned long long seed = rng_seed(a.seed_dev, a.seed), e = (unsigned long long)b;
     const long long mode = __ldg(a.scan_mode + b);
     double sp, cp, st = 0.0, cth = 1.0, dist = 1.0;
     if (mode == -1) {
@@ -188,7 +174,7 @@ __global__ void __launch_bounds__(kRayThreads) vscan_ray_kernel(ScanArgs a, Scan
     const int b = blockIdx.y;
     int sc;
     long long off, ps;
-    if (!scan_scene_of(a, b, sc, off, ps)) return;
+    if (!set_entry(a.scan_scene, b, a.s, a.offsets, sc, off, ps)) return;
     if (threadIdx.x == 0) scan_view(a, b, sc, s_v);
     __syncthreads();
     const int k = blockIdx.x * kRayThreads + threadIdx.x;
@@ -212,7 +198,7 @@ __global__ void __launch_bounds__(kCellThreads) vscan_cell_kernel(ScanArgs a, Sc
     const int b = blockIdx.x;
     int sc;
     long long off, ps;
-    if (!scan_scene_of(a, b, sc, off, ps)) return;
+    if (!set_entry(a.scan_scene, b, a.s, a.offsets, sc, off, ps)) return;
     int* ce = w.cell_end + (size_t)b * kCells;
     constexpr int kPer = (kCells + kCellThreads - 1) / kCellThreads;
     const int c0 = min((int)threadIdx.x * kPer, kCells), c1 = min(c0 + kPer, kCells);
@@ -270,7 +256,7 @@ __global__ void __launch_bounds__(kPointThreads) vscan_point_kernel(ScanArgs a, 
     const int b = blockIdx.y;
     int sc;
     long long off, ps;
-    if (!scan_scene_of(a, b, sc, off, ps)) return;
+    if (!set_entry(a.scan_scene, b, a.s, a.offsets, sc, off, ps)) return;
     const long long q0 = (long long)blockIdx.x * kPointChunk;
     if (q0 >= ps) return;
     if (pass && __ldg(w.cnt + 4 * b) < kMinNear) return;  // fewer than 100 near points: no scan
@@ -322,11 +308,6 @@ struct ScanOut {
     unsigned char* valid;
 };
 
-// (key, scene-local index) of visible point j, as one 64-bit value: the row order
-__device__ __forceinline__ unsigned long long scan_order(unsigned long long seed, int b, long long j) {
-    return (rng_draw(seed, kStreamKey, (unsigned long long)b, (unsigned long long)j) >> 32 << 32) | (unsigned long long)j;
-}
-
 // One CTA per entry.  Dynamic shared memory: the sort buffer, pow2 >= npoints 64-bit values.
 __global__ void __launch_bounds__(kSelectThreads) vscan_select_kernel(ScanArgs a, ScanWs w, int num_class,
                                                                       const float* __restrict__ label_weights, int npoints,
@@ -337,7 +318,7 @@ __global__ void __launch_bounds__(kSelectThreads) vscan_select_kernel(ScanArgs a
     const size_t row0 = (size_t)b * npoints;
     int sc;
     long long off = 0, ps = 0;
-    const bool in_range = scan_scene_of(a, b, sc, off, ps);
+    const bool in_range = set_entry(a.scan_scene, b, a.s, a.offsets, sc, off, ps);
     int vis = -1, m = 0;
     bool valid = false;
     if (in_range) {  // a scene index outside [0, S): an empty entry, visible -1
@@ -345,11 +326,11 @@ __global__ void __launch_bounds__(kSelectThreads) vscan_select_kernel(ScanArgs a
         vis = near < kMinNear ? 0 : __ldg(w.cnt + 4 * b + 1);
         m = min(vis, npoints);
         valid = vis >= min_points;
-        const unsigned long long seed = scan_seed(a);
+        const unsigned long long seed = rng_seed(a.seed_dev, a.seed);
         const unsigned* bits = w.bits + (size_t)b * w.words;
         cta_select_sorted(
             vis > 0 ? ps : 0, vis, m, [&](long long j) { return ((__ldg(bits + (j >> 5)) >> (j & 31)) & 1u) != 0u; },
-            [&](long long j) { return scan_order(seed, b, j); }, s_keys, s_sel);
+            [&](long long j) { return rng_row_key(seed, kStreamKey, (unsigned long long)b, j); }, s_keys, s_sel);
     }
     for (int r = tid; r < npoints; r += blockDim.x) {
         const size_t row = row0 + r;
@@ -376,14 +357,9 @@ __global__ void __launch_bounds__(kSelectThreads) vscan_select_kernel(ScanArgs a
     }
 }
 
-int scan_sort_n(int npoints) {
-    int n = 1;
-    while (n < npoints) n <<= 1;
-    return n;
-}
 bool scan_shape_ok(int b, int max_scene, int npoints) {
     return b >= 1 && b <= kScanMaxBatch && max_scene >= 1 && max_scene < 0x7fffffff && npoints >= 1 &&
-           npoints <= kScanMaxPoints && (long long)b * npoints * 3 < (1ll << 31);
+           npoints <= kSelectMaxRows && (long long)b * npoints * 3 < (1ll << 31);
 }
 
 AttrOnce g_scan_select_attr;
@@ -412,7 +388,7 @@ int pn2_virtual_scans(int s, int p, int max_scene, const float* xyz, const int* 
         return (int)cudaErrorInvalidValue;
     if (workspace_bytes < scan_ws_bytes(b, max_scene) || !aligned_to(workspace, 256)) return (int)cudaErrorInvalidValue;
     cudaStream_t st = as_stream(stream);
-    cudaError_t e = ensure_attrs(g_scan_select_attr, vscan_select_kernel, sizeof(unsigned long long) * kScanMaxPoints, false);
+    cudaError_t e = ensure_attrs(g_scan_select_attr, vscan_select_kernel, sizeof(unsigned long long) * kSelectMaxRows, false);
     if (e != cudaSuccess) return (int)e;
     if ((e = cudaMemsetAsync(workspace, 0, scan_zero_bytes(b, max_scene), st)) != cudaSuccess) return (int)e;
     const ScanArgs a{xyz, label, offsets, mean, scan_scene, scan_mode, seed_dev, (unsigned long long)seed, s};
@@ -428,7 +404,7 @@ int pn2_virtual_scans(int s, int p, int max_scene, const float* xyz, const int* 
         if ((rc = finish_launch())) return rc;
     }
     const ScanOut o{out_xyz, out_label, out_weight, lengths, point_idx, visible, valid};
-    vscan_select_kernel<<<(unsigned)b, kSelectThreads, sizeof(unsigned long long) * scan_sort_n(npoints), st>>>(
+    vscan_select_kernel<<<(unsigned)b, kSelectThreads, sizeof(unsigned long long) * pow2_at_least(npoints), st>>>(
         a, w, num_class, label_weights, npoints, min_points, o);
     return finish_launch();
 }

@@ -24,11 +24,11 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._tensor import DTYPE_CODES, FEATURE_DTYPES, on_device, ptr, require_cuda, stream_ptr
+from ._tensor import (DTYPE_CODES, FEATURE_DTYPES, I31, SELECT_MAX_ROWS, check_dropout, check_npoints, index_tensors,
+                      on_device, on_set_device, pack_offsets, ptr, require_cuda, seed_args, stream_ptr, to_host)
 
 CORE_MARGIN = 0.001   # scannet_dataset.py:103
 MAX_BLOCKS = 16384    # blocks in one scene's grid (pn2_api.h)
-_I31 = 2 ** 31
 
 # train.py:418: per-class weights (classes 1..20) of the calibrated voxel accuracy
 CALIBRATION_WEIGHTS = (0.388, 0.357, 0.038, 0.033, 0.017, 0.02, 0.016, 0.025, 0.002, 0.002, 0.002, 0.007, 0.006, 0.022,
@@ -117,7 +117,7 @@ def scene_blocks(xyz: torch.Tensor, block_size: float = 1.5, stride=None, paddin
         raise ValueError(f"scene_blocks expects a (num_points, 3) scene with at least one point, got {tuple(xyz.shape)}")
     xyz = require_cuda(xyz, "xyz", torch.float32)
     p = xyz.shape[0]
-    if p + 1 >= _I31:
+    if p + 1 >= I31:
         raise ValueError(f"scene_blocks takes fewer than 2^31 - 1 points, got {p}")
     block_size, stride, padding = float(block_size), float(stride), float(padding)
     dev = xyz.device
@@ -138,7 +138,7 @@ def scene_blocks(xyz: torch.Tensor, block_size: float = 1.5, stride=None, paddin
         ctx, core = host[:nblk], host[nblk:]
         sub_begin, sub_count, lengths, sub = split_plan(ctx, core, max_points)
         b, n = len(lengths), int(lengths.max())
-        if b * n * 3 >= _I31 or int(core.sum()) >= _I31:
+        if b * n * 3 >= I31 or int(core.sum()) >= I31:
             raise ValueError(f"scene_blocks: a batch of {b} x {n} rows ({int(core.sum())} core rows) passes 2^31 elements")
         tables = torch.from_numpy(np.concatenate([sub_begin, sub_count]).astype(np.int32)).to(dev)
         blk = sub[:, 0]
@@ -179,7 +179,7 @@ def merge_block_logits(blocks: SceneBlocks, logits: torch.Tensor, accum: torch.T
     if row_begin < 0 or row_begin % n or row_begin // n + logits.shape[0] > b:
         raise ValueError(f"merge_block_logits: row_begin {row_begin} with {logits.shape[0]} blocks of {n} rows is not "
                          f"a range of the {b} blocks")
-    if c < 1 or p * c >= _I31 or logits.numel() >= _I31:
+    if c < 1 or p * c >= I31 or logits.numel() >= I31:
         raise ValueError(f"merge_block_logits: ({p}, {c}) accum or {tuple(logits.shape)} logits pass 2^31 elements")
     logits = require_cuda(logits, "logits", FEATURE_DTYPES)
     if accum.dtype != torch.float32:
@@ -281,9 +281,8 @@ class VoxelAccuracy:
 
 
 # ---- training crops (scannet/scannet_dataset.py:27-60, scannet/train.py:181-197, utils/provider.py:52-70) ----------
-CROP_MAX_POINTS = 16384   # npoints cap of sample_crops: its sort buffer is npoints x 8 bytes of shared memory
+CROP_MAX_POINTS = SELECT_MAX_ROWS  # npoints cap of sample_crops and sample_virtual_scans: the shared-memory row sort
 CROP_MAX_BATCH = 65535    # crops per call
-_U64 = 2 ** 64
 
 
 class SceneSet:
@@ -305,7 +304,7 @@ class SceneSet:
         if len(xyz_list) != len(label_list):
             raise ValueError(f"SceneSet expects one label array per scene, got {len(xyz_list)} scenes and "
                              f"{len(label_list)} label arrays")
-        xyz_list, label_list = [_host(x) for x in xyz_list], [_host(lab) for lab in label_list]
+        xyz_list, label_list = [to_host(x) for x in xyz_list], [to_host(lab) for lab in label_list]
         for k, (x, lab) in enumerate(zip(xyz_list, label_list)):
             if x.ndim != 2 or x.shape[1] != 3:
                 raise ValueError(f"SceneSet: scene {k} must be (num_points, 3), got {x.shape}")
@@ -315,9 +314,7 @@ class SceneSet:
                 raise ValueError(f"SceneSet: scene {k} has {len(x)} points but labels of shape {lab.shape}")
             if not np.issubdtype(lab.dtype, np.integer):
                 raise TypeError(f"SceneSet: scene {k} has {lab.dtype} labels, expected integers")
-        self.sizes = np.array([len(x) for x in xyz_list], np.int64)
-        if int(self.sizes.sum()) >= _I31 - 1:
-            raise ValueError(f"SceneSet takes fewer than 2^31 - 1 points in all, got {int(self.sizes.sum())}")
+        self.sizes, self.offsets = pack_offsets(xyz_list, "SceneSet", device)
         pts, labs, lo, hi, mean = [], [], [], [], []
         hist = np.zeros(num_class, np.int64)
         for k, (x, lab) in enumerate(zip(xyz_list, label_list)):
@@ -337,13 +334,11 @@ class SceneSet:
             lo.append(mn)
             hi.append(mx)
             mean.append(np.mean(x.astype(np.float64), axis=0))
-        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.device = dev = self.offsets.device  # "cuda" resolved to the current index: compared against by the samplers
         self.num_class = num_class
         self.label_hist = hist
         self.xyz = torch.from_numpy(np.concatenate(pts)).to(dev)
-        self.device = self.xyz.device  # "cuda" resolves to the current index here: compared against in sample_crops
         self.label = torch.from_numpy(np.concatenate(labs)).to(dev)
-        self.offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(self.sizes)]).astype(np.int64)).to(dev)
         self.lo = torch.from_numpy(np.stack(lo)).to(dev)
         self.hi = torch.from_numpy(np.stack(hi)).to(dev)
         self.mean = torch.from_numpy(np.stack(mean)).to(dev)
@@ -359,12 +354,6 @@ class SceneSet:
         w = w / np.sum(w)
         w = 1 / np.log(1.2 + w)
         return torch.from_numpy(np.asarray(w, np.float32)).to(self.device)
-
-
-def _host(a) -> np.ndarray:
-    if isinstance(a, torch.Tensor):
-        return a.detach().cpu().numpy()
-    return np.asarray(a)
 
 
 class SceneCrops(NamedTuple):
@@ -385,6 +374,14 @@ class SceneCrops(NamedTuple):
     valid: torch.Tensor
 
 
+def _label_weights(label_weights, scenes: SceneSet, what: str) -> torch.Tensor:
+    label_weights = require_cuda(label_weights, "label_weights", torch.float32)
+    if tuple(label_weights.shape) != (scenes.num_class,):
+        raise ValueError(f"{what} expects ({scenes.num_class},) label_weights, got {tuple(label_weights.shape)}")
+    on_set_device(label_weights, "label_weights", scenes.device)
+    return label_weights
+
+
 def sample_crops(scenes: SceneSet, crop_scene: torch.Tensor, seed, label_weights: torch.Tensor, npoints: int = 8192,
                  max_dropout: float = 0.875, rotate: bool = True) -> SceneCrops:
     """B random training crops of ``scenes`` on the GPU (DESIGN.md §6.10): crop i is a 1.5 m column of scene
@@ -398,53 +395,22 @@ def sample_crops(scenes: SceneSet, crop_scene: torch.Tensor, seed, label_weights
     own seed.  ``label_weights`` (num_class,) float32 CUDA tensor, e.g. scenes.train_label_weights().  Nothing is read
     back and the same seed gives the same bits.  A crop_scene value outside [0, S) gives an empty crop (lengths 0,
     attempt -1): it cannot be reported without a read-back."""
+    what = "sample_crops"
     if not isinstance(scenes, SceneSet):
-        raise TypeError(f"sample_crops expects a SceneSet, got {type(scenes).__name__}")
-    if isinstance(npoints, bool) or not isinstance(npoints, int):
-        raise TypeError(f"sample_crops expects an integer npoints, got {type(npoints).__name__}")
-    if not 1 <= npoints <= CROP_MAX_POINTS:
-        raise ValueError(f"sample_crops expects 1 <= npoints <= {CROP_MAX_POINTS} (the shared-memory sort), got {npoints}")
-    if isinstance(max_dropout, bool) or not isinstance(max_dropout, (int, float)):
-        raise TypeError(f"sample_crops expects a number for max_dropout, got {type(max_dropout).__name__}")
-    if not 0.0 <= max_dropout <= 1.0:
-        raise ValueError(f"sample_crops expects 0 <= max_dropout <= 1, got {max_dropout}")
+        raise TypeError(f"{what} expects a SceneSet, got {type(scenes).__name__}")
+    check_npoints(npoints, what)
+    check_dropout(max_dropout, what)
     if not isinstance(rotate, bool):
-        raise TypeError(f"sample_crops expects a bool rotate, got {type(rotate).__name__}")
+        raise TypeError(f"{what} expects a bool rotate, got {type(rotate).__name__}")
     dev = scenes.device
     if dev.type != "cuda":
-        raise RuntimeError(f"sample_crops needs a SceneSet on a CUDA device: pointnet2_b200 has no CPU path (got {dev})")
-    if not isinstance(crop_scene, torch.Tensor):
-        raise TypeError(f"crop_scene must be a torch.Tensor, got {type(crop_scene).__name__}")
-    if crop_scene.dtype.is_floating_point or crop_scene.dtype.is_complex or crop_scene.dtype == torch.bool:
-        raise TypeError(f"crop_scene must be an integer tensor, got {crop_scene.dtype}")
-    if crop_scene.dim() != 1 or not 1 <= crop_scene.shape[0] <= CROP_MAX_BATCH:
-        raise ValueError(f"sample_crops expects a (B,) crop_scene with 1 <= B <= {CROP_MAX_BATCH}, got {tuple(crop_scene.shape)}")
-    if not crop_scene.is_cuda:
-        raise RuntimeError(f"crop_scene must be a CUDA tensor: pointnet2_b200 has no CPU path (got device {crop_scene.device})")
+        raise RuntimeError(f"{what} needs a SceneSet on a CUDA device: pointnet2_b200 has no CPU path (got {dev})")
+    crop_scene, = index_tensors(what, dev, CROP_MAX_BATCH, crop_scene=crop_scene)
     b = crop_scene.shape[0]
-    if b * npoints * 3 >= _I31:
-        raise ValueError(f"sample_crops: {b} crops of {npoints} rows pass 2^31 elements")
-    seed_val, seed_dev = 0, None
-    if isinstance(seed, torch.Tensor):
-        if seed.dtype != torch.int64 or tuple(seed.shape) != (1,):
-            raise TypeError(f"a tensor seed must be a (1,) int64 tensor, got {seed.dtype} {tuple(seed.shape)}")
-        if not seed.is_cuda:
-            raise RuntimeError(f"a tensor seed must be a CUDA tensor (got device {seed.device})")
-        seed_dev = seed
-    elif isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
-        raise TypeError(f"sample_crops expects an int or a (1,) int64 CUDA tensor seed, got {type(seed).__name__}")
-    else:
-        seed = int(seed)
-        if not -2 ** 63 <= seed < _U64:
-            raise ValueError(f"sample_crops expects a 64-bit seed, got {seed}")
-        seed_val = seed - _U64 if seed >= 2 ** 63 else seed   # the same 64 bits, as a signed value
-    label_weights = require_cuda(label_weights, "label_weights", torch.float32)
-    if tuple(label_weights.shape) != (scenes.num_class,):
-        raise ValueError(f"sample_crops expects ({scenes.num_class},) label_weights, got {tuple(label_weights.shape)}")
-    for name, t in (("crop_scene", crop_scene), ("label_weights", label_weights), ("seed", seed_dev)):
-        if t is not None and t.device != dev:
-            raise RuntimeError(f"{name} must be on the scene set's device {dev}, got {t.device}")
-    crop_scene = crop_scene.to(torch.int64).contiguous()
+    if b * npoints * 3 >= I31:
+        raise ValueError(f"{what}: {b} crops of {npoints} rows pass 2^31 elements")
+    seed_val, seed_dev = seed_args(seed, what, dev)
+    label_weights = _label_weights(label_weights, scenes, what)
     lib = _lib.load()
     with on_device(scenes.xyz):
         wsb = int(lib.pn2_scene_crops_workspace_bytes(b, npoints))
@@ -491,15 +457,6 @@ class SceneScans(NamedTuple):
     valid: torch.Tensor
 
 
-def _index_tensor(t, name: str, what: str, max_batch: int) -> torch.Tensor:
-    if not isinstance(t, torch.Tensor):
-        raise TypeError(f"{name} must be a torch.Tensor, got {type(t).__name__}")
-    if t.dtype.is_floating_point or t.dtype.is_complex or t.dtype == torch.bool:
-        raise TypeError(f"{name} must be an integer tensor, got {t.dtype}")
-    if t.dim() != 1 or not 1 <= t.shape[0] <= max_batch:
-        raise ValueError(f"{what} expects a (B,) {name} with 1 <= B <= {max_batch}, got {tuple(t.shape)}")
-
-
 def sample_virtual_scans(scenes: SceneSet, scan_scene: torch.Tensor, scan_mode: torch.Tensor, seed,
                          label_weights: torch.Tensor, npoints: int = 8192, min_points: int = 300) -> SceneScans:
     """B virtual scans of ``scenes`` on the GPU (DESIGN.md §6.12): entry i is what a camera 1.5 m high, behind the
@@ -516,50 +473,20 @@ def sample_virtual_scans(scenes: SceneSet, scan_scene: torch.Tensor, scan_mode: 
     what = "sample_virtual_scans"
     if not isinstance(scenes, SceneSet):
         raise TypeError(f"{what} expects a SceneSet, got {type(scenes).__name__}")
-    if isinstance(npoints, bool) or not isinstance(npoints, int):
-        raise TypeError(f"{what} expects an integer npoints, got {type(npoints).__name__}")
-    if not 1 <= npoints <= CROP_MAX_POINTS:
-        raise ValueError(f"{what} expects 1 <= npoints <= {CROP_MAX_POINTS} (the shared-memory sort), got {npoints}")
+    check_npoints(npoints, what)
     if isinstance(min_points, bool) or not isinstance(min_points, int):
         raise TypeError(f"{what} expects an integer min_points, got {type(min_points).__name__}")
-    if not 0 <= min_points < _I31:
+    if not 0 <= min_points < I31:
         raise ValueError(f"{what} expects 0 <= min_points < 2^31, got {min_points}")
     dev = scenes.device
     if dev.type != "cuda":
         raise RuntimeError(f"{what} needs a SceneSet on a CUDA device: pointnet2_b200 has no CPU path (got {dev})")
-    _index_tensor(scan_scene, "scan_scene", what, SCAN_MAX_BATCH)
-    _index_tensor(scan_mode, "scan_mode", what, SCAN_MAX_BATCH)
+    scan_scene, scan_mode = index_tensors(what, dev, SCAN_MAX_BATCH, scan_scene=scan_scene, scan_mode=scan_mode)
     b = scan_scene.shape[0]
-    if scan_mode.shape[0] != b:
-        raise ValueError(f"{what} expects one scan_mode per scan_scene, got {scan_mode.shape[0]} and {b}")
-    for name, t in (("scan_scene", scan_scene), ("scan_mode", scan_mode)):
-        if not t.is_cuda:
-            raise RuntimeError(f"{name} must be a CUDA tensor: pointnet2_b200 has no CPU path (got device {t.device})")
-    if b * npoints * 3 >= _I31:
+    if b * npoints * 3 >= I31:
         raise ValueError(f"{what}: {b} scans of {npoints} rows pass 2^31 elements")
-    seed_val, seed_dev = 0, None
-    if isinstance(seed, torch.Tensor):
-        if seed.dtype != torch.int64 or tuple(seed.shape) != (1,):
-            raise TypeError(f"a tensor seed must be a (1,) int64 tensor, got {seed.dtype} {tuple(seed.shape)}")
-        if not seed.is_cuda:
-            raise RuntimeError(f"a tensor seed must be a CUDA tensor (got device {seed.device})")
-        seed_dev = seed
-    elif isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
-        raise TypeError(f"{what} expects an int or a (1,) int64 CUDA tensor seed, got {type(seed).__name__}")
-    else:
-        seed = int(seed)
-        if not -2 ** 63 <= seed < _U64:
-            raise ValueError(f"{what} expects a 64-bit seed, got {seed}")
-        seed_val = seed - _U64 if seed >= 2 ** 63 else seed   # the same 64 bits, as a signed value
-    label_weights = require_cuda(label_weights, "label_weights", torch.float32)
-    if tuple(label_weights.shape) != (scenes.num_class,):
-        raise ValueError(f"{what} expects ({scenes.num_class},) label_weights, got {tuple(label_weights.shape)}")
-    for name, t in (("scan_scene", scan_scene), ("scan_mode", scan_mode), ("label_weights", label_weights),
-                    ("seed", seed_dev)):
-        if t is not None and t.device != dev:
-            raise RuntimeError(f"{name} must be on the scene set's device {dev}, got {t.device}")
-    scan_scene = scan_scene.to(torch.int64).contiguous()
-    scan_mode = scan_mode.to(torch.int64).contiguous()
+    seed_val, seed_dev = seed_args(seed, what, dev)
+    label_weights = _label_weights(label_weights, scenes, what)
     lib = _lib.load()
     max_scene = int(scenes.sizes.max())
     with on_device(scenes.xyz):

@@ -23,11 +23,10 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._tensor import on_device, ptr, stream_ptr
+from ._tensor import (I31, SELECT_MAX_ROWS, check_dropout, check_npoints, index_tensors, on_device, pack_offsets, ptr,
+                      seed_args, stream_ptr, to_host)
 
-MAX_POINTS = 16384   # points per shape and npoints: the kernel's (key, row) sort lives in 16384 x 8 B of shared memory
-_I31 = 2 ** 31
-_U64 = 2 ** 64
+MAX_POINTS = SELECT_MAX_ROWS  # points per shape and npoints: the kernel's (key, row) sort is in shared memory
 
 
 def pc_normalize(pc: np.ndarray) -> np.ndarray:
@@ -36,12 +35,6 @@ def pc_normalize(pc: np.ndarray) -> np.ndarray:
     pc = pc - centroid
     m = np.max(np.sqrt(np.sum(pc ** 2, axis=1)))
     return pc / m
-
-
-def _host(a) -> np.ndarray:
-    if isinstance(a, torch.Tensor):
-        return a.detach().cpu().numpy()
-    return np.asarray(a)
 
 
 class ShapeSet:
@@ -65,22 +58,18 @@ class ShapeSet:
         for name, lst in (("normal", normal_list), ("part", part_list)):
             if lst is not None and len(list(lst)) != len(xyz_list):
                 raise ValueError(f"ShapeSet expects one {name} array per shape, got {len(list(lst))} for {len(xyz_list)} shapes")
-        xyz_list = [_host(x) for x in xyz_list]
-        normal_list = None if normal_list is None else [_host(n) for n in normal_list]
-        part_list = None if part_list is None else [_host(p) for p in part_list]
-        sizes = []
+        xyz_list = [to_host(x) for x in xyz_list]
+        normal_list = None if normal_list is None else [to_host(n) for n in normal_list]
+        part_list = None if part_list is None else [to_host(p) for p in part_list]
         for k, x in enumerate(xyz_list):
             if x.ndim != 2 or x.shape[1] != 3:
                 raise ValueError(f"ShapeSet: shape {k} must be (num_points, 3), got {x.shape}")
             if not 1 <= len(x) <= MAX_POINTS:
                 raise ValueError(f"ShapeSet: shape {k} has {len(x)} points; a shape has 1 to {MAX_POINTS}")
-            sizes.append(len(x))
-        self.sizes = np.array(sizes, np.int64)
-        if int(self.sizes.sum()) >= _I31 - 1:
-            raise ValueError(f"ShapeSet takes fewer than 2^31 - 1 points in all, got {int(self.sizes.sum())}")
+        self.sizes, self.offsets = pack_offsets(xyz_list, "ShapeSet", device)
         labels = []
         for k, lab in enumerate(label_list):
-            lab = _host(lab)
+            lab = to_host(lab)
             if lab.size != 1 or not np.issubdtype(lab.dtype, np.integer):
                 raise TypeError(f"ShapeSet: shape {k} has label {lab!r}; expected one integer")
             lab = int(lab.reshape(()))
@@ -112,17 +101,15 @@ class ShapeSet:
                     raise ValueError(f"ShapeSet: shape {k} has {len(x)} points but part labels of shape {p.shape}")
                 if not np.issubdtype(p.dtype, np.integer):
                     raise TypeError(f"ShapeSet: shape {k} has {p.dtype} part labels, expected integers")
-                if p.min() < 0 or p.max() >= _I31:
+                if p.min() < 0 or p.max() >= I31:
                     raise ValueError(f"ShapeSet: shape {k} has part labels outside [0, 2^31)")
                 parts.append(p.astype(np.int32))
-        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.device = dev = self.offsets.device  # "cuda" resolved to the current index: compared against by the samplers
         self.num_class = num_class
         self.xyz = torch.from_numpy(np.concatenate(pts)).to(dev)
-        self.device = self.xyz.device  # "cuda" resolves to the current index here: compared against in sample_shapes
         self.normals = torch.from_numpy(np.concatenate(nrms)).to(dev) if normal_list is not None else None
         self.part = torch.from_numpy(np.concatenate(parts)).to(dev) if part_list is not None else None
         self.label = torch.tensor(labels, dtype=torch.int32).to(dev)
-        self.offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(self.sizes)]).astype(np.int64)).to(dev)
 
     def __len__(self) -> int:
         return len(self.sizes)
@@ -140,24 +127,6 @@ class ShapeBatch(NamedTuple):
     part: Optional[torch.Tensor]
     lengths: torch.Tensor
     point_idx: torch.Tensor
-
-
-def _seed_args(seed, dev, op):
-    """(value, device tensor or None) of an int seed or a (1,) int64 CUDA tensor seed."""
-    if isinstance(seed, torch.Tensor):
-        if seed.dtype != torch.int64 or tuple(seed.shape) != (1,):
-            raise TypeError(f"a tensor seed must be a (1,) int64 tensor, got {seed.dtype} {tuple(seed.shape)}")
-        if not seed.is_cuda:
-            raise RuntimeError(f"a tensor seed must be a CUDA tensor (got device {seed.device})")
-        if seed.device != dev:
-            raise RuntimeError(f"seed must be on the shape set's device {dev}, got {seed.device}")
-        return 0, seed
-    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)):
-        raise TypeError(f"{op} expects an int or a (1,) int64 CUDA tensor seed, got {type(seed).__name__}")
-    seed = int(seed)
-    if not -2 ** 63 <= seed < _U64:
-        raise ValueError(f"{op} expects a 64-bit seed, got {seed}")
-    return (seed - _U64 if seed >= 2 ** 63 else seed), None   # the same 64 bits, as a signed value
 
 
 def _number(v, name, op):
@@ -178,12 +147,10 @@ def _pair(v, name, op):
 
 
 def _check_call(shapes, shape_idx, npoints, with_normals, op):
+    """shape_idx as the kernel reads it, once the arguments every shape batch takes are checked."""
     if not isinstance(shapes, ShapeSet):
         raise TypeError(f"{op} expects a ShapeSet, got {type(shapes).__name__}")
-    if isinstance(npoints, bool) or not isinstance(npoints, int):
-        raise TypeError(f"{op} expects an integer npoints, got {type(npoints).__name__}")
-    if not 1 <= npoints <= MAX_POINTS:
-        raise ValueError(f"{op} expects 1 <= npoints <= {MAX_POINTS} (the shared-memory sort), got {npoints}")
+    check_npoints(npoints, op)
     if not isinstance(with_normals, bool):
         raise TypeError(f"{op} expects a bool with_normals, got {type(with_normals).__name__}")
     if with_normals and shapes.normals is None:
@@ -191,17 +158,7 @@ def _check_call(shapes, shape_idx, npoints, with_normals, op):
     dev = shapes.device
     if dev.type != "cuda":
         raise RuntimeError(f"{op} needs a ShapeSet on a CUDA device: pointnet2_b200 has no CPU path (got {dev})")
-    if not isinstance(shape_idx, torch.Tensor):
-        raise TypeError(f"shape_idx must be a torch.Tensor, got {type(shape_idx).__name__}")
-    if shape_idx.dtype.is_floating_point or shape_idx.dtype.is_complex or shape_idx.dtype == torch.bool:
-        raise TypeError(f"shape_idx must be an integer tensor, got {shape_idx.dtype}")
-    if shape_idx.dim() != 1 or shape_idx.shape[0] < 1:
-        raise ValueError(f"{op} expects a (B,) shape_idx with B >= 1, got {tuple(shape_idx.shape)}")
-    if not shape_idx.is_cuda:
-        raise RuntimeError(f"shape_idx must be a CUDA tensor: pointnet2_b200 has no CPU path (got device {shape_idx.device})")
-    if shape_idx.device != dev:
-        raise RuntimeError(f"shape_idx must be on the shape set's device {dev}, got {shape_idx.device}")
-    return dev
+    return index_tensors(op, dev, shape_idx=shape_idx)[0]
 
 
 def _launch(shapes, shape_idx, seed_val, seed_dev, votes, npoints, subset_random, rotate, perturb, scale, shift, jitter,
@@ -210,9 +167,8 @@ def _launch(shapes, shape_idx, seed_val, seed_dev, votes, npoints, subset_random
     b = shape_idx.shape[0]
     e = b * votes if votes else b
     ch = 6 if with_normals else 3
-    if e * npoints * ch >= _I31:
+    if e * npoints * ch >= I31:
         raise ValueError(f"{e} entries of {npoints} rows x {ch} channels pass 2^31 elements")
-    shape_idx = shape_idx.to(torch.int64).contiguous()
     lib = _lib.load()
     with on_device(shapes.xyz):
         out = ShapeBatch(
@@ -265,12 +221,9 @@ def sample_shapes(shapes: ShapeSet, shape_idx: torch.Tensor, seed, npoints: int 
     shift = _number(shift, "shift", op)
     if shift < 0:
         raise ValueError(f"{op} expects shift >= 0, got {shift}")
-    if isinstance(max_dropout, bool) or not isinstance(max_dropout, (int, float)):
-        raise TypeError(f"{op} expects a number for max_dropout, got {type(max_dropout).__name__}")
-    if not 0.0 <= max_dropout <= 1.0:
-        raise ValueError(f"{op} expects 0 <= max_dropout <= 1, got {max_dropout}")
-    dev = _check_call(shapes, shape_idx, npoints, with_normals, op)
-    seed_val, seed_dev = _seed_args(seed, dev, op)
+    check_dropout(max_dropout, op)
+    shape_idx = _check_call(shapes, shape_idx, npoints, with_normals, op)
+    seed_val, seed_dev = seed_args(seed, op, shapes.device)
     return _launch(shapes, shape_idx, seed_val, seed_dev, 0, npoints, subset == "random", rotate, perturb, scale, shift,
                    jitter, max_dropout, with_normals)
 
@@ -283,10 +236,10 @@ def vote_batch(shapes: ShapeSet, shape_idx: torch.Tensor, num_votes: int, seed, 
     op = "vote_batch"
     if isinstance(num_votes, bool) or not isinstance(num_votes, int) or num_votes < 1:
         raise ValueError(f"{op} expects a positive integer num_votes, got {num_votes!r}")
-    dev = _check_call(shapes, shape_idx, npoints, with_normals, op)
-    if shape_idx.shape[0] * num_votes >= _I31:
+    shape_idx = _check_call(shapes, shape_idx, npoints, with_normals, op)
+    if shape_idx.shape[0] * num_votes >= I31:
         raise ValueError(f"{op}: {shape_idx.shape[0]} shapes x {num_votes} votes pass 2^31 entries")
-    seed_val, seed_dev = _seed_args(seed, dev, op)
+    seed_val, seed_dev = seed_args(seed, op, shapes.device)
     return _launch(shapes, shape_idx, seed_val, seed_dev, num_votes, npoints, False, False, False, None, 0.0, None, 0.0,
                    with_normals)
 
