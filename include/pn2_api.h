@@ -315,6 +315,33 @@ int pn2_masked_bn_relu_backward_typed(int dtype, int rows, int c, const void* dy
                                       const float* save_invstd, void* dx, float* dgamma, float* dbeta, void* workspace,
                                       size_t workspace_bytes, void* stream);
 
+/* ---- learned layers: the inference tail of a set-abstraction level (utils/pointnet_util.py:45-54 + :115-124, MSG
+ * :179-191) in one launch -----------------------------------------------------------------------------------------------
+ * For every group (i, j) of b x m:   row k = concat(xyz[i, idx[i,j,k]] - new_xyz[i,j], points[i, idx[i,j,k]]) in the order
+ * xyz_first chooses (as pn2_group_concat; use_xyz == 0 with points: the features alone), then for each of nlayers <= 4
+ * layers   row = act((row . W^T + bias - mean) * gamma / sqrt(var + eps) + beta),   and out[i, j, :] = max over k of row.
+ * No tensor of b*m*nsample rows is written.  xyz (b,n,3) f32; new_xyz (b,m,3) f32 or NULL (zeros); points (b,n,c) in
+ * `dtype` or NULL (c is then taken as 0); idx (b,m,nsample) i32 with every index < n, or NULL (row k is point k; needs
+ * nsample == n: the one group that holds the whole cloud).  Per layer l, HOST arrays of nlayers entries holding DEVICE
+ * pointers to the module's own float32 tensors: widths[l] = C_out (<= 1024; C_in of layer 0 is c + 3 or c, <= 1027),
+ * weight[l] (C_out, C_in) row-major, bias[l] (C_out) or NULL, and for the batch norm bn_mean[l] / bn_var[l] (the running
+ * statistics; bn_mean == NULL or bn_mean[l] == NULL: the layer has none), bn_weight[l] / bn_bias[l] (NULL: not affine),
+ * bn_eps[l]; relu[l] != 0: act = max(., 0), else the identity.  The kernel derives the per-channel scale and shift
+ * itself: there is no folded copy of the parameters that could go stale.
+ * out: group (i, j) is written at out + (i*m + j) * out_row_stride, widths[nlayers-1] elements of `dtype`, so one scale
+ * of a multi-scale level can write its slice of the concatenated (b, m, sum of widths) tensor.
+ * PN2_F32: FP32 fused multiply-adds in ascending channel order.  PN2_BF16 / PN2_F16: tensor-core products of the 16-bit
+ * rows with the weights rounded to the 16-bit type, float32 accumulation; the centred xyz are rounded once (as
+ * pn2_group_concat_typed), and each layer's result is rounded once after the affine and the activation, in float32.
+ * Every output depends on its own group alone and every sum has a fixed order: the same bits on every run, whatever b is
+ * and whatever the other groups hold.  NaN propagates through the maximum as in torch.  b == 0 or m == 0 launches
+ * nothing; invalid arguments return cudaErrorInvalidValue without a launch. */
+int pn2_sa_mlp_max_typed(int dtype, int b, int n, int c, int m, int nsample, const float* xyz, const float* new_xyz,
+                         const void* points, const int* idx, int xyz_first, int use_xyz, int nlayers, const int* widths,
+                         const float* const* weight, const float* const* bias, const float* const* bn_weight,
+                         const float* const* bn_bias, const float* const* bn_mean, const float* const* bn_var,
+                         const float* bn_eps, const int* relu, void* out, long long out_row_stride, void* stream);
+
 /* ---- the sampling+grouping half of a set-abstraction layer, device-resident ------------------ */
 
 /* query_ball_point + group_point(xyz) in ONE launch (tf_grouping_g.cu:3-57 back to back, as

@@ -73,6 +73,9 @@ _SIGNATURES = {
     "pn2_masked_bn_relu_forward_typed": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, c_float, c_float, _P, _P, _P, _P, _P, _P, _P,
                                                  c_size_t, _P]),
     "pn2_masked_bn_relu_backward_typed": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    # inference tail of a set-abstraction level: gather + shared MLP (eval-mode batch norm) + max-pool
+    "pn2_sa_mlp_max_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P,
+                                     _P, _P, _P, _P, _P, _P, _P, c_longlong, _P]),
     # whole-scene segmentation: block partition of a scene and the ordered merge of block logits
     "pn2_scene_blocks_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "pn2_scene_blocks_count": (c_int, [c_int, _P, c_double, c_double, c_double, c_double, c_double, c_int, c_int, _P, _P,

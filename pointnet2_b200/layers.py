@@ -4,7 +4,9 @@ The reference builds every learned layer as a 1x1 convolution + batch norm + ReL
 tensor (tf_util.conv2d called from utils/pointnet_util.py:115-121,146-152,187-190,221-226) and finds
 its variables by TensorFlow variable scope (``scope='layer1'`` ...).  On a channels-last tensor a 1x1
 convolution is a matrix product over the last axis, so ``SharedMLP`` is Linear + BatchNorm1d + ReLU over
-the flattened leading axes (cuBLAS through torch: dense layers are outside the hand-written hot path).
+the flattened leading axes.  In training that is cuBLAS and torch's batch norm (plus the masked batch norm kernel for
+padded batches); at inference the stack of a set-abstraction level runs inside ``sa_mlp_max``, one CUDA kernel that
+gathers the groups, applies every layer with the batch norm's running statistics and max-pools (csrc/sa_mlp.cu).
 
 ``scoped_mlp`` is the registry that lets the reference's own call form run unchanged::
 
@@ -17,6 +19,7 @@ an optimiser, ``reset_scopes()`` is ``tf.reset_default_graph()``.
 """
 from __future__ import annotations
 
+import ctypes
 from typing import Dict, Optional, Sequence
 
 import torch
@@ -24,7 +27,7 @@ from torch import nn
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from ._tensor import DTYPE_CODES, FEATURE_DTYPES, on_device, ptr, stream_ptr
+from ._tensor import DTYPE_CODES, FEATURE_DTYPES, on_device, ptr, require_cuda, same_device, stream_ptr
 
 
 # tf_util.batch_norm_template calls tf.contrib.layers.batch_norm without an epsilon, so the reference normalises with
@@ -35,7 +38,9 @@ BN_EPS = 1e-3
 
 class SharedMLP(nn.Module):
     """conv2d(1x1)+BN+ReLU stack on (..., C) tensors — tf_util.conv2d with xavier weights, zero bias, and the
-    reference's batch-norm epsilon (BN_EPS)."""
+    reference's batch-norm epsilon (BN_EPS).  Calling it runs the torch layers; the set-abstraction modules hand an
+    eval-mode stack to ``sa_mlp_max`` instead when ``sa_mlp_applies`` (no grad mode, CUDA, max-pooling), which reads
+    these same parameters and buffers on every call."""
 
     def __init__(self, in_channels: int, widths: Sequence[int], bn: bool = True, last_activation: bool = True):
         super().__init__()
@@ -233,6 +238,191 @@ def masked_batch_norm_relu(bn: nn.BatchNorm1d, x: torch.Tensor, keep: torch.Tens
     weight = bn.weight if bn.affine else None
     bias = bn.bias if bn.affine else None
     return _MaskedBatchNormReLU.apply(x, weight, bias, keep, bn)
+
+
+SA_MLP_MAX_LAYERS = 4
+SA_MLP_MAX_WIDTH = 1024  # of a layer's output; the first layer takes up to SA_MLP_MAX_WIDTH + 3 input channels
+# Multiply-adds per grouped row (sum of C_in * C_out) up to which the modules take the kernel.  Above it the torch layers
+# win: measured on an NVIDIA H100 80GB HBM3 at 700 W (DESIGN.md 6.13), [256, 512, 1024] on 259 inputs (721 K) runs 0.23-0.55 ms through cuBLAS and
+# 1.1-1.3 ms fused, while [256, 256, 512] on 259 inputs (263 K) is faster fused.  A function of the widths alone, so
+# that a level takes the same route, and gives the same bits, at every batch size.
+SA_MLP_MAX_MACS = 300_000
+
+
+def _mlp_stack(mlp):
+    """The layers of a SharedMLP as [(Linear, BatchNorm1d or None, relu: bool)], or None when its body is not a sequence
+    of Linear [+ BatchNorm1d] [+ ReLU]."""
+    if not isinstance(mlp, SharedMLP):
+        return None
+    stack = []
+    for mod in mlp.body:
+        if isinstance(mod, nn.Linear):
+            stack.append([mod, None, False])
+        elif not stack or stack[-1][2]:
+            return None
+        elif isinstance(mod, nn.BatchNorm1d) and stack[-1][1] is None:
+            stack[-1][1] = mod
+        elif isinstance(mod, nn.ReLU):
+            stack[-1][2] = True
+        else:
+            return None
+    return [tuple(e) for e in stack] or None
+
+
+def _linear_misfit(lin: nn.Linear, device) -> Optional[Exception]:
+    """As _bn_tensors_misfit, for a Linear's weight and bias."""
+    for name, t in (("weight", lin.weight), ("bias", lin.bias)):
+        if t is None:
+            continue
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            return TypeError(f"linear {name} must be a contiguous torch.float32 tensor, got {t.dtype}"
+                             f"{'' if t.is_contiguous() else ' (not contiguous)'}")
+        if t.device != device:
+            return RuntimeError(f"linear {name} must be on the inputs' device {device}, got device {t.device}")
+    return None
+
+
+def sa_mlp_dtype(points: Optional[torch.Tensor]):
+    """The arithmetic (and output) type of sa_mlp_max: the autocast dtype inside torch.autocast, else that of points
+    (float32 without points)."""
+    if torch.is_autocast_enabled("cuda"):
+        return torch.get_autocast_dtype("cuda")
+    return torch.float32 if points is None else points.dtype
+
+
+def sa_mlp_applies(mlp, xyz: torch.Tensor, points: Optional[torch.Tensor] = None, pooling: str = 'max') -> bool:
+    """Whether a set-abstraction level with this learned stack runs through sa_mlp_max: ``mlp`` is a SharedMLP of at
+    most SA_MLP_MAX_LAYERS layers no wider than SA_MLP_MAX_WIDTH whose batch norms are all in eval mode with running
+    statistics and whose layers add up to at most SA_MLP_MAX_MACS multiply-adds per row (beyond that cuBLAS is faster),
+    its parameters and buffers float32 on the inputs' device, grad mode is off, the inputs are on CUDA with
+    features in float32 / bfloat16 / float16 (under autocast: an autocast dtype of bfloat16 / float16), and the pooling
+    is 'max'.  Everything else (training, grad mode, a module converted to 16 bits, other callables, other poolings)
+    keeps the torch layers."""
+    stack = _mlp_stack(mlp)
+    if stack is None or pooling != 'max' or torch.is_grad_enabled() or not xyz.is_cuda:
+        return False
+    if points is not None and (not points.is_cuda or points.dtype not in FEATURE_DTYPES):
+        return False
+    if sa_mlp_dtype(points) not in FEATURE_DTYPES:
+        return False
+    if len(stack) > SA_MLP_MAX_LAYERS or mlp.in_channels > SA_MLP_MAX_WIDTH + 3:
+        return False
+    if sum(lin.in_features * lin.out_features for lin, _, _ in stack) > SA_MLP_MAX_MACS:
+        return False
+    for lin, bn, _ in stack:
+        if lin.out_features > SA_MLP_MAX_WIDTH or _linear_misfit(lin, xyz.device) is not None:
+            return False
+        if bn is not None and (bn.training or bn.running_mean is None or _bn_tensors_misfit(bn, xyz.device) is not None):
+            return False
+    return True
+
+
+def sa_mlp_max(xyz: torch.Tensor, new_xyz: Optional[torch.Tensor], points: Optional[torch.Tensor],
+               idx: Optional[torch.Tensor], mlp: SharedMLP, xyz_first: bool = True, use_xyz: bool = True,
+               out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The inference tail of a set-abstraction level as one CUDA op (csrc/sa_mlp.cu): for every group (b, s)
+
+        rows = concat(xyz[b, idx[b, s]] - new_xyz[b, s], points[b, idx[b, s]])     ([features, xyz] when not xyz_first;
+                                                                                    the features alone when not use_xyz)
+        out[b, s] = max over the rows of mlp(rows), its batch norms using their running statistics,
+
+    without writing a tensor of B*S*K rows.  ``xyz`` (B, N, 3) float32; ``new_xyz`` (B, S, 3) float32, or None for zeros;
+    ``points`` (B, N, C) float32 / bfloat16 / float16 or None; ``idx`` (B, S, K) int32, or None for the single group
+    that holds every point in order (S = 1, K = N); ``mlp`` a SharedMLP in eval mode, whose own parameters and buffers
+    the kernel reads (nothing is folded or cached, so a loaded checkpoint is seen at once).  ``out``: an optional
+    (B, S, C_out) tensor to write, which may be a channel slice of a wider contiguous (B, S, .) tensor.
+
+    The arithmetic type is that of ``points`` (float32 without points), or the autocast dtype inside torch.autocast, and
+    the result has it: float32 is FP32 fused multiply-adds, the 16-bit types run on the tensor cores with float32
+    accumulation and one rounding per layer.  Each output depends on its own group alone, so it has the same bits on
+    every run, at every batch size and next to any other cloud, which a cuBLAS product does not promise.  NaN
+    propagates as in the torch layers.  No gradient: call it under torch.no_grad().
+
+    Raises ValueError for a batch norm in training mode (that needs batch statistics: use the module itself) or without
+    running statistics, for more than 4 layers or widths above 1024, and for shapes that do not fit together; TypeError /
+    RuntimeError for tensors of the wrong dtype or device."""
+    stack = _mlp_stack(mlp)
+    if stack is None:
+        raise TypeError(f"sa_mlp_max expects a SharedMLP of Linear [+ BatchNorm1d] [+ ReLU] layers, got {type(mlp).__name__}")
+    for _, bn, _ in stack:
+        if bn is not None and bn.training and bn.running_mean is not None:
+            raise ValueError("sa_mlp_max uses the batch norms' running statistics; in training mode call the module itself")
+        if bn is not None and bn.running_mean is None:
+            raise ValueError("sa_mlp_max needs batch norms with running statistics (track_running_stats=True)")
+    if len(stack) > SA_MLP_MAX_LAYERS or max(lin.out_features for lin, _, _ in stack) > SA_MLP_MAX_WIDTH \
+            or mlp.in_channels > SA_MLP_MAX_WIDTH + 3:
+        raise ValueError(f"sa_mlp_max takes at most {SA_MLP_MAX_LAYERS} layers of at most {SA_MLP_MAX_WIDTH} channels "
+                         f"({SA_MLP_MAX_WIDTH + 3} inputs), got {mlp.in_channels} -> {[lin.out_features for lin, _, _ in stack]}")
+    if torch.is_grad_enabled() and any(p.requires_grad for p in mlp.parameters()):
+        raise RuntimeError("sa_mlp_max has no backward: call it under torch.no_grad()")
+    xyz = require_cuda(xyz, "xyz", torch.float32)
+    if xyz.dim() != 3 or xyz.shape[2] != 3:
+        raise ValueError(f"sa_mlp_max expects (batch_size, ndataset, 3) xyz, got {tuple(xyz.shape)}")
+    b, n = xyz.shape[0], xyz.shape[1]
+    tensors = [xyz]
+    if idx is not None:
+        idx = require_cuda(idx, "idx", torch.int32)
+        if idx.dim() != 3 or idx.shape[0] != b or idx.shape[2] < 1:
+            raise ValueError(f"idx must be (batch_size, npoint, nsample >= 1) matching xyz, got {tuple(idx.shape)}")
+        s, k = idx.shape[1], idx.shape[2]
+        tensors.append(idx)
+    else:
+        s, k = 1, n
+    if new_xyz is not None:
+        new_xyz = require_cuda(new_xyz, "new_xyz", torch.float32)
+        if tuple(new_xyz.shape) != (b, s, 3):
+            raise ValueError(f"new_xyz must be (batch_size, npoint, 3) = {(b, s, 3)}, got {tuple(new_xyz.shape)}")
+        tensors.append(new_xyz)
+    dtype = sa_mlp_dtype(points)
+    if dtype not in FEATURE_DTYPES:
+        raise TypeError(f"sa_mlp_max computes in float32, bfloat16 or float16, not the autocast dtype {dtype}")
+    c = 0
+    if points is not None:
+        points = require_cuda(points, "points", FEATURE_DTYPES)
+        if points.dim() != 3 or points.shape[:2] != xyz.shape[:2]:
+            raise ValueError("points must be (batch_size, ndataset, channel) matching xyz")
+        tensors.append(points)
+        c = points.shape[2]
+        if points.dtype != dtype:
+            points = points.to(dtype)  # autocast: as the first Linear would cast its input
+    cin = c + 3 if (use_xyz or points is None) else c
+    if cin != mlp.in_channels:
+        raise ValueError(f"the grouped rows have {cin} channels, mlp expects {mlp.in_channels}")
+    same_device(*tensors)
+    dev = xyz.device
+    for lin, bn, _ in stack:
+        misfit = _linear_misfit(lin, dev) or (None if bn is None else _bn_tensors_misfit(bn, dev))
+        if misfit is not None:
+            raise misfit
+    cout = mlp.out_channels
+    if out is None:
+        out = torch.empty((b, s, cout), dtype=dtype, device=dev)
+    else:
+        if not isinstance(out, torch.Tensor) or out.dtype != dtype or tuple(out.shape) != (b, s, cout):
+            raise ValueError(f"out must be a {dtype} tensor of shape {(b, s, cout)}, got "
+                             f"{getattr(out, 'dtype', type(out).__name__)} {tuple(getattr(out, 'shape', ()))}")
+        if out.device != dev:
+            raise RuntimeError(f"out must be on the inputs' device ({dev}), got {out.device}")
+        if b * s and (out.stride(2) != 1 or out.stride(1) < cout or (b > 1 and out.stride(0) != s * out.stride(1))):
+            raise ValueError("out must be a channel slice of a contiguous (batch_size, npoint, channels) tensor")
+    if b * s == 0:
+        return out
+    nl = len(stack)
+    pa = lambda ts: (ctypes.c_void_p * nl)(*[None if t is None else t.data_ptr() for t in ts])
+    bns = [bn for _, bn, _ in stack]
+    with on_device(xyz):
+        rc = _lib.load().pn2_sa_mlp_max_typed(
+            DTYPE_CODES[dtype], b, n, c, s, k, ptr(xyz), ptr(new_xyz), ptr(points), ptr(idx), 1 if xyz_first else 0,
+            1 if use_xyz else 0, nl, (ctypes.c_int * nl)(*[lin.out_features for lin, _, _ in stack]),
+            pa([lin.weight for lin, _, _ in stack]), pa([lin.bias for lin, _, _ in stack]),
+            pa([bn.weight if bn is not None and bn.affine else None for bn in bns]),
+            pa([bn.bias if bn is not None and bn.affine else None for bn in bns]),
+            pa([None if bn is None else bn.running_mean for bn in bns]),
+            pa([None if bn is None else bn.running_var for bn in bns]),
+            (ctypes.c_float * nl)(*[0.0 if bn is None else float(bn.eps) for bn in bns]),
+            (ctypes.c_int * nl)(*[1 if relu else 0 for _, _, relu in stack]), ptr(out), out.stride(1), stream_ptr(dev))
+    _lib.check(rc, "pn2_sa_mlp_max_typed")
+    return out
 
 
 def set_bn_momentum(model: nn.Module, bn_decay: float) -> None:

@@ -1,5 +1,6 @@
-"""torch twins of the learned tails around the geometry ops (SURVEY §8f n4 — OUTSIDE the measured
-hot path: dense layers belong to cuBLAS/cuDNN through torch, not to hand-written kernels).
+"""torch twins of the learned tails around the geometry ops (SURVEY §8f n4).  Training runs them through torch
+(cuBLAS / cuDNN, plus the masked batch norm kernel on padded batches); in eval mode under no_grad the set-abstraction
+tails run in the library's own kernel (layers.sa_mlp_max), the feature-propagation tails and heads through torch.
 
 The reference builds every learned layer as a 1x1 convolution + batch norm + ReLU on a
 channels-last tensor (tf_util.conv2d called from utils/pointnet_util.py:115-121,146-152,187-190,

@@ -5,13 +5,16 @@ set-abstraction / feature-propagation geometry path.
 (utils/pointnet_util.py:22-56, :59-84).  ``pointnet_sa_module``, ``pointnet_sa_module_msg`` and
 ``pointnet_fp_module`` keep the reference's full positional signatures (:87, :156, :199 — ``mlp`` lists of
 widths, ``is_training``, ``bn_decay``, ``scope``, ``bn`` ...), so the reference's model files call them
-unchanged; the dense half (1x1 conv + BN + ReLU stacks, :115-153, :187-195, :218-228) is cuDNN/cuBLAS
-territory and outside this path: width lists resolve to torch layers kept in a variable-scope registry
-(``layers.scoped_mlp``), or pass a callable, or None to get the grouped tensor pooled as-is.
+unchanged; the dense half (1x1 conv + BN + ReLU stacks, :115-153, :187-195, :218-228) is torch layers: width lists
+resolve to ``layers.SharedMLP`` modules kept in a variable-scope registry (``layers.scoped_mlp``), or pass a callable, or
+None to get the grouped tensor pooled as-is.
 
 ``fused=True`` (default) routes through the fused kernels (FPS+gather in one launch,
 group+centre+concat in one pass); ``fused=False`` issues the reference's exact op sequence.  Both
-produce identical values.
+produce identical values.  At inference (a SharedMLP in eval mode, grad mode off, max-pooling: ``layers.sa_mlp_applies``)
+``fused=True`` also runs the learned tail of a set-abstraction level in the kernel behind ``layers.sa_mlp_max``: gather,
+every layer and the max-pool in one launch, no grouped tensor in between.  Its float32 results differ from the torch
+layers' by float32 rounding (the sums are ordered differently), and unlike theirs do not depend on the batch size.
 """
 from __future__ import annotations
 
@@ -195,6 +198,20 @@ def _apply_mlp(mlp, t: torch.Tensor, scope=None, name="mlp", bn=True, is_trainin
     return mod(t) if mask is None else mod(t, mask)
 
 
+def _sa_mlp_route(mlp, xyz, points, use_xyz, scope, name, bn, is_training, bn_decay, pooling='max'):
+    """The SharedMLP behind ``mlp`` (a module, or a width list resolved through the scope registry) when the level's
+    tail runs through layers.sa_mlp_max, else None."""
+    if mlp is None or xyz.requires_grad or torch.is_grad_enabled() or pooling != 'max':
+        return None
+    if not callable(mlp):
+        widths = [int(w) for w in mlp]
+        if not widths:
+            return None
+        cin = 3 if points is None else points.shape[-1] + (3 if use_xyz else 0)
+        mlp = layers.scoped_mlp(scope, name, cin, widths, bn, xyz.device, is_training, bn_decay)
+    return mlp if layers.sa_mlp_applies(mlp, xyz, points, pooling) else None
+
+
 def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp=None, mlp2=None, group_all=False, is_training=None,
                        bn_decay=None, scope=None, bn=True, pooling='max', knn=False, use_xyz=True, use_nchw=False, fused=True,
                        lengths=None):
@@ -209,6 +226,26 @@ def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp=None, mlp2=None
         Not with group_all or knn (ValueError).
         Return: new_xyz (b,npoint,3), new_points (b,npoint,channels), idx (b,npoint,nsample)
     '''
+    tail = _sa_mlp_route(mlp, xyz, points, use_xyz, scope, "conv", bn, is_training, bn_decay, pooling) if fused else None
+    if tail is not None:
+        # inference: the kernel gathers the groups itself, so only the centroids and the indices are made here
+        if group_all:
+            _no_lengths_with(lengths, "group_all (the max-pool over every point would need a mask)")
+            b, n = xyz.shape[0], xyz.shape[1]
+            new_xyz = xyz.new_zeros((b, 1, 3))
+            idx = torch.arange(n, dtype=torch.int32, device=xyz.device).view(1, 1, n).expand(b, 1, n).contiguous()
+            new_points = layers.sa_mlp_max(xyz, None, points, None, tail, True, use_xyz)
+        else:
+            if knn:
+                _no_lengths_with(lengths, "knn grouping")
+                _, new_xyz = farthest_point_sample_and_gather(npoint, xyz)
+                _, idx = knn_point(nsample, xyz, new_xyz)
+            else:
+                _, new_xyz, idx, _, _ = sample_group(npoint, radius, nsample, xyz, center=True, want_grouped=False,
+                                                     lengths=lengths)
+            new_points = layers.sa_mlp_max(xyz, new_xyz, points, idx, tail, True, use_xyz)
+        new_points = _apply_mlp(mlp2, new_points.unsqueeze(2), scope, "conv_post", bn, is_training, bn_decay)
+        return new_xyz, new_points.squeeze(2), idx
     if group_all:
         _no_lengths_with(lengths, "group_all (the max-pool over every point would need a mask)")
         new_xyz, new_points, idx, grouped_xyz = sample_and_group_all(xyz, points, use_xyz)
@@ -245,9 +282,23 @@ def pointnet_sa_module_msg(xyz, points, npoint, radius_list: Sequence[float], ns
     '''
     pre = None
     if fused and not xyz.requires_grad and (points is None or use_xyz):
+        tails = None if mlp_list is None else [
+            _sa_mlp_route(mlp_list[i], xyz, points, use_xyz, scope, f"conv{i}", bn, is_training, bn_decay)
+            for i in range(len(radius_list))]
+        to_kernel = bool(tails) and all(t is not None for t in tails)
         # one call: the sampling pass and every scale's ball query (+ centred grouped xyz when they are the features)
         _, new_xyz, idx_list, _, gxyz_list = sample_group_msg(npoint, radius_list, nsample_list, xyz, center=True,
-                                                              want_grouped=points is None, lengths=lengths)
+                                                              want_grouped=points is None and not to_kernel,
+                                                              lengths=lengths)
+        if to_kernel:
+            # inference: each scale's kernel gathers its groups and writes its channels of the concatenated result
+            new_points = torch.empty((xyz.shape[0], new_xyz.shape[1], sum(t.out_channels for t in tails)),
+                                     dtype=layers.sa_mlp_dtype(points), device=xyz.device)
+            lo = 0
+            for idx, t in zip(idx_list, tails):
+                layers.sa_mlp_max(xyz, new_xyz, points, idx, t, False, use_xyz, out=new_points[..., lo:lo + t.out_channels])
+                lo += t.out_channels
+            return new_xyz, new_points
         pre = (idx_list, gxyz_list)
     elif fused and not xyz.requires_grad:
         _, new_xyz = farthest_point_sample_and_gather(npoint, xyz, lengths=lengths)
