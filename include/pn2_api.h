@@ -342,6 +342,34 @@ int pn2_sa_mlp_max_typed(int dtype, int b, int n, int c, int m, int nsample, con
                          const float* const* bn_bias, const float* const* bn_mean, const float* const* bn_var,
                          const float* bn_eps, const int* relu, void* out, long long out_row_stride, void* stream);
 
+/* ---- learned layers, row by row: feature-propagation tails and heads at inference (utils/pointnet_util.py:199-229)
+ * ------------------------------------------------------------------------------------------------------------------------
+ * The layers of pn2_sa_mlp_max_typed (same per-layer HOST arrays of DEVICE pointers, same arithmetic, nlayers <= 4,
+ * widths <= 1024), applied to every row with one output row per input row and no pooling; layer 0 takes up to 1536 inputs.
+ * Row r of the result is written at out + r * out_row_stride (widths[nlayers-1] elements of `dtype`).  Every output row
+ * depends on its own input row alone and every sum has a fixed order: the same bits whatever the row count and whatever
+ * the other rows hold.  Padding rows are never read and are written as 0.  Nothing is read back to the host, so both
+ * calls can be captured in a CUDA graph.  Invalid arguments return cudaErrorInvalidValue without a launch.
+ *
+ * pn2_fp_mlp_typed: row j of cloud i (b x n rows) is concat(interpolate(points2[i] at the 3-NN of xyz1[i,j] in xyz2[i]),
+ * points1[i,j]), the first c2 inputs bit-identical to what pn2_fp_interpolate_concat_ragged_typed writes.  xyz1 (b,n,3)
+ * f32, lengths1 (b,) device int32 or NULL (rows j >= lengths1[i], clamped to [1, n], are padding), xyz2 (b,m,3) f32,
+ * points1 (b,n,c1) in `dtype` or NULL (c1 is then taken as 0), points2 (b,m,c2) in `dtype`, c2 >= 1, c2 + c1 <= 1536,
+ * b <= 65535.  The 3-NN indices and weights go through `workspace`, pn2_fp_mlp_workspace_bytes(b, n) bytes (256-byte
+ * aligned); two launches.
+ * pn2_mlp_rows_typed: row r is x[r] (rows, c) in `dtype`, 1 <= c <= 1536; mask (rows,) bytes, nonzero on the real rows,
+ * or NULL (every row is real).  One launch. */
+size_t pn2_fp_mlp_workspace_bytes(int b, int n);
+int pn2_fp_mlp_typed(int dtype, int b, int n, int m, int c2, int c1, const float* xyz1, const int* lengths1, const float* xyz2,
+                     const void* points1, const void* points2, int nlayers, const int* widths, const float* const* weight,
+                     const float* const* bias, const float* const* bn_weight, const float* const* bn_bias,
+                     const float* const* bn_mean, const float* const* bn_var, const float* bn_eps, const int* relu, void* out,
+                     long long out_row_stride, void* workspace, size_t workspace_bytes, void* stream);
+int pn2_mlp_rows_typed(int dtype, long long rows, int c, const void* x, const unsigned char* mask, int nlayers,
+                       const int* widths, const float* const* weight, const float* const* bias, const float* const* bn_weight,
+                       const float* const* bn_bias, const float* const* bn_mean, const float* const* bn_var,
+                       const float* bn_eps, const int* relu, void* out, long long out_row_stride, void* stream);
+
 /* ---- the sampling+grouping half of a set-abstraction layer, device-resident ------------------ */
 
 /* query_ball_point + group_point(xyz) in ONE launch (tf_grouping_g.cu:3-57 back to back, as

@@ -25,5 +25,6 @@ from .pointnet_util import (  # noqa: F401
     sample_and_group_all,
 )
 from .host import SetAbstractionHost, SetAbstractionPipeline  # noqa: F401
+from .layers import batch_invariant, is_batch_invariant  # noqa: F401
 
 __version__ = "0.1.0"

@@ -76,6 +76,12 @@ _SIGNATURES = {
     # inference tail of a set-abstraction level: gather + shared MLP (eval-mode batch norm) + max-pool
     "pn2_sa_mlp_max_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P,
                                      _P, _P, _P, _P, _P, _P, _P, c_longlong, _P]),
+    # learned layers row by row: feature-propagation tails (3-NN interpolation + concat in front) and heads
+    "pn2_fp_mlp_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "pn2_fp_mlp_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_int, _P, _P, _P, _P, _P, _P,
+                                 _P, _P, _P, _P, c_longlong, _P, c_size_t, _P]),
+    "pn2_mlp_rows_typed": (c_int, [c_int, c_longlong, c_int, _P, _P, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_longlong,
+                                   _P]),
     # whole-scene segmentation: block partition of a scene and the ordered merge of block logits
     "pn2_scene_blocks_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "pn2_scene_blocks_count": (c_int, [c_int, _P, c_double, c_double, c_double, c_double, c_double, c_int, c_int, _P, _P,

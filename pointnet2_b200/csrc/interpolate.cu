@@ -152,10 +152,7 @@ three_nn_kernel(int n, int m, const float* __restrict__ xyz1, const float* __res
     }
 }
 
-// ---- three_interpolate ---------------------------------------------------------------------------
-__device__ __forceinline__ float interp3(float p1, float p2, float p3, float w1, float w2, float w3) {
-    return __fadd_rn(__fadd_rn(__fmul_rn(p1, w1), __fmul_rn(p2, w2)), __fmul_rn(p3, w3));
-}
+// ---- three_interpolate (interp3: pn2_common.cuh) ------------------------------------------------
 
 constexpr int kItThreads = 256;
 

@@ -127,6 +127,12 @@ __device__ __forceinline__ unsigned long long f2_fma(unsigned long long a, unsig
     return f2_pack(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 
+// ---- inverse-distance interpolation of three neighbours (three_interpolate, the FP front ends) --------------------
+// ((p1*w1 + p2*w2) + p3*w3), every operation rounded on its own: the reference's x86 arithmetic
+__device__ __forceinline__ float interp3(float p1, float p2, float p3, float w1, float w2, float w3) {
+    return __fadd_rn(__fadd_rn(__fmul_rn(p1, w1), __fmul_rn(p2, w2)), __fmul_rn(p3, w3));
+}
+
 // ---- per-cloud lengths -----------------------------------------------------------------------
 // Points of cloud `cloud` in a padded (b, n, 3) batch: lengths[cloud] clamped to [1, n] (a value out of range can
 // never make a kernel read outside its row), or n when the batch has no lengths (lengths == NULL).  n stays the

@@ -7,6 +7,8 @@ convolution is a matrix product over the last axis, so ``SharedMLP`` is Linear +
 the flattened leading axes.  In training that is cuBLAS and torch's batch norm (plus the masked batch norm kernel for
 padded batches); at inference the stack of a set-abstraction level runs inside ``sa_mlp_max``, one CUDA kernel that
 gathers the groups, applies every layer with the batch norm's running statistics and max-pools (csrc/sa_mlp.cu).
+Inside ``batch_invariant()`` the feature-propagation tails and every other eval-mode stack run through the row-wise
+twin of that kernel (``fp_mlp``, ``mlp_rows``; csrc/fp_mlp.cu), so that no learned layer's result depends on the batch.
 
 ``scoped_mlp`` is the registry that lets the reference's own call form run unchanged::
 
@@ -19,7 +21,9 @@ an optimiser, ``reset_scopes()`` is ``tf.reset_default_graph()``.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
+import math
 from typing import Dict, Optional, Sequence
 
 import torch
@@ -27,7 +31,7 @@ from torch import nn
 from torch.autograd.function import once_differentiable
 
 from . import _lib
-from ._tensor import DTYPE_CODES, FEATURE_DTYPES, on_device, ptr, require_cuda, same_device, stream_ptr
+from ._tensor import DTYPE_CODES, FEATURE_DTYPES, device_lengths, on_device, ptr, require_cuda, same_device, stream_ptr
 
 
 # tf_util.batch_norm_template calls tf.contrib.layers.batch_norm without an epsilon, so the reference normalises with
@@ -40,7 +44,8 @@ class SharedMLP(nn.Module):
     """conv2d(1x1)+BN+ReLU stack on (..., C) tensors — tf_util.conv2d with xavier weights, zero bias, and the
     reference's batch-norm epsilon (BN_EPS).  Calling it runs the torch layers; the set-abstraction modules hand an
     eval-mode stack to ``sa_mlp_max`` instead when ``sa_mlp_applies`` (no grad mode, CUDA, max-pooling), which reads
-    these same parameters and buffers on every call."""
+    these same parameters and buffers on every call.  Inside ``batch_invariant()`` a call that ``invariant_applies`` to
+    runs through ``mlp_rows``."""
 
     def __init__(self, in_channels: int, widths: Sequence[int], bn: bool = True, last_activation: bool = True):
         super().__init__()
@@ -64,6 +69,8 @@ class SharedMLP(nn.Module):
         """``mask``: optional bool tensor of t.shape[:-1] (or as many elements), True on the real rows of a padded batch
         (see row_mask).  Batch norm then takes its training statistics from the real rows only, and the padding rows of
         every layer's output are 0 (whatever t holds there, NaN included).  Without a mask: the plain stack."""
+        if _BATCH_INVARIANT and invariant_applies(self, t):
+            return _invariant_call(mlp_rows, t, self, mask)
         lead = t.shape[:-1]
         if mask is None:
             return self.body(t.reshape(-1, t.shape[-1])).reshape(*lead, self.out_channels)
@@ -282,6 +289,51 @@ def _linear_misfit(lin: nn.Linear, device) -> Optional[Exception]:
     return None
 
 
+def _eval_stack(mlp, who: str, max_in: int):
+    """The layers of ``mlp`` (see _mlp_stack) for a kernel that applies them with the batch norms' running statistics,
+    after the checks every such kernel makes: TypeError if it is not a SharedMLP, ValueError for a batch norm in training
+    mode or without running statistics and for more layers or wider ones than the kernels take, RuntimeError in grad
+    mode (the kernels have no backward)."""
+    stack = _mlp_stack(mlp)
+    if stack is None:
+        raise TypeError(f"{who} expects a SharedMLP of Linear [+ BatchNorm1d] [+ ReLU] layers, got {type(mlp).__name__}")
+    for _, bn, _ in stack:
+        if bn is not None and bn.training and bn.running_mean is not None:
+            raise ValueError(f"{who} uses the batch norms' running statistics; in training mode call the module itself")
+        if bn is not None and bn.running_mean is None:
+            raise ValueError(f"{who} needs batch norms with running statistics (track_running_stats=True)")
+    if len(stack) > SA_MLP_MAX_LAYERS or max(lin.out_features for lin, _, _ in stack) > SA_MLP_MAX_WIDTH \
+            or mlp.in_channels > max_in:
+        raise ValueError(f"{who} takes at most {SA_MLP_MAX_LAYERS} layers of at most {SA_MLP_MAX_WIDTH} channels "
+                         f"({max_in} inputs), got {mlp.in_channels} -> {[lin.out_features for lin, _, _ in stack]}")
+    if torch.is_grad_enabled() and any(p.requires_grad for p in mlp.parameters()):
+        raise RuntimeError(f"{who} has no backward: call it under torch.no_grad()")
+    return stack
+
+
+def _check_params(stack, dev) -> None:
+    for lin, bn, _ in stack:
+        misfit = _linear_misfit(lin, dev) or (None if bn is None else _bn_tensors_misfit(bn, dev))
+        if misfit is not None:
+            raise misfit
+
+
+def _layer_args(stack):
+    """nlayers and the per-layer host arrays of the fused-MLP C entries (pn2_sa_mlp_max_typed and its row-wise twins):
+    widths, weight, bias, bn_weight, bn_bias, bn_mean, bn_var, bn_eps, relu."""
+    nl = len(stack)
+    pa = lambda ts: (ctypes.c_void_p * nl)(*[None if t is None else t.data_ptr() for t in ts])
+    bns = [bn for _, bn, _ in stack]
+    return (nl, (ctypes.c_int * nl)(*[lin.out_features for lin, _, _ in stack]),
+            pa([lin.weight for lin, _, _ in stack]), pa([lin.bias for lin, _, _ in stack]),
+            pa([bn.weight if bn is not None and bn.affine else None for bn in bns]),
+            pa([bn.bias if bn is not None and bn.affine else None for bn in bns]),
+            pa([None if bn is None else bn.running_mean for bn in bns]),
+            pa([None if bn is None else bn.running_var for bn in bns]),
+            (ctypes.c_float * nl)(*[0.0 if bn is None else float(bn.eps) for bn in bns]),
+            (ctypes.c_int * nl)(*[1 if relu else 0 for _, _, relu in stack]))
+
+
 def sa_mlp_dtype(points: Optional[torch.Tensor]):
     """The arithmetic (and output) type of sa_mlp_max: the autocast dtype inside torch.autocast, else that of points
     (float32 without points)."""
@@ -297,7 +349,8 @@ def sa_mlp_applies(mlp, xyz: torch.Tensor, points: Optional[torch.Tensor] = None
     its parameters and buffers float32 on the inputs' device, grad mode is off, the inputs are on CUDA with
     features in float32 / bfloat16 / float16 (under autocast: an autocast dtype of bfloat16 / float16), and the pooling
     is 'max'.  Everything else (training, grad mode, a module converted to 16 bits, other callables, other poolings)
-    keeps the torch layers."""
+    keeps the torch layers.  Inside ``batch_invariant()`` the SA_MLP_MAX_MACS limit does not apply: the wide group_all
+    levels take the kernel too."""
     stack = _mlp_stack(mlp)
     if stack is None or pooling != 'max' or torch.is_grad_enabled() or not xyz.is_cuda:
         return False
@@ -307,7 +360,7 @@ def sa_mlp_applies(mlp, xyz: torch.Tensor, points: Optional[torch.Tensor] = None
         return False
     if len(stack) > SA_MLP_MAX_LAYERS or mlp.in_channels > SA_MLP_MAX_WIDTH + 3:
         return False
-    if sum(lin.in_features * lin.out_features for lin, _, _ in stack) > SA_MLP_MAX_MACS:
+    if not _BATCH_INVARIANT and sum(lin.in_features * lin.out_features for lin, _, _ in stack) > SA_MLP_MAX_MACS:
         return False
     for lin, bn, _ in stack:
         if lin.out_features > SA_MLP_MAX_WIDTH or _linear_misfit(lin, xyz.device) is not None:
@@ -341,20 +394,7 @@ def sa_mlp_max(xyz: torch.Tensor, new_xyz: Optional[torch.Tensor], points: Optio
     Raises ValueError for a batch norm in training mode (that needs batch statistics: use the module itself) or without
     running statistics, for more than 4 layers or widths above 1024, and for shapes that do not fit together; TypeError /
     RuntimeError for tensors of the wrong dtype or device."""
-    stack = _mlp_stack(mlp)
-    if stack is None:
-        raise TypeError(f"sa_mlp_max expects a SharedMLP of Linear [+ BatchNorm1d] [+ ReLU] layers, got {type(mlp).__name__}")
-    for _, bn, _ in stack:
-        if bn is not None and bn.training and bn.running_mean is not None:
-            raise ValueError("sa_mlp_max uses the batch norms' running statistics; in training mode call the module itself")
-        if bn is not None and bn.running_mean is None:
-            raise ValueError("sa_mlp_max needs batch norms with running statistics (track_running_stats=True)")
-    if len(stack) > SA_MLP_MAX_LAYERS or max(lin.out_features for lin, _, _ in stack) > SA_MLP_MAX_WIDTH \
-            or mlp.in_channels > SA_MLP_MAX_WIDTH + 3:
-        raise ValueError(f"sa_mlp_max takes at most {SA_MLP_MAX_LAYERS} layers of at most {SA_MLP_MAX_WIDTH} channels "
-                         f"({SA_MLP_MAX_WIDTH + 3} inputs), got {mlp.in_channels} -> {[lin.out_features for lin, _, _ in stack]}")
-    if torch.is_grad_enabled() and any(p.requires_grad for p in mlp.parameters()):
-        raise RuntimeError("sa_mlp_max has no backward: call it under torch.no_grad()")
+    stack = _eval_stack(mlp, "sa_mlp_max", SA_MLP_MAX_WIDTH + 3)
     xyz = require_cuda(xyz, "xyz", torch.float32)
     if xyz.dim() != 3 or xyz.shape[2] != 3:
         raise ValueError(f"sa_mlp_max expects (batch_size, ndataset, 3) xyz, got {tuple(xyz.shape)}")
@@ -390,10 +430,7 @@ def sa_mlp_max(xyz: torch.Tensor, new_xyz: Optional[torch.Tensor], points: Optio
         raise ValueError(f"the grouped rows have {cin} channels, mlp expects {mlp.in_channels}")
     same_device(*tensors)
     dev = xyz.device
-    for lin, bn, _ in stack:
-        misfit = _linear_misfit(lin, dev) or (None if bn is None else _bn_tensors_misfit(bn, dev))
-        if misfit is not None:
-            raise misfit
+    _check_params(stack, dev)
     cout = mlp.out_channels
     if out is None:
         out = torch.empty((b, s, cout), dtype=dtype, device=dev)
@@ -407,22 +444,195 @@ def sa_mlp_max(xyz: torch.Tensor, new_xyz: Optional[torch.Tensor], points: Optio
             raise ValueError("out must be a channel slice of a contiguous (batch_size, npoint, channels) tensor")
     if b * s == 0:
         return out
-    nl = len(stack)
-    pa = lambda ts: (ctypes.c_void_p * nl)(*[None if t is None else t.data_ptr() for t in ts])
-    bns = [bn for _, bn, _ in stack]
     with on_device(xyz):
         rc = _lib.load().pn2_sa_mlp_max_typed(
             DTYPE_CODES[dtype], b, n, c, s, k, ptr(xyz), ptr(new_xyz), ptr(points), ptr(idx), 1 if xyz_first else 0,
-            1 if use_xyz else 0, nl, (ctypes.c_int * nl)(*[lin.out_features for lin, _, _ in stack]),
-            pa([lin.weight for lin, _, _ in stack]), pa([lin.bias for lin, _, _ in stack]),
-            pa([bn.weight if bn is not None and bn.affine else None for bn in bns]),
-            pa([bn.bias if bn is not None and bn.affine else None for bn in bns]),
-            pa([None if bn is None else bn.running_mean for bn in bns]),
-            pa([None if bn is None else bn.running_var for bn in bns]),
-            (ctypes.c_float * nl)(*[0.0 if bn is None else float(bn.eps) for bn in bns]),
-            (ctypes.c_int * nl)(*[1 if relu else 0 for _, _, relu in stack]), ptr(out), out.stride(1), stream_ptr(dev))
+            1 if use_xyz else 0, *_layer_args(stack), ptr(out), out.stride(1), stream_ptr(dev))
     _lib.check(rc, "pn2_sa_mlp_max_typed")
     return out
+
+
+ROW_MLP_MAX_IN = 1536  # first-layer inputs of fp_mlp / mlp_rows (PointNet2PartSegMSG.fp1 takes 512 + 1024)
+
+
+def _out_rows(out, lead, cout, dtype, dev, who):
+    """``out`` checked as a (*lead, cout) tensor of dtype on dev whose rows are cout-wide slices of a contiguous tensor
+    (returned with its row stride), or a new one."""
+    if out is None:
+        return torch.empty((*lead, cout), dtype=dtype, device=dev), cout
+    if not isinstance(out, torch.Tensor) or out.dtype != dtype or tuple(out.shape) != (*lead, cout):
+        raise ValueError(f"{who}: out must be a {dtype} tensor of shape {(*lead, cout)}, got "
+                         f"{getattr(out, 'dtype', type(out).__name__)} {tuple(getattr(out, 'shape', ()))}")
+    if out.device != dev:
+        raise RuntimeError(f"{who}: out must be on the inputs' device ({dev}), got {out.device}")
+    rs = out.stride(-2) if out.dim() > 1 else cout
+    ok = out.stride(-1) == 1 and rs >= cout
+    for d in range(out.dim() - 2):  # every leading axis steps whole rows
+        ok = ok and (out.shape[d] == 1 or out.stride(d) == rs * math.prod(out.shape[d + 1:-1]))
+    if out.numel() and not ok:
+        raise ValueError(f"{who}: out must be a channel slice of a contiguous (..., channels) tensor")
+    return out, rs
+
+
+def fp_mlp(xyz1: torch.Tensor, xyz2: torch.Tensor, points1: Optional[torch.Tensor], points2: torch.Tensor, mlp: SharedMLP,
+           lengths=None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The inference tail of a feature-propagation level as one CUDA op (csrc/fp_mlp.cu): for every row j of cloud i
+
+        row = concat(interpolate(points2[i] at the 3-NN of xyz1[i, j] in xyz2[i]), points1[i, j])
+        out[i, j] = mlp(row), its batch norms using their running statistics,
+
+    the row bit-identical to what fp_interpolate_concat writes, and no (B, N1, C2 + C1) tensor in between.  ``xyz1``
+    (B, N1, 3) and ``xyz2`` (B, N2, 3) float32; ``points1`` (B, N1, C1) or None; ``points2`` (B, N2, C2) float32 /
+    bfloat16 / float16; ``mlp`` a SharedMLP in eval mode, C2 + C1 <= 1536 inputs, whose own parameters and buffers the
+    kernel reads on every call.  ``lengths``: optional (B,) per-cloud row counts of xyz1 / points1 (as
+    pointnet_fp_module takes them); padding rows are never read and come out 0.  ``out``: an optional (B, N1, C_out)
+    tensor to write, which may be a channel slice of a wider contiguous one.
+
+    Arithmetic as in sa_mlp_max: the dtype of points2, or the autocast dtype inside torch.autocast (points1 and points2
+    are then cast as the first Linear would cast its input); float32 is FP32 fused multiply-adds in ascending order, the
+    16-bit types run on the tensor cores with float32 accumulation and one rounding per layer.  Each output row depends
+    on its own row alone: the same bits at every batch size and next to any other cloud.  No gradient.
+
+    Errors as sa_mlp_max: TypeError for a stack that is not a SharedMLP or tensors of the wrong dtype, ValueError for a
+    training-mode batch norm, missing running statistics, too many or too wide layers and shapes that do not fit
+    together, RuntimeError in grad mode or for tensors off CUDA."""
+    stack = _eval_stack(mlp, "fp_mlp", ROW_MLP_MAX_IN)
+    xyz1 = require_cuda(xyz1, "xyz1", torch.float32)
+    xyz2 = require_cuda(xyz2, "xyz2", torch.float32)
+    points2 = require_cuda(points2, "points2", FEATURE_DTYPES)
+    if xyz1.dim() != 3 or xyz1.shape[2] != 3 or xyz2.dim() != 3 or xyz2.shape[2] != 3 or xyz2.shape[0] != xyz1.shape[0]:
+        raise ValueError(f"fp_mlp expects (batch_size, n1, 3) xyz1 and (batch_size, n2, 3) xyz2, got "
+                         f"{tuple(xyz1.shape)} and {tuple(xyz2.shape)}")
+    b, n, m = xyz1.shape[0], xyz1.shape[1], xyz2.shape[1]
+    if points2.dim() != 3 or points2.shape[:2] != xyz2.shape[:2] or points2.shape[2] < 1:
+        raise ValueError(f"points2 must be (batch_size, n2, channel >= 1) matching xyz2, got {tuple(points2.shape)}")
+    if m < 1:
+        raise ValueError("fp_mlp needs at least one known point (n2 >= 1)")
+    tensors = [xyz1, xyz2, points2]
+    dtype = sa_mlp_dtype(points2)
+    if dtype not in FEATURE_DTYPES:
+        raise TypeError(f"fp_mlp computes in float32, bfloat16 or float16, not the autocast dtype {dtype}")
+    c1 = 0
+    if points1 is not None:
+        points1 = require_cuda(points1, "points1", FEATURE_DTYPES)
+        if points1.dim() != 3 or points1.shape[:2] != xyz1.shape[:2]:
+            raise ValueError(f"points1 must be (batch_size, n1, channel) matching xyz1, got {tuple(points1.shape)}")
+        if points1.dtype != points2.dtype and not torch.is_autocast_enabled("cuda"):
+            raise TypeError(f"points1 ({points1.dtype}) and points2 ({points2.dtype}) must have one dtype")
+        tensors.append(points1)
+        c1 = points1.shape[2]
+    c2 = points2.shape[2]
+    if c2 + c1 != mlp.in_channels:
+        raise ValueError(f"the propagated rows have {c2} + {c1} channels, mlp expects {mlp.in_channels}")
+    same_device(*tensors)
+    dev = xyz1.device
+    _check_params(stack, dev)
+    lengths = device_lengths(lengths, b, n, dev, "fp_mlp")
+    if b > 65535:
+        raise ValueError(f"fp_mlp takes at most 65535 clouds, got {b}")
+    out, rs = _out_rows(out, (b, n), mlp.out_channels, dtype, dev, "fp_mlp")
+    if b * n == 0:
+        return out
+    points2 = points2.to(dtype)  # autocast: as the first Linear would cast its input
+    if points1 is not None:
+        points1 = points1.to(dtype)
+    lib = _lib.load()
+    with on_device(xyz1):
+        wsb = int(lib.pn2_fp_mlp_workspace_bytes(b, n))
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+        rc = lib.pn2_fp_mlp_typed(DTYPE_CODES[dtype], b, n, m, c2, c1, ptr(xyz1), ptr(lengths), ptr(xyz2), ptr(points1),
+                                  ptr(points2), *_layer_args(stack), ptr(out), rs, ptr(ws), wsb, stream_ptr(dev))
+    _lib.check(rc, "pn2_fp_mlp_typed")
+    return out
+
+
+def mlp_rows(t: torch.Tensor, mlp: SharedMLP, mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``mlp`` applied to every row of ``t`` (..., C) as one CUDA op (csrc/fp_mlp.cu), its batch norms using their
+    running statistics: what SharedMLP.forward(t, mask) computes in eval mode, with the arithmetic, the errors and the
+    batch invariance of fp_mlp.  ``mask``: optional bool tensor of t.shape[:-1] (or as many elements), True on the real
+    rows; the others are never read (they may be NaN) and come out 0.  C <= 1536.  Returns (..., C_out) in the
+    arithmetic dtype."""
+    stack = _eval_stack(mlp, "mlp_rows", ROW_MLP_MAX_IN)
+    t = require_cuda(t, "t", FEATURE_DTYPES)
+    if t.dim() < 1 or t.shape[-1] != mlp.in_channels:
+        raise ValueError(f"mlp_rows: t must be (..., {mlp.in_channels}), got {tuple(t.shape)}")
+    lead = tuple(t.shape[:-1])
+    rows = math.prod(lead)
+    tensors = [t]
+    if mask is not None:
+        if not isinstance(mask, torch.Tensor) or mask.dtype != torch.bool or mask.numel() != rows:
+            raise ValueError(f"mlp_rows expects a bool mask of {rows} rows, got "
+                             f"{getattr(mask, 'dtype', type(mask).__name__)} {tuple(getattr(mask, 'shape', ()))}")
+        tensors.append(mask)
+    dtype = sa_mlp_dtype(t)
+    if dtype not in FEATURE_DTYPES:
+        raise TypeError(f"mlp_rows computes in float32, bfloat16 or float16, not the autocast dtype {dtype}")
+    same_device(*tensors)
+    dev = t.device
+    _check_params(stack, dev)
+    out = torch.empty((*lead, mlp.out_channels), dtype=dtype, device=dev)
+    if rows == 0:
+        return out
+    t = t.to(dtype)  # autocast: as the first Linear would cast its input
+    keep = None if mask is None else mask.reshape(-1).contiguous().view(torch.uint8)
+    with on_device(t):
+        rc = _lib.load().pn2_mlp_rows_typed(DTYPE_CODES[dtype], rows, t.shape[-1], ptr(t), ptr(keep), *_layer_args(stack),
+                                            ptr(out), mlp.out_channels, stream_ptr(dev))
+    _lib.check(rc, "pn2_mlp_rows_typed")
+    return out
+
+
+# ---- batch-invariant inference ----------------------------------------------------------------------------------------
+_BATCH_INVARIANT = False
+
+
+def is_batch_invariant() -> bool:
+    """Whether the batch-invariant mode (batch_invariant()) is on."""
+    return _BATCH_INVARIANT
+
+
+@contextlib.contextmanager
+def batch_invariant(enabled: bool = True):
+    """Batch-invariant inference, process-wide (as torch.use_deterministic_algorithms), restored on exit::
+
+        with torch.no_grad(), layers.batch_invariant():
+            logits, _ = net.eval()(points, lengths)
+
+    Inside it every learned layer that runs in eval mode (batch norms with running statistics), with grad mode off, on
+    CUDA, goes through the fused kernels: set-abstraction tails through sa_mlp_max whatever their width
+    (SA_MLP_MAX_MACS does not apply), pointnet_fp_module with a SharedMLP through fp_mlp, and every other SharedMLP call
+    (the heads, mlp2, the stacks of non-max poolings) through mlp_rows.  Each output row then depends on its own inputs
+    alone, with the same bits at every batch size, chunking and padding, which the cuBLAS products of the torch layers do
+    not promise.  A layer the kernels cannot take (more than 4 layers, widths above 1024, inputs above 1536, a module
+    converted to 16 bits) raises RuntimeError instead of running the torch layers.  Training steps and grad-mode calls
+    are untouched: batch statistics depend on the batch by definition.  Outside the mode nothing changes."""
+    global _BATCH_INVARIANT
+    prev = _BATCH_INVARIANT
+    _BATCH_INVARIANT = bool(enabled)
+    try:
+        yield
+    finally:
+        _BATCH_INVARIANT = prev
+
+
+def invariant_applies(mlp, x: torch.Tensor) -> bool:
+    """Whether a call of ``mlp`` on ``x`` falls under batch_invariant(): the mode is on, grad mode is off, x is on CUDA,
+    and every batch norm of mlp (when it is a SharedMLP) is in eval mode with running statistics."""
+    if not _BATCH_INVARIANT or torch.is_grad_enabled() or not getattr(x, "is_cuda", False):
+        return False
+    bns = [m for m in mlp.modules() if isinstance(m, nn.modules.batchnorm._BatchNorm)] if isinstance(mlp, nn.Module) else []
+    return all(not bn.training and bn.running_mean is not None for bn in bns)
+
+
+def _invariant_call(fn, *args, **kwargs):
+    """fn(...) for a layer that batch_invariant() sends to the kernels; an argument they cannot take is a RuntimeError
+    (the mode never falls back to the torch layers)."""
+    try:
+        return fn(*args, **kwargs)
+    except (TypeError, ValueError) as e:
+        raise RuntimeError(f"batch_invariant(): the kernels cannot take this layer ({e}); leave the mode to run the "
+                           f"torch layers") from e
+
 
 
 def set_bn_momentum(model: nn.Module, bn_decay: float) -> None:

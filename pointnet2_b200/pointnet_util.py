@@ -212,6 +212,23 @@ def _sa_mlp_route(mlp, xyz, points, use_xyz, scope, name, bn, is_training, bn_de
     return mlp if layers.sa_mlp_applies(mlp, xyz, points, pooling) else None
 
 
+def _fp_mlp_route(mlp, xyz1, points1, points2, scope, bn, is_training, bn_decay):
+    """The SharedMLP behind ``mlp`` (a module, or a width list resolved through the scope registry) when a
+    feature-propagation level runs through layers.fp_mlp: inside layers.batch_invariant(), where layers.invariant_applies.
+    Else None."""
+    if not layers.is_batch_invariant() or torch.is_grad_enabled() or not xyz1.is_cuda:
+        return None
+    if not callable(mlp):
+        widths = [int(w) for w in mlp]
+        if not widths:
+            return None
+        cin = points2.shape[-1] + (0 if points1 is None else points1.shape[-1])
+        mlp = layers.scoped_mlp(scope, "conv", cin, widths, bn, xyz1.device, is_training, bn_decay)
+    if not isinstance(mlp, layers.SharedMLP):
+        return None  # another callable: its own SharedMLP calls route themselves
+    return mlp if layers.invariant_applies(mlp, xyz1) else None
+
+
 def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp=None, mlp2=None, group_all=False, is_training=None,
                        bn_decay=None, scope=None, bn=True, pooling='max', knn=False, use_xyz=True, use_nchw=False, fused=True,
                        lengths=None):
@@ -341,6 +358,8 @@ def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp=None, is_training=None,
         batch norm statistics of the mlp come from the real rows only); padding rows are never read and come out 0.
         With lengths, mlp must be a list of widths or a layers.SharedMLP (it takes the row mask); another callable
         raises ValueError.
+        Inside layers.batch_invariant() (eval-mode batch norms, grad mode off, CUDA) a SharedMLP tail runs with the
+        interpolation and the concat in one kernel (layers.fp_mlp), with or without lengths.
         Return: new_points (b,n1,mlp[-1]) (or (b,n1,c2+c1) when mlp is None)
     '''
     mask = None
@@ -351,6 +370,10 @@ def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp=None, is_training=None,
         b, n = xyz1.shape[0], xyz1.shape[1]
         lengths = device_lengths(lengths, b, n, xyz1.device, "pointnet_fp_module")
         mask = layers.row_mask(lengths, n)
+    tail = _fp_mlp_route(mlp, xyz1, points1, points2, scope, bn, is_training, bn_decay) if mlp is not None else None
+    if tail is not None:
+        # batch-invariant inference: interpolation, concat and every layer in the row kernel behind layers.fp_mlp
+        return layers._invariant_call(layers.fp_mlp, xyz1, xyz2, points1, points2, tail, lengths=lengths)
     no_grad = not points2.requires_grad and (points1 is None or not points1.requires_grad)
     same_dtype = points1 is None or points1.dtype == points2.dtype
     if fused and no_grad and same_dtype and points2.shape[2] > 0:

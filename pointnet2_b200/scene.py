@@ -206,7 +206,8 @@ def predict_scene(model, xyz: torch.Tensor, batch_size: int = 16, **block_kw):
 
     Returns (accum, count, label): accum (P, C) float32, the sum of each point's core logits in ascending row order;
     count (P,) int32, its number of core occurrences (always >= 1); label (P,) int64, the argmax of accum over the
-    classes, the lowest class on ties."""
+    classes, the lowest class on ties.  Inside layers.batch_invariant() (an eval-mode model of SharedMLP layers) the
+    results do not depend on batch_size: every block's logits have the same bits whatever blocks share its batch."""
     if isinstance(batch_size, bool) or not isinstance(batch_size, int) or batch_size < 1:
         raise ValueError(f"predict_scene expects a positive integer batch_size, got {batch_size!r}")
     blocks = scene_blocks(xyz, **block_kw)

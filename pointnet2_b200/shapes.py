@@ -248,7 +248,8 @@ def classify_votes(model, shapes: ShapeSet, shape_idx: torch.Tensor, num_votes: 
                    chunk: Optional[int] = None) -> torch.Tensor:
     """(B, num_class) float32 logits of ``model`` summed over the votes of vote_batch, in ascending v (evaluate.py:
     126-138), under torch.no_grad() and in whatever train / eval mode the caller set.  The model is called as
-    ``model(points, lengths)`` on ``chunk`` votes of all B shapes at a time (default: every vote in one call)."""
+    ``model(points, lengths)`` on ``chunk`` votes of all B shapes at a time (default: every vote in one call).  Inside
+    layers.batch_invariant() (an eval-mode model of SharedMLP layers) the logits do not depend on ``chunk``."""
     if isinstance(num_votes, bool) or not isinstance(num_votes, int) or num_votes < 1:
         raise ValueError(f"classify_votes expects a positive integer num_votes, got {num_votes!r}")
     if chunk is None:
