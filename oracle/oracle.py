@@ -223,6 +223,55 @@ def oracle_knn_point(k: int, xyz1, xyz2):
     return np.ascontiguousarray(out[:, :, :k]), np.ascontiguousarray(outi[:, :, :k])
 
 
+def _opt(a):
+    return None if a is None else _f(a)
+
+
+def oracle_mlp_affine_f32(layer):
+    """(scale, shift) float32 of one layer as the fused MLP kernels derive them (see oracle_mlp_rows_f32)."""
+    w = _f(layer["w"])
+    n = w.shape[0]
+    args = [_opt(layer.get(k)) for k in ("b", "gamma", "beta", "mean", "var")]
+    scale, shift = np.empty(n, _F), np.empty(n, _F)
+    lib().oracle_mlp_affine_f32(c_int(n), *[None if a is None else _p(a) for a in args],
+                                c_float(layer.get("eps", 0.0)), _p(scale), _p(shift))
+    return scale, shift
+
+
+def oracle_mlp_rows_f32(x, layers):
+    """The fused inference MLPs' float32 arithmetic (csrc/mlp_tile.cuh) on every row of x (rows, cin).  ``layers``: up
+    to 4 dicts with "w" (cout, cin) and optional "b", "gamma", "beta", "mean", "var" (cout,), "eps" (rounded to
+    float32, as the kernels take it) and "relu"; no "mean" means no batch norm, no "gamma" / "beta" a batch norm
+    without affine.  Returns (rows, cout of the last layer) float32."""
+    x = _f(x)
+    rows, cin = x.shape
+    nl = len(layers)
+    prev = cin
+    for L in layers:
+        if np.ndim(L["w"]) != 2 or np.shape(L["w"])[1] != prev:
+            raise ValueError(f"oracle_mlp_rows_f32: a layer's weight is {np.shape(L['w'])}, its input has {prev} channels")
+        prev = np.shape(L["w"])[0]
+    keep = []  # the contiguous copies must outlive the call
+
+    def arr(key):
+        ps = []
+        for L in layers:
+            a = _opt(L.get(key))
+            keep.append(a)
+            ps.append(None if a is None else a.ctypes.data)
+        return (c_void_p * nl)(*ps)
+    widths = (c_int * nl)(*[int(np.shape(L["w"])[0]) for L in layers])
+    w, b, g, be, mu, var = (arr(k) for k in ("w", "b", "gamma", "beta", "mean", "var"))
+    eps = (c_float * nl)(*[float(L.get("eps", 0.0)) for L in layers])
+    relu = (c_int * nl)(*[1 if L.get("relu") else 0 for L in layers])
+    out = np.empty((rows, widths[nl - 1]), _F)
+    rc = lib().oracle_mlp_rows_f32(ctypes.c_longlong(rows), c_int(cin), c_int(nl), widths, w, b, g, be, mu, var, eps,
+                                   relu, _p(x), _p(out))
+    if rc != 0:
+        raise ValueError("oracle_mlp_rows_f32: bad arguments")
+    return out
+
+
 # ------------------------------------------------------------------ reference CPU functions
 def refcpu_query_ball_point(radius: float, nsample: int, xyz1, xyz2):
     """tf_ops/grouping/test/query_ball_point.cpp:19 (no pts_cnt output). idx pre-zeroed."""

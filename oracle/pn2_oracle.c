@@ -431,3 +431,74 @@ void oracle_prob_sample(int b, int n, int m, const float *inp_p, const float *in
     oracle_prob_cumsum(b, n, inp_p, temp);
     oracle_prob_search(b, n, m, temp, inp_r, out);
 }
+
+/* ------------------------------------------------------------------------------------------
+ * The fused inference MLPs (pointnet2_b200/csrc/mlp_tile.cuh, mlp_tile_layers), float32 path:
+ * up to 4 layers of Linear [+ eval-mode batch norm] [+ ReLU] on every row.  Not a reference op:
+ * the restatement of the arithmetic the kernels document, so that their float32 outputs can be
+ * checked bit for bit.  Per output channel, at the start of each layer,
+ *     scale = 1 / sqrt(var + eps)  [* gamma when affine],  shift = fmaf(bias - mean, scale, beta)
+ * (every operation rounded on its own; without a batch norm scale = 1, shift = bias); then per
+ * row and channel
+ *     acc = +0;  acc = fmaf(a[k], w[j][k], acc) for ascending k;  y = fmaf(acc, scale, shift)
+ * and, with ReLU, y < 0 ? 0 : y (NaN and -0 pass).  A NULL bias is 0, a NULL gamma / beta means
+ * a batch norm without affine, a NULL mean no batch norm.
+ * ------------------------------------------------------------------------------------------ */
+void oracle_mlp_affine_f32(int n, const float *bias, const float *gamma, const float *beta, const float *mean,
+                           const float *var, float eps, float *scale, float *shift) {
+    for (int j = 0; j < n; ++j) {
+        float sc = 1.f, sh = bias ? bias[j] : 0.f;
+        if (mean) {
+            sc = 1.f / sqrtf(var[j] + eps);
+            if (gamma) sc = sc * gamma[j];
+            sh = fmaf(sh - mean[j], sc, beta ? beta[j] : 0.f);
+        }
+        scale[j] = sc;
+        shift[j] = sh;
+    }
+}
+
+/* x: (rows, cin); layer l maps widths[l-1] (cin for l = 0) to widths[l] channels, w[l] is
+ * (widths[l], in) row-major; out: (rows, widths[nlayers-1]).  Returns 0, or -1 for bad arguments. */
+int oracle_mlp_rows_f32(long long rows, int cin, int nlayers, const int *widths, const float *const *w,
+                        const float *const *bias, const float *const *gamma, const float *const *beta,
+                        const float *const *mean, const float *const *var, const float *eps, const int *relu,
+                        const float *x, float *out) {
+    if (rows < 0 || cin < 1 || nlayers < 1 || nlayers > 4) return -1;
+    int widest = cin;
+    for (int l = 0; l < nlayers; ++l) {
+        if (widths[l] < 1) return -1;
+        if (widths[l] > widest) widest = widths[l];
+    }
+    float *a = (float *)malloc(sizeof(float) * (size_t)widest);
+    float *y = (float *)malloc(sizeof(float) * (size_t)widest);
+    float *scale = (float *)malloc(sizeof(float) * (size_t)widest * nlayers);
+    float *shift = (float *)malloc(sizeof(float) * (size_t)widest * nlayers);
+    for (int l = 0; l < nlayers; ++l)
+        oracle_mlp_affine_f32(widths[l], bias[l], gamma ? gamma[l] : NULL, beta ? beta[l] : NULL,
+                              mean ? mean[l] : NULL, var ? var[l] : NULL, eps ? eps[l] : 0.f,
+                              scale + (size_t)l * widest, shift + (size_t)l * widest);
+    for (long long r = 0; r < rows; ++r) {
+        int c = cin;
+        memcpy(a, x + (size_t)r * cin, sizeof(float) * (size_t)cin);
+        for (int l = 0; l < nlayers; ++l) {
+            const float *sc = scale + (size_t)l * widest, *sh = shift + (size_t)l * widest;
+            for (int j = 0; j < widths[l]; ++j) {
+                const float *wj = w[l] + (size_t)j * c;
+                float acc = 0.f;
+                for (int k = 0; k < c; ++k) acc = fmaf(a[k], wj[k], acc);
+                float v = fmaf(acc, sc[j], sh[j]);
+                if (relu[l]) v = v < 0.f ? 0.f : v;
+                y[j] = v;
+            }
+            c = widths[l];
+            memcpy(a, y, sizeof(float) * (size_t)c);
+        }
+        memcpy(out + (size_t)r * c, a, sizeof(float) * (size_t)c);
+    }
+    free(a);
+    free(y);
+    free(scale);
+    free(shift);
+    return 0;
+}
