@@ -315,6 +315,32 @@ int pn2_masked_bn_relu_backward_typed(int dtype, int rows, int c, const void* dy
                                       const float* save_invstd, void* dx, float* dgamma, float* dbeta, void* workspace,
                                       size_t workspace_bytes, void* stream);
 
+/* The same batch norm + ReLU followed by a max over each cloud's real rows (tf_util.max_pool2d over [num_point, 1],
+ * models/pointnet_cls_basic.py:52), without writing the (b, n, c) ReLU output.  x (b, n, c) in `dtype`, keep (b*n) bytes as
+ * above (row j of cloud i is real when keep[i*n + j] != 0).  b*n < 2^31.
+ * Forward: the statistics, save_mean / save_invstd and the running statistics come from the kernels of
+ * pn2_masked_bn_relu_forward_typed on the b*n rows, so they are bit-identical to it.  Then, per (cloud i, column k),
+ * out[i, k] = max over the real rows j of y[i, j, k] (y computed and rounded to `dtype` exactly as that entry writes it,
+ * values compared as order-preserving keys, so NaN wins) and argmax[i, k] (int32) = the FIRST such row j: where TF's
+ * MaxPoolGrad sends the gradient.  A cloud without a real row gets out 0 and argmax -1.
+ * Backward (out, argmax and the saved statistics from the forward): g[i, k] = out[i, k] > 0 ? dout[i, k] : 0 at row
+ * argmax[i, k] of cloud i and 0 on every other row; dbeta = sum_i g, dgamma = sum_i g * xhat(argmax row), both in
+ * ascending i; dx = keep ? gamma * invstd * (g - dbeta / cnt - xhat * dgamma / cnt) : 0 over all b*n rows, cnt the real
+ * rows.  No float atomics: bit-identical from run to run.
+ * Both take a device workspace of pn2_masked_bn_relu_max_workspace_bytes(b, n, c) bytes (16-byte aligned).  b == 0
+ * launches nothing; an unknown dtype, a NULL required pointer, b < 0, n <= 0, c <= 0 or a short workspace return
+ * cudaErrorInvalidValue without a launch. */
+size_t pn2_masked_bn_relu_max_workspace_bytes(int b, int n, int c);
+int pn2_masked_bn_relu_max_forward_typed(int dtype, int b, int n, int c, const void* x, const unsigned char* keep,
+                                         const float* gamma, const float* beta, float eps, float momentum,
+                                         const long long* num_batches_tracked, float* running_mean, float* running_var,
+                                         void* out, int* argmax, float* save_mean, float* save_invstd, void* workspace,
+                                         size_t workspace_bytes, void* stream);
+int pn2_masked_bn_relu_max_backward_typed(int dtype, int b, int n, int c, const void* dout, const void* x, const void* out,
+                                          const int* argmax, const unsigned char* keep, const float* gamma,
+                                          const float* save_mean, const float* save_invstd, void* dx, float* dgamma,
+                                          float* dbeta, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- learned layers: the inference tail of a set-abstraction level (utils/pointnet_util.py:45-54 + :115-124, MSG
  * :179-191) in one launch -----------------------------------------------------------------------------------------------
  * For every group (i, j) of b x m:   row k = concat(xyz[i, idx[i,j,k]] - new_xyz[i,j], points[i, idx[i,j,k]]) in the order
@@ -341,6 +367,25 @@ int pn2_sa_mlp_max_typed(int dtype, int b, int n, int c, int m, int nsample, con
                          const float* const* weight, const float* const* bias, const float* const* bn_weight,
                          const float* const* bn_bias, const float* const* bn_mean, const float* const* bn_var,
                          const float* bn_eps, const int* relu, void* out, long long out_row_stride, void* stream);
+
+/* pn2_sa_mlp_max_all_typed: the one group of every cloud (idx == NULL, nsample == n, m == 1), with per-cloud row counts.
+ * Arguments and arithmetic as pn2_sa_mlp_max_typed; new_xyz (b,1,3) or NULL; lengths (b,) device int32 or NULL: rows
+ * j >= lengths[i], clamped to [1, n], are padding and never read (they may hold NaN).  xyz may be NULL when the rows take
+ * no coordinates (use_xyz == 0 with points).  out row i at out + i * out_row_stride.
+ * When a cloud has more row tiles than the machine needs, they are dealt out to several CTAs, which atomicMax their
+ * partial key maxima into the workspace (zeroed on the stream first); a second launch turns the keys into values.  The
+ * split count is a function of b, n, the widths and the SM count, never of the values or the lengths, and the maximum of
+ * exact keys does not depend on it: the output is bit-identical to pn2_sa_mlp_max_typed's one-CTA walk and to each
+ * cloud computed alone.  Workspace: pn2_sa_mlp_max_all_workspace_bytes(b, widths[nlayers-1]) bytes, 16-byte aligned,
+ * required whatever the split.  Nothing is read back to the host: the call can be captured in a CUDA graph.  b == 0
+ * launches nothing; invalid arguments return cudaErrorInvalidValue without a launch. */
+size_t pn2_sa_mlp_max_all_workspace_bytes(int b, int c_out);
+int pn2_sa_mlp_max_all_typed(int dtype, int b, int n, int c, const float* xyz, const float* new_xyz, const void* points,
+                             const int* lengths, int xyz_first, int use_xyz, int nlayers, const int* widths,
+                             const float* const* weight, const float* const* bias, const float* const* bn_weight,
+                             const float* const* bn_bias, const float* const* bn_mean, const float* const* bn_var,
+                             const float* bn_eps, const int* relu, void* out, long long out_row_stride, void* workspace,
+                             size_t workspace_bytes, void* stream);
 
 /* ---- learned layers, row by row: feature-propagation tails and heads at inference (utils/pointnet_util.py:199-229)
  * ------------------------------------------------------------------------------------------------------------------------

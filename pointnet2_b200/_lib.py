@@ -73,9 +73,19 @@ _SIGNATURES = {
     "pn2_masked_bn_relu_forward_typed": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, c_float, c_float, _P, _P, _P, _P, _P, _P, _P,
                                                  c_size_t, _P]),
     "pn2_masked_bn_relu_backward_typed": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    # ... followed by a max over each cloud's real rows of a padded (b, n, c) tensor
+    "pn2_masked_bn_relu_max_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "pn2_masked_bn_relu_max_forward_typed": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_float, c_float, _P, _P, _P,
+                                                     _P, _P, _P, _P, _P, c_size_t, _P]),
+    "pn2_masked_bn_relu_max_backward_typed": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                                      _P, c_size_t, _P]),
     # inference tail of a set-abstraction level: gather + shared MLP (eval-mode batch norm) + max-pool
     "pn2_sa_mlp_max_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P,
                                      _P, _P, _P, _P, _P, _P, _P, c_longlong, _P]),
+    # ... on the one group of every cloud, with per-cloud lengths, split over CTAs
+    "pn2_sa_mlp_max_all_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "pn2_sa_mlp_max_all_typed": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, c_int, c_int, c_int, _P, _P, _P, _P, _P,
+                                         _P, _P, _P, _P, _P, c_longlong, _P, c_size_t, _P]),
     # learned layers row by row: feature-propagation tails (3-NN interpolation + concat in front) and heads
     "pn2_fp_mlp_workspace_bytes": (c_size_t, [c_int, c_int]),
     "pn2_fp_mlp_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, c_int, _P, _P, _P, _P, _P, _P,

@@ -298,7 +298,221 @@ __global__ void __launch_bounds__(kMbnThreads) mbn_norm_relu_kernel(const T* __r
     }
 }
 
+// One CTA per (cloud, column tile) of a (b, n, c) x: y as mbn_norm_relu_kernel computes and rounds it, and per column
+// its maximum over the cloud's real rows with the FIRST row that reaches it (where TF's MaxPoolGrad sends the gradient).
+// Values are compared as max_key keys, so NaN wins.  Each thread walks rows threadIdx.y, + ty, ... and keeps the first
+// of equal keys; the ty threads of a column are merged in a fixed tree that prefers the lower row on equal keys.
+// A cloud without a real row gets out 0 and argmax -1.  Only out (b, c) and argmax (b, c) are written.
+template <typename T, int V, bool VEC>
+__global__ void __launch_bounds__(kMbnThreads) mbn_norm_relu_max_kernel(const T* __restrict__ x,
+                                                                        const unsigned char* __restrict__ keep, int n, int c,
+                                                                        const float* __restrict__ mean,
+                                                                        const float* __restrict__ invstd,
+                                                                        const float* __restrict__ gamma,
+                                                                        const float* __restrict__ beta, T* __restrict__ out,
+                                                                        int* __restrict__ argmax) {
+    __shared__ unsigned s_key[kMbnThreads * V];
+    __shared__ int s_row[kMbnThreads * V];
+    const int tx = blockDim.x, ty = blockDim.y, tid = threadIdx.y * tx + threadIdx.x;
+    const int col = (blockIdx.y * tx + threadIdx.x) * V;
+    const bool active = col < c;
+    const long long cloud = blockIdx.x;
+    float mu[V], sc[V], sh[V];
+    unsigned key[V];
+    int arg[V];
+#pragma unroll
+    for (int i = 0; i < V; ++i) {
+        mu[i] = active ? __ldg(mean + col + i) : 0.f;
+        const float is = active ? __ldg(invstd + col + i) : 0.f;
+        sc[i] = gamma && active ? __fmul_rn(is, __ldg(gamma + col + i)) : is;
+        sh[i] = beta && active ? __ldg(beta + col + i) : 0.f;
+        key[i] = 0u;
+        arg[i] = -1;
+    }
+    if (active) {
+        const T* xc = x + (size_t)cloud * n * c + col;
+        const unsigned char* kc = keep + (size_t)cloud * n;
+        for (int jb = threadIdx.y; jb < n; jb += ty * kMbnUnroll) {
+            bool kf[kMbnUnroll];
+            float v[kMbnUnroll][V];
+#pragma unroll
+            for (int u = 0; u < kMbnUnroll; ++u) {
+                const int j = jb + u * ty;
+                kf[u] = j < n && __ldg(kc + j) != 0;
+                if (kf[u]) {
+                    load_cols<T, V, VEC>(xc + (size_t)j * c, v[u]);
+                } else {
+#pragma unroll
+                    for (int i = 0; i < V; ++i) v[u][i] = 0.f;
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < kMbnUnroll; ++u) {
+#pragma unroll
+                for (int i = 0; i < V; ++i) {
+                    const float t = __fmaf_rn(__fsub_rn(v[u][i], mu[i]), sc[i], sh[i]);
+                    // the value y holds in T, compared as a key: the maximum and its first row are those of the
+                    // rounded tensor masked_batch_norm_relu would write
+                    const unsigned k = max_key(to_f32(from_f32<T>(t < 0.f ? 0.f : t)));
+                    if (kf[u] && k > key[i]) {
+                        key[i] = k;
+                        arg[i] = jb + u * ty;
+                    }
+                }
+            }
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < V; ++i) {
+        s_key[tid * V + i] = key[i];
+        s_row[tid * V + i] = arg[i];
+    }
+    __syncthreads();
+    for (int s = ty >> 1; s > 0; s >>= 1) {
+        if ((int)threadIdx.y < s) {
+            const int o = tid + s * tx;
+#pragma unroll
+            for (int i = 0; i < V; ++i) {
+                const unsigned kb = s_key[o * V + i];
+                const int rb = s_row[o * V + i];
+                if (kb > key[i] || (kb == key[i] && kb != 0u && rb < arg[i])) {
+                    key[i] = kb;
+                    arg[i] = rb;
+                }
+                s_key[tid * V + i] = key[i];
+                s_row[tid * V + i] = arg[i];
+            }
+        }
+        __syncthreads();
+    }
+    if (threadIdx.y == 0 && active) {
+#pragma unroll
+        for (int i = 0; i < V; ++i) {
+            out[(size_t)cloud * c + col + i] = from_f32<T>(key[i] ? key_value(key[i]) : 0.f);
+            argmax[(size_t)cloud * c + col + i] = key[i] ? arg[i] : -1;
+        }
+    }
+}
+
 // ---- backward --------------------------------------------------------------------------------------------------------
+
+// Backward of the max-pooled form, step 1.  One CTA per 32 columns: the CTA counts the real rows (an integer sum), then
+// for each column g[i] = out[i] > 0 ? dout[i] : 0 (the gradient of the ReLU at the argmax row; the other rows get none),
+// dbeta = sum_i g[i] and dgamma = sum_i g[i] * xhat(argmax row), both over the clouds i in ascending order: the warps
+// take 32 clouds at a time and warp 0 adds their terms in order.  Writes dgamma / dbeta (either may be NULL), gsel (b, c)
+// and the dx coefficients coef[3][c] of mbn_bwd_dx_kernel.
+template <typename T>
+__global__ void __launch_bounds__(32 * kMbnMergeWarps) mbn_max_bwd_finalize_kernel(
+    const T* __restrict__ dout, const T* __restrict__ x, const T* __restrict__ out, const int* __restrict__ argmax,
+    const unsigned char* __restrict__ keep, int b, int n, int c, const float* __restrict__ gamma,
+    const float* __restrict__ mean, const float* __restrict__ invstd, float* __restrict__ dgamma, float* __restrict__ dbeta,
+    float* __restrict__ gsel, float* __restrict__ coef) {
+    __shared__ float s_g[kMbnMergeWarps][32], s_xh[kMbnMergeWarps][32];
+    __shared__ int s_cnt;
+    const int lane = threadIdx.x, w = threadIdx.y, tid = w * 32 + lane;
+    const int col = blockIdx.x * 32 + lane;
+    const bool active = col < c;
+    if (tid == 0) s_cnt = 0;
+    __syncthreads();
+    const long long rows = (long long)b * n;
+    int cnt = 0;
+    for (long long r = tid; r < rows; r += 32 * kMbnMergeWarps) cnt += __ldg(keep + r) != 0;
+    cnt += __shfl_xor_sync(kFullMask, cnt, 16);
+    cnt += __shfl_xor_sync(kFullMask, cnt, 8);
+    cnt += __shfl_xor_sync(kFullMask, cnt, 4);
+    cnt += __shfl_xor_sync(kFullMask, cnt, 2);
+    cnt += __shfl_xor_sync(kFullMask, cnt, 1);
+    if (lane == 0) atomicAdd(&s_cnt, cnt);  // an integer sum: exact in any order
+    const float mu = active ? __ldg(mean + col) : 0.f, is = active ? __ldg(invstd + col) : 0.f;
+    float sg = 0.f, sgx = 0.f;
+    for (int i0 = 0; i0 < b; i0 += kMbnMergeWarps) {
+        const int i = i0 + w;
+        float g = 0.f, xh = 0.f;
+        if (active && i < b) {
+            const size_t o = (size_t)i * c + col;
+            const int r = __ldg(argmax + o);
+            if (r >= 0 && to_f32(out[o]) > 0.f) {
+                g = to_f32(dout[o]);
+                xh = __fmul_rn(__fsub_rn(to_f32(x[((size_t)i * n + r) * c + col]), mu), is);
+            }
+            gsel[o] = g;
+        }
+        s_g[w][lane] = g;
+        s_xh[w][lane] = xh;
+        __syncthreads();
+        if (w == 0) {
+            const int m = min(kMbnMergeWarps, b - i0);
+            for (int k = 0; k < m; ++k) {
+                sg = __fadd_rn(sg, s_g[k][lane]);
+                sgx = __fmaf_rn(s_g[k][lane], s_xh[k][lane], sgx);
+            }
+        }
+        __syncthreads();
+    }
+    if (w != 0 || !active) return;
+    if (dbeta) dbeta[col] = sg;
+    if (dgamma) dgamma[col] = sgx;
+    const float fc = (float)s_cnt;
+    coef[col] = gamma ? __fmul_rn(__ldg(gamma + col), is) : is;
+    coef[c + col] = __fdiv_rn(sg, fc);
+    coef[2 * c + col] = __fdiv_rn(sgx, fc);
+}
+
+// Step 2: dx = keep ? gamma * invstd * (g - sum g / cnt - xhat * sum g * xhat / cnt) : 0 with g = gsel[i] at the argmax
+// row of cloud i and 0 elsewhere (the arithmetic of mbn_bwd_dx_kernel)
+template <typename T, int V, bool VEC>
+__global__ void __launch_bounds__(kMbnThreads) mbn_max_bwd_dx_kernel(const T* __restrict__ x, const unsigned char* __restrict__ keep,
+                                                                     int rows, int n, int c, const int* __restrict__ argmax,
+                                                                     const float* __restrict__ gsel,
+                                                                     const float* __restrict__ mean,
+                                                                     const float* __restrict__ invstd,
+                                                                     const float* __restrict__ coef, T* __restrict__ dx) {
+    const int tx = blockDim.x, ty = blockDim.y;
+    const int col = (blockIdx.y * tx + threadIdx.x) * V;
+    if (col >= c) return;  // no barrier in this kernel
+    float mu[V], is[V], a[V], mg[V], mgx[V];
+#pragma unroll
+    for (int i = 0; i < V; ++i) {
+        mu[i] = __ldg(mean + col + i);
+        is[i] = __ldg(invstd + col + i);
+        a[i] = __ldg(coef + col + i);
+        mg[i] = __ldg(coef + c + col + i);
+        mgx[i] = __ldg(coef + 2 * c + col + i);
+    }
+    const long long step = (long long)gridDim.x * ty * kMbnUnroll;
+    for (long long rb = (long long)blockIdx.x * ty * kMbnUnroll + threadIdx.y; rb < rows; rb += step) {
+        bool kf[kMbnUnroll];
+        float xv[kMbnUnroll][V];
+#pragma unroll
+        for (int u = 0; u < kMbnUnroll; ++u) {
+            const long long r = rb + (long long)u * ty;
+            kf[u] = r < rows && __ldg(keep + r) != 0;
+            if (kf[u]) {
+                load_cols<T, V, VEC>(x + (size_t)r * c + col, xv[u]);
+            } else {
+#pragma unroll
+                for (int i = 0; i < V; ++i) xv[u][i] = 0.f;
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < kMbnUnroll; ++u) {
+            const long long r = rb + (long long)u * ty;
+            if (r >= rows) break;
+            const long long cloud = r / n;
+            const int j = (int)(r - cloud * n);
+            float o[V];
+#pragma unroll
+            for (int i = 0; i < V; ++i) {
+                const size_t bc = (size_t)cloud * c + col + i;
+                const float g = __ldg(argmax + bc) == j ? __ldg(gsel + bc) : 0.f;
+                const float xh = __fmul_rn(__fsub_rn(xv[u][i], mu[i]), is[i]);
+                const float t = __fmaf_rn(-xh, mgx[i], __fsub_rn(g, mg[i]));
+                o[i] = kf[u] ? __fmul_rn(a[i], t) : 0.f;
+            }
+            store_cols<T, V, VEC>(dx + (size_t)r * c + col, o);
+        }
+    }
+}
 
 // Per CTA (same chunks as the forward): count and column sums of g = dy * [y > 0] and g * xhat over the real rows, each
 // thread adding its rows in ascending order, then a fixed tree over the ty threads of each column.
@@ -555,6 +769,63 @@ bool mbn_args_ok(int rows, int c, const MbnGeom& g) {
     return rows >= 0 && c > 0 && g.col_tiles <= 65535;
 }
 
+// ---- the max-pooled form: statistics as the plain form, then one pass that keeps each cloud's column maxima ----------
+
+// Workspace of the backward: coef[3][c], then gsel (b, c)
+struct MaxBwdLayout {
+    size_t coef, gsel, total;
+};
+MaxBwdLayout max_bwd_layout(int b, int c) {
+    MaxBwdLayout L;
+    L.coef = 0;
+    L.gsel = align256(sizeof(float) * 3 * (size_t)c);
+    L.total = L.gsel + align256(sizeof(float) * (size_t)b * c);
+    return L;
+}
+
+template <typename T, int V, bool VEC>
+int max_forward_launch(const MbnGeom& g, int b, int n, int c, const T* x, const unsigned char* keep, const float* gamma,
+                       const float* beta, float eps, float momentum, const long long* nbt, float* running_mean,
+                       float* running_var, T* out, int* argmax, float* save_mean, float* save_invstd, char* ws,
+                       const MbnLayout& L, cudaStream_t st) {
+    float* pa = reinterpret_cast<float*>(ws + L.pa);
+    float* pb = reinterpret_cast<float*>(ws + L.pb);
+    int* pc = reinterpret_cast<int*>(ws + L.cnt);
+    const dim3 block(g.tx, g.ty);
+    const int rows = b * n;
+    mbn_stats_kernel<T, V, VEC><<<dim3((unsigned)g.chunks, g.col_tiles), block, 0, st>>>(x, keep, rows, c, pa, pb, pc);
+    int rc = finish_launch();
+    if (rc) return rc;
+    mbn_finalize_kernel<<<ceil_div_u(c, 32), dim3(32, kMbnMergeWarps), 0, st>>>(pa, pb, pc, g.chunks, c, eps, momentum, nbt,
+                                                                                 running_mean, running_var, save_mean, save_invstd);
+    rc = finish_launch();
+    if (rc) return rc;
+    mbn_norm_relu_max_kernel<T, V, VEC><<<dim3((unsigned)b, g.col_tiles), block, 0, st>>>(
+        x, keep, n, c, save_mean, save_invstd, gamma, beta, out, argmax);
+    return finish_launch();
+}
+
+template <typename T, int V, bool VEC>
+int max_backward_launch(const MbnGeom& g, int b, int n, int c, const T* dout, const T* x, const T* out, const int* argmax,
+                        const unsigned char* keep, const float* gamma, const float* save_mean, const float* save_invstd,
+                        T* dx, float* dgamma, float* dbeta, char* ws, const MaxBwdLayout& L, cudaStream_t st) {
+    float* coef = reinterpret_cast<float*>(ws + L.coef);
+    float* gsel = reinterpret_cast<float*>(ws + L.gsel);
+    const int rows = b * n;
+    mbn_max_bwd_finalize_kernel<T><<<ceil_div_u(c, 32), dim3(32, kMbnMergeWarps), 0, st>>>(
+        dout, x, out, argmax, keep, b, n, c, gamma, save_mean, save_invstd, dgamma, dbeta, gsel, coef);
+    int rc = finish_launch();
+    if (rc) return rc;
+    mbn_max_bwd_dx_kernel<T, V, VEC><<<dim3(elementwise_row_blocks(g, rows), g.col_tiles), dim3(g.tx, g.ty), 0, st>>>(
+        x, keep, rows, n, c, argmax, gsel, save_mean, save_invstd, coef, dx);
+    return finish_launch();
+}
+
+bool max_args_ok(int b, int n, int c) {
+    return b >= 0 && n > 0 && c > 0 && (long long)b * n <= 0x7fffffffLL && b <= 0x7fffffff &&
+           mbn_geom(b * n, c).col_tiles <= 65535;
+}
+
 template <typename T>
 int forward_typed(int rows, int c, const void* x, const unsigned char* keep, const float* gamma, const float* beta, float eps,
                   float momentum, const long long* nbt, float* running_mean, float* running_var, void* y, float* save_mean,
@@ -638,6 +909,72 @@ int pn2_masked_bn_relu_backward_typed(int dtype, int rows, int c, const void* dy
         return backward_typed<__nv_bfloat16>(rows, c, dy, x, y, keep, gamma, save_mean, save_invstd, dx, dgamma, dbeta, ws, g, L,
                                              st);
     return backward_typed<__half>(rows, c, dy, x, y, keep, gamma, save_mean, save_invstd, dx, dgamma, dbeta, ws, g, L, st);
+}
+
+size_t pn2_masked_bn_relu_max_workspace_bytes(int b, int n, int c) {
+    using namespace pn2;
+    if (b <= 0 || n <= 0 || c <= 0 || (long long)b * n > 0x7fffffffLL) return 0;
+    const size_t fwd = mbn_layout(mbn_geom(b * n, c), c).total, bwd = max_bwd_layout(b, c).total;
+    return fwd > bwd ? fwd : bwd;
+}
+
+int pn2_masked_bn_relu_max_forward_typed(int dtype, int b, int n, int c, const void* x, const unsigned char* keep,
+                                         const float* gamma, const float* beta, float eps, float momentum,
+                                         const long long* num_batches_tracked, float* running_mean, float* running_var,
+                                         void* out, int* argmax, float* save_mean, float* save_invstd, void* workspace,
+                                         size_t workspace_bytes, void* stream) {
+    using namespace pn2;
+    if (!valid_dtype(dtype) || !max_args_ok(b, n, c)) return (int)cudaErrorInvalidValue;
+    if (!x || !keep || !out || !argmax || !save_mean || !save_invstd) return (int)cudaErrorInvalidValue;
+    if (!running_mean != !running_var) return (int)cudaErrorInvalidValue;
+    if (running_mean && momentum < 0.f && !num_batches_tracked) return (int)cudaErrorInvalidValue;
+    if (b == 0) return 0;
+    if (!workspace || workspace_bytes < pn2_masked_bn_relu_max_workspace_bytes(b, n, c) || !aligned_to(workspace, 16))
+        return (int)cudaErrorInvalidValue;
+    const MbnGeom g = mbn_geom(b * n, c);
+    const MbnLayout L = mbn_layout(g, c);
+    char* ws = static_cast<char*>(workspace);
+    const cudaStream_t st = as_stream(stream);
+    auto run = [&](auto t) {
+        using T = decltype(t);
+        // the statistics read x in the plain form's geometry; the vector loads need x aligned to 4 elements
+        return dispatch_vec<T>(g, aligned_to(x, 4 * sizeof(T)), [&](auto v, auto vec) {
+            return max_forward_launch<T, decltype(v)::value, decltype(vec)::value>(
+                g, b, n, c, static_cast<const T*>(x), keep, gamma, beta, eps, momentum, num_batches_tracked, running_mean,
+                running_var, static_cast<T*>(out), argmax, save_mean, save_invstd, ws, L, st);
+        });
+    };
+    if (dtype == PN2_F32) return run(float());
+    if (dtype == PN2_BF16) return run(__nv_bfloat16());
+    return run(__half());
+}
+
+int pn2_masked_bn_relu_max_backward_typed(int dtype, int b, int n, int c, const void* dout, const void* x, const void* out,
+                                          const int* argmax, const unsigned char* keep, const float* gamma,
+                                          const float* save_mean, const float* save_invstd, void* dx, float* dgamma,
+                                          float* dbeta, void* workspace, size_t workspace_bytes, void* stream) {
+    using namespace pn2;
+    if (!valid_dtype(dtype) || !max_args_ok(b, n, c)) return (int)cudaErrorInvalidValue;
+    if (!dout || !x || !out || !argmax || !keep || !save_mean || !save_invstd || !dx) return (int)cudaErrorInvalidValue;
+    if (b == 0) return 0;
+    if (!workspace || workspace_bytes < pn2_masked_bn_relu_max_workspace_bytes(b, n, c) || !aligned_to(workspace, 16))
+        return (int)cudaErrorInvalidValue;
+    const MbnGeom g = mbn_geom(b * n, c);
+    const MaxBwdLayout L = max_bwd_layout(b, c);
+    char* ws = static_cast<char*>(workspace);
+    const cudaStream_t st = as_stream(stream);
+    auto run = [&](auto t) {
+        using T = decltype(t);
+        const bool aligned = aligned_to(x, 4 * sizeof(T)) && aligned_to(dx, 4 * sizeof(T));
+        return dispatch_vec<T>(g, aligned, [&](auto v, auto vec) {
+            return max_backward_launch<T, decltype(v)::value, decltype(vec)::value>(
+                g, b, n, c, static_cast<const T*>(dout), static_cast<const T*>(x), static_cast<const T*>(out), argmax, keep,
+                gamma, save_mean, save_invstd, static_cast<T*>(dx), dgamma, dbeta, ws, L, st);
+        });
+    };
+    if (dtype == PN2_F32) return run(float());
+    if (dtype == PN2_BF16) return run(__nv_bfloat16());
+    return run(__half());
 }
 
 }  // extern "C"

@@ -515,6 +515,18 @@ template <> __device__ __forceinline__ float from_f32<float>(float x) { return x
 template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
 template <> __device__ __forceinline__ __half from_f32<__half>(float x) { return __float2half_rn(x); }
 
+// ---- maxima that keep NaN (torch's max does; fmaxf would drop it) ------------------------------
+// float -> key with  a < b  <=>  key(a) < key(b)  as unsigned, every NaN the largest key; 0 is below every key.  The
+// maximum of exact keys is exact, so it does not depend on the order or the grouping of the comparisons.
+__device__ __forceinline__ unsigned max_key(float v) {
+    if (v != v) return 0xffffffffu;
+    const unsigned u = __float_as_uint(v);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key_value(unsigned k) {
+    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
 // Four consecutive elements as one vector: float4 (16 bytes) for float, uint2 (8 bytes) for 2-byte types.
 template <typename T> struct Pack4 { using type = uint2; };
 template <> struct Pack4<float> { using type = float4; };

@@ -8,7 +8,12 @@
 // The tile, the weight slabs and the per-layer loop are mlp_tile.cuh's (shared with fp_mlp.cu).
 // Every output depends on its own group only and every sum has a fixed order, so results are bit-identical from run to
 // run and whatever else is in the batch.  The maximum keeps NaN (torch's max does; fmaxf would drop it): values are
-// compared as order-preserving integer keys in which NaN is the largest.
+// compared as order-preserving integer keys in which NaN is the largest (max_key, pn2_common.cuh).
+//
+// The whole-cloud form (pn2_sa_mlp_max_all_typed: no idx, optional per-cloud lengths) may deal the TM-row pieces of a
+// cloud out to several CTAs.  Each CTA then atomicMax'es its partial key maxima into a (groups, C_out) key workspace and
+// a second launch turns the keys into values.  The maximum of exact keys does not depend on which CTA saw which row,
+// so the output has the bits of the one-CTA walk.
 #include <type_traits>
 
 #include "mlp_tile.cuh"
@@ -18,10 +23,13 @@ namespace pn2 {
 constexpr int kMlpMaxIn = kMlpMaxWidth + 3;
 
 struct SaMlpParams {
-    const float* xyz;
+    const float* xyz;      // nullptr only when the rows take no xyz (xyz_lo < 0)
     const float* new_xyz;  // nullptr: zeros
     const void* points;    // nullptr: no features
     const int* idx;        // nullptr: row k of every group is point k (nsample == n)
+    const int* lengths;    // nullptr: every row of a group is real; else (idx == nullptr, m == 1) rows k >= lengths[g],
+                           // clamped to [1, nsample], are padding and never read
+    unsigned* keys;        // nullptr: the CTA writes out; else its partial maxima go into keys (groups, C_out)
     void* out;
     long long out_stride;  // elements between consecutive groups of out
     long long groups;      // b * m
@@ -29,19 +37,15 @@ struct SaMlpParams {
     int xyz_lo, feat_lo;   // first column of the centred xyz (-1: none) and of the features in a row
     int nlayers;
     int groups_per_tile;   // whole groups in a tile (nsample <= TM), or 1 with the group walked in pieces of TM rows
+    int splits;            // CTAs per tile: CTA s walks pieces s, s + splits, ... (1 unless keys is set)
     int stride0, stride1;  // row strides of the two activation buffers, in elements
     int max_cout;
     MlpLayer layer[kMlpMaxLayers];
 };
 
-// float -> key with  a < b  <=>  key(a) < key(b)  as unsigned, every NaN the largest key; 0 is below every key
-__device__ __forceinline__ unsigned max_key(float v) {
-    if (v != v) return 0xffffffffu;
-    const unsigned u = __float_as_uint(v);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key_value(unsigned k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+// Real rows of group g: nsample, or its length clamped to [1, nsample] (as layers.row_mask clamps it)
+__device__ __forceinline__ int group_rows(const SaMlpParams& p, long long g) {
+    return p.lengths ? min(max(__ldg(p.lengths + g), 1), p.nsample) : p.nsample;
 }
 
 template <typename T, int TM>
@@ -60,14 +64,17 @@ sa_mlp_max_kernel(const __grid_constant__ SaMlpParams p) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int K = p.nsample;
     const int cout_last = p.layer[p.nlayers - 1].cout;
-    const long long group0 = (long long)blockIdx.x * p.groups_per_tile;
-    const int pieces = K > TM ? (K + TM - 1) / TM : 1;
+    const long long tile = blockIdx.x / p.splits;
+    const int split = (int)(blockIdx.x - tile * p.splits);
+    const long long group0 = tile * p.groups_per_tile;
+    // pieces mode holds one group per tile: its real rows set the piece count
+    const int pieces = K > TM ? (group_rows(p, group0) + TM - 1) / TM : 1;
     const int cin0 = p.layer[0].cin;
     const int cin0_pad = slab_pad(cin0);
 
     for (int e = tid; e < p.groups_per_tile * cout_last; e += kMlpThreads) s_max[e] = 0u;
 
-    for (int piece = 0; piece < pieces; ++piece) {
+    for (int piece = split; piece < pieces; piece += p.splits) {
         // ---- gather: one warp per row, lanes over the row's channels; unused rows and the padding columns are 0 ----
         for (int r = warp; r < TM; r += kMlpThreads / 32) {
             int slot, k;
@@ -79,7 +86,7 @@ sa_mlp_max_kernel(const __grid_constant__ SaMlpParams p) {
                 k = r - slot * K;
             }
             const long long g = group0 + slot;
-            const bool live = k < K && slot < p.groups_per_tile && g < p.groups;
+            const bool live = k < K && slot < p.groups_per_tile && g < p.groups && (!p.lengths || k < group_rows(p, g));
             if (lane == 0) s_slot[r] = live ? slot : -1;
             T* row = act0 + (size_t)r * p.stride0;
             if (!live) {
@@ -141,12 +148,28 @@ sa_mlp_max_kernel(const __grid_constant__ SaMlpParams p) {
         });
     }
 
-    // ---- the groups' maxima, rounded once to the output type ----
+    // ---- the groups' maxima, rounded once to the output type (or this CTA's share of them, as keys) ----
     T* out = static_cast<T*>(p.out);
     for (int e = tid; e < p.groups_per_tile * cout_last; e += kMlpThreads) {
         const int slot = e / cout_last, col = e - slot * cout_last;
         const long long g = group0 + slot;
-        if (g < p.groups) out[g * p.out_stride + col] = from_f32<T>(key_value(s_max[e]));
+        if (g >= p.groups) continue;
+        if (p.keys) {
+            if (s_max[e]) atomicMax(p.keys + g * cout_last + col, s_max[e]);  // 0: this CTA saw no row
+        } else {
+            out[g * p.out_stride + col] = from_f32<T>(key_value(s_max[e]));
+        }
+    }
+}
+
+// The split walk's second step: every group's key maxima as values of the output type
+template <typename T>
+__global__ void __launch_bounds__(256) sa_mlp_keys_out_kernel(const unsigned* __restrict__ keys, long long groups, int cout,
+                                                              T* __restrict__ out, long long out_stride) {
+    const long long total = groups * cout;
+    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+        const long long g = e / cout;
+        out[g * out_stride + (e - g * cout)] = from_f32<T>(key_value(__ldg(keys + e)));
     }
 }
 
@@ -158,22 +181,54 @@ static size_t sa_mlp_smem(const SaMlpParams& p, int tm, int slots) {
            sizeof(float) * 2 * (size_t)p.max_cout + sizeof(int) * (size_t)tm + sizeof(unsigned) * (size_t)slots * cout_last;
 }
 
+// Multiply-adds of a whole cloud below which it is never split: a CTA's fixed cost (its key slots, the workspace memset
+// and the second launch) is then not small against the work, and the call is bound by launches anyway.
+constexpr long long kSplitMinMacs = 1ll << 22;
+
+// CTAs per tile for the whole-cloud form: enough for every SM to hold as many CTAs as fit (at most the two of the
+// launch bounds), never more than the pieces of the longest possible cloud, and one for a cloud of little work.  A
+// function of the shapes and the device alone, never of the values or the lengths.
+static int sa_mlp_splits(const SaMlpParams& p, int tm, size_t smem) {
+    const long long groups = p.groups;
+    const int nsample = p.nsample;
+    long long macs = 0;
+    for (int l = 0; l < p.nlayers; ++l) macs += (long long)p.layer[l].cin * p.layer[l].cout;
+    if (nsample <= tm || macs * nsample < kSplitMinMacs) return 1;
+    const long long pieces = (nsample + tm - 1) / tm;
+    const long long per_sm = smem * 2 + 2048 <= 228 * 1024 ? 2 : 1;
+    const long long want = ((long long)num_sms() * per_sm + groups - 1) / groups;
+    return (int)(want < pieces ? want : pieces);
+}
+
 template <typename T, int TM>
-static int sa_mlp_launch(const SaMlpParams& p, size_t smem, cudaStream_t st) {
+static int sa_mlp_launch(SaMlpParams& p, size_t smem, unsigned* keys, cudaStream_t st) {
     static AttrOnce once;
     // the opt-in is raised to the limit once, so that one setting serves every shape
     cudaError_t e = ensure_attrs(once, sa_mlp_max_kernel<T, TM>, kMlpSmemLimit, false);
     if (e != cudaSuccess) return (int)e;
     const long long tiles = (p.groups + p.groups_per_tile - 1) / p.groups_per_tile;
-    if (tiles > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
-    sa_mlp_max_kernel<T, TM><<<(unsigned)tiles, kMlpThreads, smem, st>>>(p);
+    p.splits = keys ? sa_mlp_splits(p, TM, smem) : 1;
+    p.keys = p.splits > 1 ? keys : nullptr;
+    if (tiles * p.splits > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
+    const int cout = p.layer[p.nlayers - 1].cout;
+    if (p.keys) {
+        // zeroed on the stream (0 is below every key), so the call stays capturable in a CUDA graph
+        e = cudaMemsetAsync(p.keys, 0, sizeof(unsigned) * (size_t)p.groups * cout, st);
+        if (e != cudaSuccess) return (int)e;
+    }
+    sa_mlp_max_kernel<T, TM><<<(unsigned)(tiles * p.splits), kMlpThreads, smem, st>>>(p);
+    int rc = finish_launch();
+    if (rc || !p.keys) return rc;
+    sa_mlp_keys_out_kernel<T><<<grid_for((unsigned long long)p.groups * cout, 256), 256, 0, st>>>(
+        p.keys, p.groups, cout, static_cast<T*>(p.out), p.out_stride);
     return finish_launch();
 }
 
 // The row tile is the largest of 64 / 32 / 16 whose buffers fit (the widths decide: [256, 512, 1024] on 643 inputs
-// takes 32 rows in float32 and 64 in 16 bits); groups of at most TM rows share a tile, as many as fit.
+// takes 32 rows in float32 and 64 in 16 bits); groups of at most TM rows share a tile, as many as fit.  keys: the
+// whole-cloud form's key workspace, which lets a cloud of several pieces be split over CTAs (nullptr: one CTA per tile).
 template <typename T>
-static int sa_mlp_plan_launch(SaMlpParams& p, cudaStream_t st) {
+static int sa_mlp_plan_launch(SaMlpParams& p, unsigned* keys, cudaStream_t st) {
     int w0 = p.layer[0].cin, w1 = 1;  // widest rows of buffer 0 (input, outputs of layers 1, 3) and 1 (layers 0, 2)
     for (int l = 0; l + 1 < p.nlayers; ++l) {
         int& w = (l & 1) ? w0 : w1;
@@ -187,41 +242,28 @@ static int sa_mlp_plan_launch(SaMlpParams& p, cudaStream_t st) {
         while (slots > 1 && sa_mlp_smem<T>(p, tm, slots) > kMlpSmemLimit) --slots;
         p.groups_per_tile = slots;
         const size_t smem = sa_mlp_smem<T>(p, tm, slots);
-        if (tm == 64) return sa_mlp_launch<T, 64>(p, smem, st);
-        if (tm == 32) return sa_mlp_launch<T, 32>(p, smem, st);
-        return sa_mlp_launch<T, 16>(p, smem, st);
+        if (tm == 64) return sa_mlp_launch<T, 64>(p, smem, keys, st);
+        if (tm == 32) return sa_mlp_launch<T, 32>(p, smem, keys, st);
+        return sa_mlp_launch<T, 16>(p, smem, keys, st);
     }
     return (int)cudaErrorInvalidValue;
 }
 
-}  // namespace pn2
-
-extern "C" int pn2_sa_mlp_max_typed(int dtype, int b, int n, int c, int m, int nsample, const float* xyz,
-                                    const float* new_xyz, const void* points, const int* idx, int xyz_first, int use_xyz,
-                                    int nlayers, const int* widths, const float* const* weight, const float* const* bias,
-                                    const float* const* bn_weight, const float* const* bn_bias,
-                                    const float* const* bn_mean, const float* const* bn_var, const float* bn_eps,
-                                    const int* relu, void* out, long long out_row_stride, void* stream) {
-    using namespace pn2;
-    if (!valid_dtype(dtype) || b < 0 || n <= 0 || c < 0 || m < 0 || nsample <= 0) return (int)cudaErrorInvalidValue;
+// The checks and the parameters both entries share; false: an invalid argument (nothing may be launched)
+static bool sa_mlp_params(SaMlpParams& p, int dtype, int b, int n, int c, int m, int nsample, const void* points,
+                          int xyz_first, int use_xyz, int nlayers, const int* widths, const float* const* weight,
+                          const float* const* bias, const float* const* bn_weight, const float* const* bn_bias,
+                          const float* const* bn_mean, const float* const* bn_var, const float* bn_eps, const int* relu,
+                          long long out_row_stride) {
+    if (!valid_dtype(dtype) || b < 0 || n <= 0 || c < 0 || m < 0 || nsample <= 0) return false;
     if (!points) c = 0;
     const bool with_xyz = use_xyz || c == 0;
     const int cin = c + (with_xyz ? 3 : 0);
-    if (cin > kMlpMaxIn || (!idx && nsample != n)) return (int)cudaErrorInvalidValue;
-    SaMlpParams p{};
+    if (cin > kMlpMaxIn) return false;
     if (!mlp_layers_from_args(p.layer, p.max_cout, cin, nlayers, widths, weight, bias, bn_weight, bn_bias, bn_mean, bn_var,
                               bn_eps, relu))
-        return (int)cudaErrorInvalidValue;
-    const int prev = widths[nlayers - 1];
-    if (out_row_stride < prev) return (int)cudaErrorInvalidValue;
-    if (b == 0 || m == 0) return 0;
-    if (!xyz || !out) return (int)cudaErrorInvalidValue;
-    p.xyz = xyz;
-    p.new_xyz = new_xyz;
-    p.points = points;
-    p.idx = idx;
-    p.out = out;
-    p.out_stride = out_row_stride;
+        return false;
+    if (out_row_stride < widths[nlayers - 1]) return false;
     p.groups = (long long)b * m;
     p.n = n;
     p.c = c;
@@ -230,7 +272,70 @@ extern "C" int pn2_sa_mlp_max_typed(int dtype, int b, int n, int c, int m, int n
     p.xyz_lo = with_xyz ? (xyz_first ? 0 : c) : -1;
     p.feat_lo = with_xyz && xyz_first ? 3 : 0;
     p.nlayers = nlayers;
-    if (dtype == PN2_F32) return sa_mlp_plan_launch<float>(p, as_stream(stream));
-    if (dtype == PN2_BF16) return sa_mlp_plan_launch<__nv_bfloat16>(p, as_stream(stream));
-    return sa_mlp_plan_launch<__half>(p, as_stream(stream));
+    p.splits = 1;
+    return true;
+}
+
+template <typename F>
+static int sa_mlp_dispatch(int dtype, F&& f) {
+    if (dtype == PN2_F32) return f(float());
+    if (dtype == PN2_BF16) return f(__nv_bfloat16());
+    return f(__half());
+}
+
+}  // namespace pn2
+
+extern "C" size_t pn2_sa_mlp_max_all_workspace_bytes(int b, int c_out) {
+    if (b <= 0 || c_out <= 0) return 0;
+    return ((size_t)b * c_out * sizeof(unsigned) + 255) / 256 * 256;
+}
+
+extern "C" int pn2_sa_mlp_max_all_typed(int dtype, int b, int n, int c, const float* xyz, const float* new_xyz,
+                                        const void* points, const int* lengths, int xyz_first, int use_xyz, int nlayers,
+                                        const int* widths, const float* const* weight, const float* const* bias,
+                                        const float* const* bn_weight, const float* const* bn_bias,
+                                        const float* const* bn_mean, const float* const* bn_var, const float* bn_eps,
+                                        const int* relu, void* out, long long out_row_stride, void* workspace,
+                                        size_t workspace_bytes, void* stream) {
+    using namespace pn2;
+    SaMlpParams p{};
+    if (!sa_mlp_params(p, dtype, b, n, c, 1, n, points, xyz_first, use_xyz, nlayers, widths, weight, bias, bn_weight,
+                       bn_bias, bn_mean, bn_var, bn_eps, relu, out_row_stride))
+        return (int)cudaErrorInvalidValue;
+    if (b == 0) return 0;
+    if (!out || (p.xyz_lo >= 0 && !xyz)) return (int)cudaErrorInvalidValue;
+    if (!workspace || workspace_bytes < pn2_sa_mlp_max_all_workspace_bytes(b, widths[nlayers - 1]) ||
+        !aligned_to(workspace, 16))
+        return (int)cudaErrorInvalidValue;
+    p.xyz = xyz;
+    p.new_xyz = new_xyz;
+    p.points = points;
+    p.lengths = lengths;
+    p.out = out;
+    p.out_stride = out_row_stride;
+    unsigned* keys = static_cast<unsigned*>(workspace);
+    return sa_mlp_dispatch(dtype, [&](auto t) { return sa_mlp_plan_launch<decltype(t)>(p, keys, as_stream(stream)); });
+}
+
+extern "C" int pn2_sa_mlp_max_typed(int dtype, int b, int n, int c, int m, int nsample, const float* xyz,
+                                    const float* new_xyz, const void* points, const int* idx, int xyz_first, int use_xyz,
+                                    int nlayers, const int* widths, const float* const* weight, const float* const* bias,
+                                    const float* const* bn_weight, const float* const* bn_bias,
+                                    const float* const* bn_mean, const float* const* bn_var, const float* bn_eps,
+                                    const int* relu, void* out, long long out_row_stride, void* stream) {
+    using namespace pn2;
+    SaMlpParams p{};
+    if (!sa_mlp_params(p, dtype, b, n, c, m, nsample, points, xyz_first, use_xyz, nlayers, widths, weight, bias, bn_weight,
+                       bn_bias, bn_mean, bn_var, bn_eps, relu, out_row_stride) ||
+        (!idx && nsample != n))
+        return (int)cudaErrorInvalidValue;
+    if (b == 0 || m == 0) return 0;
+    if (!xyz || !out) return (int)cudaErrorInvalidValue;
+    p.xyz = xyz;
+    p.new_xyz = new_xyz;
+    p.points = points;
+    p.idx = idx;
+    p.out = out;
+    p.out_stride = out_row_stride;
+    return sa_mlp_dispatch(dtype, [&](auto t) { return sa_mlp_plan_launch<decltype(t)>(p, nullptr, as_stream(stream)); });
 }

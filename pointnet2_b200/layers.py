@@ -75,28 +75,34 @@ class SharedMLP(nn.Module):
         if mask is None:
             return self.body(t.reshape(-1, t.shape[-1])).reshape(*lead, self.out_channels)
         keep = mask.reshape(-1, 1)
-        # torch.where, not a multiply: NaN * 0 is NaN.  This one stays even before the fused op: NaN input rows would
-        # reach the Linear's weight gradient through x^T dy.
-        x = torch.where(keep, t.reshape(-1, t.shape[-1]), 0)
-        mods = list(self.body)
-        i = 0
-        while i < len(mods):
-            mod = mods[i]
-            if isinstance(mod, nn.BatchNorm1d):
-                if _fuses_at(mods, i, x):
-                    # BatchNorm1d + the ReLU after it in the CUDA op, which reads no padding row and writes 0 there
-                    x = masked_batch_norm_relu(mod, x, keep.reshape(-1))
-                    i += 2
-                    continue
-                x = torch.where(keep, masked_batch_norm(mod, x, keep), 0)
-            elif isinstance(mod, nn.Linear):
-                x = mod(x)
-                if not _fuses_at(mods, i + 1, x):
-                    x = torch.where(keep, x, 0)
-            else:
-                x = mod(x)  # ReLU keeps the zeros
-            i += 1
-        return x.reshape(*lead, self.out_channels)
+        return _masked_layers(list(self.body), t.reshape(-1, t.shape[-1]), keep).reshape(*lead, self.out_channels)
+
+
+def _masked_layers(mods, x: torch.Tensor, keep: torch.Tensor, fuse_last: bool = False) -> torch.Tensor:
+    """The modules ``mods`` of a SharedMLP body on the rows of x (R, C) where keep (R, 1) is True: batch norms take
+    their statistics from those rows, and every output's padding rows are 0.  fuse_last: mods ends with a Linear whose
+    output goes straight to a fused op that reads no padding row (its padding rows are left as they come)."""
+    # torch.where, not a multiply: NaN * 0 is NaN.  This one stays even before the fused op: NaN input rows would
+    # reach the Linear's weight gradient through x^T dy.
+    x = torch.where(keep, x, 0)
+    i = 0
+    while i < len(mods):
+        mod = mods[i]
+        if isinstance(mod, nn.BatchNorm1d):
+            if _fuses_at(mods, i, x):
+                # BatchNorm1d + the ReLU after it in the CUDA op, which reads no padding row and writes 0 there
+                x = masked_batch_norm_relu(mod, x, keep.reshape(-1))
+                i += 2
+                continue
+            x = torch.where(keep, masked_batch_norm(mod, x, keep), 0)
+        elif isinstance(mod, nn.Linear):
+            x = mod(x)
+            if not (_fuses_at(mods, i + 1, x) or (fuse_last and i + 1 == len(mods))):
+                x = torch.where(keep, x, 0)
+        else:
+            x = mod(x)  # ReLU keeps the zeros
+        i += 1
+    return x
 
 
 def row_mask(lengths: torch.Tensor, n: int) -> torch.Tensor:
@@ -247,6 +253,141 @@ def masked_batch_norm_relu(bn: nn.BatchNorm1d, x: torch.Tensor, keep: torch.Tens
     return _MaskedBatchNormReLU.apply(x, weight, bias, keep, bn)
 
 
+class _MaskedBatchNormReLUMax(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, keep, bn, b, n):
+        c = x.shape[1]
+        dev = x.device
+        tracking = bn.track_running_stats and bn.running_mean is not None
+        momentum = -1.0 if bn.momentum is None else float(bn.momentum)
+        out = torch.empty((b, c), dtype=x.dtype, device=dev)
+        argmax = torch.empty((b, c), dtype=torch.int32, device=dev)
+        save_mean = torch.empty(c, dtype=torch.float32, device=dev)
+        save_invstd = torch.empty(c, dtype=torch.float32, device=dev)
+        lib = _lib.load()
+        with on_device(x):
+            if tracking:
+                bn.num_batches_tracked.add_(1)  # on the device; the kernel reads it for the cumulative average
+            wsb = int(lib.pn2_masked_bn_relu_max_workspace_bytes(b, n, c))
+            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+            rc = lib.pn2_masked_bn_relu_max_forward_typed(
+                DTYPE_CODES[x.dtype], b, n, c, ptr(x), ptr(keep), ptr(weight), ptr(bias), float(bn.eps), momentum,
+                ptr(bn.num_batches_tracked if tracking else None), ptr(bn.running_mean if tracking else None),
+                ptr(bn.running_var if tracking else None), ptr(out), ptr(argmax), ptr(save_mean), ptr(save_invstd),
+                ptr(ws), wsb, stream_ptr(dev))
+        _lib.check(rc, "pn2_masked_bn_relu_max_forward_typed")
+        ctx.save_for_backward(x, out, argmax, keep, weight, save_mean, save_invstd)
+        ctx.affine = weight is not None
+        ctx.mark_non_differentiable(argmax)
+        return out, argmax
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout, _dargmax):
+        x, out, argmax, keep, weight, save_mean, save_invstd = ctx.saved_tensors
+        b, c = out.shape
+        n = x.shape[0] // max(b, 1)
+        dev = x.device
+        dout = dout.to(x.dtype).contiguous()
+        dx = torch.empty_like(x)
+        dgamma = torch.empty(c, dtype=torch.float32, device=dev) if ctx.affine else None
+        dbeta = torch.empty(c, dtype=torch.float32, device=dev) if ctx.affine else None
+        lib = _lib.load()
+        with on_device(x):
+            wsb = int(lib.pn2_masked_bn_relu_max_workspace_bytes(b, n, c))
+            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+            rc = lib.pn2_masked_bn_relu_max_backward_typed(
+                DTYPE_CODES[x.dtype], b, n, c, ptr(dout), ptr(x), ptr(out), ptr(argmax), ptr(keep), ptr(weight),
+                ptr(save_mean), ptr(save_invstd), ptr(dx), ptr(dgamma), ptr(dbeta), ptr(ws), wsb, stream_ptr(dev))
+        _lib.check(rc, "pn2_masked_bn_relu_max_backward_typed")
+        return dx, dgamma, dbeta, None, None, None, None
+
+
+def masked_bn_relu_max(bn: nn.BatchNorm1d, x: torch.Tensor, lengths=None, *, with_indices: bool = False):
+    """max over each cloud's real rows of relu(bn(x)), the batch norm taking its statistics from the real rows, as one
+    CUDA op forward and backward (csrc/masked_bn.cu): the last layer of PointNet's point features and its max-pool
+    (models/pointnet_cls_basic.py:46-53) on a padded batch.  ``x`` (B, N, C) float32 / bfloat16 / float16 on CUDA, the
+    Linear output; ``lengths`` (B,) per-cloud row counts (see device_lengths; None: every row is real).  Returns (B, C)
+    in x's dtype, and with ``with_indices`` also the (B, C) int32 row of each maximum: the FIRST row that reaches it,
+    where TF's MaxPoolGrad sends the gradient.  The (B, N, C) ReLU output is never stored.
+
+    The statistics, the running-statistics update and every value are bit-identical to masked_batch_norm_relu on the
+    same rows followed by a max over the real rows (NaN wins, as in torch).  The padding rows of x are never read (they
+    may be NaN).  Backward: the gradient reaches each maximum's row only, through the ReLU and the batch norm, with
+    fixed-order sums and no float atomics, so it is bit-identical from run to run.  For batch statistics only, as
+    masked_batch_norm_relu; CPU tensors raise RuntimeError."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype in FEATURE_DTYPES):
+        raise RuntimeError(f"masked_bn_relu_max needs a float32/bfloat16/float16 CUDA tensor, got "
+                           f"{getattr(x, 'dtype', type(x).__name__)} on {getattr(x, 'device', '?')}")
+    if x.dim() != 3 or x.shape[2] != bn.num_features:
+        raise ValueError(f"masked_bn_relu_max expects (batch_size, num_point, {bn.num_features}) x, got {tuple(x.shape)}")
+    if not bn.training and bn.running_mean is not None:
+        raise ValueError("masked_bn_relu_max computes batch statistics; in eval mode with running statistics use bn(x)")
+    misfit = _bn_tensors_misfit(bn, x.device)
+    if misfit is not None:
+        raise misfit
+    b, n, c = x.shape
+    if b * n >= 2 ** 31:
+        raise ValueError(f"masked_bn_relu_max takes fewer than 2^31 rows, got {b} x {n}")
+    lengths = device_lengths(lengths, b, n, x.device, "masked_bn_relu_max")
+    if lengths is None:
+        keep = torch.ones(b * n, dtype=torch.uint8, device=x.device)
+    else:
+        keep = row_mask(lengths, n).reshape(-1).view(torch.uint8)  # the bool mask as bytes, no copy
+    weight = bn.weight if bn.affine else None
+    bias = bn.bias if bn.affine else None
+    if b == 0:
+        out = x.new_empty((0, c))
+        return (out, torch.empty((0, c), dtype=torch.int32, device=x.device)) if with_indices else out
+    out, argmax = _MaskedBatchNormReLUMax.apply(x.reshape(b * n, c).contiguous(), weight, bias, keep, bn, b, n)
+    return (out, argmax) if with_indices else out
+
+
+def _first_max(y: torch.Tensor) -> torch.Tensor:
+    """y (B, N, C) -> (B, C): the maximum over N (NaN wins, as in torch's max), its gradient going to the first row that
+    reaches it only (TF's MaxPoolGrad), whatever the device"""
+    m = y.amax(1, keepdim=True)
+    hit = (y == m) | (torch.isnan(y) & torch.isnan(m))
+    rows = torch.arange(y.shape[1], device=y.device).view(1, -1, 1)
+    first = torch.where(hit, rows, y.shape[1]).amin(1, keepdim=True)
+    return y.gather(1, first).squeeze(1)
+
+
+def shared_mlp_max(mlp: "SharedMLP", t: torch.Tensor, lengths=None) -> torch.Tensor:
+    """max over each cloud's real rows of mlp(t): t (B, N, C), ``lengths`` (B,) per-cloud row counts (None: every row
+    is real; the padding rows are never read and may be NaN).  Returns (B, C_out).  The one place that routes
+    "SharedMLP, then a whole-cloud max-pool":
+
+    * training on CUDA: the earlier layers through SharedMLP's masked path, then the last Linear, then masked_bn_relu_max
+      when its batch norm and ReLU fuse (fused_bn_applies);
+    * eval under no_grad: sa_mlp_max(idx=None, lengths=...) when sa_mlp_applies, and inside batch_invariant() always (a
+      stack the kernel cannot take raises RuntimeError there);
+    * anything else (CPU, float64, grad mode in eval): the masked layers, the padding rows set to -inf, and a max whose
+      gradient goes to the first maximal row."""
+    if t.dim() != 3:
+        raise ValueError(f"shared_mlp_max expects (batch_size, num_point, channels) t, got {tuple(t.shape)}")
+    b, n = t.shape[0], t.shape[1]
+    lengths = device_lengths(lengths, b, n, t.device, "shared_mlp_max")
+    if t.is_cuda and not torch.is_grad_enabled():
+        if _BATCH_INVARIANT and invariant_applies(mlp, t):
+            return _invariant_call(sa_mlp_max, None, None, t, None, mlp, True, False, lengths=lengths)[:, 0]
+        if sa_mlp_applies(mlp, t, t):
+            return sa_mlp_max(None, None, t, None, mlp, True, False, lengths=lengths)[:, 0]
+    mask = torch.ones(b, n, dtype=torch.bool, device=t.device) if lengths is None else row_mask(lengths, n)
+    keep = mask.reshape(-1, 1)
+    mods = list(mlp.body) if isinstance(mlp, SharedMLP) else []
+    if (len(mods) >= 3 and isinstance(mods[-3], nn.Linear) and isinstance(mods[-2], nn.BatchNorm1d)
+            and isinstance(mods[-1], nn.ReLU)):
+        # the layers SharedMLP(t, mask) runs, split before the last batch norm, whose input may go to the fused op
+        x = _masked_layers(mods[:-2], t.reshape(-1, t.shape[-1]), keep, fuse_last=True)
+        if fused_bn_applies(mods[-2], x):
+            return masked_bn_relu_max(mods[-2], x.reshape(b, n, -1), lengths)
+        y = _masked_layers(mods[-2:], x, keep).reshape(b, n, -1)
+    else:
+        y = mlp(t, mask)
+    return _first_max(torch.where(mask.unsqueeze(-1), y, float("-inf")))
+
+
 SA_MLP_MAX_LAYERS = 4
 SA_MLP_MAX_WIDTH = 1024  # of a layer's output; the first layer takes up to SA_MLP_MAX_WIDTH + 3 input channels
 # Multiply-adds per grouped row (sum of C_in * C_out) up to which the modules take the kernel.  Above it the torch layers
@@ -370,9 +511,9 @@ def sa_mlp_applies(mlp, xyz: torch.Tensor, points: Optional[torch.Tensor] = None
     return True
 
 
-def sa_mlp_max(xyz: torch.Tensor, new_xyz: Optional[torch.Tensor], points: Optional[torch.Tensor],
+def sa_mlp_max(xyz: Optional[torch.Tensor], new_xyz: Optional[torch.Tensor], points: Optional[torch.Tensor],
                idx: Optional[torch.Tensor], mlp: SharedMLP, xyz_first: bool = True, use_xyz: bool = True,
-               out: Optional[torch.Tensor] = None) -> torch.Tensor:
+               out: Optional[torch.Tensor] = None, *, lengths=None) -> torch.Tensor:
     """The inference tail of a set-abstraction level as one CUDA op (csrc/sa_mlp.cu): for every group (b, s)
 
         rows = concat(xyz[b, idx[b, s]] - new_xyz[b, s], points[b, idx[b, s]])     ([features, xyz] when not xyz_first;
@@ -391,15 +532,33 @@ def sa_mlp_max(xyz: torch.Tensor, new_xyz: Optional[torch.Tensor], points: Optio
     every run, at every batch size and next to any other cloud, which a cuBLAS product does not promise.  NaN
     propagates as in the torch layers.  No gradient: call it under torch.no_grad().
 
+    With ``idx=None`` (the group_all form) the call goes to the whole-cloud entry (pn2_sa_mlp_max_all_typed), which
+    deals the row tiles of a cloud out to several CTAs when the batch is too small to fill the GPU; the maximum of exact
+    keys does not depend on that split, so the bits are those of one CTA per cloud.  There ``lengths`` (B,) may give
+    per-cloud row counts (see device_lengths): rows from lengths[i] on are never read and may hold NaN.  ``lengths``
+    with an ``idx`` raises ValueError.  ``xyz`` may be None there when the rows take no coordinates (use_xyz=False with
+    points).
+
     Raises ValueError for a batch norm in training mode (that needs batch statistics: use the module itself) or without
     running statistics, for more than 4 layers or widths above 1024, and for shapes that do not fit together; TypeError /
     RuntimeError for tensors of the wrong dtype or device."""
+    if lengths is not None and idx is not None:
+        raise ValueError("sa_mlp_max takes lengths only with idx=None (the one group of every cloud)")
     stack = _eval_stack(mlp, "sa_mlp_max", SA_MLP_MAX_WIDTH + 3)
-    xyz = require_cuda(xyz, "xyz", torch.float32)
-    if xyz.dim() != 3 or xyz.shape[2] != 3:
-        raise ValueError(f"sa_mlp_max expects (batch_size, ndataset, 3) xyz, got {tuple(xyz.shape)}")
-    b, n = xyz.shape[0], xyz.shape[1]
-    tensors = [xyz]
+    if xyz is None and (idx is not None or points is None or use_xyz):
+        raise ValueError("sa_mlp_max needs xyz unless idx is None and the rows are the features alone (use_xyz=False)")
+    if xyz is not None:
+        xyz = require_cuda(xyz, "xyz", torch.float32)
+        if xyz.dim() != 3 or xyz.shape[2] != 3:
+            raise ValueError(f"sa_mlp_max expects (batch_size, ndataset, 3) xyz, got {tuple(xyz.shape)}")
+        b, n = xyz.shape[0], xyz.shape[1]
+        tensors = [xyz]
+    else:
+        points = require_cuda(points, "points", FEATURE_DTYPES)
+        if points.dim() != 3:
+            raise ValueError(f"sa_mlp_max expects (batch_size, ndataset, channel) points, got {tuple(points.shape)}")
+        b, n = points.shape[0], points.shape[1]
+        tensors = []
     if idx is not None:
         idx = require_cuda(idx, "idx", torch.int32)
         if idx.dim() != 3 or idx.shape[0] != b or idx.shape[2] < 1:
@@ -419,7 +578,7 @@ def sa_mlp_max(xyz: torch.Tensor, new_xyz: Optional[torch.Tensor], points: Optio
     c = 0
     if points is not None:
         points = require_cuda(points, "points", FEATURE_DTYPES)
-        if points.dim() != 3 or points.shape[:2] != xyz.shape[:2]:
+        if points.dim() != 3 or tuple(points.shape[:2]) != (b, n):
             raise ValueError("points must be (batch_size, ndataset, channel) matching xyz")
         tensors.append(points)
         c = points.shape[2]
@@ -429,7 +588,7 @@ def sa_mlp_max(xyz: torch.Tensor, new_xyz: Optional[torch.Tensor], points: Optio
     if cin != mlp.in_channels:
         raise ValueError(f"the grouped rows have {cin} channels, mlp expects {mlp.in_channels}")
     same_device(*tensors)
-    dev = xyz.device
+    dev = tensors[0].device
     _check_params(stack, dev)
     cout = mlp.out_channels
     if out is None:
@@ -444,8 +603,19 @@ def sa_mlp_max(xyz: torch.Tensor, new_xyz: Optional[torch.Tensor], points: Optio
             raise ValueError("out must be a channel slice of a contiguous (batch_size, npoint, channels) tensor")
     if b * s == 0:
         return out
+    lib = _lib.load()
+    if idx is None:
+        lengths = device_lengths(lengths, b, n, dev, "sa_mlp_max")
+        with on_device(tensors[0]):
+            wsb = int(lib.pn2_sa_mlp_max_all_workspace_bytes(b, cout))
+            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+            rc = lib.pn2_sa_mlp_max_all_typed(
+                DTYPE_CODES[dtype], b, n, c, ptr(xyz), ptr(new_xyz), ptr(points), ptr(lengths), 1 if xyz_first else 0,
+                1 if use_xyz else 0, *_layer_args(stack), ptr(out), out.stride(1), ptr(ws), wsb, stream_ptr(dev))
+        _lib.check(rc, "pn2_sa_mlp_max_all_typed")
+        return out
     with on_device(xyz):
-        rc = _lib.load().pn2_sa_mlp_max_typed(
+        rc = lib.pn2_sa_mlp_max_typed(
             DTYPE_CODES[dtype], b, n, c, s, k, ptr(xyz), ptr(new_xyz), ptr(points), ptr(idx), 1 if xyz_first else 0,
             1 if use_xyz else 0, *_layer_args(stack), ptr(out), out.stride(1), stream_ptr(dev))
     _lib.check(rc, "pn2_sa_mlp_max_typed")

@@ -13,12 +13,14 @@ Networks (layer hyper-parameters quoted from the reference's model files):
     PointNet2SemSeg   models/pointnet2_sem_seg.py:28-46
     PointNet2PartSeg     models/pointnet2_part_seg.py:17-41
     PointNet2PartSegMSG  models/pointnet2_part_seg_msg_one_hot.py:19-47
+    PointNetClsBasic  models/pointnet_cls_basic.py:21-60 (PointNet v1, the baseline classifier)
 Losses and metrics: cls_loss, sem_seg_loss, part_seg_loss; for part segmentation PART_OFFSETS, part_seg_predict and
 part_seg_iou (part_seg/train.py:274-300).
 Geometry goes through pointnet2_b200.pointnet_util (the CUDA ops); there is no CPU path.
 """
 from __future__ import annotations
 
+import math
 from typing import Optional, Sequence
 
 import numpy as np
@@ -26,7 +28,7 @@ import torch
 from torch import nn
 
 from ._tensor import device_lengths
-from .layers import SharedMLP, row_mask, set_bn_momentum  # noqa: F401
+from .layers import SharedMLP, row_mask, set_bn_momentum, shared_mlp_max  # noqa: F401
 from .pointnet_util import pointnet_fp_module, pointnet_sa_module, pointnet_sa_module_msg
 
 
@@ -129,6 +131,49 @@ class PointNet2ClsMSG(nn.Module):
         l2_xyz, l2_points = self.sa2(l1_xyz, l1_points)
         _, l3_points, _ = self.sa3(l2_xyz, l2_points)
         return self.head(l3_points.reshape(point_cloud.shape[0], -1)), {}
+
+
+class PointNetClsBasic(nn.Module):
+    """PointNet (v1) classification net, input (B,N,3) -> logits (B,num_class).  models/pointnet_cls_basic.py:21-60:
+    conv1-conv5 (64, 64, 64, 128, 1024, each with batch norm and ReLU) on every point, a max over the cloud, fc1 512 and
+    fc2 256 with batch norm, dropout (keep 0.7) after fc2 only, fc3 without activation.  No T-nets (the reference has
+    none).
+
+    conv1 is a [1, 3] convolution over the (N, 3, 1) image of the cloud (weight [1, 3, 1, 64]), so its xavier bound uses
+    fan_in 3 and fan_out 3 * 64 = 192; the other layers are 1x1 and initialise as SharedMLP does.  conv1-conv4 are
+    ``feat``, conv5 is ``conv5``: conv5 and the max form one step (layers.shared_mlp_max) that trains through the fused
+    masked batch norm + ReLU + max-pool and infers through sa_mlp_max's whole-cloud kernel.
+
+    ``lengths`` (B,), optional: cloud i is ``point_cloud[i, :lengths[i]]`` (variable-size clouds padded to N, as
+    shapes.sample_shapes makes them with point dropout).  The padding rows are never read (they may be NaN), the batch
+    norms of conv1-conv5 take their statistics from the real rows, and the max runs over the real rows only.  A lengths
+    tensor on the GPU is never read back.  On CUDA dense and ragged batches run the same kernels (lengths=None means
+    every row is real); on the CPU or in float64 the layers run as the torch composition."""
+
+    def __init__(self, num_class: int = 40):
+        super().__init__()
+        self.feat = SharedMLP(3, [64, 64, 64, 128])
+        bound = math.sqrt(6.0 / (3 + 3 * 64))  # xavier on the [1, 3, 1, 64] kernel: fan_in 3, fan_out 192
+        nn.init.uniform_(self.feat.body[0].weight, -bound, bound)
+        self.conv5 = SharedMLP(128, [1024])
+        self.fc1 = SharedMLP(1024, [512])
+        self.fc2 = SharedMLP(512, [256])
+        self.dp1 = nn.Dropout(1.0 - 0.7)
+        self.fc3 = SharedMLP(256, [num_class], bn=False, last_activation=False)
+
+    def forward(self, point_cloud, lengths=None):
+        if not isinstance(point_cloud, torch.Tensor) or point_cloud.dim() != 3 or point_cloud.shape[-1] != 3:
+            shape = tuple(point_cloud.shape) if isinstance(point_cloud, torch.Tensor) else type(point_cloud).__name__
+            raise ValueError(f"PointNetClsBasic expects a (batch_size, num_point, 3) point cloud, got {shape}")
+        b, n = point_cloud.shape[0], point_cloud.shape[1]
+        lengths = device_lengths(lengths, b, n, point_cloud.device, "PointNetClsBasic")
+        if lengths is None:
+            mask = torch.ones(b, n, dtype=torch.bool, device=point_cloud.device)
+        else:
+            mask = row_mask(lengths, n)
+        net = self.feat(point_cloud, mask)
+        net = shared_mlp_max(self.conv5, net, lengths)
+        return self.fc3(self.dp1(self.fc2(self.fc1(net)))), {}
 
 
 class PointNet2SemSeg(nn.Module):

@@ -27,6 +27,8 @@ SHOW = ["fps_cta_kernel<16, 256, 0, false>", "fps_cta_kernel<16, 256, 1, false>"
         "mbn_stats_kernel<float, 4, true>", "mbn_stats_kernel<__nv_bfloat16, 4, true>", "mbn_stats_kernel<float, 1, false>", "mbn_finalize_kernel",
         "mbn_norm_relu_kernel<float, 4, true>", "mbn_norm_relu_kernel<__nv_bfloat16, 4, true>", "mbn_bwd_sums_kernel<float, 4, true>",
         "mbn_bwd_sums_kernel<__nv_bfloat16, 4, true>", "mbn_bwd_finalize_kernel", "mbn_bwd_dx_kernel<float, 4, true>", "mbn_bwd_dx_kernel<__nv_bfloat16, 4, true>",
+        "mbn_norm_relu_max_kernel<float, 4, true>", "mbn_norm_relu_max_kernel<__nv_bfloat16, 4, true>", "mbn_max_bwd_finalize_kernel<float>",
+        "mbn_max_bwd_dx_kernel<float, 4, true>", "mbn_max_bwd_dx_kernel<__nv_bfloat16, 4, true>", "sa_mlp_keys_out_kernel<float>",
         "scene_count_kernel", "scene_scan_kernel", "scene_fill_kernel", "scene_merge_kernel<float>", "scene_merge_kernel<__nv_bfloat16>",
         "scene_merge_kernel<__half>", "crop_attempt_kernel", "crop_select_kernel", "shape_batch_kernel",
         "vscan_ray_kernel", "vscan_cell_kernel", "vscan_point_kernel", "vscan_select_kernel"]

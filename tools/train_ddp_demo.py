@@ -14,6 +14,7 @@ min(0.99, 1 - 0.5 * 0.5^(samples/200000)).
     python tools/train_ddp_demo.py --model part_seg_msg --ragged --steps 30     # part segmentation, variable sizes
     python tools/train_ddp_demo.py --model sem_seg --scene-crops --steps 30     # training crops of synthetic rooms
     python tools/train_ddp_demo.py --shape-set --votes 12 --steps 30            # augmented shape batches, voted accuracy
+    python tools/train_ddp_demo.py --model cls_basic --shape-set --votes 12 --steps 30   # PointNet v1 on the same
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 \
         tools/train_ddp_demo.py --steps 20                                      # one rank per GPU
 
@@ -26,7 +27,7 @@ models) draws each cloud's length from U[N/2, N], fills the padding rows with Na
 --scene-crops (sem_seg) trains on scene.sample_crops of a SceneSet of synthetic rooms (workloads.scene_room, 21
 classes): each step's scenes come from a seeded permutation of the set, each rank draws its crops on its own GPU with a
 seed derived from (step, rank), with dropout and rotation, and passes the crops' lengths and sample weights.
---shape-set (cls_ssg, cls_msg, part_seg, part_seg_msg) builds one shapes.ShapeSet of synthetic shapes (--set-shapes of
+--shape-set (cls_ssg, cls_msg, cls_basic, part_seg, part_seg_msg) builds one shapes.ShapeSet of synthetic shapes (--set-shapes of
 --set-points points: the parametric shapes above, or workloads.part_shapes for the part models) and trains on
 shapes.sample_shapes batches drawn on the GPU with a seed derived from (step, rank): ModelNet's augmentation for the
 classification nets, the ShapeNet part recipe (random rows, jitter, normals) for the part nets.  --votes V then prints
@@ -85,7 +86,8 @@ def synthetic_shapes(batch: int, num_point: int, num_class: int, rs: np.random.R
 
 def main() -> None:
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", choices=["cls_ssg", "cls_msg", "sem_seg", "part_seg", "part_seg_msg"], default="cls_ssg")
+    ap.add_argument("--model", choices=["cls_ssg", "cls_msg", "cls_basic", "sem_seg", "part_seg", "part_seg_msg"],
+                    default="cls_ssg")
     ap.add_argument("--batch", type=int, default=32, help="GLOBAL batch (split across ranks)")
     ap.add_argument("--num-point", type=int, default=1024)
     ap.add_argument("--num-class", type=int, default=10)
@@ -113,7 +115,7 @@ def main() -> None:
     args = ap.parse_args()
     if args.shape_set and (args.model == "sem_seg" or args.ragged or args.scene_crops):
         raise SystemExit("--shape-set trains the cls / part models on their own ragged batches (no --ragged)")
-    if args.votes and (not args.shape_set or args.model not in ("cls_ssg", "cls_msg")):
+    if args.votes and (not args.shape_set or args.model not in ("cls_ssg", "cls_msg", "cls_basic")):
         raise SystemExit("--votes scores a classification model trained with --shape-set")
     if args.scene_crops and (args.model != "sem_seg" or args.ragged):
         raise SystemExit("--scene-crops trains the sem_seg model on its own ragged crops (no --ragged)")
@@ -143,6 +145,8 @@ def main() -> None:
         model = nets.PointNet2ClsSSG(args.num_class)
     elif args.model == "cls_msg":
         model = nets.PointNet2ClsMSG(args.num_class)
+    elif args.model == "cls_basic":  # PointNet v1, the reference's baseline classifier
+        model = nets.PointNetClsBasic(args.num_class)
     elif args.model == "part_seg":  # 50 ShapeNet parts: --num-class does not apply
         model = nets.PointNet2PartSeg()
     elif args.model == "part_seg_msg":
