@@ -570,6 +570,35 @@ int pn2_virtual_scans(int s, int p, int max_scene, const float* xyz, const int* 
                       float* out_xyz, long long* out_label, float* out_weight, int* lengths, int* point_idx, int* visible,
                       unsigned char* valid, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- point-cloud rendering (utils/render_balls_so.cpp render_ball, utils/show3d_balls.py; DESIGN.md §6.16) --------
+ * Image i of b (out (b, h, w, 3) u8) is what render_ball(h, w, show, len_i, xyz_i, c0, c1, c2, r) writes for cloud i
+ * alone on a canvas filled with background[0..2] (a host array of 3 bytes): xyz (b, n, 3) int32 (x the row, y the
+ * column), colors (b, n, 3) f32 holding c0, c1, c2 per point (NULL: 255 everywhere), lengths (b,) int32 on the device
+ * (NULL: n), clamped to [0, n]; padding rows are never read and a cloud of length 0 renders as background.  r < 1 is
+ * taken as 1; r <= 4096.  Every coordinate of a real point must satisfy |x|, |y|, |z| <= 2^30 (not checked).  Bit for
+ * bit: the pixel goes to the largest key (z2 + 2^31) << 32 | ~i over the (point, pattern entry) pairs on the canvas
+ * with z2 > -2100000000, and its colour is recomputed in render_ball's arithmetic order.  b <= 65535, h * w < 2^31,
+ * n < 2^30 / 3.  The workspace is pn2_render_balls_workspace_bytes(b, h, w) bytes, 256-byte aligned (0 = invalid
+ * shape): 8 bytes per pixel per image and 8 per image.  Nothing is read back, so the call can be captured in a CUDA
+ * graph.  b = 0 does nothing; invalid arguments return cudaErrorInvalidValue without a launch. */
+size_t pn2_render_balls_workspace_bytes(int b, int h, int w);
+int pn2_render_balls(int b, int n, int h, int w, const int* xyz, const float* colors, const int* lengths, int r,
+                     const unsigned char* background, void* workspace, size_t workspace_bytes, unsigned char* out,
+                     void* stream);
+/* pn2_render_balls, and counters (2 u64 on the device, added to) += the pixel atomics issued and the ones skipped
+ * because the pixel already held a key at least as large: for measurement. */
+int pn2_render_balls_counted(int b, int n, int h, int w, const int* xyz, const float* colors, const int* lengths, int r,
+                             const unsigned char* background, void* workspace, size_t workspace_bytes,
+                             unsigned char* out, unsigned long long* counters, void* stream);
+/* showpoints' view transform of b clouds xyz (b, n, 3) f64 with lengths as above, for v views: p' = (p - mean) /
+ * ((radius * 2.2) / size) over the cloud's real points in float64 (mean in a fixed order, so a cloud's result does not
+ * depend on the rest of the batch; a cloud whose points coincide maps to 0), then p' R_v + (size/2, size/2, 0) with
+ * rotations (v, 3, 3) f64 on the host (row-major, R_v = Rx Ry zoom), clamped to +-2^30 and truncated toward zero into
+ * out (b, v, n, 3) int32; padding rows are 0.  The workspace holds 32 * b bytes, 8-byte aligned.  b <= 65535,
+ * n < 2^30 / 3, v >= 1, size >= 1. */
+int pn2_project_points(int b, int n, int v, const double* xyz, const int* lengths, const double* rotations, int size,
+                       void* workspace, size_t workspace_bytes, int* out, void* stream);
+
 /* ---- host-buffer entry point (the reference feeds numpy through feed_dict) ----------------- */
 
 /* One SSG set-abstraction sampling+grouping layer (farthest_point_sample + gather_point +

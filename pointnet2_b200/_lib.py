@@ -111,6 +111,11 @@ _SIGNATURES = {
     "pn2_virtual_scans_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "pn2_virtual_scans": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, c_int, _P, c_int, _P, _P, c_longlong, _P, c_int, c_int,
                                   _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    # point-cloud rendering: z-buffered ball splats of a ragged batch, and the viewer's projection
+    "pn2_render_balls_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "pn2_render_balls": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P, c_size_t, _P, _P]),
+    "pn2_render_balls_counted": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P, c_size_t, _P, _P, _P]),
+    "pn2_project_points": (c_int, [c_int, c_int, c_int, _P, _P, _P, c_int, _P, c_size_t, _P, _P]),
     "pn2_sa_layer_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "pn2_sa_layer_host": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_api_version": (c_int, []),
