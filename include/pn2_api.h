@@ -466,6 +466,36 @@ int pn2_sa_layer_msg_device_ragged(int b, int n, int m, int nscales, const float
                                    int* const* idx, int* const* pts_cnt, float* const* grouped_xyz, int center,
                                    void* workspace, size_t workspace_bytes, void* stream);
 
+/* farthest_point_sample + gather_point + knn_point + group_point(xyz) (sample_and_group(..., knn=True),
+ * utils/pointnet_util.py:40-46) on DEVICE buffers, results bit-identical to pn2_fps_gather, pn2_knn_point and
+ * group_point(xyz, idx) [- new_xyz] called one after the other: fps_idx (b,m) i32 (required: it is also the channel
+ * between the two kernels), new_xyz (b,m,3), idx (b,m,k) i32, dist (b,m,k) f32 = knn_point's val or NULL,
+ * grouped_xyz (b,m,k,3) or NULL, centred on new_xyz when center != 0 (one rounding per coordinate).
+ * 1 <= k <= min(n, 128), as for pn2_knn_point; otherwise cudaErrorInvalidValue, as for NULL xyz / fps_idx /
+ * new_xyz / idx, before any device is touched.
+ * The kNN grouping can run as a programmatically dependent grid on the SMs the sampling chain leaves idle (each
+ * consumer CTA holds the cloud in shared memory and serves centroids as they are picked) when sampling runs one CTA
+ * per cloud (n <= 8192), pn2_sa_knn_layer_fits(n, k) and b < SMs / 2.  It does when a cost comparison from
+ * (b, n, m, k) and the SM count says the consumers beat the sequential ops (DESIGN.md §6.2.1: at N 4096 -> 1024 on
+ * 132 SMs, b <= 33 at k = 32 and b <= 26 at k = 64).  Otherwise the kernels run back to back, using `workspace`
+ * (pn2_sa_knn_layer_workspace_bytes bytes) for the sampling scratch and, when dist is NULL, knn_point's distances.
+ * The workspace size follows the same choice: 0 when the call will overlap; on the sequential path it includes the
+ * distances, so it is an upper bound when dist is given.  Ask for it on the device, and under the
+ * pn2_set_sa_knn_path / pn2_set_sa_consumer_ctas settings, of the call; a workspace that turns out too small is
+ * refused with cudaErrorInvalidValue.  Asynchronous; capturable in a CUDA graph after the first call on a device.
+ * pn2_set_sa_consumer_ctas also sets the kNN consumer CTAs per cloud (0 = automatic: every SM the sampling
+ * leaves per cloud).
+ * pn2_sa_knn_layer_fits(n, k) only says that the consumer's shared memory holds the cloud and its W buffers
+ * (1 <= k <= min(n, 64)); the overlapped path also needs the conditions above. */
+int pn2_sa_knn_layer_fits(int n, int k);
+size_t pn2_sa_knn_layer_workspace_bytes(int b, int n, int m, int k);
+int pn2_sa_knn_layer_device(int b, int n, int m, int k, const float* xyz, int* fps_idx, float* new_xyz, int* idx,
+                            float* dist, float* grouped_xyz, int center, void* workspace, size_t workspace_bytes,
+                            void* stream);
+/* measurement switch for pn2_sa_knn_layer_device: 0 = the cost rule (default), 1 = overlapped wherever it can run
+ * (fits, one sampling CTA per cloud, an idle SM per cloud), 2 = always sequential.  The outputs do not depend on it. */
+void pn2_set_sa_knn_path(int mode);
+
 /* ---- whole-scene segmentation (scannet/scannet_dataset.py:83-118, scannet/train.py:326-427; DESIGN.md §6.9) --------
  * A scene xyz (p,3) f32 (finite) is cut into nx x ny xy blocks, i-major: block (i,j) spans bmin = (lo_x + i*stride,
  * lo_y + j*stride), bmax = bmin + block_size.  Every test is in double on the float32 coordinate, each operation rounded:

@@ -56,6 +56,11 @@ _SIGNATURES = {
     "pn2_sa_layer_device": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, c_int, _P, c_size_t, _P]),
     "pn2_sa_layer_msg_device": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, c_int, _P, c_size_t, _P]),
     "pn2_set_sa_consumer_ctas": (None, [c_int]),
+    # the same layer with kNN grouping
+    "pn2_sa_knn_layer_fits": (c_int, [c_int, c_int]),
+    "pn2_sa_knn_layer_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "pn2_sa_knn_layer_device": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, c_int, _P, c_size_t, _P]),
+    "pn2_set_sa_knn_path": (None, [c_int]),
     # variable-size clouds: the entries above with a (b,) int32 device array of lengths
     "pn2_fps_gather_ragged": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     "pn2_query_ball_point_ragged": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),

@@ -22,54 +22,19 @@
 //
 // One warp per query; the data points of the query's cloud are staged through shared-memory tiles
 // shared by the CTA's 8 warps (coordinates as SoA: consecutive lanes read consecutive words).
-#include <math.h>
-
-#include "pn2_common.cuh"
+//
+// knn_warp.cuh holds the same per-query algorithm as a KnnWarp routine for the overlapped kNN set-abstraction layer
+// (sa_fused.cu), and the distance and the sort this kernel uses.  This kernel keeps its own inline copy of the
+// scan and the replay: built on KnnWarp it returned the same bits but ran 4-18 % slower on the H100
+// (32 x 1024 queries x 4096 points, k = 8..128: ptxas needed up to 16 more registers), so a change to
+// either copy must be made to both (test_parity_gpu.py and test_knn_layer_gpu.py pin both to the oracle).
+#include "knn_warp.cuh"
 
 namespace pn2 {
 
 constexpr int kKnnThreads = 256;
 constexpr int kKnnWarps = kKnnThreads / 32;
 constexpr int kKnnTile = 1024;  // data points per shared-memory tile
-constexpr int kKnnMaxK = 128;
-
-// Ascending bitonic sort of 32*E 64-bit keys held E per lane (element i = register i/32 of lane i%32; E a power of 2).
-template <int E>
-__device__ __forceinline__ void bitonic_sort_u64(unsigned long long (&key)[E], int lane) {
-#pragma unroll
-    for (int size = 2; size <= 32 * E; size <<= 1) {
-#pragma unroll
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            if (stride >= 32) {  // partner in the same lane, another register
-                const int js = stride >> 5;
-#pragma unroll
-                for (int j = 0; j < E; ++j) {
-                    if ((j & js) == 0) {
-                        const bool up = (((32 * j) & size) == 0);
-                        const unsigned long long x = key[j], y = key[j | js];
-                        const bool sw = up ? (x > y) : (x < y);
-                        key[j] = sw ? y : x;
-                        key[j | js] = sw ? x : y;
-                    }
-                }
-            } else {
-#pragma unroll
-                for (int j = 0; j < E; ++j) {
-                    const int i = 32 * j + lane;
-                    const unsigned long long other = __shfl_xor_sync(kFullMask, key[j], stride);
-                    const bool up = ((i & size) == 0), lower = ((lane & stride) == 0);
-                    const bool keep_min = (up == lower);  // the lower element of an ascending pair keeps the minimum
-                    key[j] = (keep_min == (other < key[j])) ? other : key[j];
-                }
-            }
-        }
-    }
-}
-
-__device__ __forceinline__ float knn_dist(float x, float y, float z, float qx, float qy, float qz) {
-    const float dx = __fsub_rn(x, qx), dy = __fsub_rn(y, qy), dz = __fsub_rn(z, qz);
-    return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-}
 
 template <int KC>  // registers per lane that hold the list B: k <= 32 * KC
 __global__ void __launch_bounds__(kKnnThreads)

@@ -26,6 +26,10 @@
 // bit-identical; grouped_xyz is emitted in the same pass (raw gather, or centred on the query with
 // one __fsub_rn per coordinate — utils/pointnet_util.py:46), so group_point(xyz) disappears.
 //
+// kNN grouping (sample_and_group(..., knn=True)) gets the same overlap from knn_group_kernel below: the
+// consumer keeps the whole cloud in shared memory and runs knn_point's per-query warp routine
+// (knn_warp.cuh) on each centroid as it appears.
+//
 // The same kernel also serves query_ball_point + group_point(xyz) on their own (all queries known up
 // front: several CTAs per cloud, no polling) — one launch instead of grid build + grid query +
 // brute-force + group.
@@ -34,6 +38,7 @@
 
 #include <atomic>
 
+#include "knn_warp.cuh"
 #include "pn2_common.cuh"
 
 namespace pn2 {
@@ -541,6 +546,235 @@ static int sa_layer_msg(int b, int n, int m, int nscales, const float* radii, co
     return rc;
 }
 
+
+// ================================================================================================
+// kNN grouping overlapped with the sampling chain: pn2_sa_knn_layer_device.
+//
+// knn_group_kernel<KC> (k <= 32 * KC) has ctas_per_cloud CTAs per cloud.  Each copies its cloud (n points, SoA) into
+// shared memory once; warp gw of the cloud's CTAs then serves centroids gw, gw + stride, ...: it polls fps_idx as
+// ball_group_kernel does, reads the centroid's coordinates from the copy (the floats gather_point writes into
+// new_xyz), and runs knn_point's per-query routine (knn_warp.cuh) over the whole cloud in one offer.  The results are
+// knn_point's bit for bit; grouped_xyz is the gather of the result row, raw or centred with one __fsub_rn per
+// coordinate as group_point(xyz, idx) - new_xyz computes it.
+//
+// Shared memory: 12 n bytes of cloud + 24 k bytes of W buffers per warp (2k entries of value, original index and
+// current position).  The warp count per CTA follows from what the cloud leaves, up to 32: 32 warps up to k = 64 at
+// n = 8192, fewer for larger clouds; below kKgMinWarps the layer takes the sequential path.
+// ================================================================================================
+constexpr int kKgMinWarps = 4;
+constexpr int kKgMaxWarps = 32;
+// Largest k the overlapped layer takes.  Measured on the H100 (DESIGN.md §6.2.1): at k = 128 the consumer's per-query
+// cost is 3.5x the sampling step's and the layer trailed the sequential ops (0.63 against 0.54 ms at 16 x 1024 -> 512),
+// so k > 64 takes the sequential path.
+constexpr int kKgMaxK = 64;
+constexpr size_t kKgSmemMax = 200 * 1024;
+
+__host__ __device__ inline size_t kg_cloud_bytes(int n) { return ((size_t)n * 12 + 15) / 16 * 16; }
+
+// warps per consumer CTA for (n, k); 0 = the overlapped layer does not hold this shape
+static int kg_warps(int n, int k) {
+    if (n <= 0 || k <= 0 || k > kKgMaxK || k > n) return 0;
+    const size_t cloud = kg_cloud_bytes(n);
+    if (cloud >= kKgSmemMax) return 0;
+    const size_t w = (kKgSmemMax - cloud) / ((size_t)24 * k);
+    const int nw = w < (size_t)kKgMaxWarps ? (int)w : kKgMaxWarps;
+    return nw >= kKgMinWarps ? nw : 0;
+}
+
+__device__ __forceinline__ void kg_load(const float* __restrict__ s_x, int n, int pos, float& x, float& y, float& z) {
+    x = s_x[pos];
+    y = s_x[n + pos];
+    z = s_x[2 * n + pos];
+}
+
+template <int KC>
+__global__ void __launch_bounds__(kKgMaxWarps * 32, 1)
+knn_group_kernel(int n, int m, int k, const float* __restrict__ xyz, const int* q_idx, int* __restrict__ idx,
+                 float* __restrict__ dist, float* __restrict__ grouped, int center, int ctas_per_cloud) {
+    extern __shared__ __align__(16) unsigned char s_raw[];
+    float* __restrict__ s_x = reinterpret_cast<float*>(s_raw);  // [3][n]: x, then y, then z
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
+    float* __restrict__ wv = reinterpret_cast<float*>(s_raw + kg_cloud_bytes(n)) + (size_t)warp * 6 * k;
+    int* __restrict__ wo = reinterpret_cast<int*>(wv + 2 * k);
+    int* __restrict__ wp = wo + 2 * k;
+    const int cloud = blockIdx.x / ctas_per_cloud, part = blockIdx.x - cloud * ctas_per_cloud;
+    const float* __restrict__ pts = xyz + (size_t)cloud * n * 3;
+    for (int p = tid; p < 3 * n; p += blockDim.x) {  // coalesced reads, transposed into SoA
+        const int pt = p / 3, c = p - 3 * pt;
+        s_x[c * n + pt] = __ldg(pts + p);
+    }
+    __syncthreads();
+
+    const int qstride = ctas_per_cloud * nwarps;
+    const long long t_start = clock64();
+    for (int q = part * nwarps + warp; q < m; q += qstride) {
+        // wait for the sampling kernel to publish centroid q (its index turns non-negative)
+        int qi = 0;
+        if (lane == 0) {
+            const int* src = q_idx + (size_t)cloud * m + q;
+            qi = ld_volatile_s32(src);
+            unsigned backoff = 32;
+            while (qi < 0) {
+                __nanosleep(backoff);
+                if (backoff < 256) backoff <<= 1;
+                qi = ld_volatile_s32(src);
+                if (clock64() - t_start > 4000000000ll) break;  // ~2 s: never hang the device on a lost producer
+            }
+        }
+        qi = __shfl_sync(kFullMask, qi, 0);
+        const size_t row = ((size_t)cloud * m + q) * k;
+        int* __restrict__ orow = idx + row;
+        if (qi < 0 || qi >= n) {  // producer lost / corrupt index: flag the row instead of faulting
+            for (int e = lane; e < k; e += 32) orow[e] = -1;
+            continue;
+        }
+        float qx, qy, qz;
+        kg_load(s_x, n, qi, qx, qy, qz);
+        KnnWarp<KC> w(k, lane, qx, qy, qz);
+        w.fill_a(wv, wo, k, [&](int pos, float& x, float& y, float& z) { kg_load(s_x, n, pos, x, y, z); });
+        w.offer(s_x, s_x + n, s_x + 2 * n, n, 0);
+        float* __restrict__ drow = dist ? dist + row : nullptr;
+        w.finish(wv, wo, wp, k, [&](int e, float v, int i) {
+            orow[e] = i;
+            if (drow) drow[e] = v;
+        });
+        if (grouped) {
+            __syncwarp();  // the replay's columns were written by lane 0
+            float* __restrict__ grow = grouped + row * 3;
+            for (int e = lane; e < k; e += 32) {
+                float x, y, z;
+                kg_load(s_x, n, orow[e], x, y, z);
+                // centred: xyz[idx] - new_xyz, one rounding per coordinate; a raw copy otherwise (x - 0 would
+                // canonicalise a NaN payload, which a gather never does)
+                grow[3 * e + 0] = center ? __fsub_rn(x, qx) : x;
+                grow[3 * e + 1] = center ? __fsub_rn(y, qy) : y;
+                grow[3 * e + 2] = center ? __fsub_rn(z, qz) : z;
+            }
+        }
+        __syncwarp();  // W is reused by this warp's next query
+    }
+    // completion of this grid must imply completion of the sampling grid it overlaps (see ball_group_kernel)
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+}
+
+static int launch_knn_group(int b, int n, int m, int k, const float* xyz, const int* q_idx, int* idx, float* dist, float* grouped,
+                            int center, int ctas_per_cloud, cudaStream_t st) {
+    static std::atomic<long long> max_dyn_once[2][64];  // [KC instance][device]: 0 = not asked yet
+    const int nw = kg_warps(n, k);
+    if (nw == 0) return (int)cudaErrorInvalidValue;
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return (int)e;
+    if (dev < 0 || dev >= 64) return (int)cudaErrorInvalidDevice;
+    const int kc = k <= 32 ? 0 : 1;
+    auto kern = kc == 0 ? knn_group_kernel<1> : knn_group_kernel<2>;
+    long long max_dyn = max_dyn_once[kc][dev].load(std::memory_order_acquire);
+    if (max_dyn == 0) {
+        int optin = 0;
+        cudaFuncAttributes fa;
+        e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+        if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, kern);
+        if (e != cudaSuccess) return (int)e;
+        max_dyn = (long long)optin - (long long)fa.sharedSizeBytes;
+        if (max_dyn < (long long)kKgSmemMax) return (int)cudaErrorInvalidValue;
+        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_dyn);
+        if (e != cudaSuccess) return (int)e;
+        max_dyn_once[kc][dev].store(max_dyn, std::memory_order_release);
+    }
+    // an SM to itself, as for the ball query: every byte of shared memory rules out co-residency with a sampling CTA
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)b * (unsigned)ctas_per_cloud, 1, 1);
+    cfg.blockDim = dim3((unsigned)nw * 32, 1, 1);
+    cfg.dynamicSmemBytes = (size_t)max_dyn;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    e = cudaLaunchKernelEx(&cfg, kern, n, m, k, xyz, q_idx, idx, dist, grouped, center, ctas_per_cloud);
+    count_launch();
+    if (e != cudaSuccess) return (int)e;
+    return (int)cudaGetLastError();
+}
+
+// SMs the sampling chain leaves per cloud (b sampling CTAs, one SM each)
+static int knn_room(int b) {
+    const int sms = num_sms();
+    return b < sms ? (sms - b) / b : 0;
+}
+
+// Consumer CTAs per cloud: every SM the sampling chain leaves, but no more CTAs than give each warp one centroid.
+// pn2_set_sa_consumer_ctas overrides (0 = automatic), within the same bounds.
+static int knn_consumer_ctas(int b, int m, int k, int n) {
+    const int room = knn_room(b), nw = kg_warps(n, k);
+    int r = g_sa_consumer_ctas.load(std::memory_order_relaxed);
+    if (r <= 0) r = room;
+    if (r > room) r = room;
+    const int rmax = (m + nw - 1) / nw;
+    if (r > rmax) r = rmax;
+    return r < 1 ? 1 : r;
+}
+
+// pn2_set_sa_knn_path: 0 = the rule below, 1 = overlapped wherever it can run, 2 = sequential (measurement)
+static std::atomic<int> g_sa_knn_path{0};
+
+// Overlapped or sequential.  The overlapped layer can run when the sampling is one CTA per cloud, k <= 64, the cloud
+// and the W buffers fit in shared memory (kg_warps) and at least one idle SM is left per cloud.  Whether it WINS is a
+// cost comparison, in units of one sampling step t (the sampling takes m t either way).  Let C = c / t, c the SM time
+// of one kNN query, r the consumer CTAs per cloud, nw their warps, S the SMs.  Each consumer warp serves
+// ceil(m / (r nw)) centroids and nw warps share an SM, so the consumers need about ceil(m / (r nw)) nw C; the
+// sequential ops need m for the sampling plus b m C / S for knn_point on every SM:
+//     overlapped  <=>  ceil(m / (r nw)) nw C <= m + b m C / S.
+// C was measured on the H100 (DESIGN.md §6.2.1: knn_point against the sampling kernel, uniform and duplicate-heavy
+// clouds): up to 4.0 at k = 8, 8.2 at k = 32 and 16.6 at k = 64 for N 4096, 20.9 at k = 64 for N 1024.
+// max(4, k (0.26 + 80 / n)) bounds those.  At N 4096 -> 1024 on 132 SMs it overlaps k = 32 for b <= 33 (3 or more
+// consumer CTAs per cloud) and k = 64 for b <= 26.
+static bool knn_overlapped(int b, int n, int m, int k) {
+    const int mode = g_sa_knn_path.load(std::memory_order_relaxed);
+    if (mode == 2 || kg_warps(n, k) == 0 || knn_room(b) < 1 || !fps_single_cta(b, n)) return false;
+    if (mode == 1) return true;
+    const double S = num_sms(), r = knn_consumer_ctas(b, m, k, n), nw = kg_warps(n, k);
+    const double C = fmax(4.0, k * (0.26 + 80.0 / n));
+    const double per_warp = ceil((double)m / (r * nw));
+    return per_warp * nw * C <= (double)m + (double)b * m * C / S;
+}
+
+static size_t knn_val_bytes(int b, int m, int k) { return (size_t)b * (size_t)m * (size_t)k * sizeof(float); }
+
+static int sa_knn_layer(int b, int n, int m, int k, const float* xyz, int* fps_idx, float* new_xyz, int* idx, float* dist,
+                        float* grouped_xyz, int center, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+    if (b < 0 || n <= 0 || m < 0 || k <= 0 || k > kKnnMaxK || k > n) return (int)cudaErrorInvalidValue;
+    if (b == 0 || m == 0) return 0;
+    if (!xyz || !fps_idx || !new_xyz || !idx || b > 65535) return (int)cudaErrorInvalidValue;
+    if (knn_overlapped(b, n, m, k)) {
+        int rc = fps_dispatch(b, n, m, xyz, nullptr, nullptr, fps_idx, new_xyz, /*sentinel=*/1, st);
+        if (rc == 0)
+            rc = launch_knn_group(b, n, m, k, xyz, fps_idx, idx, dist, grouped_xyz, center, knn_consumer_ctas(b, m, k, n), st);
+        return rc;
+    }
+    // sequential path: the sampling, knn_point and the xyz grouping one after the other
+    const size_t fps_b = align256(pn2_fps_scratch_bytes(b, n));
+    char* ws = static_cast<char*>(workspace);
+    float* temp = nullptr;
+    float* val = dist;
+    if (fps_b) {
+        if (!ws || workspace_bytes < fps_b) return (int)cudaErrorInvalidValue;
+        temp = reinterpret_cast<float*>(ws);
+    }
+    if (!val) {  // knn_point writes the distances somewhere
+        if (!ws || workspace_bytes < fps_b + knn_val_bytes(b, m, k)) return (int)cudaErrorInvalidValue;
+        val = reinterpret_cast<float*>(ws + fps_b);
+    }
+    void* stream = static_cast<void*>(st);
+    int rc = fps_dispatch(b, n, m, xyz, nullptr, temp, fps_idx, new_xyz, 0, st);
+    if (rc == 0) rc = pn2_knn_point(b, n, m, k, xyz, new_xyz, val, idx, stream);
+    if (rc == 0 && grouped_xyz)
+        rc = center ? pn2_group_concat(b, n, 0, m, k, xyz, new_xyz, nullptr, idx, 1, grouped_xyz, nullptr, stream)
+                    : pn2_group_point(b, n, 3, m, k, xyz, idx, grouped_xyz, stream);
+    return rc;
+}
+
 }  // namespace pn2
 
 extern "C" {
@@ -593,6 +827,24 @@ int pn2_sa_layer_device(int b, int n, int m, float radius, int nsample, const fl
     return pn2_sa_layer_device_ragged(b, n, m, radius, nsample, xyz, nullptr, fps_idx, new_xyz, idx, pts_cnt, grouped_xyz, center,
                                       workspace, workspace_bytes, stream);
 }
+
+int pn2_sa_knn_layer_fits(int n, int k) { return pn2::kg_warps(n, k) > 0 ? 1 : 0; }
+
+size_t pn2_sa_knn_layer_workspace_bytes(int b, int n, int m, int k) {
+    if (b <= 0 || n <= 0 || m <= 0 || k <= 0 || k > pn2::kKnnMaxK || k > n) return 0;
+    // the overlapped path needs none; the sequential one FPS scratch for clouds beyond the cluster capacity +
+    // knn_point's distances when the caller does not want them
+    if (pn2::knn_overlapped(b, n, m, k)) return 0;
+    return pn2::align256(pn2_fps_scratch_bytes(b, n)) + pn2::align256(pn2::knn_val_bytes(b, m, k));
+}
+
+int pn2_sa_knn_layer_device(int b, int n, int m, int k, const float* xyz, int* fps_idx, float* new_xyz, int* idx, float* dist,
+                            float* grouped_xyz, int center, void* workspace, size_t workspace_bytes, void* stream) {
+    return pn2::sa_knn_layer(b, n, m, k, xyz, fps_idx, new_xyz, idx, dist, grouped_xyz, center, workspace, workspace_bytes,
+                             pn2::as_stream(stream));
+}
+
+void pn2_set_sa_knn_path(int mode) { pn2::g_sa_knn_path.store(mode >= 0 && mode <= 2 ? mode : 0, std::memory_order_relaxed); }
 
 void pn2_set_sa_consumer_ctas(int ctas_per_cloud) { pn2::g_sa_consumer_ctas.store(ctas_per_cloud, std::memory_order_relaxed); }
 

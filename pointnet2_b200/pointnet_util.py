@@ -26,7 +26,7 @@ from . import _lib, layers
 from ._tensor import DTYPE_CODES, FEATURE_DTYPES, device_lengths, on_device, ptr, require_cuda, same_device, stream_ptr
 from .tf_grouping import group_point, group_point_grad, knn_point, query_ball_point
 from .tf_interpolate import fp_interpolate_concat, three_interpolate, three_nn, three_nn_interpolate
-from .sa_layer import sample_group, sample_group_msg
+from .sa_layer import KNN_MAX_K, sample_group, sample_group_msg, sample_knn
 from .tf_sampling import farthest_point_sample, farthest_point_sample_and_gather, gather_point
 
 
@@ -122,13 +122,24 @@ def sample_and_group(npoint, radius, nsample, xyz, points, knn=False, use_xyz=Tr
         n.  Sampling and the ball query then see each cloud alone; every index is below its length, so the grouping
         never reads the padding.  Not with knn (ValueError).
 
-    ``fused=True`` uses the overlapped sampling+grouping layer (sa_layer.sample_group) and the
-    single-pass concat kernel; ``fused=False`` issues the reference's op sequence one by one.  Both
+    ``fused=True`` uses the overlapped sampling+grouping layer (sa_layer.sample_group, or sa_layer.sample_knn for
+    knn with nsample <= 128) and the single-pass concat kernel; ``fused=False`` issues the reference's op sequence one by one.  Both
     return identical values.
     """
     if knn:
         _no_lengths_with(lengths, "knn grouping")
     no_grad_xyz = not xyz.requires_grad
+    if fused and no_grad_xyz and knn and 0 < int(nsample) <= min(KNN_MAX_K, xyz.shape[1]):
+        # one call: FPS + gather + kNN (+ centred grouped xyz when they are the whole output), the kNN grouping
+        # overlapping the sampling chain
+        need_g = points is None or not use_xyz
+        _, new_xyz, idx, _, grouped_xyz = sample_knn(npoint, nsample, xyz, center=True, want_grouped=need_g)
+        if points is None:
+            return new_xyz, grouped_xyz, idx, grouped_xyz
+        if not use_xyz:
+            return new_xyz, group_point(points, idx), idx, grouped_xyz
+        new_points, grouped_xyz = group_and_concat(xyz, new_xyz, points, idx, xyz_first=True)
+        return new_xyz, new_points, idx, grouped_xyz
     if fused and no_grad_xyz and not knn:
         # one call: FPS + gather + ball query (+ centred grouped xyz when they are the whole output)
         need_g = points is None or not use_xyz
@@ -255,8 +266,11 @@ def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp=None, mlp2=None
         else:
             if knn:
                 _no_lengths_with(lengths, "knn grouping")
-                _, new_xyz = farthest_point_sample_and_gather(npoint, xyz)
-                _, idx = knn_point(nsample, xyz, new_xyz)
+                if 0 < int(nsample) <= min(KNN_MAX_K, xyz.shape[1]):
+                    _, new_xyz, idx, _, _ = sample_knn(npoint, nsample, xyz, center=True, want_grouped=False)
+                else:
+                    _, new_xyz = farthest_point_sample_and_gather(npoint, xyz)
+                    _, idx = knn_point(nsample, xyz, new_xyz)
             else:
                 _, new_xyz, idx, _, _ = sample_group(npoint, radius, nsample, xyz, center=True, want_grouped=False,
                                                      lengths=lengths)

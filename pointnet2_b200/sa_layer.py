@@ -6,6 +6,10 @@
 grouping run as a programmatically dependent grid on the SMs the sampling chain leaves idle.  The
 results are bit-identical to the four separate ops.
 
+``sample_knn`` is the kNN-grouping form (sample_and_group(..., knn=True)): FPS + gather_point + knn_point +
+group_point(xyz) in ONE C-ABI call, ``pn2_sa_knn_layer_device``, whose kNN grouping overlaps the sampling chain in
+the same way; bit-identical to the separate ops.
+
 ``ball_group`` is the same consumer kernel on its own (queries known up front): query_ball_point +
 group_point(xyz) in one launch.
 
@@ -118,6 +122,50 @@ def sample_group_msg(npoint: int, radius_list, nsample_list, xyz: torch.Tensor, 
                                                     stream_ptr(dev))
     _lib.check(rc, "pn2_sa_layer_msg_device")
     return fps_idx, new_xyz, idx, cnt, grouped
+
+
+KNN_MAX_K = 128  # pn2_sa_knn_layer_device's (and pn2_knn_point's) largest k
+
+
+def sample_knn(npoint: int, k: int, xyz: torch.Tensor, center: bool = True, want_grouped: bool = True,
+               want_dist: bool = False):
+    """FPS + gather_point + knn_point(k, xyz, new_xyz) + group_point(xyz) [- new_xyz] in one call.
+
+    Returns (fps_idx (b,npoint) i32, new_xyz (b,npoint,3), idx (b,npoint,k) i32, dist (b,npoint,k) f32 or None,
+    grouped_xyz (b,npoint,k,3) or None).  ``dist`` is knn_point's ``val`` (squared distances, ascending);
+    ``center=True`` subtracts the centroid.  Bit-identical to the separate ops; no gradients.  Needs
+    1 <= k <= min(n, 128) (ValueError otherwise: larger k keep knn_point's composite path)."""
+    npoint, k = int(npoint), int(k)
+    if npoint <= 0:
+        raise ValueError("FarthestPointSample expects positive npoint")
+    if k <= 0:
+        raise ValueError("knn_point expects positive k")
+    xyz = require_cuda(xyz, "xyz", torch.float32)
+    if xyz.dim() != 3 or xyz.shape[2] != 3:
+        raise ValueError(f"expected (batch_size, ndataset, 3) xyz shape, got {tuple(xyz.shape)}")
+    b, n, _ = xyz.shape
+    if n <= 0:
+        raise ValueError("FarthestPointSample expects at least one point per batch entry")
+    if k > n:
+        raise ValueError(f"knn_point expects k <= ndataset (the reference slices k columns of an n-column matrix), got k={k}, n={n}")
+    if k > KNN_MAX_K:
+        raise ValueError(f"sample_knn expects k <= {KNN_MAX_K}, got k={k}")
+    dev = xyz.device
+    fps_idx = torch.empty((b, npoint), dtype=torch.int32, device=dev)
+    new_xyz = torch.empty((b, npoint, 3), dtype=torch.float32, device=dev)
+    idx = torch.empty((b, npoint, k), dtype=torch.int32, device=dev)
+    dist = torch.empty((b, npoint, k), dtype=torch.float32, device=dev) if want_dist else None
+    grouped = torch.empty((b, npoint, k, 3), dtype=torch.float32, device=dev) if want_grouped else None
+    if b == 0:
+        return fps_idx, new_xyz, idx, dist, grouped
+    lib = _lib.load()
+    with on_device(xyz):
+        wsb = int(lib.pn2_sa_knn_layer_workspace_bytes(b, n, npoint, k))
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev) if wsb else None
+        rc = lib.pn2_sa_knn_layer_device(b, n, npoint, k, ptr(xyz.detach()), ptr(fps_idx), ptr(new_xyz), ptr(idx), ptr(dist),
+                                         ptr(grouped), 1 if center else 0, ptr(ws), wsb, stream_ptr(dev))
+    _lib.check(rc, "pn2_sa_knn_layer_device")
+    return fps_idx, new_xyz, idx, dist, grouped
 
 
 def ball_group(radius: float, nsample: int, xyz1: torch.Tensor, xyz2: torch.Tensor, center: bool = True,
