@@ -644,6 +644,26 @@ size_t pn2_sa_layer_workspace_bytes(int b, int n, int m, int nsample);
 int pn2_sa_layer_host(int b, int n, int m, float radius, int nsample, const float* h_xyz,
                       float* h_new_xyz, int* h_idx, int* h_pts_cnt, float* h_grouped_xyz,
                       void* workspace, size_t workspace_bytes, void* stream);
+/* The same layer on a batch of variable-size clouds, packed on the host (DESIGN.md §6.8).
+ * h_xyz is PACKED: cloud i is rows [off_i, off_i + h_lengths[i]) of a (sum of lengths, 3) float32 host array, off
+ * the exclusive prefix sum of the lengths, no padding.  n is the capacity: every length must satisfy
+ * 1 <= h_lengths[i] <= n, otherwise cudaErrorInvalidValue before anything is enqueued (no clamping).  The outputs
+ * and their NULL rules are pn2_sa_layer_host's; cloud i's are bit for bit what pn2_sa_layer_host returns for that
+ * cloud alone with n = h_lengths[i].
+ * h_lengths is read synchronously during the call (validation, copy size and row stride) and again by the
+ * asynchronous copy that carries it to the device; h_xyz is read only by the asynchronous copy.  Keep both
+ * unchanged until the stream has passed the copies.
+ * Enqueued on `stream`: one copy of the b lengths, one copy of the 12 * sum(lengths) packed bytes, one kernel that
+ * writes the real rows into a padded (b, n_run, 3) device batch, n_run = max(lengths) (padding rows are neither
+ * written nor read), pn2_sa_layer_device_ragged(b, n_run, ...), then the copies back.  The sampling plan and the
+ * ball-query path are therefore chosen for the longest cloud of the batch, not for the capacity.  Nothing is
+ * synchronised.  `workspace`: a 256-byte-aligned device buffer of at least
+ * pn2_sa_layer_host_ragged_workspace_bytes(b,n,m,nsample) bytes (cudaErrorInvalidValue when smaller,
+ * cudaErrorMisalignedAddress when misaligned). */
+size_t pn2_sa_layer_host_ragged_workspace_bytes(int b, int n, int m, int nsample);
+int pn2_sa_layer_host_ragged(int b, int n, int m, float radius, int nsample, const float* h_xyz,
+                             const int* h_lengths, float* h_new_xyz, int* h_idx, int* h_pts_cnt,
+                             float* h_grouped_xyz, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- introspection ------------------------------------------------------------------------- */
 int pn2_api_version(void);

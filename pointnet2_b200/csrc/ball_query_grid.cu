@@ -287,6 +287,9 @@ int query_ball_point_ws(int b, int n, int m, float radius, int nsample, const fl
     return query_ball_point_prebuilt(b, n, m, radius, nsample, xyz1, lengths, xyz2, idx, pts_cnt, workspace, workspace_bytes, st);
 }
 
+// the largest pn2_query_ball_point_workspace_bytes(b, k) over k <= n (0 outside [kGridMinN, kGridMaxN], growing inside)
+size_t query_ball_point_workspace_bound(int b, int n) { return pn2_query_ball_point_workspace_bytes(b, n < kGridMaxN ? n : kGridMaxN); }
+
 }  // namespace pn2
 
 extern "C" {

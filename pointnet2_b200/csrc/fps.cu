@@ -1209,6 +1209,11 @@ size_t fps_scratch_bytes(int b, int n) {
     return plan_fps(b, n).cluster == 0 ? sizeof(float) * (size_t)(b < 32 ? b : 32) * (size_t)n : 0;
 }
 
+size_t fps_scratch_bound(int b, int n) {
+    if (b <= 0 || n <= 0) return 0;
+    return sizeof(float) * (size_t)(b < 32 ? b : 32) * (size_t)n;  // fps_scratch_bytes(b, k) for every k <= n is at most this
+}
+
 int fps_dispatch(int b, int n, int m, const float* inp, const int* lengths, float* temp, int* out, float* new_xyz,
                  int sentinel, cudaStream_t st) {
     if (b < 0 || n <= 0 || m < 0) return (int)cudaErrorInvalidValue;

@@ -486,6 +486,10 @@ int fps_dispatch(int b, int n, int m, const float* inp, const int* lengths, floa
                  int sentinel, cudaStream_t st);
 bool fps_single_cta(int b, int n);
 size_t fps_scratch_bytes(int b, int n);
+// upper bounds of fps_scratch_bytes(b, k) and pn2_query_ball_point_workspace_bytes(b, k) over every k <= n: a caller
+// that picks the row stride per call (the ragged host layer) sizes its workspace once for the largest stride
+size_t fps_scratch_bound(int b, int n);
+size_t query_ball_point_workspace_bound(int b, int n);
 
 // ordered-sum scatter through an inverse index (scatter_det.cu), shared by three_interpolate's gradient and the
 // group_point / gather_point gradients: dst[b, i, :] = sum over the entries e with idx[b, e] == i, e ascending, of

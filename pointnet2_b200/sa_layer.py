@@ -223,6 +223,10 @@ class SetAbstractionDevice:
     ``submit`` never blocks; the tensors ``collect`` returns belong to the slot and stay valid until
     the slot is reused (``depth`` submits later).  ``collect`` makes the caller's current stream wait
     for the batch (no host synchronisation unless ``sync=True``).
+
+    ``submit(xyz, lengths)`` takes a padded batch of variable-size clouds (``lengths`` as for ``sample_group``:
+    a device tensor is never read back, so ``enqueue`` with one can be captured in a CUDA graph and replayed
+    with new lengths written into it).
     """
 
     def __init__(self, b, n, npoint, radius, nsample, depth: int = 2, center: bool = False, want_grouped: bool = True,
@@ -245,7 +249,7 @@ class SetAbstractionDevice:
                 idx=torch.empty((self.b, self.m, self.s), dtype=torch.int32, device=dev),
                 pts_cnt=torch.empty((self.b, self.m), dtype=torch.int32, device=dev),
                 grouped=torch.empty((self.b, self.m, self.s, 3), dtype=torch.float32, device=dev) if want_grouped else None,
-                ws=torch.empty(wsb, dtype=torch.uint8, device=dev) if wsb else None, wsb=wsb, xyz=None,
+                ws=torch.empty(wsb, dtype=torch.uint8, device=dev) if wsb else None, wsb=wsb, xyz=None, lengths=None,
                 stream=torch.cuda.Stream(dev), done=torch.cuda.Event()))
         self._next = 0
         self._inflight: collections.deque[int] = collections.deque()
@@ -260,26 +264,34 @@ class SetAbstractionDevice:
     def full(self) -> bool:
         return len(self._inflight) == len(self.slots)
 
-    def enqueue(self, slot: dict, xyz: torch.Tensor, stream: torch.cuda.Stream) -> None:
-        """Issue the layer for ``xyz`` into ``slot``'s buffers on ``stream`` (capturable in a CUDA graph)."""
+    def enqueue(self, slot: dict, xyz: torch.Tensor, stream: torch.cuda.Stream, lengths: torch.Tensor | None = None) -> None:
+        """Issue the layer for ``xyz`` into ``slot``'s buffers on ``stream`` (capturable in a CUDA graph).
+        ``lengths``: None, or the (b,) int32 device tensor of per-cloud lengths."""
         with torch.cuda.device(self.device):
-            rc = self.lib.pn2_sa_layer_device(self.b, self.n, self.m, self.radius, self.s, ptr(xyz), ptr(slot["fps_idx"]),
-                                              ptr(slot["new_xyz"]), ptr(slot["idx"]), ptr(slot["pts_cnt"]), ptr(slot["grouped"]),
-                                              1 if self.center else 0, ptr(slot["ws"]), slot["wsb"], stream.cuda_stream)
+            if lengths is None:
+                rc = self.lib.pn2_sa_layer_device(self.b, self.n, self.m, self.radius, self.s, ptr(xyz), ptr(slot["fps_idx"]),
+                                                  ptr(slot["new_xyz"]), ptr(slot["idx"]), ptr(slot["pts_cnt"]), ptr(slot["grouped"]),
+                                                  1 if self.center else 0, ptr(slot["ws"]), slot["wsb"], stream.cuda_stream)
+            else:
+                rc = self.lib.pn2_sa_layer_device_ragged(self.b, self.n, self.m, self.radius, self.s, ptr(xyz), ptr(lengths),
+                                                         ptr(slot["fps_idx"]), ptr(slot["new_xyz"]), ptr(slot["idx"]),
+                                                         ptr(slot["pts_cnt"]), ptr(slot["grouped"]), 1 if self.center else 0,
+                                                         ptr(slot["ws"]), slot["wsb"], stream.cuda_stream)
         _lib.check(rc, "pn2_sa_layer_device")
 
-    def submit(self, xyz: torch.Tensor) -> int:
+    def submit(self, xyz: torch.Tensor, lengths=None) -> int:
         if self.full():
             raise RuntimeError("SetAbstractionDevice is full: collect() the oldest batch first")
         xyz = require_cuda(xyz, "xyz", torch.float32)
         if tuple(xyz.shape) != (self.b, self.n, 3):
             raise ValueError(f"expected xyz of shape {(self.b, self.n, 3)}, got {tuple(xyz.shape)}")
+        lens = device_lengths(lengths, self.b, self.n, self.device, "SetAbstractionDevice")
         i = self._next
         slot = self.slots[i]
-        slot["xyz"] = xyz  # keep the input alive while the kernels read it
+        slot["xyz"], slot["lengths"] = xyz, lens  # keep the inputs alive while the kernels read them
         st = slot["stream"]
-        st.wait_stream(torch.cuda.current_stream(self.device))  # xyz was produced on the caller's stream
-        self.enqueue(slot, xyz, st)
+        st.wait_stream(torch.cuda.current_stream(self.device))  # xyz (and lengths) were produced on the caller's stream
+        self.enqueue(slot, xyz, st, lens)
         slot["done"].record(st)
         self._inflight.append(i)
         self._next = (i + 1) % len(self.slots)

@@ -33,7 +33,7 @@ SHOW = ["fps_cta_kernel<16, 256, 0, false>", "fps_cta_kernel<16, 256, 1, false>"
         "scene_merge_kernel<__half>", "crop_attempt_kernel", "crop_select_kernel", "shape_batch_kernel",
         "vscan_ray_kernel", "vscan_cell_kernel", "vscan_point_kernel", "vscan_select_kernel",
         "render_zrange_kernel", "render_splat_kernel<false>", "render_splat_kernel<true>", "render_resolve_kernel",
-        "project_stats_kernel", "project_points_kernel"]
+        "project_stats_kernel", "project_points_kernel", "ragged_unpack_kernel"]
 
 
 def demangle(names):
