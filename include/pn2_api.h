@@ -664,6 +664,33 @@ size_t pn2_sa_layer_host_ragged_workspace_bytes(int b, int n, int m, int nsample
 int pn2_sa_layer_host_ragged(int b, int n, int m, float radius, int nsample, const float* h_xyz,
                              const int* h_lengths, float* h_new_xyz, int* h_idx, int* h_pts_cnt,
                              float* h_grouped_xyz, void* workspace, size_t workspace_bytes, void* stream);
+/* The multi-scale layer (pointnet_sa_module_msg, utils/pointnet_util.py:156-196) on HOST buffers (DESIGN.md §6.8):
+ * ONE farthest_point_sample + gather_point for every scale, then query_ball_point + group_point(xyz) per scale,
+ * through pn2_sa_layer_msg_device.  radii, nsamples, h_idx, h_pts_cnt and h_grouped_xyz are HOST arrays of nscales
+ * (1..16) entries, as for pn2_sa_layer_msg_device: h_new_xyz (b,m,3), every h_idx[k] (b,m,nsamples[k]) and
+ * h_pts_cnt[k] (b,m) are required; h_grouped_xyz, or any entry of it, may be NULL, and such a scale's grouped_xyz
+ * (b,m,nsamples[k],3; NOT centred) is neither computed nor copied back.  Scale k's outputs are bit for bit those of
+ * pn2_sa_layer_host with (radii[k], nsamples[k]) alone: the sampling is shared.
+ * Enqueued on `stream`: one copy of the 12*b*n input bytes, pn2_sa_layer_msg_device(center = 0), then the copies
+ * back: new_xyz, then each scale's idx, pts_cnt and (when wanted) grouped_xyz.  Nothing is synchronised.
+ * A bad count or shape, nscales outside 1..16, a radius that is not positive (or NaN), a non-positive nsample, a NULL
+ * required pointer or a workspace smaller than pn2_sa_layer_msg_host_workspace_bytes(b,n,m,nscales,nsamples) returns
+ * cudaErrorInvalidValue, a workspace not 256-byte aligned cudaErrorMisalignedAddress, before any device call.  The
+ * workspace size is 0 for invalid arguments. */
+size_t pn2_sa_layer_msg_host_workspace_bytes(int b, int n, int m, int nscales, const int* nsamples);
+int pn2_sa_layer_msg_host(int b, int n, int m, int nscales, const float* radii, const int* nsamples,
+                          const float* h_xyz, float* h_new_xyz, int* const* h_idx, int* const* h_pts_cnt,
+                          float* const* h_grouped_xyz, void* workspace, size_t workspace_bytes, void* stream);
+/* The multi-scale layer on packed variable-size clouds: h_xyz and h_lengths as for pn2_sa_layer_host_ragged (every
+ * length checked on the host, 1 <= h_lengths[i] <= n, before anything is enqueued), everything else as for
+ * pn2_sa_layer_msg_host.  Enqueued: the lengths copy, one copy of the 12 * sum(lengths) packed bytes, the unpack
+ * kernel at the row stride n_run = max(lengths), pn2_sa_layer_msg_device_ragged(b, n_run, ...), then the copies back.
+ * Cloud i's outputs are bit for bit what pn2_sa_layer_msg_host returns for that cloud alone with n = h_lengths[i]. */
+size_t pn2_sa_layer_msg_host_ragged_workspace_bytes(int b, int n, int m, int nscales, const int* nsamples);
+int pn2_sa_layer_msg_host_ragged(int b, int n, int m, int nscales, const float* radii, const int* nsamples,
+                                 const float* h_xyz, const int* h_lengths, float* h_new_xyz, int* const* h_idx,
+                                 int* const* h_pts_cnt, float* const* h_grouped_xyz, void* workspace,
+                                 size_t workspace_bytes, void* stream);
 
 /* ---- introspection ------------------------------------------------------------------------- */
 int pn2_api_version(void);

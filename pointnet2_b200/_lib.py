@@ -125,6 +125,10 @@ _SIGNATURES = {
     "pn2_sa_layer_host": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_sa_layer_host_ragged_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "pn2_sa_layer_host_ragged": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    "pn2_sa_layer_msg_host_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, _P]),
+    "pn2_sa_layer_msg_host": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
+    "pn2_sa_layer_msg_host_ragged_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, _P]),
+    "pn2_sa_layer_msg_host_ragged": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_api_version": (c_int, []),
     "pn2_error_string": (ctypes.c_char_p, [c_int]),
     "pn2_launch_count": (c_ulonglong, []),

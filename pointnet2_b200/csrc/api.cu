@@ -7,12 +7,16 @@ unsigned long long g_launch_count = 0;
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 struct SaLayout {
-    size_t lengths, packed, xyz, new_xyz, fps_idx, idx, cnt, grouped, dev_ws, dev_ws_bytes, total;
+    size_t lengths, packed, xyz, new_xyz, fps_idx, dev_ws, dev_ws_bytes, total;
+    size_t idx[kSaMaxScales], cnt[kSaMaxScales], grouped[kSaMaxScales];
 };
 
+// The workspace of the host-buffer layer with nscales ball-query scales (1 <= nscales <= kSaMaxScales, every
+// nsamples[k] > 0): the input batch, new_xyz, fps_idx, then each scale's idx, pts_cnt and grouped_xyz in turn, then
+// the device layer's scratch, which does not depend on nsample.  With one scale this is the single-scale layout.
 // ragged: the lengths and the packed staging area come first, and the device layer's workspace is sized for every
-// row stride up to n, since the ragged entry runs the layer at the stride of each batch's longest cloud
-static SaLayout sa_layout(int b, int n, int m, int nsample, bool ragged = false) {
+// row stride up to n, since the ragged entries run the layer at the stride of each batch's longest cloud
+static SaLayout sa_layout(int b, int n, int m, int nscales, const int* nsamples, bool ragged) {
     SaLayout L;
     size_t off = 0;
     L.lengths = off;
@@ -22,29 +26,48 @@ static SaLayout sa_layout(int b, int n, int m, int nsample, bool ragged = false)
     L.xyz = off;     off = align_up(off + sizeof(float) * (size_t)b * n * 3, 256);
     L.new_xyz = off; off = align_up(off + sizeof(float) * (size_t)b * m * 3, 256);
     L.fps_idx = off; off = align_up(off + sizeof(int) * (size_t)b * m, 256);  // also the channel between the two overlapped kernels
-    L.idx = off;     off = align_up(off + sizeof(int) * (size_t)b * m * nsample, 256);
-    L.cnt = off;     off = align_up(off + sizeof(int) * (size_t)b * m, 256);
-    L.grouped = off; off = align_up(off + sizeof(float) * (size_t)b * m * nsample * 3, 256);
+    for (int k = 0; k < nscales; ++k) {
+        const size_t s = (size_t)nsamples[k];
+        L.idx[k] = off;     off = align_up(off + sizeof(int) * (size_t)b * m * s, 256);
+        L.cnt[k] = off;     off = align_up(off + sizeof(int) * (size_t)b * m, 256);
+        L.grouped[k] = off; off = align_up(off + sizeof(float) * (size_t)b * m * s * 3, 256);
+    }
     L.dev_ws_bytes = ragged ? align_up(fps_scratch_bound(b, n), 256) + align_up(query_ball_point_workspace_bound(b, n), 256)
-                            : pn2_sa_layer_device_workspace_bytes(b, n, m, nsample);  // 0 on the overlapped path
+                            : pn2_sa_layer_device_workspace_bytes(b, n, m, nsamples[0]);  // 0 on the overlapped path
     L.dev_ws = off;  off = align_up(off + L.dev_ws_bytes, 256);
     L.total = off;
     return L;
 }
 
-// The D2H copies of the host-buffer layer: each output whose host pointer is not NULL.
-static int copy_out(int b, int m, int nsample, const char* ws, const SaLayout& L, float* h_new_xyz, int* h_idx, int* h_pts_cnt,
-                    float* h_grouped_xyz, cudaStream_t st) {
-    const struct { void* dst; size_t off, bytes; } outs[4] = {
-        {h_new_xyz, L.new_xyz, sizeof(float) * (size_t)b * m * 3},
-        {h_idx, L.idx, sizeof(int) * (size_t)b * m * nsample},
-        {h_pts_cnt, L.cnt, sizeof(int) * (size_t)b * m},
-        {h_grouped_xyz, L.grouped, sizeof(float) * (size_t)b * m * nsample * 3},
-    };
-    for (const auto& o : outs) {
-        if (!o.dst) continue;
-        const cudaError_t e = cudaMemcpyAsync(o.dst, ws + o.off, o.bytes, cudaMemcpyDeviceToHost, st);
+// the scale list of a multi-scale call: 1 <= nscales <= kSaMaxScales, every nsample positive and, with check_radii,
+// every radius too (the workspace size takes no radii)
+static bool valid_scales(int nscales, const float* radii, const int* nsamples, bool check_radii) {
+    if (nscales < 1 || nscales > kSaMaxScales || !nsamples || (check_radii && !radii)) return false;
+    for (int k = 0; k < nscales; ++k)
+        if (nsamples[k] <= 0 || (check_radii && !(radii[k] > 0.f))) return false;
+    return true;
+}
+
+// The D2H copies of the host-buffer layer: new_xyz, then each scale's idx, pts_cnt and grouped_xyz, each whose host
+// pointer is not NULL (h_grouped_xyz itself may be NULL).
+static int copy_out(int b, int m, int nscales, const int* nsamples, const char* ws, const SaLayout& L, float* h_new_xyz,
+                    int* const* h_idx, int* const* h_pts_cnt, float* const* h_grouped_xyz, cudaStream_t st) {
+    if (h_new_xyz) {
+        const cudaError_t e = cudaMemcpyAsync(h_new_xyz, ws + L.new_xyz, sizeof(float) * (size_t)b * m * 3, cudaMemcpyDeviceToHost, st);
         if (e != cudaSuccess) return (int)e;
+    }
+    for (int k = 0; k < nscales; ++k) {
+        const size_t s = (size_t)nsamples[k];
+        const struct { void* dst; size_t off, bytes; } outs[3] = {
+            {h_idx[k], L.idx[k], sizeof(int) * (size_t)b * m * s},
+            {h_pts_cnt[k], L.cnt[k], sizeof(int) * (size_t)b * m},
+            {h_grouped_xyz ? h_grouped_xyz[k] : nullptr, L.grouped[k], sizeof(float) * (size_t)b * m * s * 3},
+        };
+        for (const auto& o : outs) {
+            if (!o.dst) continue;
+            const cudaError_t e = cudaMemcpyAsync(o.dst, ws + o.off, o.bytes, cudaMemcpyDeviceToHost, st);
+            if (e != cudaSuccess) return (int)e;
+        }
     }
     return 0;
 }
@@ -101,6 +124,78 @@ static int launch_ragged_unpack(int b, int stride, const float* packed, const in
     ragged_unpack_kernel<<<dim3((unsigned)b, (unsigned)chunks, 1), kUnpackThreads, 0, st>>>(packed, lengths, stride, xyz);
     return finish_launch();
 }
+
+// The host-buffer layer behind the four entries.  Dense (ragged false): h_xyz is (b, n, 3).  Ragged: h_xyz is packed
+// with the host lengths h_lengths, which are checked here, and the device layer runs at the stride of the longest
+// cloud.  Everything is checked before the first enqueue.  The outputs follow copy_out; a scale whose grouped_xyz is
+// not wanted is not computed either.
+static int sa_layer_host(int b, int n, int m, int nscales, const float* radii, const int* nsamples, const float* h_xyz,
+                         const int* h_lengths, bool ragged, float* h_new_xyz, int* const* h_idx, int* const* h_pts_cnt,
+                         float* const* h_grouped_xyz, void* workspace, size_t workspace_bytes, void* stream) {
+    if (b <= 0 || n <= 0 || m <= 0 || !valid_scales(nscales, radii, nsamples, true)) return (int)cudaErrorInvalidValue;
+    if (!h_xyz || (ragged && !h_lengths) || !workspace) return (int)cudaErrorInvalidValue;
+    // the lengths are host memory: checked here, and the row stride is this batch's longest cloud
+    size_t rows = (size_t)b * n;
+    int n_run = n;
+    if (ragged) {
+        rows = 0;
+        n_run = 0;
+        for (int i = 0; i < b; ++i) {
+            const int l = h_lengths[i];
+            if (l < 1 || l > n) return (int)cudaErrorInvalidValue;
+            rows += (size_t)l;
+            n_run = l > n_run ? l : n_run;
+        }
+    }
+    const SaLayout L = sa_layout(b, n, m, nscales, nsamples, ragged);
+    if (workspace_bytes < L.total) return (int)cudaErrorInvalidValue;
+    if ((reinterpret_cast<uintptr_t>(workspace) & 255u) != 0) return (int)cudaErrorMisalignedAddress;
+    const size_t dev_ws_bytes = ragged ? pn2_sa_layer_device_workspace_bytes(b, n_run, m, nsamples[0]) : L.dev_ws_bytes;
+    if (dev_ws_bytes > L.dev_ws_bytes) return (int)cudaErrorInvalidValue;  // the bounds in sa_layout cover every stride <= n
+    cudaStream_t st = as_stream(stream);
+    char* ws = static_cast<char*>(workspace);
+    int* d_len = ragged ? reinterpret_cast<int*>(ws + L.lengths) : nullptr;
+    float* d_xyz = reinterpret_cast<float*>(ws + L.xyz);
+    int* d_idx[kSaMaxScales];
+    int* d_cnt[kSaMaxScales];
+    float* d_grp[kSaMaxScales];
+    bool grouped = false;
+    for (int k = 0; k < nscales; ++k) {
+        d_idx[k] = reinterpret_cast<int*>(ws + L.idx[k]);
+        d_cnt[k] = reinterpret_cast<int*>(ws + L.cnt[k]);
+        // not wanted: not computed
+        d_grp[k] = h_grouped_xyz && h_grouped_xyz[k] ? reinterpret_cast<float*>(ws + L.grouped[k]) : nullptr;
+        grouped = grouped || d_grp[k];
+    }
+
+    cudaError_t e;
+    if (ragged) {
+        float* d_packed = reinterpret_cast<float*>(ws + L.packed);
+        e = cudaMemcpyAsync(d_len, h_lengths, sizeof(int) * (size_t)b, cudaMemcpyHostToDevice, st);
+        if (e != cudaSuccess) return (int)e;
+        e = cudaMemcpyAsync(d_packed, h_xyz, sizeof(float) * 3 * rows, cudaMemcpyHostToDevice, st);
+        if (e != cudaSuccess) return (int)e;
+        const int rc = launch_ragged_unpack(b, n_run, d_packed, d_len, d_xyz, st);
+        if (rc) return rc;
+    } else {
+        e = cudaMemcpyAsync(d_xyz, h_xyz, sizeof(float) * 3 * rows, cudaMemcpyHostToDevice, st);
+        if (e != cudaSuccess) return (int)e;
+    }
+    const int rc = pn2_sa_layer_msg_device_ragged(b, n_run, m, nscales, radii, nsamples, d_xyz, d_len,
+                                                  reinterpret_cast<int*>(ws + L.fps_idx), reinterpret_cast<float*>(ws + L.new_xyz),
+                                                  d_idx, d_cnt, grouped ? d_grp : nullptr, /*center=*/0,
+                                                  dev_ws_bytes ? ws + L.dev_ws : nullptr, dev_ws_bytes, stream);
+    if (rc) return rc;
+    return copy_out(b, m, nscales, nsamples, ws, L, h_new_xyz, h_idx, h_pts_cnt, h_grouped_xyz, st);
+}
+
+// the multi-scale entries' required outputs: new_xyz, and every scale's idx and pts_cnt
+static bool msg_outputs_given(int nscales, const float* h_new_xyz, int* const* h_idx, int* const* h_pts_cnt) {
+    if (nscales < 1 || nscales > kSaMaxScales || !h_new_xyz || !h_idx || !h_pts_cnt) return false;
+    for (int k = 0; k < nscales; ++k)
+        if (!h_idx[k] || !h_pts_cnt[k]) return false;
+    return true;
+}
 }  // namespace pn2
 
 extern "C" {
@@ -113,79 +208,52 @@ unsigned long long pn2_launch_count(void) { return __atomic_load_n(&pn2::g_launc
 
 size_t pn2_sa_layer_workspace_bytes(int b, int n, int m, int nsample) {
     if (b <= 0 || n <= 0 || m <= 0 || nsample <= 0) return 0;
-    return pn2::sa_layout(b, n, m, nsample).total;
+    return pn2::sa_layout(b, n, m, 1, &nsample, /*ragged=*/false).total;
 }
 
 int pn2_sa_layer_host(int b, int n, int m, float radius, int nsample, const float* h_xyz, float* h_new_xyz,
                       int* h_idx, int* h_pts_cnt, float* h_grouped_xyz, void* workspace, size_t workspace_bytes,
                       void* stream) {
-    using namespace pn2;
-    if (b <= 0 || n <= 0 || m <= 0 || nsample <= 0 || !(radius > 0.f)) return (int)cudaErrorInvalidValue;
-    if (!h_xyz || !workspace) return (int)cudaErrorInvalidValue;
-    const SaLayout L = sa_layout(b, n, m, nsample);
-    if (workspace_bytes < L.total) return (int)cudaErrorInvalidValue;
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255u) != 0) return (int)cudaErrorMisalignedAddress;
-    cudaStream_t st = as_stream(stream);
-    char* ws = static_cast<char*>(workspace);
-    float* d_xyz = reinterpret_cast<float*>(ws + L.xyz);
-    float* d_new = reinterpret_cast<float*>(ws + L.new_xyz);
-    int* d_fps = reinterpret_cast<int*>(ws + L.fps_idx);
-    int* d_idx = reinterpret_cast<int*>(ws + L.idx);
-    int* d_cnt = reinterpret_cast<int*>(ws + L.cnt);
-    float* d_grp = h_grouped_xyz ? reinterpret_cast<float*>(ws + L.grouped) : nullptr;  // not wanted: not computed
-
-    cudaError_t e = cudaMemcpyAsync(d_xyz, h_xyz, sizeof(float) * (size_t)b * n * 3, cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) return (int)e;
-    int rc = pn2_sa_layer_device(b, n, m, radius, nsample, d_xyz, d_fps, d_new, d_idx, d_cnt, d_grp, /*center=*/0,
-                                 L.dev_ws_bytes ? ws + L.dev_ws : nullptr, L.dev_ws_bytes, stream);
-    if (rc) return rc;
-    return copy_out(b, m, nsample, ws, L, h_new_xyz, h_idx, h_pts_cnt, h_grouped_xyz, st);
+    return pn2::sa_layer_host(b, n, m, 1, &radius, &nsample, h_xyz, nullptr, /*ragged=*/false, h_new_xyz, &h_idx, &h_pts_cnt,
+                              &h_grouped_xyz, workspace, workspace_bytes, stream);
 }
 
 size_t pn2_sa_layer_host_ragged_workspace_bytes(int b, int n, int m, int nsample) {
     if (b <= 0 || n <= 0 || m <= 0 || nsample <= 0) return 0;
-    return pn2::sa_layout(b, n, m, nsample, /*ragged=*/true).total;
+    return pn2::sa_layout(b, n, m, 1, &nsample, /*ragged=*/true).total;
 }
 
 int pn2_sa_layer_host_ragged(int b, int n, int m, float radius, int nsample, const float* h_xyz, const int* h_lengths,
                              float* h_new_xyz, int* h_idx, int* h_pts_cnt, float* h_grouped_xyz, void* workspace,
                              size_t workspace_bytes, void* stream) {
-    using namespace pn2;
-    if (b <= 0 || n <= 0 || m <= 0 || nsample <= 0 || !(radius > 0.f)) return (int)cudaErrorInvalidValue;
-    if (!h_xyz || !h_lengths || !workspace) return (int)cudaErrorInvalidValue;
-    // the lengths are host memory: checked here, and the row stride is this batch's longest cloud
-    size_t rows = 0;
-    int n_run = 0;
-    for (int i = 0; i < b; ++i) {
-        const int l = h_lengths[i];
-        if (l < 1 || l > n) return (int)cudaErrorInvalidValue;
-        rows += (size_t)l;
-        n_run = l > n_run ? l : n_run;
-    }
-    const SaLayout L = sa_layout(b, n, m, nsample, /*ragged=*/true);
-    if (workspace_bytes < L.total) return (int)cudaErrorInvalidValue;
-    if ((reinterpret_cast<uintptr_t>(workspace) & 255u) != 0) return (int)cudaErrorMisalignedAddress;
-    const size_t dev_ws_bytes = pn2_sa_layer_device_workspace_bytes(b, n_run, m, nsample);
-    if (dev_ws_bytes > L.dev_ws_bytes) return (int)cudaErrorInvalidValue;  // the bounds in sa_layout cover every stride <= n
-    cudaStream_t st = as_stream(stream);
-    char* ws = static_cast<char*>(workspace);
-    int* d_len = reinterpret_cast<int*>(ws + L.lengths);
-    float* d_packed = reinterpret_cast<float*>(ws + L.packed);
-    float* d_xyz = reinterpret_cast<float*>(ws + L.xyz);
-    float* d_grp = h_grouped_xyz ? reinterpret_cast<float*>(ws + L.grouped) : nullptr;  // not wanted: not computed
+    return pn2::sa_layer_host(b, n, m, 1, &radius, &nsample, h_xyz, h_lengths, /*ragged=*/true, h_new_xyz, &h_idx, &h_pts_cnt,
+                              &h_grouped_xyz, workspace, workspace_bytes, stream);
+}
 
-    cudaError_t e = cudaMemcpyAsync(d_len, h_lengths, sizeof(int) * (size_t)b, cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) return (int)e;
-    e = cudaMemcpyAsync(d_packed, h_xyz, sizeof(float) * 3 * rows, cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) return (int)e;
-    int rc = launch_ragged_unpack(b, n_run, d_packed, d_len, d_xyz, st);
-    if (rc) return rc;
-    rc = pn2_sa_layer_device_ragged(b, n_run, m, radius, nsample, d_xyz, d_len, reinterpret_cast<int*>(ws + L.fps_idx),
-                                    reinterpret_cast<float*>(ws + L.new_xyz), reinterpret_cast<int*>(ws + L.idx),
-                                    reinterpret_cast<int*>(ws + L.cnt), d_grp, /*center=*/0,
-                                    dev_ws_bytes ? ws + L.dev_ws : nullptr, dev_ws_bytes, stream);
-    if (rc) return rc;
-    return copy_out(b, m, nsample, ws, L, h_new_xyz, h_idx, h_pts_cnt, h_grouped_xyz, st);
+size_t pn2_sa_layer_msg_host_workspace_bytes(int b, int n, int m, int nscales, const int* nsamples) {
+    if (b <= 0 || n <= 0 || m <= 0 || !pn2::valid_scales(nscales, nullptr, nsamples, false)) return 0;
+    return pn2::sa_layout(b, n, m, nscales, nsamples, /*ragged=*/false).total;
+}
+
+int pn2_sa_layer_msg_host(int b, int n, int m, int nscales, const float* radii, const int* nsamples, const float* h_xyz,
+                          float* h_new_xyz, int* const* h_idx, int* const* h_pts_cnt, float* const* h_grouped_xyz,
+                          void* workspace, size_t workspace_bytes, void* stream) {
+    if (!pn2::msg_outputs_given(nscales, h_new_xyz, h_idx, h_pts_cnt)) return (int)cudaErrorInvalidValue;
+    return pn2::sa_layer_host(b, n, m, nscales, radii, nsamples, h_xyz, nullptr, /*ragged=*/false, h_new_xyz, h_idx, h_pts_cnt,
+                              h_grouped_xyz, workspace, workspace_bytes, stream);
+}
+
+size_t pn2_sa_layer_msg_host_ragged_workspace_bytes(int b, int n, int m, int nscales, const int* nsamples) {
+    if (b <= 0 || n <= 0 || m <= 0 || !pn2::valid_scales(nscales, nullptr, nsamples, false)) return 0;
+    return pn2::sa_layout(b, n, m, nscales, nsamples, /*ragged=*/true).total;
+}
+
+int pn2_sa_layer_msg_host_ragged(int b, int n, int m, int nscales, const float* radii, const int* nsamples, const float* h_xyz,
+                                 const int* h_lengths, float* h_new_xyz, int* const* h_idx, int* const* h_pts_cnt,
+                                 float* const* h_grouped_xyz, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!pn2::msg_outputs_given(nscales, h_new_xyz, h_idx, h_pts_cnt)) return (int)cudaErrorInvalidValue;
+    return pn2::sa_layer_host(b, n, m, nscales, radii, nsamples, h_xyz, h_lengths, /*ragged=*/true, h_new_xyz, h_idx, h_pts_cnt,
+                              h_grouped_xyz, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -490,6 +490,8 @@ size_t fps_scratch_bytes(int b, int n);
 // that picks the row stride per call (the ragged host layer) sizes its workspace once for the largest stride
 size_t fps_scratch_bound(int b, int n);
 size_t query_ball_point_workspace_bound(int b, int n);
+// most ball-query scales of one multi-scale layer call (pn2_sa_layer_msg_device and its host-buffer entries)
+constexpr int kSaMaxScales = 16;
 
 // ordered-sum scatter through an inverse index (scatter_det.cu), shared by three_interpolate's gradient and the
 // group_point / gather_point gradients: dst[b, i, :] = sum over the entries e with idx[b, e] == i, e ascending, of

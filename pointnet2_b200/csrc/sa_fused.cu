@@ -505,7 +505,7 @@ int ball_group(int b, int n, int m, float radius, int nsample, const float* xyz1
 static int sa_layer_msg(int b, int n, int m, int nscales, const float* radii, const int* nsamples, const float* xyz,
                         const int* lengths, int* fps_idx, float* new_xyz, int* const* idx, int* const* pts_cnt,
                         float* const* grouped_xyz, int center, void* workspace, size_t workspace_bytes, cudaStream_t st) {
-    if (b < 0 || n <= 0 || m < 0 || nscales <= 0 || nscales > 16 || !radii || !nsamples || !idx || !pts_cnt)
+    if (b < 0 || n <= 0 || m < 0 || nscales <= 0 || nscales > kSaMaxScales || !radii || !nsamples || !idx || !pts_cnt)
         return (int)cudaErrorInvalidValue;
     for (int k = 0; k < nscales; ++k)
         if (nsamples[k] <= 0 || !(radii[k] > 0.0f) || !idx[k] || !pts_cnt[k]) return (int)cudaErrorInvalidValue;
