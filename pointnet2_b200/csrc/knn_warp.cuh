@@ -1,12 +1,11 @@
-// knn_warp.cuh — the per-query work of knn_point, one warp per query, as the KnnWarp routine that
-// knn_group_kernel (sa_fused.cu: the whole cloud in shared memory, queries taken from a concurrently running
-// sampling kernel) runs; and the distance and the sort that knn_kernel (knn.cu) uses as well.  knn_kernel keeps an
-// inline copy of the scan and the replay below (see knn.cu for why): a change here must be made there too.
+// knn_warp.cuh — the per-query work of knn_point, one warp per query, as the KnnWarp routine that both kNN kernels
+// run: knn_kernel (knn.cu: the cloud staged through shared-memory tiles) and knn_group_kernel (sa_fused.cu: the whole
+// cloud in shared memory, queries taken from a concurrently running sampling kernel).
 //
 // Semantics (see knn.cu for the derivation): the first k columns of the reference's selection sort over the row of
 // squared distances, ties included.  Only set A (positions < k) and set B (the k smallest of the rest under
 // (value, position)) can ever be selected or moved, so a query
-//   1. fills A into its W buffer          (fill_a: from wherever the caller keeps the cloud),
+//   1. fills A into its W buffer          (put_a for each position < min(k, n), from wherever the caller keeps the cloud),
 //   2. offers the positions >= k to B     (offer: points [0, tn) of SoA arrays in shared memory at global position
 //                                          base, once per tile or once for a cloud held whole),
 //   3. replays the k rounds on A and B    (finish: sorted fast path, or the exact replay with current positions),
@@ -61,13 +60,13 @@ __device__ __forceinline__ float knn_dist(float x, float y, float z, float qx, f
 
 template <int KC>  // registers per lane that hold the list B: k <= 32 * KC
 struct KnnWarp {
+    const int k, lane;
+    const float qx, qy, qz;
     // the list B lives in REGISTERS while the row is scanned: entry e = register e/32 of lane e%32 (no shared memory,
     // no __syncwarp): round 2's first version kept a sorted B in shared memory and spent most of its time in the
     // read-sync-write shifts (1.02 ms at 32 x 1024 x 4096, k = 32).
     float bv[KC];
     int bo[KC];
-    const int k, lane;
-    const float qx, qy, qz;
     int nb = 0;            // |B| so far (<= k)
     float tau = INFINITY;  // B full: its largest value; a later position must be strictly smaller to enter
     int ev_pos = -1;       // B's current maximum under (value, position) — the entry a better candidate evicts
@@ -81,68 +80,69 @@ struct KnnWarp {
         }
     }
 
-    // set A: positions 0..ka-1 keep their own slot; load(pos, x, y, z) reads data point pos
-    template <class Load>
-    __device__ __forceinline__ void fill_a(float* __restrict__ wv, int* __restrict__ wo, int ka, Load load) const {
-        for (int pos = lane; pos < ka; pos += 32) {
-            float x, y, z;
-            load(pos, x, y, z);
-            wv[pos] = knn_dist(x, y, z, qx, qy, qz);
-            wo[pos] = pos;
-        }
-    }
-
-    // B's maximum: ev_pos and tau
-    __device__ __forceinline__ void find_max() {
-        unsigned loc = 0u;  // distances are non-negative and never NaN here: unsigned order of the bits == float order
-#pragma unroll
-        for (int c = 0; c < KC; ++c)
-            if (32 * c + lane < k) loc = max(loc, __float_as_uint(bv[c]));
-        const unsigned mx = __reduce_max_sync(kFullMask, loc);
-        int lp = -1;
-#pragma unroll
-        for (int c = 0; c < KC; ++c)
-            if (32 * c + lane < k && __float_as_uint(bv[c]) == mx) lp = max(lp, bo[c]);
-        ev_pos = __reduce_max_sync(kFullMask, lp);  // among equal values the latest position goes first
-        tau = __uint_as_float(mx);
-    }
-
-    // one candidate group (32 consecutive positions, ascending): offer every lane of `cand` to the list.  B is kept
-    // UNSORTED (phase 2 sorts W anyway): while it is open a candidate is appended, afterwards it replaces the current
-    // maximum, and two redux.sync find the next one — ~20 instructions whatever k is (the sorted list this replaces
-    // shifted KC registers per insertion: 35 instructions at k <= 32, ~70 at k = 128, 35 % of the kernel at k = 32).
-    __device__ __forceinline__ void insert_group(unsigned cand, float d, int pos0) {
-        while (cand) {  // ascending position
-            const int src = __ffs(cand) - 1;
-            cand &= cand - 1;
-            const float dv = __shfl_sync(kFullMask, d, src);
-            const int dpos = pos0 + src;
-            if (nb < k) {
-#pragma unroll
-                for (int c = 0; c < KC; ++c)
-                    if (32 * c + lane == nb) {
-                        bv[c] = dv;
-                        bo[c] = dpos;
-                    }
-                if (++nb == k) find_max();
-            } else if (dv < tau) {  // tau may have dropped since the ballot (warp-uniform)
-#pragma unroll
-                for (int c = 0; c < KC; ++c)
-                    if (bo[c] == ev_pos && 32 * c + lane < k) {
-                        bv[c] = dv;
-                        bo[c] = dpos;
-                    }
-                find_max();
-            }
-        }
+    // set A: position pos < min(k, n) keeps its own slot; (x, y, z) is data point pos.  The caller loops over the
+    // positions: handed a loader callable instead, the front end re-associated knn_kernel's 64-bit address arithmetic
+    // (a separate base per coordinate in the tile loads too) and ptxas took 48 / 40 + 8 bytes of spill / 64 registers.
+    __device__ __forceinline__ void put_a(float* __restrict__ wv, int* __restrict__ wo, int pos, float x, float y, float z) const {
+        wv[pos] = knn_dist(x, y, z, qx, qy, qz);
+        wo[pos] = pos;
     }
 
     // candidates for B among the points [0, tn) of s_x / s_y / s_z, which sit at global positions base + p: those at
     // positions >= k that beat the current k-th best (strictly, once B is full).  Positions must be offered in
     // ascending order across calls.  ncu (k = 32, n = 4096): the kernel is issue-bound (91 % issue-active) and this
     // loop was 27 % of its instructions at 44 per 32 points — now two groups per trip and nothing about set A inside.
+    //
+    // nb, tau and ev_pos are copied into locals for the call.  Updated through `this` inside the loop, tau became an
+    // integer and the eviction below a different chain of selects, and knn_kernel<2> took 43 registers instead of 40.
     __device__ __forceinline__ void offer(const float* __restrict__ s_x, const float* __restrict__ s_y,
                                           const float* __restrict__ s_z, int tn, int base) {
+        int nb = this->nb;
+        float tau = this->tau;
+        int ev_pos = this->ev_pos;
+        // B's maximum: ev_pos and tau
+        auto find_max = [&]() {
+            unsigned loc = 0u;  // distances are non-negative and never NaN here: unsigned order of the bits == float order
+#pragma unroll
+            for (int c = 0; c < KC; ++c)
+                if (32 * c + lane < k) loc = max(loc, __float_as_uint(bv[c]));
+            const unsigned mx = __reduce_max_sync(kFullMask, loc);
+            int lp = -1;
+#pragma unroll
+            for (int c = 0; c < KC; ++c)
+                if (32 * c + lane < k && __float_as_uint(bv[c]) == mx) lp = max(lp, bo[c]);
+            ev_pos = __reduce_max_sync(kFullMask, lp);  // among equal values the latest position goes first
+            tau = __uint_as_float(mx);
+        };
+        // one candidate group (32 consecutive positions, ascending): offer every lane of `cand` to the list.  B is kept
+        // UNSORTED (phase 2 sorts W anyway): while it is open a candidate is appended, afterwards it replaces the current
+        // maximum, and two redux.sync find the next one — ~20 instructions whatever k is (the sorted list this replaces
+        // shifted KC registers per insertion: 35 instructions at k <= 32, ~70 at k = 128, 35 % of the kernel at k = 32).
+        auto insert_group = [&](unsigned cand, float d, int pos0) {
+            while (cand) {  // ascending position
+                const int src = __ffs(cand) - 1;
+                cand &= cand - 1;
+                const float dv = __shfl_sync(kFullMask, d, src);
+                const int dpos = pos0 + src;
+                if (nb < k) {
+#pragma unroll
+                    for (int c = 0; c < KC; ++c)
+                        if (32 * c + lane == nb) {
+                            bv[c] = dv;
+                            bo[c] = dpos;
+                        }
+                    if (++nb == k) find_max();
+                } else if (dv < tau) {  // tau may have dropped since the ballot (warp-uniform)
+#pragma unroll
+                    for (int c = 0; c < KC; ++c)
+                        if (bo[c] == ev_pos && 32 * c + lane < k) {
+                            bv[c] = dv;
+                            bo[c] = dpos;
+                        }
+                    find_max();
+                }
+            }
+        };
         for (int p0 = max(0, k - base); p0 < tn; p0 += 64) {
             const int pa = p0 + lane, pb = pa + 32;
             float d0 = INFINITY, d1 = INFINITY;
@@ -155,6 +155,9 @@ struct KnnWarp {
             if (c0) insert_group(c0, d0, base + p0);
             if (c1) insert_group(c1, d1, base + p0 + 32);  // insert_group re-checks every candidate against the current tau
         }
+        this->nb = nb;
+        this->tau = tau;
+        this->ev_pos = ev_pos;
     }
 
     // ---- phase 2: replay the selection sort on W = A ∪ B; emit(column, value, index) for columns 0..ka-1 ----------

@@ -631,7 +631,11 @@ knn_group_kernel(int n, int m, int k, const float* __restrict__ xyz, const int* 
         float qx, qy, qz;
         kg_load(s_x, n, qi, qx, qy, qz);
         KnnWarp<KC> w(k, lane, qx, qy, qz);
-        w.fill_a(wv, wo, k, [&](int pos, float& x, float& y, float& z) { kg_load(s_x, n, pos, x, y, z); });
+        for (int pos = lane; pos < k; pos += 32) {
+            float x, y, z;
+            kg_load(s_x, n, pos, x, y, z);
+            w.put_a(wv, wo, pos, x, y, z);
+        }
         w.offer(s_x, s_x + n, s_x + 2 * n, n, 0);
         float* __restrict__ drow = dist ? dist + row : nullptr;
         w.finish(wv, wo, wp, k, [&](int e, float v, int i) {
