@@ -161,6 +161,21 @@ int pn2_selection_sort(int b, int n, int m, int k, const float* dist, int* outi,
 int pn2_knn_point(int b, int n, int m, int k, const float* xyz1, const float* xyz2, float* val, int* idx,
                   void* stream);
 
+/* pn2_knn_point on ragged clouds (see pn2_fps_gather_ragged): lengths1 (b,) device int32, the lengths of the data
+ * clouds xyz1, and lengths2 (b,) device int32, the lengths of the query clouds xyz2; either may be NULL (every cloud
+ * has n points / m queries).  Each value is clamped to [1, n] (lengths1) or [1, m] (lengths2) on the device; the
+ * kernel (and so the cost) is chosen from n and k.  With len_i = lengths1[i], k_i = min(k, len_i) and qlen_i =
+ * lengths2[i], every query row j < qlen_i of cloud i holds:
+ *   - columns [0, k_i): bit for bit what pn2_knn_point(k_i) returns for the truncated cloud xyz1[i, :len_i] and that
+ *     query, ties and NaN / inf distances included;
+ *   - columns [k_i, k) (a cloud shorter than k): column 0 again, in val and idx, as the ball query pads a short row
+ *     with its first hit (a max-pool over the row is unchanged, and group_point on idx gives the grouped points).
+ * Query rows j >= qlen_i are never read and hold idx 0 / val +inf (the missing-neighbour filler of
+ * pn2_three_nn_ragged).  Padding rows of xyz1 and xyz2 may hold NaN, inf or anything else.  Still 1 <= k <=
+ * min(n, 128).  lengths1 = lengths2 = NULL is pn2_knn_point; self-kNN of a ragged batch passes the same lengths twice. */
+int pn2_knn_point_ragged(int b, int n, int m, int k, const float* xyz1, const int* lengths1, const float* xyz2,
+                         const int* lengths2, float* val, int* idx, void* stream);
+
 /* ---- 3d_interpolation (replaces the CPU functions of tf_interpolate.cpp; now on the GPU) -- */
 
 /* threenn_cpu(b,n,m,xyz1,xyz2,dist,idx), tf_interpolate.cpp:60-103.
@@ -492,6 +507,14 @@ size_t pn2_sa_knn_layer_workspace_bytes(int b, int n, int m, int k);
 int pn2_sa_knn_layer_device(int b, int n, int m, int k, const float* xyz, int* fps_idx, float* new_xyz, int* idx,
                             float* dist, float* grouped_xyz, int center, void* workspace, size_t workspace_bytes,
                             void* stream);
+/* pn2_sa_knn_layer_device on ragged clouds (see pn2_fps_gather_ragged): `lengths` (b,) device int32 after xyz,
+ * otherwise the arguments, paths (still chosen from (b, n, m, k)) and workspace of pn2_sa_knn_layer_device.  Cloud i's
+ * fps_idx and new_xyz are pn2_fps_gather_ragged's; idx, dist and grouped_xyz are pn2_knn_point_ragged's (lengths1 =
+ * lengths, no query lengths) and their gather, including the column-0 filler of a cloud shorter than k.  Every index
+ * is < lengths[i], so the grouping and any later layer need no lengths. */
+int pn2_sa_knn_layer_device_ragged(int b, int n, int m, int k, const float* xyz, const int* lengths, int* fps_idx,
+                                   float* new_xyz, int* idx, float* dist, float* grouped_xyz, int center,
+                                   void* workspace, size_t workspace_bytes, void* stream);
 /* measurement switch for pn2_sa_knn_layer_device: 0 = the cost rule (default), 1 = overlapped wherever it can run
  * (fits, one sampling CTA per cloud, an idle SM per cloud), 2 = always sequential.  The outputs do not depend on it. */
 void pn2_set_sa_knn_path(int mode);

@@ -66,6 +66,8 @@ _SIGNATURES = {
     "pn2_query_ball_point_ragged": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_sa_layer_device_ragged": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, _P, c_int, _P, c_size_t, _P]),
     "pn2_sa_layer_msg_device_ragged": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, _P, c_size_t, _P]),
+    "pn2_knn_point_ragged": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P]),
+    "pn2_sa_knn_layer_device_ragged": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, c_int, _P, c_size_t, _P]),
     # ... and with the lengths of the unknown side of the interpolation ops
     "pn2_three_nn_ragged": (c_int, [c_int, c_int, c_int, _P, _P, _P, _P, _P, _P]),
     "pn2_three_nn_interpolate_ragged_typed": (c_int, [c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P]),

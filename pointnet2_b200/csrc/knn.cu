@@ -33,10 +33,15 @@ constexpr int kKnnThreads = 256;
 constexpr int kKnnWarps = kKnnThreads / 32;
 constexpr int kKnnTile = 1024;  // data points per shared-memory tile
 
-template <int KC>  // registers per lane that hold the list B: k <= 32 * KC
+// L (ragged batch): data cloud i is its first cloud_length(lengths1, i, n) points, query cloud i its first
+// cloud_length(lengths2, i, m) queries (lengths2 == NULL: all m).  A template flag, so that the instances without lengths
+// compile to the code they always did.  A cloud shorter than k runs KnnWarp with k_i = min(k, len) (KC still chosen
+// from k): its columns [0, k_i) are knn_point(k_i) on the truncated cloud, and finish takes its usual ka == k entry;
+// columns [k_i, k) repeat column 0.  Query rows past their length get idx 0 / val +inf.
+template <int KC, bool L>  // KC: registers per lane that hold the list B: k <= 32 * KC
 __global__ void __launch_bounds__(kKnnThreads)
 knn_kernel(int n, int m, int k, const float* __restrict__ xyz1, const float* __restrict__ xyz2, float* __restrict__ val,
-           int* __restrict__ idx) {
+           int* __restrict__ idx, const int* __restrict__ lengths1, const int* __restrict__ lengths2) {
     __shared__ float s_x[kKnnTile], s_y[kKnnTile], s_z[kKnnTile];
     // per warp: W[0..k) = set A (positions 0..k-1), W[k..2k) = set B (in no particular order)
     __shared__ float s_wv[kKnnWarps][2 * kKnnMaxK];
@@ -46,7 +51,8 @@ knn_kernel(int n, int m, int k, const float* __restrict__ xyz1, const float* __r
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int cloud = blockIdx.y;
     const int q = blockIdx.x * kKnnWarps + warp;
-    const bool valid = q < m;
+    const int len = L ? cloud_length(lengths1, cloud, n) : n;  // data points of this cloud: padding is never loaded
+    const bool valid = q < (L ? cloud_length(lengths2, cloud, m) : m);
     const float* __restrict__ data = xyz1 + (size_t)cloud * n * 3;
     float qx = 0.f, qy = 0.f, qz = 0.f;
     if (valid) {
@@ -57,16 +63,17 @@ knn_kernel(int n, int m, int k, const float* __restrict__ xyz1, const float* __r
     }
     float* __restrict__ wv = s_wv[warp];
     int* __restrict__ wo = s_wo[warp];
-    KnnWarp<KC> w(k, lane, qx, qy, qz);
-    const int ka = min(k, n);  // |A|
+    const int kq = L ? min(k, len) : k;  // columns the selection produces for this cloud
+    KnnWarp<KC> w(kq, lane, qx, qy, qz);
+    const int ka = min(kq, len);  // |A|
     // set A straight from global memory: at most 128 points
     if (valid)
         for (int pos = lane; pos < ka; pos += 32) {
             const float* s = data + (size_t)pos * 3;
             w.put_a(wv, wo, pos, __ldg(s), __ldg(s + 1), __ldg(s + 2));
         }
-    for (int base = 0; base < n; base += kKnnTile) {
-        const int tn = min(kKnnTile, n - base);
+    for (int base = 0; base < len; base += kKnnTile) {
+        const int tn = min(kKnnTile, len - base);
         __syncthreads();  // previous tile consumed
         for (int p = tid; p < tn; p += kKnnThreads) {
             const float* s = data + (size_t)(base + p) * 3;
@@ -77,13 +84,42 @@ knn_kernel(int n, int m, int k, const float* __restrict__ xyz1, const float* __r
         __syncthreads();
         if (valid) w.offer(s_x, s_y, s_z, tn, base);
     }
-    if (!valid) return;
+    if (!valid) {
+        if (L && q < m)  // a query row past its cloud's length: the missing-neighbour filler
+            for (int e = lane; e < k; e += 32) {
+                val[((size_t)cloud * m + q) * k + e] = INFINITY;
+                idx[((size_t)cloud * m + q) * k + e] = 0;
+            }
+        return;
+    }
     float* __restrict__ oval = val + ((size_t)cloud * m + q) * k;
     int* __restrict__ oidx = idx + ((size_t)cloud * m + q) * k;
     w.finish(wv, wo, s_wp[warp], ka, [&](int e, float v, int i) {
         oval[e] = v;
         oidx[e] = i;
     });
+    if (L && kq < k) {  // a cloud shorter than k: columns [kq, k) repeat column 0, as the ball query pads a short row
+        __syncwarp();   // the replay's column 0 was written by lane 0
+        const float v0 = oval[0];
+        const int i0 = oidx[0];
+        for (int e = kq + lane; e < k; e += 32) {
+            oval[e] = v0;
+            oidx[e] = i0;
+        }
+    }
+}
+
+// pn2_knn_point on the clouds' first lengths1[b] points and the first lengths2[b] queries (NULL: all n / all m)
+static int knn_point(int b, int n, int m, int k, const float* xyz1, const int* lengths1, const float* xyz2, const int* lengths2,
+                     float* val, int* idx, cudaStream_t st) {
+    if (b < 0 || n <= 0 || m < 0 || k <= 0 || k > kKnnMaxK || k > n) return (int)cudaErrorInvalidValue;
+    if (b == 0 || m == 0) return 0;
+    if (!xyz1 || !xyz2 || !val || !idx || b > 65535) return (int)cudaErrorInvalidValue;
+    dim3 grid((m + kKnnWarps - 1) / kKnnWarps, b, 1);
+    auto kern = k <= 32 ? knn_kernel<1, false> : k <= 64 ? knn_kernel<2, false> : knn_kernel<4, false>;
+    if (lengths1 || lengths2) kern = k <= 32 ? knn_kernel<1, true> : k <= 64 ? knn_kernel<2, true> : knn_kernel<4, true>;
+    kern<<<grid, kKnnThreads, 0, st>>>(n, m, k, xyz1, xyz2, val, idx, lengths1, lengths2);
+    return finish_launch();
 }
 
 }  // namespace pn2
@@ -91,15 +127,12 @@ knn_kernel(int n, int m, int k, const float* __restrict__ xyz1, const float* __r
 extern "C" {
 
 int pn2_knn_point(int b, int n, int m, int k, const float* xyz1, const float* xyz2, float* val, int* idx, void* stream) {
-    using namespace pn2;
-    if (b < 0 || n <= 0 || m < 0 || k <= 0 || k > kKnnMaxK || k > n) return (int)cudaErrorInvalidValue;
-    if (b == 0 || m == 0) return 0;
-    if (!xyz1 || !xyz2 || !val || !idx || b > 65535) return (int)cudaErrorInvalidValue;
-    dim3 grid((m + kKnnWarps - 1) / kKnnWarps, b, 1);
-    if (k <= 32) knn_kernel<1><<<grid, kKnnThreads, 0, as_stream(stream)>>>(n, m, k, xyz1, xyz2, val, idx);
-    else if (k <= 64) knn_kernel<2><<<grid, kKnnThreads, 0, as_stream(stream)>>>(n, m, k, xyz1, xyz2, val, idx);
-    else knn_kernel<4><<<grid, kKnnThreads, 0, as_stream(stream)>>>(n, m, k, xyz1, xyz2, val, idx);
-    return finish_launch();
+    return pn2::knn_point(b, n, m, k, xyz1, nullptr, xyz2, nullptr, val, idx, pn2::as_stream(stream));
+}
+
+int pn2_knn_point_ragged(int b, int n, int m, int k, const float* xyz1, const int* lengths1, const float* xyz2, const int* lengths2,
+                         float* val, int* idx, void* stream) {
+    return pn2::knn_point(b, n, m, k, xyz1, lengths1, xyz2, lengths2, val, idx, pn2::as_stream(stream));
 }
 
 }  // extern "C"

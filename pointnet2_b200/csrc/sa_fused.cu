@@ -560,6 +560,10 @@ static int sa_layer_msg(int b, int n, int m, int nscales, const float* radii, co
 // Shared memory: 12 n bytes of cloud + 24 k bytes of W buffers per warp (2k entries of value, original index and
 // current position).  The warp count per CTA follows from what the cloud leaves, up to 32: 32 warps up to k = 64 at
 // n = 8192, fewer for larger clouds; below kKgMinWarps the layer takes the sequential path.
+//
+// Ragged batches (L): cloud i is its first len_i = cloud_length(lengths, i, n) points.  Only those are copied into
+// shared memory (the SoA stride stays n), a centroid index >= len_i is flagged like a lost one, and a cloud shorter than
+// k runs KnnWarp with k_i = min(k, len_i) and repeats column 0 in columns [k_i, k), as knn_kernel<KC, true> does.
 // ================================================================================================
 constexpr int kKgMinWarps = 4;
 constexpr int kKgMaxWarps = 32;
@@ -587,10 +591,11 @@ __device__ __forceinline__ void kg_load(const float* __restrict__ s_x, int n, in
     z = s_x[2 * n + pos];
 }
 
-template <int KC>
+template <int KC, bool L>  // L: per-cloud lengths (a template flag: the instances without them keep their code)
 __global__ void __launch_bounds__(kKgMaxWarps * 32, 1)
 knn_group_kernel(int n, int m, int k, const float* __restrict__ xyz, const int* q_idx, int* __restrict__ idx,
-                 float* __restrict__ dist, float* __restrict__ grouped, int center, int ctas_per_cloud) {
+                 float* __restrict__ dist, float* __restrict__ grouped, int center, int ctas_per_cloud,
+                 const int* __restrict__ lengths) {
     extern __shared__ __align__(16) unsigned char s_raw[];
     float* __restrict__ s_x = reinterpret_cast<float*>(s_raw);  // [3][n]: x, then y, then z
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
@@ -599,7 +604,8 @@ knn_group_kernel(int n, int m, int k, const float* __restrict__ xyz, const int* 
     int* __restrict__ wp = wo + 2 * k;
     const int cloud = blockIdx.x / ctas_per_cloud, part = blockIdx.x - cloud * ctas_per_cloud;
     const float* __restrict__ pts = xyz + (size_t)cloud * n * 3;
-    for (int p = tid; p < 3 * n; p += blockDim.x) {  // coalesced reads, transposed into SoA
+    const int len = L ? cloud_length(lengths, cloud, n) : n;
+    for (int p = tid; p < 3 * len; p += blockDim.x) {  // coalesced reads, transposed into SoA
         const int pt = p / 3, c = p - 3 * pt;
         s_x[c * n + pt] = __ldg(pts + p);
     }
@@ -624,26 +630,36 @@ knn_group_kernel(int n, int m, int k, const float* __restrict__ xyz, const int* 
         qi = __shfl_sync(kFullMask, qi, 0);
         const size_t row = ((size_t)cloud * m + q) * k;
         int* __restrict__ orow = idx + row;
-        if (qi < 0 || qi >= n) {  // producer lost / corrupt index: flag the row instead of faulting
+        if (qi < 0 || qi >= len) {  // producer lost / corrupt index: flag the row instead of faulting
             for (int e = lane; e < k; e += 32) orow[e] = -1;
             continue;
         }
         float qx, qy, qz;
         kg_load(s_x, n, qi, qx, qy, qz);
-        KnnWarp<KC> w(k, lane, qx, qy, qz);
-        for (int pos = lane; pos < k; pos += 32) {
+        const int kq = L ? min(k, len) : k;  // columns the selection produces for this cloud
+        KnnWarp<KC> w(kq, lane, qx, qy, qz);
+        for (int pos = lane; pos < kq; pos += 32) {
             float x, y, z;
             kg_load(s_x, n, pos, x, y, z);
             w.put_a(wv, wo, pos, x, y, z);
         }
-        w.offer(s_x, s_x + n, s_x + 2 * n, n, 0);
+        w.offer(s_x, s_x + n, s_x + 2 * n, len, 0);
         float* __restrict__ drow = dist ? dist + row : nullptr;
-        w.finish(wv, wo, wp, k, [&](int e, float v, int i) {
+        w.finish(wv, wo, wp, kq, [&](int e, float v, int i) {
             orow[e] = i;
             if (drow) drow[e] = v;
         });
+        if (L && kq < k) {  // a cloud shorter than k: columns [kq, k) repeat column 0
+            __syncwarp();   // the replay's column 0 was written by lane 0
+            const int i0 = orow[0];
+            const float v0 = drow ? drow[0] : 0.f;
+            for (int e = kq + lane; e < k; e += 32) {
+                orow[e] = i0;
+                if (drow) drow[e] = v0;
+            }
+        }
         if (grouped) {
-            __syncwarp();  // the replay's columns were written by lane 0
+            __syncwarp();  // the replay's columns (and the filler) were written by other lanes
             float* __restrict__ grow = grouped + row * 3;
             for (int e = lane; e < k; e += 32) {
                 float x, y, z;
@@ -661,17 +677,18 @@ knn_group_kernel(int n, int m, int k, const float* __restrict__ xyz, const int* 
     asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 
-static int launch_knn_group(int b, int n, int m, int k, const float* xyz, const int* q_idx, int* idx, float* dist, float* grouped,
-                            int center, int ctas_per_cloud, cudaStream_t st) {
-    static std::atomic<long long> max_dyn_once[2][64];  // [KC instance][device]: 0 = not asked yet
+static int launch_knn_group(int b, int n, int m, int k, const float* xyz, const int* lengths, const int* q_idx, int* idx,
+                            float* dist, float* grouped, int center, int ctas_per_cloud, cudaStream_t st) {
+    static std::atomic<long long> max_dyn_once[4][64];  // [ragged * 2 + KC instance][device]: 0 = not asked yet
     const int nw = kg_warps(n, k);
     if (nw == 0) return (int)cudaErrorInvalidValue;
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return (int)e;
     if (dev < 0 || dev >= 64) return (int)cudaErrorInvalidDevice;
-    const int kc = k <= 32 ? 0 : 1;
-    auto kern = kc == 0 ? knn_group_kernel<1> : knn_group_kernel<2>;
+    const int kc = (lengths ? 2 : 0) + (k <= 32 ? 0 : 1);
+    auto kern = kc == 0 ? knn_group_kernel<1, false> : kc == 1 ? knn_group_kernel<2, false> : kc == 2 ? knn_group_kernel<1, true>
+                                                                                                   : knn_group_kernel<2, true>;
     long long max_dyn = max_dyn_once[kc][dev].load(std::memory_order_acquire);
     if (max_dyn == 0) {
         int optin = 0;
@@ -696,7 +713,7 @@ static int launch_knn_group(int b, int n, int m, int k, const float* xyz, const 
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    e = cudaLaunchKernelEx(&cfg, kern, n, m, k, xyz, q_idx, idx, dist, grouped, center, ctas_per_cloud);
+    e = cudaLaunchKernelEx(&cfg, kern, n, m, k, xyz, q_idx, idx, dist, grouped, center, ctas_per_cloud, lengths);
     count_launch();
     if (e != cudaSuccess) return (int)e;
     return (int)cudaGetLastError();
@@ -746,18 +763,21 @@ static bool knn_overlapped(int b, int n, int m, int k) {
 
 static size_t knn_val_bytes(int b, int m, int k) { return (size_t)b * (size_t)m * (size_t)k * sizeof(float); }
 
-static int sa_knn_layer(int b, int n, int m, int k, const float* xyz, int* fps_idx, float* new_xyz, int* idx, float* dist,
-                        float* grouped_xyz, int center, void* workspace, size_t workspace_bytes, cudaStream_t st) {
+// pn2_sa_knn_layer_device on the clouds' first lengths[b] points (lengths == NULL: all n); the path and the workspace are
+// chosen from (b, n, m, k) either way
+static int sa_knn_layer(int b, int n, int m, int k, const float* xyz, const int* lengths, int* fps_idx, float* new_xyz, int* idx,
+                        float* dist, float* grouped_xyz, int center, void* workspace, size_t workspace_bytes, cudaStream_t st) {
     if (b < 0 || n <= 0 || m < 0 || k <= 0 || k > kKnnMaxK || k > n) return (int)cudaErrorInvalidValue;
     if (b == 0 || m == 0) return 0;
     if (!xyz || !fps_idx || !new_xyz || !idx || b > 65535) return (int)cudaErrorInvalidValue;
     if (knn_overlapped(b, n, m, k)) {
-        int rc = fps_dispatch(b, n, m, xyz, nullptr, nullptr, fps_idx, new_xyz, /*sentinel=*/1, st);
+        int rc = fps_dispatch(b, n, m, xyz, lengths, nullptr, fps_idx, new_xyz, /*sentinel=*/1, st);
         if (rc == 0)
-            rc = launch_knn_group(b, n, m, k, xyz, fps_idx, idx, dist, grouped_xyz, center, knn_consumer_ctas(b, m, k, n), st);
+            rc = launch_knn_group(b, n, m, k, xyz, lengths, fps_idx, idx, dist, grouped_xyz, center, knn_consumer_ctas(b, m, k, n), st);
         return rc;
     }
-    // sequential path: the sampling, knn_point and the xyz grouping one after the other
+    // sequential path: the sampling, knn_point and the xyz grouping one after the other; every index the sampling and
+    // knn_point return is below the cloud's length, so the grouping needs no lengths
     const size_t fps_b = align256(pn2_fps_scratch_bytes(b, n));
     char* ws = static_cast<char*>(workspace);
     float* temp = nullptr;
@@ -771,8 +791,8 @@ static int sa_knn_layer(int b, int n, int m, int k, const float* xyz, int* fps_i
         val = reinterpret_cast<float*>(ws + fps_b);
     }
     void* stream = static_cast<void*>(st);
-    int rc = fps_dispatch(b, n, m, xyz, nullptr, temp, fps_idx, new_xyz, 0, st);
-    if (rc == 0) rc = pn2_knn_point(b, n, m, k, xyz, new_xyz, val, idx, stream);
+    int rc = fps_dispatch(b, n, m, xyz, lengths, temp, fps_idx, new_xyz, 0, st);
+    if (rc == 0) rc = pn2_knn_point_ragged(b, n, m, k, xyz, lengths, new_xyz, nullptr, val, idx, stream);
     if (rc == 0 && grouped_xyz)
         rc = center ? pn2_group_concat(b, n, 0, m, k, xyz, new_xyz, nullptr, idx, 1, grouped_xyz, nullptr, stream)
                     : pn2_group_point(b, n, 3, m, k, xyz, idx, grouped_xyz, stream);
@@ -844,7 +864,14 @@ size_t pn2_sa_knn_layer_workspace_bytes(int b, int n, int m, int k) {
 
 int pn2_sa_knn_layer_device(int b, int n, int m, int k, const float* xyz, int* fps_idx, float* new_xyz, int* idx, float* dist,
                             float* grouped_xyz, int center, void* workspace, size_t workspace_bytes, void* stream) {
-    return pn2::sa_knn_layer(b, n, m, k, xyz, fps_idx, new_xyz, idx, dist, grouped_xyz, center, workspace, workspace_bytes,
+    return pn2::sa_knn_layer(b, n, m, k, xyz, nullptr, fps_idx, new_xyz, idx, dist, grouped_xyz, center, workspace, workspace_bytes,
+                             pn2::as_stream(stream));
+}
+
+int pn2_sa_knn_layer_device_ragged(int b, int n, int m, int k, const float* xyz, const int* lengths, int* fps_idx, float* new_xyz,
+                                   int* idx, float* dist, float* grouped_xyz, int center, void* workspace, size_t workspace_bytes,
+                                   void* stream) {
+    return pn2::sa_knn_layer(b, n, m, k, xyz, lengths, fps_idx, new_xyz, idx, dist, grouped_xyz, center, workspace, workspace_bytes,
                              pn2::as_stream(stream));
 }
 

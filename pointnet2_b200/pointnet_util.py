@@ -120,20 +120,28 @@ def sample_and_group(npoint, radius, nsample, xyz, points, knn=False, use_xyz=Tr
         centred on new_xyz.
         lengths: optional (b,) integers: cloud i is ``xyz[i, :lengths[i]]`` (and ``points[i, :lengths[i]]``), padded to
         n.  Sampling and the ball query then see each cloud alone; every index is below its length, so the grouping
-        never reads the padding.  Not with knn (ValueError).
+        never reads the padding.  Not with knn (ValueError): kNN grouping of variable-size clouds is
+        ``pointnet_sa_module(..., knn=True, lengths=)``, or ``sa_layer.sample_knn(..., lengths=)`` for the grouped xyz.
 
     ``fused=True`` uses the overlapped sampling+grouping layer (sa_layer.sample_group, or sa_layer.sample_knn for
     knn with nsample <= 128) and the single-pass concat kernel; ``fused=False`` issues the reference's op sequence one by one.  Both
     return identical values.
     """
     if knn:
-        _no_lengths_with(lengths, "knn grouping")
+        _no_lengths_with(lengths, "knn grouping in sample_and_group (pointnet_sa_module(knn=True) and sa_layer.sample_knn "
+                                  "take them)")
+    return _sample_and_group(npoint, radius, nsample, xyz, points, knn, use_xyz, fused, lengths)
+
+
+def _sample_and_group(npoint, radius, nsample, xyz, points, knn, use_xyz, fused, lengths):
+    """sample_and_group, with lengths for kNN grouping too: knn_point(lengths=) semantics, so a cloud shorter than
+    nsample repeats its nearest neighbour (column 0) in the rest of each row, as the ball query pads a short row."""
     no_grad_xyz = not xyz.requires_grad
     if fused and no_grad_xyz and knn and 0 < int(nsample) <= min(KNN_MAX_K, xyz.shape[1]):
         # one call: FPS + gather + kNN (+ centred grouped xyz when they are the whole output), the kNN grouping
         # overlapping the sampling chain
         need_g = points is None or not use_xyz
-        _, new_xyz, idx, _, grouped_xyz = sample_knn(npoint, nsample, xyz, center=True, want_grouped=need_g)
+        _, new_xyz, idx, _, grouped_xyz = sample_knn(npoint, nsample, xyz, center=True, want_grouped=need_g, lengths=lengths)
         if points is None:
             return new_xyz, grouped_xyz, idx, grouped_xyz
         if not use_xyz:
@@ -156,7 +164,7 @@ def sample_and_group(npoint, radius, nsample, xyz, points, knn=False, use_xyz=Tr
     else:
         new_xyz = gather_point(xyz, farthest_point_sample(npoint, xyz, lengths=lengths))
     if knn:
-        _, idx = knn_point(nsample, xyz, new_xyz)
+        _, idx = knn_point(nsample, xyz, new_xyz, lengths=lengths)
     else:
         idx, _ = query_ball_point(radius, nsample, xyz, new_xyz, lengths=lengths)
     if fused:
@@ -251,7 +259,9 @@ def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp=None, mlp2=None
         and bn_decay set their mode and batch-norm momentum), or callables on a (batch, npoint, nsample, channel) tensor,
         or None.  use_nchw is accepted and ignored (a layout hint for TensorFlow's conv2d).
         lengths: optional (b,) per-cloud point counts of a padded batch (see sample_and_group); the outputs are dense.
-        Not with group_all or knn (ValueError).
+        With knn, a cloud shorter than nsample repeats its nearest neighbour in the rest of each group
+        (tf_grouping.knn_point), which leaves the max-pool unchanged (the other poolings count that neighbour again).
+        Not with group_all (ValueError).
         Return: new_xyz (b,npoint,3), new_points (b,npoint,channels), idx (b,npoint,nsample)
     '''
     tail = _sa_mlp_route(mlp, xyz, points, use_xyz, scope, "conv", bn, is_training, bn_decay, pooling) if fused else None
@@ -265,12 +275,11 @@ def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp=None, mlp2=None
             new_points = layers.sa_mlp_max(xyz, None, points, None, tail, True, use_xyz)
         else:
             if knn:
-                _no_lengths_with(lengths, "knn grouping")
                 if 0 < int(nsample) <= min(KNN_MAX_K, xyz.shape[1]):
-                    _, new_xyz, idx, _, _ = sample_knn(npoint, nsample, xyz, center=True, want_grouped=False)
+                    _, new_xyz, idx, _, _ = sample_knn(npoint, nsample, xyz, center=True, want_grouped=False, lengths=lengths)
                 else:
-                    _, new_xyz = farthest_point_sample_and_gather(npoint, xyz)
-                    _, idx = knn_point(nsample, xyz, new_xyz)
+                    _, new_xyz = farthest_point_sample_and_gather(npoint, xyz, lengths=lengths)
+                    _, idx = knn_point(nsample, xyz, new_xyz, lengths=lengths)
             else:
                 _, new_xyz, idx, _, _ = sample_group(npoint, radius, nsample, xyz, center=True, want_grouped=False,
                                                      lengths=lengths)
@@ -281,8 +290,8 @@ def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp=None, mlp2=None
         _no_lengths_with(lengths, "group_all (the max-pool over every point would need a mask)")
         new_xyz, new_points, idx, grouped_xyz = sample_and_group_all(xyz, points, use_xyz)
     else:
-        new_xyz, new_points, idx, grouped_xyz = sample_and_group(npoint, radius, nsample, xyz, points, knn, use_xyz,
-                                                                 fused=fused, lengths=lengths)
+        new_xyz, new_points, idx, grouped_xyz = _sample_and_group(npoint, radius, nsample, xyz, points, knn, use_xyz, fused,
+                                                                  lengths)
     new_points = _apply_mlp(mlp, new_points, scope, "conv", bn, is_training, bn_decay)
     if pooling == 'max':
         new_points = new_points.max(dim=2, keepdim=True).values

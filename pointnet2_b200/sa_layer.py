@@ -128,13 +128,18 @@ KNN_MAX_K = 128  # pn2_sa_knn_layer_device's (and pn2_knn_point's) largest k
 
 
 def sample_knn(npoint: int, k: int, xyz: torch.Tensor, center: bool = True, want_grouped: bool = True,
-               want_dist: bool = False):
+               want_dist: bool = False, *, lengths=None):
     """FPS + gather_point + knn_point(k, xyz, new_xyz) + group_point(xyz) [- new_xyz] in one call.
 
     Returns (fps_idx (b,npoint) i32, new_xyz (b,npoint,3), idx (b,npoint,k) i32, dist (b,npoint,k) f32 or None,
     grouped_xyz (b,npoint,k,3) or None).  ``dist`` is knn_point's ``val`` (squared distances, ascending);
     ``center=True`` subtracts the centroid.  Bit-identical to the separate ops; no gradients.  Needs
-    1 <= k <= min(n, 128) (ValueError otherwise: larger k keep knn_point's composite path)."""
+    1 <= k <= min(n, 128) (ValueError otherwise: larger k keep knn_point's composite path).
+    ``lengths`` (b,) integers, optional: cloud i is ``xyz[i, :lengths[i]]``.  Its fps_idx and new_xyz are what the
+    sampling returns for it alone; idx, dist and grouped_xyz are ``knn_point(k, xyz, new_xyz, lengths=lengths)`` and
+    its gather, so a cloud shorter than k repeats its nearest neighbour (column 0) in columns [lengths[i], k).  Every
+    index is below its length.  A device tensor is never read on the host, so the call can be captured in a CUDA graph
+    and replayed with new lengths written into the same tensor."""
     npoint, k = int(npoint), int(k)
     if npoint <= 0:
         raise ValueError("FarthestPointSample expects positive npoint")
@@ -151,6 +156,7 @@ def sample_knn(npoint: int, k: int, xyz: torch.Tensor, center: bool = True, want
     if k > KNN_MAX_K:
         raise ValueError(f"sample_knn expects k <= {KNN_MAX_K}, got k={k}")
     dev = xyz.device
+    lens = device_lengths(lengths, b, n, dev, "sample_knn")
     fps_idx = torch.empty((b, npoint), dtype=torch.int32, device=dev)
     new_xyz = torch.empty((b, npoint, 3), dtype=torch.float32, device=dev)
     idx = torch.empty((b, npoint, k), dtype=torch.int32, device=dev)
@@ -162,8 +168,13 @@ def sample_knn(npoint: int, k: int, xyz: torch.Tensor, center: bool = True, want
     with on_device(xyz):
         wsb = int(lib.pn2_sa_knn_layer_workspace_bytes(b, n, npoint, k))
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev) if wsb else None
-        rc = lib.pn2_sa_knn_layer_device(b, n, npoint, k, ptr(xyz.detach()), ptr(fps_idx), ptr(new_xyz), ptr(idx), ptr(dist),
-                                         ptr(grouped), 1 if center else 0, ptr(ws), wsb, stream_ptr(dev))
+        if lens is None:
+            rc = lib.pn2_sa_knn_layer_device(b, n, npoint, k, ptr(xyz.detach()), ptr(fps_idx), ptr(new_xyz), ptr(idx), ptr(dist),
+                                             ptr(grouped), 1 if center else 0, ptr(ws), wsb, stream_ptr(dev))
+        else:
+            rc = lib.pn2_sa_knn_layer_device_ragged(b, n, npoint, k, ptr(xyz.detach()), ptr(lens), ptr(fps_idx), ptr(new_xyz),
+                                                    ptr(idx), ptr(dist), ptr(grouped), 1 if center else 0, ptr(ws), wsb,
+                                                    stream_ptr(dev))
     _lib.check(rc, "pn2_sa_knn_layer_device")
     return fps_idx, new_xyz, idx, dist, grouped
 

@@ -176,7 +176,7 @@ def group_point(points: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
     return _GroupPoint.apply(points, idx)
 
 
-def knn_point(k: int, xyz1: torch.Tensor, xyz2: torch.Tensor):
+def knn_point(k: int, xyz1: torch.Tensor, xyz2: torch.Tensor, *, lengths=None, query_lengths=None):
     """The k nearest data points of every query point, by squared Euclidean distance.
 
     Arguments: ``k`` neighbours per query; ``xyz1`` float32 (B, N, c), the cloud that is searched; ``xyz2`` float32
@@ -186,6 +186,15 @@ def knn_point(k: int, xyz1: torch.Tensor, xyz2: torch.Tensor):
     sum((xyz1 - xyz2)**2, -1) and runs select_top_k on it; for 3-D points and k <= 128 this runs one
     tiled top-k kernel instead (pn2_knn_point: no matrix), whose val / idx equal the first k columns
     of that composite bit for bit, ties included.  Other shapes take the composite itself.
+
+    ``lengths`` (B,) integers, optional: the data cloud b is ``xyz1[b, :lengths[b]]`` (variable-size clouds padded to
+    N).  With k_b = min(k, lengths[b]), columns [0, k_b) of each row are what this function returns for that cloud
+    alone with k_b neighbours; a cloud shorter than k repeats column 0 in columns [k_b, k) (``val`` and ``idx``), as
+    the ball query pads a short row with its first hit.  ``query_lengths`` (B,) integers, optional: the query cloud b
+    is ``xyz2[b, :query_lengths[b]]``; rows past it come back as idx 0 / val +inf.  Padding rows are never read.  A
+    device tensor is never read on the host (its values are clamped to [1, N] / [1, M] on the device), so the call
+    can be captured in a CUDA graph; a host tensor or sequence is checked here.  Lengths need the kernel: 3-D points
+    and k <= 128 (ValueError otherwise).
     """
     k = int(k)
     if k <= 0:
@@ -199,13 +208,22 @@ def knn_point(k: int, xyz1: torch.Tensor, xyz2: torch.Tensor):
     m = xyz2.shape[1]
     if k > n:
         raise ValueError(f"knn_point expects k <= ndataset (the reference slices k columns of an n-column matrix), got k={k}, n={n}")
+    ragged = lengths is not None or query_lengths is not None
+    if ragged and not (c == 3 and k <= 128):
+        raise ValueError(f"knn_point takes lengths only for 3-D points and k <= 128 (the kernel), got c={c}, k={k}")
+    lens = device_lengths(lengths, b, n, xyz1.device, "knn_point")
+    qlens = device_lengths(query_lengths, b, m, xyz1.device, "knn_point") if m else None
     if c == 3 and k <= 128:
         val = torch.empty((b, m, k), dtype=torch.float32, device=xyz1.device)
         idx = torch.empty((b, m, k), dtype=torch.int32, device=xyz1.device)
         if b * m:
             with on_device(xyz1):
-                rc = _lib.load().pn2_knn_point(b, n, m, k, ptr(xyz1.detach()), ptr(xyz2.detach()), ptr(val), ptr(idx),
-                                               stream_ptr(xyz1.device))
+                if ragged:
+                    rc = _lib.load().pn2_knn_point_ragged(b, n, m, k, ptr(xyz1.detach()), ptr(lens), ptr(xyz2.detach()), ptr(qlens),
+                                                          ptr(val), ptr(idx), stream_ptr(xyz1.device))
+                else:
+                    rc = _lib.load().pn2_knn_point(b, n, m, k, ptr(xyz1.detach()), ptr(xyz2.detach()), ptr(val), ptr(idx),
+                                                   stream_ptr(xyz1.device))
             _lib.check(rc, "pn2_knn_point")
         return val, idx
     diff = xyz1.unsqueeze(1) - xyz2.unsqueeze(2)  # (b,m,n,c): tile(xyz1) - tile(xyz2), tf_grouping.py:64-66

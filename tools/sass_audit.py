@@ -19,7 +19,9 @@ WATCH = [("CREDUX", r"^CREDUX"), ("REDUX", r"^REDUX"), ("FADD2", r"^FADD2"), ("F
          ("POPC", r"^POPC"), ("MUFU", r"^MUFU"), ("LDL", r"^LDL"), ("STL", r"^STL")]
 SHOW = ["fps_cta_kernel<16, 256, 0, false>", "fps_cta_kernel<16, 256, 1, false>", "fps_cta_kernel<16, 256, 1, true>", "fps_cta_kernel<32, 256, 1, false>", "fps_cluster_kernel<16, 128, 16, 1, false>", "fps_cluster_kernel<32, 128, 32, 0, false>", "fps_cluster_kernel<32, 128, 32, 1, false>", "fps_cluster_kernel<32, 512, 16, 1, false>",
         "fps_cluster_big_kernel<52, 512, 16, 0, false>", "fps_cluster_big_kernel<52, 512, 16, 1, false>",
-        "ball_group_kernel", "knn_kernel", "knn_group_kernel<1>", "knn_group_kernel<2>", "ball_query_kernel<16>", "bq_grid_build_kernel", "bq_grid_query_kernel",
+        "ball_group_kernel", "knn_kernel<1, false>", "knn_kernel<2, false>", "knn_kernel<4, false>", "knn_kernel<1, true>",
+        "knn_kernel<2, true>", "knn_kernel<4, true>", "knn_group_kernel<1, false>", "knn_group_kernel<2, false>", "knn_group_kernel<1, true>",
+        "knn_group_kernel<2, true>", "ball_query_kernel<16>", "bq_grid_build_kernel", "bq_grid_query_kernel",
         "group_rows_vec4_kernel<32, 4>", "group_narrow_kernel<false, float>", "group_rows_kernel<32, true, float>", "group_concat_vec_kernel<16, 2>",
         "group_point_grad_vec4_kernel<unsigned int, float>", "group_point_grad_vec4_kernel<unsigned int, __nv_bfloat16>", "three_nn_kernel", "fp_front_kernel<1, float>", "fp_front_kernel<8, float>", "fp_front_kernel<8, unsigned short>", "group_rows_kernel<32, true, unsigned short>",
         "three_interp_vec4_kernel<unsigned int, float, false, float4>", "three_interp_vec4_kernel<unsigned int, __nv_bfloat16, false, uint2>", "three_interp_grad_vec4_kernel<unsigned int>", "inv_build_kernel",
