@@ -414,11 +414,14 @@ __device__ __forceinline__ GridGeometry grid_geometry(const float* __restrict__ 
         g.ext[c] = warp_max_f32(s_red[3 + c][lane]) - g.mn[c];
     }
     const float emax = fmaxf(fmaxf(g.ext[0], g.ext[1]), g.ext[2]);
+    // an axis that is NaN in every point has mn = mx = +inf, so ext = inf - inf = NaN there, which fmaxf skips: such a
+    // box is not finite either
+    const bool ext_nan = (g.ext[0] != g.ext[0]) || (g.ext[1] != g.ext[1]) || (g.ext[2] != g.ext[2]);
     // cell edge: at least 1.01 * radius (any point within the radius of a query is then at most one cell away on
     // every axis, with margin for the rounding of the cell function), and large enough for kGridMaxDim cells to span
     // the box
     g.h = fmaxf(1.01f * radius, emax / (float)(kGridMaxDim - 1));
-    g.finite_box = (emax >= 0.f) && (emax < 1e30f) && (g.h > 0.f) && (g.h < 1e30f);
+    g.finite_box = !ext_nan && (emax >= 0.f) && (emax < 1e30f) && (g.h > 0.f) && (g.h < 1e30f);
     if (!g.finite_box) g.h = 1.0f;
     g.inv_h = 1.0f / g.h;
 #pragma unroll

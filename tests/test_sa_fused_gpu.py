@@ -23,10 +23,21 @@ def T(a, dev):
     return torch.from_numpy(np.ascontiguousarray(a)).to(dev)
 
 
+def brute_force_query(radius, nsample, x, q):
+    """query_ball_point on the brute-force kernel: in the automatic mode, 2048 <= n <= 9727 with b * m >= 4096 runs
+    ball_group_kernel, and the layer and ball_group would be compared with themselves"""
+    lib = _lib.load()
+    try:
+        lib.pn2_set_bq_mode(1)
+        return query_ball_point(radius, nsample, x, q)
+    finally:
+        lib.pn2_set_bq_mode(0)
+
+
 def sequential(npoint, radius, nsample, x, center):
     fi = farthest_point_sample(npoint, x)
     nx = gather_point(x, fi)
-    idx, cnt = query_ball_point(radius, nsample, x, nx)
+    idx, cnt = brute_force_query(radius, nsample, x, nx)
     g = group_point(x, idx)
     if center:
         g = g - nx.unsqueeze(2)
@@ -167,7 +178,7 @@ def test_multi_scale_layer_is_bit_identical_to_the_separate_ops(dev, gen, b, n, 
     wnx = gather_point(x, wfi)
     assert torch.equal(fi, wfi) and torch.equal(nx, wnx)
     for r, s, idx, cnt, g in zip(radii, nsamples, idxs, cnts, grps):
-        widx, wcnt = query_ball_point(r, s, x, wnx)
+        widx, wcnt = brute_force_query(r, s, x, wnx)
         assert torch.equal(idx, widx) and torch.equal(cnt, wcnt)
         assert torch.equal(g, group_point(x, widx) - wnx.unsqueeze(2))
 
@@ -198,7 +209,7 @@ def test_ball_group_matches_query_plus_group(dev, gen, b, n, m, r, s, center):
     q[:, ::3] = xyz[:, np.arange(0, m, 3) % n]
     qt = T(q.astype(np.float32), dev)
     idx, cnt, g = ball_group(r, s, x, qt, center=center)
-    widx, wcnt = query_ball_point(r, s, x, qt)
+    widx, wcnt = brute_force_query(r, s, x, qt)
     wg = group_point(x, widx)
     if center:
         wg = wg - qt.unsqueeze(2)
