@@ -105,6 +105,23 @@ def oracle_fps(npoint: int, xyz, keyorder: bool = False):
     return out
 
 
+TRACE_TIED = 64  # tied points oracle_fps_trace records per step
+
+
+def oracle_fps_trace(npoint: int, xyz):
+    """oracle_fps with a record of each step j >= 1: (idx (b, m) int32, top (b, m) float32 = the largest running
+    minimum, count (b, m) int32 = how many points attain it, tied (b, m, 64) int32 = the first 64 of them in tie-break
+    order, padded with -1).  idx[:, j] == tied[:, j, 0]; step 0 holds top -1, count 0 and no points."""
+    xyz = _f(xyz)
+    b, n, _ = xyz.shape
+    idx = np.zeros((b, npoint), _I)
+    top = np.zeros((b, npoint), _F)
+    count = np.zeros((b, npoint), _I)
+    tied = np.full((b, npoint, TRACE_TIED), -1, _I)
+    lib().oracle_fps_trace(c_int(b), c_int(n), c_int(npoint), _p(xyz), _p(idx), _p(top), _p(count), _p(tied))
+    return idx, top, count, tied
+
+
 def oracle_prob_cumsum(inp):
     inp = _f(inp)
     b, n = inp.shape

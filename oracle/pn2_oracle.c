@@ -134,6 +134,53 @@ void oracle_fps_keyorder(int b, int n, int m, const float *xyz, int *idx) {
     free(mind);
 }
 
+/* oracle_fps with a record of every step j >= 1: top[j] = the largest running minimum, count[j] = how many points
+ * attain it, tied[j*64 ..] = the first 64 of them in tie-break order (slot k mod 512 ascending, then k ascending),
+ * padded with -1.  The pick of step j is tied[j*64].  Same arithmetic as oracle_fps (d2_gpu_pattern, fminf, the 1e38
+ * start); step 0 is recorded as top -1, count 0 and no points.  idx (b, m), top (b, m), count (b, m), tied (b, m, 64). */
+#define PN2_TRACE_TIED 64
+void oracle_fps_trace(int b, int n, int m, const float *xyz, int *idx, float *top, int *count, int *tied) {
+    if (m <= 0 || n <= 0) return;
+    float *mind = (float *)malloc(sizeof(float) * (size_t)n);
+    for (int c = 0; c < b; ++c) {
+        const float *p = xyz + (size_t)c * n * 3;
+        int *o = idx + (size_t)c * m;
+        float *tp = top + (size_t)c * m;
+        int *cn = count + (size_t)c * m;
+        int *td = tied + (size_t)c * m * PN2_TRACE_TIED;
+        for (int k = 0; k < n; ++k) mind[k] = 1e38f;
+        for (int e = 0; e < PN2_TRACE_TIED; ++e) td[e] = -1;
+        int last = 0;
+        o[0] = 0;
+        tp[0] = -1.0f;
+        cn[0] = 0;
+        for (int j = 1; j < m; ++j) {
+            const float lx = p[last * 3 + 0], ly = p[last * 3 + 1], lz = p[last * 3 + 2];
+            float best = -1.0f;
+            for (int k = 0; k < n; ++k) {
+                float d = d2_gpu_pattern(p[k * 3 + 0], p[k * 3 + 1], p[k * 3 + 2], lx, ly, lz);
+                float d2 = fminf(d, mind[k]);
+                mind[k] = d2;
+                if (d2 > best) best = d2;
+            }
+            int *row = td + (size_t)j * PN2_TRACE_TIED;
+            int cnt = 0;
+            for (int e = 0; e < PN2_TRACE_TIED; ++e) row[e] = -1;
+            for (int s = 0; s < PN2_FPS_SLOTS && s < n; ++s)
+                for (int k = s; k < n; k += PN2_FPS_SLOTS)
+                    if (mind[k] == best) {
+                        if (cnt < PN2_TRACE_TIED) row[cnt] = k;
+                        ++cnt;
+                    }
+            tp[j] = best;
+            cn[j] = cnt;
+            last = row[0];
+            o[j] = last;
+        }
+    }
+    free(mind);
+}
+
 /* gatherpointKernel, tf_ops/sampling/tf_sampling_g.cu:172-181 : out[b,j,:] = inp[b,idx[b,j],:] */
 void oracle_gather_point(int b, int n, int m, const float *inp, const int *idx, float *out) {
     for (int c = 0; c < b; ++c)
