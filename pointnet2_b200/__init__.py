@@ -27,5 +27,6 @@ from .pointnet_util import (  # noqa: F401
 from .host import SetAbstractionHost, SetAbstractionPipeline  # noqa: F401
 from .layers import batch_invariant, is_batch_invariant  # noqa: F401
 from .render import project_points, render_balls, show_points  # noqa: F401
+from . import _ops  # noqa: F401  (registers the pn2:: torch operators; loads nothing)
 
 __version__ = "0.1.0"

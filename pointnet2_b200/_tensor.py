@@ -58,6 +58,17 @@ def device_lengths(lengths, b: int, n: int, device: torch.device, op: str):
         if tuple(lengths.shape) != (b,):
             raise ValueError(f"{op} expects (batch_size,) lengths shape ({b},), got {tuple(lengths.shape)}")
         return lengths.to(torch.int32).contiguous()
+    if not isinstance(lengths, torch.Tensor) and torch.compiler.is_compiling():
+        # traced (torch.export): a host sequence is checked here, in Python, and enters the graph as a constant
+        arr = np.asarray(lengths)
+        if arr.size and not np.issubdtype(arr.dtype, np.integer):
+            raise TypeError(f"{op} expects integer lengths, got {arr.dtype}")
+        if tuple(arr.shape) != (b,):
+            raise ValueError(f"{op} expects (batch_size,) lengths shape ({b},), got {tuple(arr.shape)}")
+        vals = [int(v) for v in arr.tolist()]
+        if b and (min(vals) < 1 or max(vals) > n):
+            raise ValueError(f"{op} expects 1 <= lengths <= {n} (the padded number of points), got {vals}")
+        return torch.tensor(vals, dtype=torch.int32, device=device)
     if isinstance(lengths, torch.Tensor):
         if lengths.dtype not in _INT_DTYPES:
             raise TypeError(f"{op} expects integer lengths, got {lengths.dtype}")

@@ -176,51 +176,67 @@ def _fuses_at(mods, i: int, x: torch.Tensor) -> bool:
             and fused_bn_applies(mods[i], x))
 
 
+def _bn_state(bn: nn.BatchNorm1d):
+    """(eps, momentum, num_batches_tracked, running_mean, running_var) of ``bn`` as the masked batch-norm kernels take
+    them: momentum -1 for the cumulative average, the three buffers None when bn keeps no running statistics."""
+    tracking = bn.track_running_stats and bn.running_mean is not None
+    return (float(bn.eps), -1.0 if bn.momentum is None else float(bn.momentum),
+            *((bn.num_batches_tracked, bn.running_mean, bn.running_var) if tracking else (None, None, None)))
+
+
+def masked_bn_relu_forward_launch(x, weight, bias, keep, eps: float, momentum: float, nbt, running_mean, running_var):
+    """masked_batch_norm_relu's forward on x (R, C) and the uint8 keep (R,): (y, save_mean, save_invstd).  Adds 1 to
+    ``nbt`` and updates the running statistics in place when they are given."""
+    rows, c = x.shape
+    dev = x.device
+    y = torch.empty_like(x)
+    save_mean = torch.empty(c, dtype=torch.float32, device=dev)
+    save_invstd = torch.empty(c, dtype=torch.float32, device=dev)
+    lib = _lib.load()
+    with on_device(x):
+        if nbt is not None:
+            nbt.add_(1)  # on the device; the kernel reads it for the cumulative average
+        wsb = int(lib.pn2_masked_bn_workspace_bytes(rows, c))
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+        rc = lib.pn2_masked_bn_relu_forward_typed(
+            DTYPE_CODES[x.dtype], rows, c, ptr(x), ptr(keep), ptr(weight), ptr(bias), eps, momentum, ptr(nbt),
+            ptr(running_mean), ptr(running_var), ptr(y), ptr(save_mean), ptr(save_invstd), ptr(ws), wsb, stream_ptr(dev))
+    _lib.check(rc, "pn2_masked_bn_relu_forward_typed")
+    return y, save_mean, save_invstd
+
+
+def masked_bn_relu_backward_launch(dy, x, y, keep, weight, save_mean, save_invstd):
+    """masked_batch_norm_relu's backward from the contiguous dy in x's dtype: (dx, dgamma, dbeta), the last two None
+    without weight."""
+    rows, c = x.shape
+    dev = x.device
+    dx = torch.empty_like(x)
+    dgamma = torch.empty(c, dtype=torch.float32, device=dev) if weight is not None else None
+    dbeta = torch.empty(c, dtype=torch.float32, device=dev) if weight is not None else None
+    lib = _lib.load()
+    with on_device(x):
+        wsb = int(lib.pn2_masked_bn_workspace_bytes(rows, c))
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+        rc = lib.pn2_masked_bn_relu_backward_typed(
+            DTYPE_CODES[x.dtype], rows, c, ptr(dy), ptr(x), ptr(y), ptr(keep), ptr(weight), ptr(save_mean),
+            ptr(save_invstd), ptr(dx), ptr(dgamma), ptr(dbeta), ptr(ws), wsb, stream_ptr(dev))
+    _lib.check(rc, "pn2_masked_bn_relu_backward_typed")
+    return dx, dgamma, dbeta
+
+
 class _MaskedBatchNormReLU(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, keep, bn):
-        rows, c = x.shape
-        dev = x.device
-        tracking = bn.track_running_stats and bn.running_mean is not None
-        momentum = -1.0 if bn.momentum is None else float(bn.momentum)
-        y = torch.empty_like(x)
-        save_mean = torch.empty(c, dtype=torch.float32, device=dev)
-        save_invstd = torch.empty(c, dtype=torch.float32, device=dev)
-        lib = _lib.load()
-        with on_device(x):
-            if tracking:
-                bn.num_batches_tracked.add_(1)  # on the device; the kernel reads it for the cumulative average
-            wsb = int(lib.pn2_masked_bn_workspace_bytes(rows, c))
-            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-            rc = lib.pn2_masked_bn_relu_forward_typed(
-                DTYPE_CODES[x.dtype], rows, c, ptr(x), ptr(keep), ptr(weight), ptr(bias), float(bn.eps), momentum,
-                ptr(bn.num_batches_tracked if tracking else None), ptr(bn.running_mean if tracking else None),
-                ptr(bn.running_var if tracking else None), ptr(y), ptr(save_mean), ptr(save_invstd), ptr(ws), wsb,
-                stream_ptr(dev))
-        _lib.check(rc, "pn2_masked_bn_relu_forward_typed")
+        y, save_mean, save_invstd = masked_bn_relu_forward_launch(x, weight, bias, keep, *_bn_state(bn))
         ctx.save_for_backward(x, y, keep, weight, save_mean, save_invstd)
-        ctx.affine = weight is not None
         return y
 
     @staticmethod
     @once_differentiable
     def backward(ctx, dy):
         x, y, keep, weight, save_mean, save_invstd = ctx.saved_tensors
-        rows, c = x.shape
-        dev = x.device
-        dy = dy.to(x.dtype).contiguous()
-        dx = torch.empty_like(x)
-        dgamma = torch.empty(c, dtype=torch.float32, device=dev) if ctx.affine else None
-        dbeta = torch.empty(c, dtype=torch.float32, device=dev) if ctx.affine else None
-        lib = _lib.load()
-        with on_device(x):
-            wsb = int(lib.pn2_masked_bn_workspace_bytes(rows, c))
-            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-            rc = lib.pn2_masked_bn_relu_backward_typed(
-                DTYPE_CODES[x.dtype], rows, c, ptr(dy), ptr(x), ptr(y), ptr(keep), ptr(weight), ptr(save_mean),
-                ptr(save_invstd), ptr(dx), ptr(dgamma), ptr(dbeta), ptr(ws), wsb, stream_ptr(dev))
-        _lib.check(rc, "pn2_masked_bn_relu_backward_typed")
-        return dx, dgamma, dbeta, None, None
+        return (*masked_bn_relu_backward_launch(dy.to(x.dtype).contiguous(), x, y, keep, weight, save_mean, save_invstd),
+                None, None)
 
 
 def masked_batch_norm_relu(bn: nn.BatchNorm1d, x: torch.Tensor, keep: torch.Tensor) -> torch.Tensor:
@@ -247,37 +263,76 @@ def masked_batch_norm_relu(bn: nn.BatchNorm1d, x: torch.Tensor, keep: torch.Tens
     if misfit is not None:
         raise misfit
     x = x.contiguous()
-    keep = keep.reshape(-1).contiguous().view(torch.uint8)  # the bool mask as bytes, no copy
     weight = bn.weight if bn.affine else None
     bias = bn.bias if bn.affine else None
+    if torch.compiler.is_compiling():  # the mask as bytes by a cast: inductor cannot view bool as uint8
+        eps, momentum, nbt, rm, rv = _bn_state(bn)
+        y, _, _, *stats = torch.ops.pn2.masked_batch_norm_relu(x, weight, bias, keep.reshape(-1).to(torch.uint8), rm, rv,
+                                                               nbt, eps, momentum)
+        _write_back(stats, nbt, rm, rv)
+        return y
+    keep = keep.reshape(-1).contiguous().view(torch.uint8)  # the bool mask as bytes, no copy
     return _MaskedBatchNormReLU.apply(x, weight, bias, keep, bn)
+
+
+def _write_back(stats, nbt, rm, rv) -> None:
+    """Copy the running statistics a registered masked batch-norm op returns into the module's buffers: the op is
+    functional so that it can carry an autograd formula, and this copy is the in-place update the eager kernel makes."""
+    if nbt is not None:
+        with torch.no_grad():
+            for buf, new in zip((rm, rv, nbt), stats):
+                buf.copy_(new)
+
+
+def masked_bn_relu_max_forward_launch(x, weight, bias, keep, eps: float, momentum: float, nbt, running_mean, running_var,
+                                      b: int, n: int):
+    """masked_bn_relu_max's forward on x (b * n, C) and the uint8 keep (b * n,): (out, argmax, save_mean, save_invstd),
+    the running statistics updated as masked_bn_relu_forward_launch updates them."""
+    c = x.shape[1]
+    dev = x.device
+    out = torch.empty((b, c), dtype=x.dtype, device=dev)
+    argmax = torch.empty((b, c), dtype=torch.int32, device=dev)
+    save_mean = torch.empty(c, dtype=torch.float32, device=dev)
+    save_invstd = torch.empty(c, dtype=torch.float32, device=dev)
+    lib = _lib.load()
+    with on_device(x):
+        if nbt is not None:
+            nbt.add_(1)  # on the device; the kernel reads it for the cumulative average
+        wsb = int(lib.pn2_masked_bn_relu_max_workspace_bytes(b, n, c))
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+        rc = lib.pn2_masked_bn_relu_max_forward_typed(
+            DTYPE_CODES[x.dtype], b, n, c, ptr(x), ptr(keep), ptr(weight), ptr(bias), eps, momentum, ptr(nbt),
+            ptr(running_mean), ptr(running_var), ptr(out), ptr(argmax), ptr(save_mean), ptr(save_invstd),
+            ptr(ws), wsb, stream_ptr(dev))
+    _lib.check(rc, "pn2_masked_bn_relu_max_forward_typed")
+    return out, argmax, save_mean, save_invstd
+
+
+def masked_bn_relu_max_backward_launch(dout, x, out, argmax, keep, weight, save_mean, save_invstd):
+    """masked_bn_relu_max's backward from the contiguous dout (b, C) in x's dtype: (dx (b * n, C), dgamma, dbeta), the
+    last two None without weight."""
+    b, c = out.shape
+    n = x.shape[0] // max(b, 1)
+    dev = x.device
+    dx = torch.empty_like(x)
+    dgamma = torch.empty(c, dtype=torch.float32, device=dev) if weight is not None else None
+    dbeta = torch.empty(c, dtype=torch.float32, device=dev) if weight is not None else None
+    lib = _lib.load()
+    with on_device(x):
+        wsb = int(lib.pn2_masked_bn_relu_max_workspace_bytes(b, n, c))
+        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+        rc = lib.pn2_masked_bn_relu_max_backward_typed(
+            DTYPE_CODES[x.dtype], b, n, c, ptr(dout), ptr(x), ptr(out), ptr(argmax), ptr(keep), ptr(weight),
+            ptr(save_mean), ptr(save_invstd), ptr(dx), ptr(dgamma), ptr(dbeta), ptr(ws), wsb, stream_ptr(dev))
+    _lib.check(rc, "pn2_masked_bn_relu_max_backward_typed")
+    return dx, dgamma, dbeta
 
 
 class _MaskedBatchNormReLUMax(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, keep, bn, b, n):
-        c = x.shape[1]
-        dev = x.device
-        tracking = bn.track_running_stats and bn.running_mean is not None
-        momentum = -1.0 if bn.momentum is None else float(bn.momentum)
-        out = torch.empty((b, c), dtype=x.dtype, device=dev)
-        argmax = torch.empty((b, c), dtype=torch.int32, device=dev)
-        save_mean = torch.empty(c, dtype=torch.float32, device=dev)
-        save_invstd = torch.empty(c, dtype=torch.float32, device=dev)
-        lib = _lib.load()
-        with on_device(x):
-            if tracking:
-                bn.num_batches_tracked.add_(1)  # on the device; the kernel reads it for the cumulative average
-            wsb = int(lib.pn2_masked_bn_relu_max_workspace_bytes(b, n, c))
-            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-            rc = lib.pn2_masked_bn_relu_max_forward_typed(
-                DTYPE_CODES[x.dtype], b, n, c, ptr(x), ptr(keep), ptr(weight), ptr(bias), float(bn.eps), momentum,
-                ptr(bn.num_batches_tracked if tracking else None), ptr(bn.running_mean if tracking else None),
-                ptr(bn.running_var if tracking else None), ptr(out), ptr(argmax), ptr(save_mean), ptr(save_invstd),
-                ptr(ws), wsb, stream_ptr(dev))
-        _lib.check(rc, "pn2_masked_bn_relu_max_forward_typed")
+        out, argmax, save_mean, save_invstd = masked_bn_relu_max_forward_launch(x, weight, bias, keep, *_bn_state(bn), b, n)
         ctx.save_for_backward(x, out, argmax, keep, weight, save_mean, save_invstd)
-        ctx.affine = weight is not None
         ctx.mark_non_differentiable(argmax)
         return out, argmax
 
@@ -285,22 +340,8 @@ class _MaskedBatchNormReLUMax(torch.autograd.Function):
     @once_differentiable
     def backward(ctx, dout, _dargmax):
         x, out, argmax, keep, weight, save_mean, save_invstd = ctx.saved_tensors
-        b, c = out.shape
-        n = x.shape[0] // max(b, 1)
-        dev = x.device
-        dout = dout.to(x.dtype).contiguous()
-        dx = torch.empty_like(x)
-        dgamma = torch.empty(c, dtype=torch.float32, device=dev) if ctx.affine else None
-        dbeta = torch.empty(c, dtype=torch.float32, device=dev) if ctx.affine else None
-        lib = _lib.load()
-        with on_device(x):
-            wsb = int(lib.pn2_masked_bn_relu_max_workspace_bytes(b, n, c))
-            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-            rc = lib.pn2_masked_bn_relu_max_backward_typed(
-                DTYPE_CODES[x.dtype], b, n, c, ptr(dout), ptr(x), ptr(out), ptr(argmax), ptr(keep), ptr(weight),
-                ptr(save_mean), ptr(save_invstd), ptr(dx), ptr(dgamma), ptr(dbeta), ptr(ws), wsb, stream_ptr(dev))
-        _lib.check(rc, "pn2_masked_bn_relu_max_backward_typed")
-        return dx, dgamma, dbeta, None, None, None, None
+        return (*masked_bn_relu_max_backward_launch(dout.to(x.dtype).contiguous(), x, out, argmax, keep, weight, save_mean,
+                                                    save_invstd), None, None, None, None)
 
 
 def masked_bn_relu_max(bn: nn.BatchNorm1d, x: torch.Tensor, lengths=None, *, with_indices: bool = False):
@@ -333,13 +374,21 @@ def masked_bn_relu_max(bn: nn.BatchNorm1d, x: torch.Tensor, lengths=None, *, wit
     if lengths is None:
         keep = torch.ones(b * n, dtype=torch.uint8, device=x.device)
     else:
-        keep = row_mask(lengths, n).reshape(-1).view(torch.uint8)  # the bool mask as bytes, no copy
+        keep = row_mask(lengths, n).reshape(-1)
+        # the bool mask as bytes: a view, no copy (a cast under compile: inductor cannot view bool as uint8)
+        keep = keep.to(torch.uint8) if torch.compiler.is_compiling() else keep.view(torch.uint8)
     weight = bn.weight if bn.affine else None
     bias = bn.bias if bn.affine else None
     if b == 0:
         out = x.new_empty((0, c))
         return (out, torch.empty((0, c), dtype=torch.int32, device=x.device)) if with_indices else out
-    out, argmax = _MaskedBatchNormReLUMax.apply(x.reshape(b * n, c).contiguous(), weight, bias, keep, bn, b, n)
+    if torch.compiler.is_compiling():
+        eps, momentum, nbt, rm, rv = _bn_state(bn)
+        out, argmax, _, _, *stats = torch.ops.pn2.masked_bn_relu_max(x.contiguous(), weight, bias, keep, rm, rv, nbt, eps,
+                                                                     momentum)
+        _write_back(stats, nbt, rm, rv)
+    else:
+        out, argmax = _MaskedBatchNormReLUMax.apply(x.reshape(b * n, c).contiguous(), weight, bias, keep, bn, b, n)
     return (out, argmax) if with_indices else out
 
 
@@ -459,20 +508,32 @@ def _check_params(stack, dev) -> None:
             raise misfit
 
 
+def _stack_params(stack):
+    """The tensors and flags of a layer stack (see _mlp_stack) as the fused-MLP kernels read them: a flat list of six
+    tensors per layer (Linear weight and bias, batch-norm weight, bias, running mean and running variance, None where
+    absent), the batch-norm epsilons and the ReLU flags."""
+    params, eps, relu = [], [], []
+    for lin, bn, r in stack:
+        affine = bn is not None and bn.affine
+        params += [lin.weight, lin.bias, bn.weight if affine else None, bn.bias if affine else None,
+                   None if bn is None else bn.running_mean, None if bn is None else bn.running_var]
+        eps.append(0.0 if bn is None else float(bn.eps))
+        relu.append(bool(r))
+    return params, eps, relu
+
+
 def _layer_args(stack):
     """nlayers and the per-layer host arrays of the fused-MLP C entries (pn2_sa_mlp_max_typed and its row-wise twins):
     widths, weight, bias, bn_weight, bn_bias, bn_mean, bn_var, bn_eps, relu."""
-    nl = len(stack)
-    pa = lambda ts: (ctypes.c_void_p * nl)(*[None if t is None else t.data_ptr() for t in ts])
-    bns = [bn for _, bn, _ in stack]
-    return (nl, (ctypes.c_int * nl)(*[lin.out_features for lin, _, _ in stack]),
-            pa([lin.weight for lin, _, _ in stack]), pa([lin.bias for lin, _, _ in stack]),
-            pa([bn.weight if bn is not None and bn.affine else None for bn in bns]),
-            pa([bn.bias if bn is not None and bn.affine else None for bn in bns]),
-            pa([None if bn is None else bn.running_mean for bn in bns]),
-            pa([None if bn is None else bn.running_var for bn in bns]),
-            (ctypes.c_float * nl)(*[0.0 if bn is None else float(bn.eps) for bn in bns]),
-            (ctypes.c_int * nl)(*[1 if relu else 0 for _, _, relu in stack]))
+    return _param_args(*_stack_params(stack))
+
+
+def _param_args(params, eps, relu):
+    """_layer_args from the tensors and flags _stack_params gives"""
+    nl = len(eps)
+    pa = lambda j: (ctypes.c_void_p * nl)(*[None if t is None else t.data_ptr() for t in params[j::6]])
+    return (nl, (ctypes.c_int * nl)(*[w.shape[0] for w in params[0::6]]), pa(0), pa(1), pa(2), pa(3), pa(4), pa(5),
+            (ctypes.c_float * nl)(*eps), (ctypes.c_int * nl)(*[1 if r else 0 for r in relu]))
 
 
 def sa_mlp_dtype(points: Optional[torch.Tensor]):
@@ -582,8 +643,6 @@ def sa_mlp_max(xyz: Optional[torch.Tensor], new_xyz: Optional[torch.Tensor], poi
             raise ValueError("points must be (batch_size, ndataset, channel) matching xyz")
         tensors.append(points)
         c = points.shape[2]
-        if points.dtype != dtype:
-            points = points.to(dtype)  # autocast: as the first Linear would cast its input
     cin = c + 3 if (use_xyz or points is None) else c
     if cin != mlp.in_channels:
         raise ValueError(f"the grouped rows have {cin} channels, mlp expects {mlp.in_channels}")
@@ -591,9 +650,7 @@ def sa_mlp_max(xyz: Optional[torch.Tensor], new_xyz: Optional[torch.Tensor], poi
     dev = tensors[0].device
     _check_params(stack, dev)
     cout = mlp.out_channels
-    if out is None:
-        out = torch.empty((b, s, cout), dtype=dtype, device=dev)
-    else:
+    if out is not None:
         if not isinstance(out, torch.Tensor) or out.dtype != dtype or tuple(out.shape) != (b, s, cout):
             raise ValueError(f"out must be a {dtype} tensor of shape {(b, s, cout)}, got "
                              f"{getattr(out, 'dtype', type(out).__name__)} {tuple(getattr(out, 'shape', ()))}")
@@ -601,23 +658,43 @@ def sa_mlp_max(xyz: Optional[torch.Tensor], new_xyz: Optional[torch.Tensor], poi
             raise RuntimeError(f"out must be on the inputs' device ({dev}), got {out.device}")
         if b * s and (out.stride(2) != 1 or out.stride(1) < cout or (b > 1 and out.stride(0) != s * out.stride(1))):
             raise ValueError("out must be a channel slice of a contiguous (batch_size, npoint, channels) tensor")
+    if idx is None:
+        lengths = device_lengths(lengths, b, n, dev, "sa_mlp_max") if b * s else None
+    if torch.compiler.is_compiling():
+        res = torch.ops.pn2.sa_mlp_max(xyz, new_xyz, points, idx, lengths, *_stack_params(stack), bool(xyz_first),
+                                       bool(use_xyz), dtype)
+        return res if out is None else out.copy_(res)
+    return sa_mlp_max_launch(xyz, new_xyz, points, idx, lengths, *_stack_params(stack), xyz_first, use_xyz, dtype, out)
+
+
+def sa_mlp_max_launch(xyz, new_xyz, points, idx, lengths, params, eps, relu, xyz_first: bool, use_xyz: bool, dtype, out=None):
+    """sa_mlp_max on checked arguments: the layers as _stack_params gives them, ``lengths`` None or the device tensor,
+    ``out`` None (a new (b, s, C_out) tensor) or a checked one."""
+    ref = xyz if xyz is not None else points
+    b, n = ref.shape[0], ref.shape[1]
+    s, k = (1, n) if idx is None else (idx.shape[1], idx.shape[2])
+    c = 0 if points is None else points.shape[2]
+    dev = ref.device
+    if out is None:
+        out = torch.empty((b, s, params[-6].shape[0]), dtype=dtype, device=dev)
     if b * s == 0:
         return out
+    if points is not None and points.dtype != dtype:
+        points = points.to(dtype)  # autocast: as the first Linear would cast its input
     lib = _lib.load()
     if idx is None:
-        lengths = device_lengths(lengths, b, n, dev, "sa_mlp_max")
-        with on_device(tensors[0]):
-            wsb = int(lib.pn2_sa_mlp_max_all_workspace_bytes(b, cout))
+        with on_device(ref):
+            wsb = int(lib.pn2_sa_mlp_max_all_workspace_bytes(b, out.shape[2]))
             ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
             rc = lib.pn2_sa_mlp_max_all_typed(
                 DTYPE_CODES[dtype], b, n, c, ptr(xyz), ptr(new_xyz), ptr(points), ptr(lengths), 1 if xyz_first else 0,
-                1 if use_xyz else 0, *_layer_args(stack), ptr(out), out.stride(1), ptr(ws), wsb, stream_ptr(dev))
+                1 if use_xyz else 0, *_param_args(params, eps, relu), ptr(out), out.stride(1), ptr(ws), wsb, stream_ptr(dev))
         _lib.check(rc, "pn2_sa_mlp_max_all_typed")
         return out
     with on_device(xyz):
         rc = lib.pn2_sa_mlp_max_typed(
             DTYPE_CODES[dtype], b, n, c, s, k, ptr(xyz), ptr(new_xyz), ptr(points), ptr(idx), 1 if xyz_first else 0,
-            1 if use_xyz else 0, *_layer_args(stack), ptr(out), out.stride(1), stream_ptr(dev))
+            1 if use_xyz else 0, *_param_args(params, eps, relu), ptr(out), out.stride(1), stream_ptr(dev))
     _lib.check(rc, "pn2_sa_mlp_max_typed")
     return out
 
@@ -701,6 +778,21 @@ def fp_mlp(xyz1: torch.Tensor, xyz2: torch.Tensor, points1: Optional[torch.Tenso
     if b > 65535:
         raise ValueError(f"fp_mlp takes at most 65535 clouds, got {b}")
     out, rs = _out_rows(out, (b, n), mlp.out_channels, dtype, dev, "fp_mlp")
+    if torch.compiler.is_compiling():
+        res = torch.ops.pn2.fp_mlp(xyz1, xyz2, points1, points2, lengths, *_stack_params(stack), dtype)
+        return res if out is None else out.copy_(res)
+    return fp_mlp_launch(xyz1, xyz2, points1, points2, lengths, *_stack_params(stack), dtype, out, rs)
+
+
+def fp_mlp_launch(xyz1, xyz2, points1, points2, lengths, params, eps, relu, dtype, out=None, rs=None):
+    """fp_mlp on checked arguments (layers as _stack_params gives them); ``out`` None (a new tensor) or checked, with its
+    row stride ``rs``."""
+    b, n, m = xyz1.shape[0], xyz1.shape[1], xyz2.shape[1]
+    c1 = 0 if points1 is None else points1.shape[2]
+    c2 = points2.shape[2]
+    dev = xyz1.device
+    if out is None:
+        out, rs = torch.empty((b, n, params[-6].shape[0]), dtype=dtype, device=dev), params[-6].shape[0]
     if b * n == 0:
         return out
     points2 = points2.to(dtype)  # autocast: as the first Linear would cast its input
@@ -711,7 +803,7 @@ def fp_mlp(xyz1: torch.Tensor, xyz2: torch.Tensor, points1: Optional[torch.Tenso
         wsb = int(lib.pn2_fp_mlp_workspace_bytes(b, n))
         ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
         rc = lib.pn2_fp_mlp_typed(DTYPE_CODES[dtype], b, n, m, c2, c1, ptr(xyz1), ptr(lengths), ptr(xyz2), ptr(points1),
-                                  ptr(points2), *_layer_args(stack), ptr(out), rs, ptr(ws), wsb, stream_ptr(dev))
+                                  ptr(points2), *_param_args(params, eps, relu), ptr(out), rs, ptr(ws), wsb, stream_ptr(dev))
     _lib.check(rc, "pn2_fp_mlp_typed")
     return out
 
@@ -738,16 +830,24 @@ def mlp_rows(t: torch.Tensor, mlp: SharedMLP, mask: Optional[torch.Tensor] = Non
     if dtype not in FEATURE_DTYPES:
         raise TypeError(f"mlp_rows computes in float32, bfloat16 or float16, not the autocast dtype {dtype}")
     same_device(*tensors)
-    dev = t.device
-    _check_params(stack, dev)
-    out = torch.empty((*lead, mlp.out_channels), dtype=dtype, device=dev)
+    _check_params(stack, t.device)
+    if torch.compiler.is_compiling():
+        return torch.ops.pn2.mlp_rows(t, None if mask is None else mask.reshape(-1), *_stack_params(stack), dtype)
+    return mlp_rows_launch(t, mask, *_stack_params(stack), dtype)
+
+
+def mlp_rows_launch(t, mask, params, eps, relu, dtype):
+    """mlp_rows on checked arguments (layers as _stack_params gives them): a new (..., C_out) tensor."""
+    cout = params[-6].shape[0]
+    out = torch.empty((*t.shape[:-1], cout), dtype=dtype, device=t.device)
+    rows = math.prod(t.shape[:-1])
     if rows == 0:
         return out
     t = t.to(dtype)  # autocast: as the first Linear would cast its input
     keep = None if mask is None else mask.reshape(-1).contiguous().view(torch.uint8)
     with on_device(t):
-        rc = _lib.load().pn2_mlp_rows_typed(DTYPE_CODES[dtype], rows, t.shape[-1], ptr(t), ptr(keep), *_layer_args(stack),
-                                            ptr(out), mlp.out_channels, stream_ptr(dev))
+        rc = _lib.load().pn2_mlp_rows_typed(DTYPE_CODES[dtype], rows, t.shape[-1], ptr(t), ptr(keep),
+                                            *_param_args(params, eps, relu), ptr(out), cout, stream_ptr(t.device))
     _lib.check(rc, "pn2_mlp_rows_typed")
     return out
 

@@ -30,53 +30,67 @@ from .sa_layer import KNN_MAX_K, sample_group, sample_group_msg, sample_knn
 from .tf_sampling import farthest_point_sample, farthest_point_sample_and_gather, gather_point
 
 
-class _GroupConcat(torch.autograd.Function):
-    """out = concat(xyz[idx]-new_xyz, points[idx]) in either channel order, plus grouped_xyz.  out has the dtype of
-    ``points`` (float32 without points); grouped_xyz is float32."""
+def group_and_concat_launch(xyz, new_xyz, points, idx, xyz_first: bool):
+    """(out, grouped_xyz) of group_and_concat: out has the dtype of ``points`` (float32 without points); grouped_xyz is
+    float32."""
+    b, n, _ = xyz.shape
+    _, m, s = idx.shape
+    c = 0 if points is None else points.shape[2]
+    dtype = torch.float32 if points is None else points.dtype
+    out = torch.empty((b, m, s, 3 + c), dtype=dtype, device=xyz.device)
+    gxyz = torch.empty((b, m, s, 3), dtype=torch.float32, device=xyz.device)
+    if out.numel():
+        with on_device(xyz):
+            if dtype == torch.float32:
+                rc = _lib.load().pn2_group_concat(b, n, c, m, s, ptr(xyz), ptr(new_xyz), ptr(points), ptr(idx),
+                                                  1 if xyz_first else 0, ptr(out), ptr(gxyz), stream_ptr(xyz.device))
+            else:
+                rc = _lib.load().pn2_group_concat_typed(DTYPE_CODES[dtype], b, n, c, m, s, ptr(xyz), ptr(new_xyz), ptr(points),
+                                                        ptr(idx), 1 if xyz_first else 0, ptr(out), ptr(gxyz),
+                                                        stream_ptr(xyz.device))
+        _lib.check(rc, "pn2_group_concat")
+    return out, gxyz
 
+
+def group_and_concat_backward(g_out, g_gxyz, idx, n: int, xyz_first: bool, has_points: bool, need_xyz: bool,
+                              need_new_xyz: bool):
+    """Gradients (xyz, new_xyz, points) of group_and_concat from those of (out, grouped_xyz), each None when not wanted;
+    ``g_out`` in the dtype of out, ``g_gxyz`` float32 or None."""
+    c = g_out.shape[-1] - 3
+    lo = 0 if xyz_first else c
+    g_xyz = g_new_xyz = g_points = None
+    if need_xyz or need_new_xyz:  # in the networks the coordinates need none
+        g_xyz_part = g_out[..., lo:lo + 3].float()  # the coordinates' gradient is float32 (an exact upcast)
+        if g_gxyz is not None:
+            g_xyz_part = g_xyz_part + g_gxyz
+        g_xyz_part = g_xyz_part.contiguous()
+        if need_xyz:
+            g_xyz = group_point_grad(g_xyz_part, idx, (idx.shape[0], n, 3))
+        if need_new_xyz:
+            g_new_xyz = -g_xyz_part.sum(dim=2)
+    if has_points:
+        g_feat = (g_out[..., 3:] if xyz_first else g_out[..., :c]).contiguous()
+        g_points = group_point_grad(g_feat, idx, (idx.shape[0], n, c))
+    return g_xyz, g_new_xyz, g_points
+
+
+class _GroupConcat(torch.autograd.Function):
     @staticmethod
     def forward(ctx, xyz, new_xyz, points, idx, xyz_first):
         b, n, _ = xyz.shape
         _, m, s = idx.shape
         c = 0 if points is None else points.shape[2]
-        dtype = torch.float32 if points is None else points.dtype
-        out = torch.empty((b, m, s, 3 + c), dtype=dtype, device=xyz.device)
-        gxyz = torch.empty((b, m, s, 3), dtype=torch.float32, device=xyz.device)
-        if out.numel():
-            with on_device(xyz):
-                if dtype == torch.float32:
-                    rc = _lib.load().pn2_group_concat(b, n, c, m, s, ptr(xyz), ptr(new_xyz), ptr(points), ptr(idx),
-                                                      1 if xyz_first else 0, ptr(out), ptr(gxyz), stream_ptr(xyz.device))
-                else:
-                    rc = _lib.load().pn2_group_concat_typed(DTYPE_CODES[dtype], b, n, c, m, s, ptr(xyz), ptr(new_xyz), ptr(points),
-                                                            ptr(idx), 1 if xyz_first else 0, ptr(out), ptr(gxyz),
-                                                            stream_ptr(xyz.device))
-            _lib.check(rc, "pn2_group_concat")
         ctx.save_for_backward(idx)
         ctx.meta = (b, n, c, m, s, bool(xyz_first), points is not None)
-        ctx.dtype = dtype
-        return out, gxyz
+        ctx.dtype = torch.float32 if points is None else points.dtype
+        return group_and_concat_launch(xyz, new_xyz, points, idx, xyz_first)
 
     @staticmethod
     def backward(ctx, g_out, g_gxyz):
         (idx,) = ctx.saved_tensors
-        b, n, c, m, s, xyz_first, has_points = ctx.meta
-        lo = 0 if xyz_first else c
-        g_out = g_out.to(ctx.dtype)
-        g_xyz = g_new_xyz = g_points = None
-        if ctx.needs_input_grad[0] or ctx.needs_input_grad[1]:  # in the networks the coordinates need none
-            g_xyz_part = g_out[..., lo:lo + 3].float()  # the coordinates' gradient is float32 (an exact upcast)
-            if g_gxyz is not None:
-                g_xyz_part = g_xyz_part + g_gxyz
-            g_xyz_part = g_xyz_part.contiguous()
-            if ctx.needs_input_grad[0]:
-                g_xyz = group_point_grad(g_xyz_part, idx, (b, n, 3))
-            if ctx.needs_input_grad[1]:
-                g_new_xyz = -g_xyz_part.sum(dim=2)
-        if has_points:
-            g_feat = (g_out[..., 3:] if xyz_first else g_out[..., :c]).contiguous()
-            g_points = group_point_grad(g_feat, idx, (b, n, c))
-        return g_xyz, g_new_xyz, g_points, None, None
+        _, n, _, _, _, xyz_first, has_points = ctx.meta
+        return (*group_and_concat_backward(g_out.to(ctx.dtype), g_gxyz, idx, n, xyz_first, has_points,
+                                           ctx.needs_input_grad[0], ctx.needs_input_grad[1]), None, None)
 
 
 def group_and_concat(xyz, new_xyz, points, idx, xyz_first: bool = True):
@@ -96,6 +110,8 @@ def group_and_concat(xyz, new_xyz, points, idx, xyz_first: bool = True):
         same_device(xyz, new_xyz, idx)
     if idx.dim() != 3 or idx.shape[0] != xyz.shape[0] or new_xyz.shape[:2] != idx.shape[:2]:
         raise ValueError("idx must be (batch_size, npoint, nsample) matching new_xyz")
+    if torch.compiler.is_compiling():
+        return torch.ops.pn2.group_and_concat(xyz, new_xyz, points, idx, bool(xyz_first))
     return _GroupConcat.apply(xyz, new_xyz, points, idx, xyz_first)
 
 
@@ -325,7 +341,7 @@ def pointnet_sa_module_msg(xyz, points, npoint, radius_list: Sequence[float], ns
         tails = None if mlp_list is None else [
             _sa_mlp_route(mlp_list[i], xyz, points, use_xyz, scope, f"conv{i}", bn, is_training, bn_decay)
             for i in range(len(radius_list))]
-        to_kernel = bool(tails) and all(t is not None for t in tails)
+        to_kernel = tails is not None and len(tails) > 0 and all(t is not None for t in tails)
         # one call: the sampling pass and every scale's ball query (+ centred grouped xyz when they are the features)
         _, new_xyz, idx_list, _, gxyz_list = sample_group_msg(npoint, radius_list, nsample_list, xyz, center=True,
                                                               want_grouped=points is None and not to_kernel,

@@ -58,6 +58,15 @@ def sample_group(npoint: int, radius: float, nsample: int, xyz: torch.Tensor, ce
     b, n, _ = xyz.shape
     dev = xyz.device
     lens = device_lengths(lengths, b, n, dev, "sample_group")
+    if torch.compiler.is_compiling():
+        *res, grouped = torch.ops.pn2.sample_group(npoint, radius, nsample, xyz.detach(), bool(center), bool(want_grouped), lens)
+        return (*res, grouped if want_grouped else None)
+    return sample_group_launch(npoint, radius, nsample, xyz, center, want_grouped, lens)
+
+
+def sample_group_launch(npoint: int, radius: float, nsample: int, xyz: torch.Tensor, center: bool, want_grouped: bool, lens):
+    b, n, _ = xyz.shape
+    dev = xyz.device
     fps_idx = torch.empty((b, npoint), dtype=torch.int32, device=dev)
     new_xyz = torch.empty((b, npoint, 3), dtype=torch.float32, device=dev)
     idx = torch.empty((b, npoint, nsample), dtype=torch.int32, device=dev)
@@ -87,16 +96,28 @@ def sample_group_msg(npoint: int, radius_list, nsample_list, xyz: torch.Tensor, 
     ``lengths``: as for sample_group.
 
     Returns (fps_idx, new_xyz, [idx_k], [pts_cnt_k], [grouped_xyz_k] or None)."""
-    import ctypes
     if len(radius_list) != len(nsample_list) or not len(radius_list):
         raise ValueError("radius_list and nsample_list must be non-empty and of equal length")
-    k = len(radius_list)
     npoint, _, _, xyz = _check_layer_args(npoint, radius_list[0], nsample_list[0], xyz)
     for r, s in zip(radius_list, nsample_list):
         _check_layer_args(npoint, r, s, xyz)
     b, n, _ = xyz.shape
     dev = xyz.device
     lens = device_lengths(lengths, b, n, dev, "sample_group_msg")
+    if torch.compiler.is_compiling():
+        fps_idx, new_xyz, idx, cnt, grouped = torch.ops.pn2.sample_group_msg(npoint, [float(r) for r in radius_list],
+                                                                             [int(s) for s in nsample_list], xyz.detach(),
+                                                                             bool(center), bool(want_grouped), lens)
+        return fps_idx, new_xyz, idx, cnt, grouped if want_grouped else None
+    return sample_group_msg_launch(npoint, radius_list, nsample_list, xyz, center, want_grouped, lens)
+
+
+def sample_group_msg_launch(npoint: int, radius_list, nsample_list, xyz: torch.Tensor, center: bool, want_grouped: bool,
+                            lens):
+    import ctypes
+    k = len(radius_list)
+    b, n, _ = xyz.shape
+    dev = xyz.device
     fps_idx = torch.empty((b, npoint), dtype=torch.int32, device=dev)
     new_xyz = torch.empty((b, npoint, 3), dtype=torch.float32, device=dev)
     idx = [torch.empty((b, npoint, int(s)), dtype=torch.int32, device=dev) for s in nsample_list]
@@ -157,6 +178,16 @@ def sample_knn(npoint: int, k: int, xyz: torch.Tensor, center: bool = True, want
         raise ValueError(f"sample_knn expects k <= {KNN_MAX_K}, got k={k}")
     dev = xyz.device
     lens = device_lengths(lengths, b, n, dev, "sample_knn")
+    if torch.compiler.is_compiling():
+        fps_idx, new_xyz, idx, dist, grouped = torch.ops.pn2.sample_knn(npoint, k, xyz.detach(), bool(center),
+                                                                        bool(want_grouped), bool(want_dist), lens)
+        return fps_idx, new_xyz, idx, dist if want_dist else None, grouped if want_grouped else None
+    return sample_knn_launch(npoint, k, xyz, center, want_grouped, want_dist, lens)
+
+
+def sample_knn_launch(npoint: int, k: int, xyz: torch.Tensor, center: bool, want_grouped: bool, want_dist: bool, lens):
+    b, n, _ = xyz.shape
+    dev = xyz.device
     fps_idx = torch.empty((b, npoint), dtype=torch.int32, device=dev)
     new_xyz = torch.empty((b, npoint, 3), dtype=torch.float32, device=dev)
     idx = torch.empty((b, npoint, k), dtype=torch.int32, device=dev)
@@ -195,6 +226,13 @@ def ball_group(radius: float, nsample: int, xyz1: torch.Tensor, xyz2: torch.Tens
     same_device(xyz1, xyz2)
     if xyz1.dim() != 3 or xyz1.shape[2] != 3 or xyz2.dim() != 3 or xyz2.shape[2] != 3 or xyz1.shape[0] != xyz2.shape[0]:
         raise ValueError("QueryBallPoint expects (batch_size, ndataset, 3) xyz1 and (batch_size, npoint, 3) xyz2")
+    if torch.compiler.is_compiling():
+        idx, cnt, g = torch.ops.pn2.ball_group(radius, nsample, xyz1.detach(), xyz2.detach(), bool(center), bool(want_grouped))
+        return idx, cnt, g if want_grouped else None
+    return ball_group_launch(radius, nsample, xyz1, xyz2, center, want_grouped)
+
+
+def ball_group_launch(radius: float, nsample: int, xyz1: torch.Tensor, xyz2: torch.Tensor, center: bool, want_grouped: bool):
     b, n, _ = xyz1.shape
     m = xyz2.shape[1]
     lib = _lib.load()

@@ -43,6 +43,14 @@ def query_ball_point(radius: float, nsample: int, xyz1: torch.Tensor, xyz2: torc
     if n <= 0 and b * m:
         raise ValueError("QueryBallPoint expects a non-empty xyz1")
     lens = device_lengths(lengths, b, n, xyz1.device, "QueryBallPoint")
+    if torch.compiler.is_compiling():
+        return torch.ops.pn2.query_ball_point(radius, nsample, xyz1.detach(), xyz2.detach(), lens)
+    return query_ball_point_launch(radius, nsample, xyz1, xyz2, lens)
+
+
+def query_ball_point_launch(radius: float, nsample: int, xyz1: torch.Tensor, xyz2: torch.Tensor, lens):
+    b, n, _ = xyz1.shape
+    m = xyz2.shape[1]
     idx = torch.empty((b, m, nsample), dtype=torch.int32, device=xyz1.device)
     pts_cnt = torch.empty((b, m), dtype=torch.int32, device=xyz1.device)
     if b * m:
@@ -80,6 +88,12 @@ def select_top_k(k: int, dist: torch.Tensor):
     dist = require_cuda(dist, "dist", torch.float32)
     if dist.dim() != 3:
         raise ValueError(f"SelectionSort expects (b,m,n) dist shape, got {tuple(dist.shape)}")
+    if torch.compiler.is_compiling():
+        return torch.ops.pn2.select_top_k(k, dist.detach())
+    return select_top_k_launch(k, dist)
+
+
+def select_top_k_launch(k: int, dist: torch.Tensor):
     b, m, n = dist.shape
     outi = torch.empty((b, m, n), dtype=torch.int32, device=dist.device)
     out = torch.empty((b, m, n), dtype=torch.float32, device=dist.device)
@@ -90,31 +104,33 @@ def select_top_k(k: int, dist: torch.Tensor):
     return outi, out
 
 
+def group_point_launch(points: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
+    b, n, c = points.shape
+    _, m, s = idx.shape
+    out = torch.empty((b, m, s, c), dtype=points.dtype, device=points.device)
+    if out.numel():
+        with on_device(points):
+            if points.dtype == torch.float32:
+                rc = _lib.load().pn2_group_point(b, n, c, m, s, ptr(points), ptr(idx), ptr(out),
+                                                 stream_ptr(points.device))
+            else:
+                rc = _lib.load().pn2_group_point_typed(DTYPE_CODES[points.dtype], b, n, c, m, s, ptr(points), ptr(idx),
+                                                       ptr(out), stream_ptr(points.device))
+        _lib.check(rc, "pn2_group_point")
+    return out
+
+
 class _GroupPoint(torch.autograd.Function):
     @staticmethod
     def forward(ctx, points, idx):
-        b, n, c = points.shape
-        _, m, s = idx.shape
-        out = torch.empty((b, m, s, c), dtype=points.dtype, device=points.device)
-        if out.numel():
-            with on_device(points):
-                if points.dtype == torch.float32:
-                    rc = _lib.load().pn2_group_point(b, n, c, m, s, ptr(points), ptr(idx), ptr(out),
-                                                     stream_ptr(points.device))
-                else:
-                    rc = _lib.load().pn2_group_point_typed(DTYPE_CODES[points.dtype], b, n, c, m, s, ptr(points), ptr(idx),
-                                                           ptr(out), stream_ptr(points.device))
-            _lib.check(rc, "pn2_group_point")
         ctx.save_for_backward(idx)
-        ctx.shape = (b, n, c)
+        ctx.shape = tuple(points.shape)
         ctx.dtype = points.dtype
-        return out
+        return group_point_launch(points, idx)
 
     @staticmethod
     def backward(ctx, grad_out):
         (idx,) = ctx.saved_tensors
-        b, n, c = ctx.shape
-        _, m, s = idx.shape
         return group_point_grad(grad_out.to(ctx.dtype).contiguous(), idx, ctx.shape), None
 
 
@@ -173,6 +189,8 @@ def group_point(points: torch.Tensor, idx: torch.Tensor) -> torch.Tensor:
         raise ValueError(f"GroupPoint expects (batch_size, npoints, nsample) idx shape, got {tuple(idx.shape)}")
     if points.shape[1] <= 0 and idx.numel():
         raise ValueError("GroupPoint expects a non-empty points tensor")
+    if torch.compiler.is_compiling():
+        return torch.ops.pn2.group_point(points, idx)
     return _GroupPoint.apply(points, idx)
 
 
@@ -214,19 +232,29 @@ def knn_point(k: int, xyz1: torch.Tensor, xyz2: torch.Tensor, *, lengths=None, q
     lens = device_lengths(lengths, b, n, xyz1.device, "knn_point")
     qlens = device_lengths(query_lengths, b, m, xyz1.device, "knn_point") if m else None
     if c == 3 and k <= 128:
-        val = torch.empty((b, m, k), dtype=torch.float32, device=xyz1.device)
-        idx = torch.empty((b, m, k), dtype=torch.int32, device=xyz1.device)
-        if b * m:
-            with on_device(xyz1):
-                if ragged:
-                    rc = _lib.load().pn2_knn_point_ragged(b, n, m, k, ptr(xyz1.detach()), ptr(lens), ptr(xyz2.detach()), ptr(qlens),
-                                                          ptr(val), ptr(idx), stream_ptr(xyz1.device))
-                else:
-                    rc = _lib.load().pn2_knn_point(b, n, m, k, ptr(xyz1.detach()), ptr(xyz2.detach()), ptr(val), ptr(idx),
-                                                   stream_ptr(xyz1.device))
-            _lib.check(rc, "pn2_knn_point")
-        return val, idx
+        if torch.compiler.is_compiling():
+            return torch.ops.pn2.knn_point(k, xyz1.detach(), xyz2.detach(), lens, qlens)
+        return knn_point_launch(k, xyz1, xyz2, lens, qlens)
     diff = xyz1.unsqueeze(1) - xyz2.unsqueeze(2)  # (b,m,n,c): tile(xyz1) - tile(xyz2), tf_grouping.py:64-66
     dist = (diff * diff).sum(-1)
     outi, out = select_top_k(k, dist)
     return out[:, :, :k].contiguous(), outi[:, :, :k].contiguous()
+
+
+def knn_point_launch(k: int, xyz1: torch.Tensor, xyz2: torch.Tensor, lens, qlens):
+    """knn_point's kernel (3-D points, k <= 128): (val, idx)"""
+    b, n, _ = xyz1.shape
+    m = xyz2.shape[1]
+    ragged = lens is not None or qlens is not None
+    val = torch.empty((b, m, k), dtype=torch.float32, device=xyz1.device)
+    idx = torch.empty((b, m, k), dtype=torch.int32, device=xyz1.device)
+    if b * m:
+        with on_device(xyz1):
+            if ragged:
+                rc = _lib.load().pn2_knn_point_ragged(b, n, m, k, ptr(xyz1.detach()), ptr(lens), ptr(xyz2.detach()), ptr(qlens),
+                                                      ptr(val), ptr(idx), stream_ptr(xyz1.device))
+            else:
+                rc = _lib.load().pn2_knn_point(b, n, m, k, ptr(xyz1.detach()), ptr(xyz2.detach()), ptr(val), ptr(idx),
+                                               stream_ptr(xyz1.device))
+        _lib.check(rc, "pn2_knn_point")
+    return val, idx

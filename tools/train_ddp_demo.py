@@ -99,6 +99,9 @@ def main() -> None:
                     help="mixed precision: torch.autocast in bfloat16, or float16 with a GradScaler")
     ap.add_argument("--deterministic", action="store_true",
                     help="torch.use_deterministic_algorithms(True): run-to-run identical weights; prints their SHA-256")
+    ap.add_argument("--compile", choices=["none", "cudagraphs", "inductor"], default="none",
+                    help="torch.compile the forward: cudagraphs = dynamo + AOTAutograd + CUDA graphs, inductor = "
+                         "mode='reduce-overhead' (the library's ops are pn2:: operators inside the graph)")
     ap.add_argument("--ragged", action="store_true", help="cloud lengths from U[N/2, N], NaN padding, passed as lengths=")
     ap.add_argument("--scene-crops", action="store_true",
                     help="sem_seg only: train on seeded crops of synthetic rooms drawn on the GPU by scene.sample_crops")
@@ -156,6 +159,12 @@ def main() -> None:
     model = model.to(dev)
     net = torch.nn.parallel.DistributedDataParallel(model, device_ids=[local]) if world > 1 else model
     opt = torch.optim.Adam(net.parameters(), lr=args.lr)
+    if args.compile == "cudagraphs":
+        fwd = torch.compile(net, backend="cudagraphs")
+    elif args.compile == "inductor":
+        fwd = torch.compile(net, mode="reduce-overhead")
+    else:
+        fwd = net
     amp_dtype = {"none": None, "bf16": torch.bfloat16, "fp16": torch.float16}[args.amp]
     scaler = torch.amp.GradScaler("cuda") if args.amp == "fp16" else None
 
@@ -221,9 +230,9 @@ def main() -> None:
         net.train()
         with torch.autocast(device_type="cuda", dtype=amp_dtype, enabled=amp_dtype is not None):
             if args.model == "part_seg_msg":
-                pred, _ = net(xyz, lab, lengths=lengths)
+                pred, _ = fwd(xyz, lab, lengths=lengths)
             else:
-                pred, _ = net(xyz, lengths=lengths)
+                pred, _ = fwd(xyz, lengths=lengths)
             if part:
                 loss = nets.part_seg_loss(pred, lab_part, lengths=lengths)
             elif args.scene_crops:  # the crops' labels and sample weights (label weight on core rows)
@@ -311,7 +320,7 @@ def main() -> None:
                "clouds_per_s": args.batch / float(np.median(steady)),
                "data": ("synthetic room crops" if args.scene_crops else
                         "synthetic part shapes" if part else "synthetic parametric shapes"),
-               "deterministic": args.deterministic, "ragged": args.ragged, "scene_crops": args.scene_crops,
+               "deterministic": args.deterministic, "compile": args.compile, "ragged": args.ragged, "scene_crops": args.scene_crops,
                "shape_set": args.shape_set}
         if voted is not None:
             out["voted"] = voted
