@@ -332,8 +332,9 @@ static int launch_group_rows(int b, int n, int c, int m, int nsample, const floa
     if (std::is_same<T, float>::value && HAS_XYZ && c >= 8 && c <= 64 && c % 4 == 0 && aligned_to(points, 16) && aligned_to(out, 16)) {
         // vectorised tail (see group_concat_vec_kernel).  Measured: it wins at C = 64 (30.7 against 35.6 us, cfg4 SA256) and
         // loses to the row kernel below from C = 128 up (C = 320 + 3, S = 64: 125 against 94 us), so only narrow rows take it
+        // c4 <= 16 <= LPR: one pass over the row's vectors, so the last lane never loads a next pass's first vector
         const int c4 = c / 4;
-        const int lpr = c4 <= 8 ? 8 : (c4 <= 16 ? 16 : 32);
+        const int lpr = c4 <= 8 ? 8 : 16;
         constexpr int R = 2;
         const unsigned rows_per_block = (kCopyThreads / 32) * (32 / lpr) * R;
         unsigned gx = (rpc + rows_per_block - 1) / rows_per_block;
@@ -344,8 +345,7 @@ static int launch_group_rows(int b, int n, int c, int m, int nsample, const floa
         const float4* p4 = reinterpret_cast<const float4*>(points);
         float* o = reinterpret_cast<float*>(out);  // (float here: the condition above)
         if (lpr == 8) group_concat_vec_kernel<8, R><<<grid, kCopyThreads, 0, st>>>(n, c4, nsample, rpc, xyz, new_xyz, p4, idx, xyz_lo, feat_lo, o, grouped_xyz);
-        else if (lpr == 16) group_concat_vec_kernel<16, R><<<grid, kCopyThreads, 0, st>>>(n, c4, nsample, rpc, xyz, new_xyz, p4, idx, xyz_lo, feat_lo, o, grouped_xyz);
-        else group_concat_vec_kernel<32, R><<<grid, kCopyThreads, 0, st>>>(n, c4, nsample, rpc, xyz, new_xyz, p4, idx, xyz_lo, feat_lo, o, grouped_xyz);
+        else group_concat_vec_kernel<16, R><<<grid, kCopyThreads, 0, st>>>(n, c4, nsample, rpc, xyz, new_xyz, p4, idx, xyz_lo, feat_lo, o, grouped_xyz);
         return finish_launch();
     }
     const int lpr = w <= 4 ? 4 : (w <= 8 ? 8 : (w <= 16 ? 16 : 32));
@@ -411,6 +411,9 @@ round_to_kernel(unsigned long long total, const float* __restrict__ src, T* __re
 // k rounds of "find the first minimum of v[s..n) (strict '<'), swap it into position s", indices
 // carried along — the same permutation the reference's thread-per-row loop produces, with the
 // argmin parallelised across the warp on the key (value, position).
+// NaN, as the reference's scan `if (v[t] < v[min]) min = t` from min = s treats it: a NaN at v[s]
+// is never replaced (nothing is '<' NaN), so the round keeps s; otherwise NaN candidates are
+// never taken, and the round picks the first minimum of the non-NaN values.
 __global__ void __launch_bounds__(kCopyThreads)
 selection_sort_kernel(int n, int k, long long rows, const float* __restrict__ dist, int* __restrict__ outi,
                       float* __restrict__ out) {
@@ -427,11 +430,13 @@ selection_sort_kernel(int n, int k, long long rows, const float* __restrict__ di
     __syncwarp();
     const int rounds = k < n ? k : n;
     for (int s = 0; s < rounds; ++s) {
+        const float vs = v[s];
+        if (vs != vs) continue;  // warp-uniform: v[s] is NaN, the round keeps s
         float bv = 0.f;
         int bt = -1;
         for (int t = s + lane; t < n; t += 32) {
             const float x = v[t];
-            if (bt < 0 || x < bv) {  // ascending t within a lane: strict '<' keeps the earliest
+            if (bt < 0 ? x == x : x < bv) {  // ascending t within a lane: strict '<' keeps the earliest; NaN never
                 bv = x;
                 bt = t;
             }
@@ -440,7 +445,7 @@ selection_sort_kernel(int n, int k, long long rows, const float* __restrict__ di
         for (int off = 16; off > 0; off >>= 1) {
             const float ov = __shfl_xor_sync(kFullMask, bv, off);
             const int ot = __shfl_xor_sync(kFullMask, bt, off);
-            // NaN-free total order on (value, position); lanes without candidates carry bt = -1
+            // total order on non-NaN (value, position); lanes without candidates carry bt = -1
             const bool take = (ot >= 0) && (bt < 0 || ov < bv || (ov == bv && ot < bt));
             if (take) {
                 bv = ov;
