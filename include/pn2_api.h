@@ -314,6 +314,8 @@ int pn2_three_interpolate_grad_det_ragged_typed(int dtype, int b, int n, int c, 
  * updates them from the real rows as torch's BatchNorm1d would from a batch of them alone: unbiased variance
  * var * cnt / max(cnt - 1, 1), weight `momentum`, or 1 / *num_batches_tracked (read on the device, already incremented by
  * the caller) when momentum < 0.  gamma / beta may be NULL (affine = False).
+ * No real row at all (rows > 0, every keep 0): the mean is 0 / 0 as in layers.masked_batch_norm, so save_mean,
+ * save_invstd, running_mean and running_var become NaN; y is all 0, and the backward writes dx 0 and dgamma = dbeta = 0.
  * Backward (y and the saved statistics from the forward): g = keep ? dy * [y > 0] : 0, xhat = (x - mean) * invstd,
  *   dx = keep ? gamma * invstd * (g - sum(g) / cnt - xhat * sum(g * xhat) / cnt) : 0,  dgamma = sum(g * xhat),
  *   dbeta = sum(g)   (sums over the real rows; dgamma / dbeta may be NULL, gamma NULL means 1).

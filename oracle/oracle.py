@@ -289,6 +289,70 @@ def oracle_mlp_rows_f32(x, layers):
     return out
 
 
+def _u8(a):
+    return np.ascontiguousarray(a, dtype=np.uint8)
+
+
+def oracle_mbn_stats(x, keep, eps: float, momentum: float = 0.1, nbt: int = 1, running_mean=None, running_var=None):
+    """The masked batch norm's statistics (csrc/masked_bn.cu's merge order) of x (rows, c), the float32 values of the
+    tensor, over the rows where keep (rows,) is nonzero.  Returns (mean, var_eps, count, running_mean, running_var):
+    var_eps is the float32 var + eps the kernel takes rsqrtf of; the running buffers are updated copies (None when
+    not given).  ``momentum`` < 0 is the cumulative average 1 / nbt."""
+    x, keep = _f(x), _u8(keep)
+    rows, c = x.shape
+    mean, var_eps = np.empty(c, _F), np.empty(c, _F)
+    count = c_int(0)
+    rm = None if running_mean is None else _f(running_mean).copy()
+    rv = None if running_var is None else _f(running_var).copy()
+    lib().oracle_mbn_stats(c_int(rows), c_int(c), _p(x), _p(keep), c_float(eps), c_float(momentum),
+                           ctypes.c_longlong(nbt), None if rm is None else _p(rm), None if rv is None else _p(rv),
+                           _p(mean), _p(var_eps), ctypes.byref(count))
+    return mean, var_eps, count.value, rm, rv
+
+
+def oracle_mbn_norm_relu(x, keep, mean, invstd, gamma=None, beta=None):
+    """y (rows, c) float32 before the rounding to the tensor's dtype; padding rows 0."""
+    x, keep, mean, invstd = _f(x), _u8(keep), _f(mean), _f(invstd)
+    gamma, beta = _opt(gamma), _opt(beta)
+    rows, c = x.shape
+    y = np.empty((rows, c), _F)
+    lib().oracle_mbn_norm_relu(c_int(rows), c_int(c), _p(x), _p(keep), _p(mean), _p(invstd),
+                               None if gamma is None else _p(gamma), None if beta is None else _p(beta), _p(y))
+    return y
+
+
+def oracle_mbn_backward(dy, x, y, keep, mean, invstd, gamma=None):
+    """(dx float32 before rounding, dgamma, dbeta) of the plain form from the float32 values of dy, x and y."""
+    dy, x, y, keep, mean, invstd, gamma = _f(dy), _f(x), _f(y), _u8(keep), _f(mean), _f(invstd), _opt(gamma)
+    rows, c = x.shape
+    dx = np.empty((rows, c), _F)
+    dg, db = np.empty(c, _F), np.empty(c, _F)
+    lib().oracle_mbn_backward(c_int(rows), c_int(c), _p(dy), _p(x), _p(y), _p(keep),
+                              None if gamma is None else _p(gamma), _p(mean), _p(invstd), _p(dx), _p(dg), _p(db))
+    return dx, dg, db
+
+
+def oracle_mbn_max_pool(y, keep):
+    """(out (b, c) float32, argmax (b, c) int32) of y (b, n, c), the values as rounded to the tensor's dtype."""
+    y, keep = _f(y), _u8(keep)
+    b, n, c = y.shape
+    out, arg = np.empty((b, c), _F), np.empty((b, c), _I)
+    lib().oracle_mbn_max_pool(c_int(b), c_int(n), c_int(c), _p(y), _p(keep), _p(out), _p(arg))
+    return out, arg
+
+
+def oracle_mbn_max_backward(dout, x, out, argmax, keep, mean, invstd, gamma=None):
+    """(dx (b, n, c) float32 before rounding, dgamma, dbeta) of the max-pooled form."""
+    dout, x, out, argmax, keep = _f(dout), _f(x), _f(out), _i(argmax), _u8(keep)
+    mean, invstd, gamma = _f(mean), _f(invstd), _opt(gamma)
+    b, n, c = x.shape
+    dx = np.empty((b, n, c), _F)
+    dg, db = np.empty(c, _F), np.empty(c, _F)
+    lib().oracle_mbn_max_backward(c_int(b), c_int(n), c_int(c), _p(dout), _p(x), _p(out), _p(argmax), _p(keep),
+                                  None if gamma is None else _p(gamma), _p(mean), _p(invstd), _p(dx), _p(dg), _p(db))
+    return dx, dg, db
+
+
 # ------------------------------------------------------------------ reference CPU functions
 def refcpu_query_ball_point(radius: float, nsample: int, xyz1, xyz2):
     """tf_ops/grouping/test/query_ball_point.cpp:19 (no pts_cnt output). idx pre-zeroed."""

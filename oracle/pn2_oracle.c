@@ -549,3 +549,290 @@ int oracle_mlp_rows_f32(long long rows, int cin, int nlayers, const int *widths,
     free(shift);
     return 0;
 }
+
+/* ---- masked batch norm + ReLU (csrc/masked_bn.cu), float32 -----------------------------------
+ * A restatement of the documented order, not of the kernels' code: every result but invstd is
+ * pinned bit for bit.  rsqrtf on the device is not correctly rounded, so the statistics return
+ * the float32 var + eps it is applied to, and the later stages take the device's invstd.
+ *
+ * Geometry (a function of c): vec = 4 when c % 4 == 0 else 1; tx = the power of two >= the
+ * lanes ceil(c / vec), capped at 32; ty = 256 / tx; chunk_rows = 32 * ty.  Row o of a chunk
+ * belongs to thread y = o % ty, which holds it in group (o / ty) / 8; a thread's rows ascend.
+ * Statistics per column: per group, s = the sum from +0 of its 8 rows (padding adds 0),
+ * gmean = s * (1 / ng), q = fmaf(d, d, q) over the real rows; the groups Chan-merged in order;
+ * the ty threads in a tree (slot y absorbs slot y + s, s = ty/2 .. 1); the chunks split into 32
+ * contiguous ranges of ceil(chunks / 32), each merged in order, then a tree over the 32 ranges.
+ * Chan's merge of (nb, mb, m2b) into (na, ma, m2a): wb = nb / n, d = mb - ma,
+ * ma = fmaf(d, wb, ma), m2a = (m2a + m2b) + (d * d) * (na * wb).
+ * With no real row at all the mean is 0 / 0 (NaN), as layers.masked_batch_norm computes it.
+ * Backward sums: g = y > 0 ? dy : 0, xhat = (x - mean) * invstd, each thread adds its real rows
+ * in order (sg += g, sgx = fmaf(g, xhat, sgx)), then the same two trees with plain adds.
+ * ------------------------------------------------------------------------------------------ */
+#define MBN_THREADS 256
+#define MBN_ROWS 8
+#define MBN_GROUPS 4
+#define MBN_MERGE_WARPS 32
+
+static int mbn_ty(int c) {
+    const int vec = (c % 4 == 0) ? 4 : 1;
+    const int lanes = (c + vec - 1) / vec;
+    int tx = 1;
+    while (tx < lanes && tx < 32) tx <<= 1;
+    return MBN_THREADS / tx;
+}
+
+static void mbn_chan(int *na, float *ma, float *m2a, int nb, float mb, float m2b) {
+    if (nb == 0) return;
+    if (*na == 0) {
+        *na = nb;
+        *ma = mb;
+        *m2a = m2b;
+        return;
+    }
+    const int n = *na + nb;
+    const float wb = (float)nb / (float)n;
+    const float wab = (float)*na * wb;
+    const float d = mb - *ma;
+    *ma = fmaf(d, wb, *ma);
+    *m2a = (*m2a + m2b) + (d * d) * wab;
+    *na = n;
+}
+
+/* chunks of one column: the per-thread merge of its groups, then the tree over ty */
+static void mbn_chunk_stats(long long rows, int c, int ty, long long chunk, int col, const float *x,
+                            const unsigned char *keep, int *sn, float *smean, float *sm2) {
+    const long long base = chunk * (long long)ty * MBN_ROWS * MBN_GROUPS;
+    for (int y = 0; y < ty; ++y) {
+        int n = 0;
+        float mean = 0.f, m2 = 0.f;
+        for (int grp = 0; grp < MBN_GROUPS; ++grp) {
+            float v[MBN_ROWS];
+            int kf[MBN_ROWS], ng = 0;
+            for (int k = 0; k < MBN_ROWS; ++k) {
+                const long long r = base + y + (long long)(grp * MBN_ROWS + k) * ty;
+                kf[k] = r < rows && keep[r] != 0;
+                v[k] = kf[k] ? x[(size_t)r * c + col] : 0.f;
+                ng += kf[k];
+            }
+            if (ng == 0) continue;
+            const float inv = 1.0f / (float)ng;
+            float s = 0.f;
+            for (int k = 0; k < MBN_ROWS; ++k) s = s + v[k];
+            const float gm = s * inv;
+            float q = 0.f;
+            for (int k = 0; k < MBN_ROWS; ++k) {
+                const float d = kf[k] ? v[k] - gm : 0.f;
+                q = fmaf(d, d, q);
+            }
+            mbn_chan(&n, &mean, &m2, ng, gm, q);
+        }
+        sn[y] = n;
+        smean[y] = mean;
+        sm2[y] = m2;
+    }
+    for (int s = ty >> 1; s > 0; s >>= 1)
+        for (int y = 0; y < s; ++y) mbn_chan(&sn[y], &smean[y], &sm2[y], sn[y + s], smean[y + s], sm2[y + s]);
+}
+
+/* x (rows, c) float32 values, keep (rows,).  Writes mean (c), var_eps (c) = var + eps with var
+ * = M2 / cnt (biased) and *count = cnt.  When running_mean is given, updates running_mean /
+ * running_var as the kernel does: f = momentum, or 1 / (float)nbt when momentum < 0;
+ * unbiased = var * cnt / max(cnt - 1, 1); r = r * (1 - f) + stat * f. */
+void oracle_mbn_stats(int rows, int c, const float *x, const unsigned char *keep, float eps, float momentum,
+                      long long nbt, float *running_mean, float *running_var, float *mean, float *var_eps,
+                      int *count) {
+    const int ty = mbn_ty(c);
+    const long long chunk_rows = (long long)ty * MBN_ROWS * MBN_GROUPS;
+    const long long chunks = rows > 0 ? (rows + chunk_rows - 1) / chunk_rows : 0;
+    int *pcnt = (int *)malloc(sizeof(int) * (size_t)(chunks + 1));
+    float *pmean = (float *)malloc(sizeof(float) * (size_t)(chunks + 1));
+    float *pm2 = (float *)malloc(sizeof(float) * (size_t)(chunks + 1));
+    int *sn = (int *)malloc(sizeof(int) * MBN_THREADS);
+    float *smean = (float *)malloc(sizeof(float) * MBN_THREADS);
+    float *sm2 = (float *)malloc(sizeof(float) * MBN_THREADS);
+    const long long per = (chunks + MBN_MERGE_WARPS - 1) / MBN_MERGE_WARPS;
+    for (int col = 0; col < c; ++col) {
+        for (long long k = 0; k < chunks; ++k) {
+            mbn_chunk_stats(rows, c, ty, k, col, x, keep, sn, smean, sm2);
+            pcnt[k] = sn[0];
+            pmean[k] = smean[0];
+            pm2[k] = sm2[0];
+        }
+        int wn[MBN_MERGE_WARPS];
+        float wmean[MBN_MERGE_WARPS], wm2[MBN_MERGE_WARPS];
+        for (int w = 0; w < MBN_MERGE_WARPS; ++w) {
+            const long long k0 = (long long)w * per < chunks ? (long long)w * per : chunks;
+            const long long k1 = k0 + per < chunks ? k0 + per : chunks;
+            wn[w] = 0;
+            wmean[w] = 0.f;
+            wm2[w] = 0.f;
+            for (long long k = k0; k < k1; ++k) mbn_chan(&wn[w], &wmean[w], &wm2[w], pcnt[k], pmean[k], pm2[k]);
+        }
+        for (int s = MBN_MERGE_WARPS >> 1; s > 0; s >>= 1)
+            for (int w = 0; w < s; ++w) mbn_chan(&wn[w], &wmean[w], &wm2[w], wn[w + s], wmean[w + s], wm2[w + s]);
+        const float cnt = (float)wn[0];
+        const float mu = wn[0] > 0 ? wmean[0] : 0.f / cnt;
+        const float var = wm2[0] / cnt;
+        mean[col] = mu;
+        var_eps[col] = var + eps;
+        *count = wn[0];
+        if (running_mean) {
+            const float f = momentum < 0.f ? 1.0f / (float)nbt : momentum;
+            const float keepf = 1.0f - f;
+            const float unbiased = (var * cnt) / fmaxf(cnt - 1.0f, 1.0f);
+            running_mean[col] = running_mean[col] * keepf + mu * f;
+            running_var[col] = running_var[col] * keepf + unbiased * f;
+        }
+    }
+    free(pcnt);
+    free(pmean);
+    free(pm2);
+    free(sn);
+    free(smean);
+    free(sm2);
+}
+
+/* y = keep ? (t < 0 ? 0 : t) : 0 with t = fmaf(x - mean, invstd * gamma, beta) (gamma NULL: 1,
+ * beta NULL: 0).  float32, before the rounding to the tensor's dtype. */
+void oracle_mbn_norm_relu(int rows, int c, const float *x, const unsigned char *keep, const float *mean,
+                          const float *invstd, const float *gamma, const float *beta, float *y) {
+    for (long long r = 0; r < rows; ++r)
+        for (int col = 0; col < c; ++col) {
+            const size_t o = (size_t)r * c + col;
+            const float sc = gamma ? invstd[col] * gamma[col] : invstd[col];
+            const float t = fmaf(x[o] - mean[col], sc, beta ? beta[col] : 0.f);
+            y[o] = keep[r] ? (t < 0.f ? 0.f : t) : 0.f;
+        }
+}
+
+static float mbn_dx(float g, float xh, float a, float mg, float mgx) { return a * fmaf(-xh, mgx, g - mg); }
+
+/* backward of the plain form from dy, x and y (the values of the tensors, y as the forward
+ * rounded it): dx (float32, before rounding), dgamma = sum g * xhat, dbeta = sum g. */
+void oracle_mbn_backward(int rows, int c, const float *dy, const float *x, const float *y, const unsigned char *keep,
+                         const float *gamma, const float *mean, const float *invstd, float *dx, float *dgamma,
+                         float *dbeta) {
+    const int ty = mbn_ty(c);
+    const long long chunk_rows = (long long)ty * MBN_ROWS * MBN_GROUPS;
+    const long long chunks = rows > 0 ? (rows + chunk_rows - 1) / chunk_rows : 0;
+    const long long per = (chunks + MBN_MERGE_WARPS - 1) / MBN_MERGE_WARPS;
+    float *psg = (float *)malloc(sizeof(float) * (size_t)(chunks + 1));
+    float *psgx = (float *)malloc(sizeof(float) * (size_t)(chunks + 1));
+    float sg[MBN_THREADS], sgx[MBN_THREADS];
+    int cnt = 0;
+    for (long long r = 0; r < rows; ++r) cnt += keep[r] != 0;
+    for (int col = 0; col < c; ++col) {
+        const float mu = mean[col], is = invstd[col];
+        for (long long k = 0; k < chunks; ++k) {
+            for (int t = 0; t < ty; ++t) {
+                sg[t] = 0.f;
+                sgx[t] = 0.f;
+                for (int i = 0; i < MBN_ROWS * MBN_GROUPS; ++i) {
+                    const long long r = k * chunk_rows + t + (long long)i * ty;
+                    if (r >= rows || !keep[r]) continue;
+                    const size_t o = (size_t)r * c + col;
+                    const float g = y[o] > 0.f ? dy[o] : 0.f;
+                    sg[t] = sg[t] + g;
+                    sgx[t] = fmaf(g, (x[o] - mu) * is, sgx[t]);
+                }
+            }
+            for (int s = ty >> 1; s > 0; s >>= 1)
+                for (int t = 0; t < s; ++t) {
+                    sg[t] = sg[t] + sg[t + s];
+                    sgx[t] = sgx[t] + sgx[t + s];
+                }
+            psg[k] = sg[0];
+            psgx[k] = sgx[0];
+        }
+        float wg[MBN_MERGE_WARPS], wgx[MBN_MERGE_WARPS];
+        for (int w = 0; w < MBN_MERGE_WARPS; ++w) {
+            const long long k0 = (long long)w * per < chunks ? (long long)w * per : chunks;
+            const long long k1 = k0 + per < chunks ? k0 + per : chunks;
+            wg[w] = 0.f;
+            wgx[w] = 0.f;
+            for (long long k = k0; k < k1; ++k) {
+                wg[w] = wg[w] + psg[k];
+                wgx[w] = wgx[w] + psgx[k];
+            }
+        }
+        for (int s = MBN_MERGE_WARPS >> 1; s > 0; s >>= 1)
+            for (int w = 0; w < s; ++w) {
+                wg[w] = wg[w] + wg[w + s];
+                wgx[w] = wgx[w] + wgx[w + s];
+            }
+        if (dbeta) dbeta[col] = wg[0];
+        if (dgamma) dgamma[col] = wgx[0];
+        const float a = gamma ? gamma[col] * is : is;
+        const float mg = wg[0] / (float)cnt, mgx = wgx[0] / (float)cnt;
+        for (long long r = 0; r < rows; ++r) {
+            const size_t o = (size_t)r * c + col;
+            const float g = y[o] > 0.f ? dy[o] : 0.f;
+            dx[o] = keep[r] ? mbn_dx(g, (x[o] - mu) * is, a, mg, mgx) : 0.f;
+        }
+    }
+    free(psg);
+    free(psgx);
+}
+
+static uint32_t mbn_key(float v) {
+    if (v != v) return 0xffffffffu;
+    uint32_t u;
+    memcpy(&u, &v, sizeof u);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+/* max-pool of y (b, n, c), the values as rounded to the tensor's dtype: per (cloud, column) the
+ * FIRST real row with the largest key (NaN largest, -0 < +0): out = y there, argmax = the row;
+ * a cloud without a real row gets out 0, argmax -1. */
+void oracle_mbn_max_pool(int b, int n, int c, const float *y, const unsigned char *keep, float *out, int *argmax) {
+    for (long long i = 0; i < b; ++i)
+        for (int col = 0; col < c; ++col) {
+            uint32_t best = 0;
+            int arg = -1;
+            for (int j = 0; j < n; ++j) {
+                if (!keep[i * n + j]) continue;
+                const uint32_t k = mbn_key(y[((size_t)i * n + j) * c + col]);
+                if (k > best) {
+                    best = k;
+                    arg = j;
+                }
+            }
+            out[i * c + col] = arg >= 0 ? y[((size_t)i * n + arg) * c + col] : 0.f;
+            argmax[i * c + col] = arg;
+        }
+}
+
+/* backward of the max-pooled form: g_i = argmax >= 0 && out_i > 0 ? dout_i : 0 and xhat at the
+ * argmax row, dbeta = sum_i g_i and dgamma = fmaf(g_i, xhat_i, .) over ascending clouds i;
+ * dx = keep ? a * fmaf(-xhat, dgamma / cnt, g - dbeta / cnt) : 0 (g = g_i on the argmax row). */
+void oracle_mbn_max_backward(int b, int n, int c, const float *dout, const float *x, const float *out,
+                             const int *argmax, const unsigned char *keep, const float *gamma, const float *mean,
+                             const float *invstd, float *dx, float *dgamma, float *dbeta) {
+    int cnt = 0;
+    for (long long r = 0; r < (long long)b * n; ++r) cnt += keep[r] != 0;
+    for (int col = 0; col < c; ++col) {
+        const float mu = mean[col], is = invstd[col];
+        float sg = 0.f, sgx = 0.f;
+        for (long long i = 0; i < b; ++i) {
+            const int r = argmax[i * c + col];
+            float g = 0.f, xh = 0.f;
+            if (r >= 0 && out[i * c + col] > 0.f) {
+                g = dout[i * c + col];
+                xh = (x[((size_t)i * n + r) * c + col] - mu) * is;
+            }
+            sg = sg + g;
+            sgx = fmaf(g, xh, sgx);
+        }
+        if (dbeta) dbeta[col] = sg;
+        if (dgamma) dgamma[col] = sgx;
+        const float a = gamma ? gamma[col] * is : is;
+        const float mg = sg / (float)cnt, mgx = sgx / (float)cnt;
+        for (long long i = 0; i < b; ++i)
+            for (int j = 0; j < n; ++j) {
+                const size_t o = ((size_t)i * n + j) * c + col;
+                const int r = argmax[i * c + col];
+                const float g = r == j && out[i * c + col] > 0.f ? dout[i * c + col] : 0.f;
+                dx[o] = keep[i * n + j] ? mbn_dx(g, (x[o] - mu) * is, a, mg, mgx) : 0.f;
+            }
+    }
+}

@@ -236,15 +236,18 @@ __global__ void __launch_bounds__(32 * kMbnMergeWarps) mbn_finalize_kernel(
     }
     if (w != 0 || !active) return;
     const float cnt = (float)n;
+    // without a real row the mean is 0 / 0 (NaN) as layers.masked_batch_norm computes it, and so are the variance and
+    // both running statistics
+    const float mu = n > 0 ? mean[0] : __fdiv_rn(0.f, cnt);
     const float var = __fdiv_rn(m2[0], cnt);  // biased
-    save_mean[col] = mean[0];
+    save_mean[col] = mu;
     save_invstd[col] = rsqrtf(__fadd_rn(var, eps));
     if (running_mean) {
         // as layers.masked_batch_norm: momentum, or the cumulative average 1 / num_batches_tracked (already incremented)
         const float f = momentum < 0.f ? __fdiv_rn(1.0f, (float)__ldg(num_batches_tracked)) : momentum;
         const float keepf = __fsub_rn(1.0f, f);
         const float unbiased = __fdiv_rn(__fmul_rn(var, cnt), fmaxf(__fsub_rn(cnt, 1.0f), 1.0f));
-        running_mean[col] = __fadd_rn(__fmul_rn(running_mean[col], keepf), __fmul_rn(mean[0], f));
+        running_mean[col] = __fadd_rn(__fmul_rn(running_mean[col], keepf), __fmul_rn(mu, f));
         running_var[col] = __fadd_rn(__fmul_rn(running_var[col], keepf), __fmul_rn(unbiased, f));
     }
 }
