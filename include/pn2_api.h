@@ -625,6 +625,36 @@ int pn2_virtual_scans(int s, int p, int max_scene, const float* xyz, const int* 
                       float* out_xyz, long long* out_label, float* out_weight, int* lengths, int* point_idx, int* visible,
                       unsigned char* valid, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- dataset text (modelnet_dataset.py:84, part_seg/part_dataset_all_normal.py:88; DESIGN.md §6.18) --------------
+ * F files, concatenated: text (nbytes) u8 on the device, file f at bytes file_off[f] .. file_off[f+1]-1 (file_off
+ * (F+1) int64, device; offsets are clamped to [0, nbytes]).  A file is parsed on the device when every line of it is
+ * exactly ncol fields and a terminator ("\n", "\r\n", or none on the last line); fields are separated by one ','
+ * (PN2_DELIM_COMMA) or by runs of ' ' / '\t' that may also lead and trail the line (PN2_DELIM_WHITESPACE), and a field
+ * is [+-]? (digits [. digits]? | . digits) ([eE] [+-]? digits)? whose significant digits M (leading zeros stripped)
+ * and decimal exponent E satisfy M <= 2^53 and |E| <= 22.  Its rows then hold exactly
+ * np.loadtxt(file, delimiter=...).astype(np.float32) (one row stays a row).  Any other file gets the reason code of
+ * its first line outside that grammar and is the caller's to parse.
+ *
+ * pn2_text_rows_scan: rows (F) int64, the file's lines; status (F) int32, PN2_TEXT_OK or a reason code.
+ * pn2_text_rows_parse: for every file whose status (the scan's, device) is PN2_TEXT_OK, its first min(rows, keep)
+ * rows as float32 to out (out_rows, ncol) from row row_off[f] (int64, device) on; rows past out_rows are not written.
+ * 1 <= ncol <= 64, keep >= 0.  Nothing is allocated or read back.  Invalid arguments return cudaErrorInvalidValue
+ * without a launch. */
+#define PN2_DELIM_WHITESPACE 0
+#define PN2_DELIM_COMMA 1
+#define PN2_TEXT_OK 0
+#define PN2_TEXT_SYNTAX 1   /* a byte or a field outside the grammar ("nan", "inf", "1_0", "1.", ", " ...) */
+#define PN2_TEXT_FIELDS 2   /* a line of other than ncol fields */
+#define PN2_TEXT_BLANK 3    /* an empty or all-blank line */
+#define PN2_TEXT_CR 4       /* a '\r' that does not end a "\r\n" */
+#define PN2_TEXT_COMMENT 5  /* a '#' */
+#define PN2_TEXT_INEXACT 6  /* a value outside the exact conversion: M > 2^53 or |E| > 22 */
+int pn2_text_rows_scan(int num_files, const unsigned char* text, const long long* file_off, long long nbytes, int ncol,
+                       int delim, long long* rows, int* status, void* stream);
+int pn2_text_rows_parse(int num_files, const unsigned char* text, const long long* file_off, long long nbytes, int ncol,
+                        int delim, const int* status, long long keep, const long long* row_off, float* out,
+                        long long out_rows, void* stream);
+
 /* ---- point-cloud rendering (utils/render_balls_so.cpp render_ball, utils/show3d_balls.py; DESIGN.md §6.16) --------
  * Image i of b (out (b, h, w, 3) u8) is what render_ball(h, w, show, len_i, xyz_i, c0, c1, c2, r) writes for cloud i
  * alone on a canvas filled with background[0..2] (a host array of 3 bytes): xyz (b, n, 3) int32 (x the row, y the

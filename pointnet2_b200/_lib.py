@@ -123,6 +123,9 @@ _SIGNATURES = {
     "pn2_render_balls": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P, c_size_t, _P, _P]),
     "pn2_render_balls_counted": (c_int, [c_int, c_int, c_int, c_int, _P, _P, _P, c_int, _P, _P, c_size_t, _P, _P, _P]),
     "pn2_project_points": (c_int, [c_int, c_int, c_int, _P, _P, _P, c_int, _P, c_size_t, _P, _P]),
+    # dataset text files parsed into float32 rows, or marked for the host
+    "pn2_text_rows_scan": (c_int, [c_int, _P, _P, c_longlong, c_int, c_int, _P, _P, _P]),
+    "pn2_text_rows_parse": (c_int, [c_int, _P, _P, c_longlong, c_int, c_int, _P, c_longlong, _P, _P, c_longlong, _P]),
     "pn2_sa_layer_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "pn2_sa_layer_host": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_sa_layer_host_ragged_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),

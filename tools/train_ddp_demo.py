@@ -18,7 +18,7 @@ min(0.99, 1 - 0.5 * 0.5^(samples/200000)).
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 \
         tools/train_ddp_demo.py --steps 20                                      # one rank per GPU
 
-Data is synthetic (no dataset in this image): each cloud is one of `num_class` parametric shapes
+Data is synthetic unless a dataset flag below is given: each cloud is one of `num_class` parametric shapes
 (sphere, box, cylinder, cone, torus ... scaled/rotated/jittered like utils/provider.py), so the
 loss has something to learn and the demo can assert that it goes down.  The part segmentation models
 (part_seg, part_seg_msg) train on workloads.part_shapes instead: (B, N, 6) points with normals, one
@@ -32,6 +32,11 @@ seed derived from (step, rank), with dropout and rotation, and passes the crops'
 shapes.sample_shapes batches drawn on the GPU with a seed derived from (step, rank): ModelNet's augmentation for the
 classification nets, the ShapeNet part recipe (random rows, jitter, normals) for the part nets.  --votes V then prints
 the accuracy of shapes.classify_votes with V rotated votes on a held-out synthetic set (classification nets).
+--modelnet ROOT (cls models), --shapenet-part ROOT (part models) and --scannet ROOT (sem_seg) train on the reference's
+dataset files instead (datasets.load_modelnet / load_shapenet_part / load_scannet): each implies --shape-set or
+--scene-crops, the train split replaces the synthetic set and the test split the held-out one.
+
+    python tools/train_ddp_demo.py --model cls_ssg --modelnet data/modelnet40_normal_resampled --steps 30 --votes 12
 """
 from __future__ import annotations
 
@@ -47,7 +52,7 @@ import torch
 import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from pointnet2_b200 import nets, scene, shapes, workloads as W  # noqa: E402
+from pointnet2_b200 import datasets, nets, scene, shapes, workloads as W  # noqa: E402
 from pointnet2_b200.parallel import shard_batch  # noqa: E402
 
 
@@ -115,7 +120,22 @@ def main() -> None:
     ap.add_argument("--set-points", type=int, default=2048, help="points per shape of the --shape-set sets")
     ap.add_argument("--votes", type=int, default=0,
                     help="with --shape-set (cls models): accuracy of shapes.classify_votes with this many votes")
+    ap.add_argument("--modelnet", default=None, metavar="ROOT",
+                    help="cls models: train on modelnet40_normal_resampled/ at ROOT (implies --shape-set)")
+    ap.add_argument("--shapenet-part", default=None, metavar="ROOT",
+                    help="part models: train on shapenetcore_partanno_segmentation_benchmark_v0_normal/ at ROOT "
+                         "(implies --shape-set)")
+    ap.add_argument("--scannet", default=None, metavar="ROOT",
+                    help="sem_seg: train on scannet_{train,test}.pickle at ROOT (implies --scene-crops)")
     args = ap.parse_args()
+    if args.modelnet and args.model not in ("cls_ssg", "cls_msg", "cls_basic"):
+        raise SystemExit("--modelnet trains a classification model")
+    if args.shapenet_part and args.model not in ("part_seg", "part_seg_msg"):
+        raise SystemExit("--shapenet-part trains a part segmentation model")
+    args.shape_set = args.shape_set or bool(args.modelnet or args.shapenet_part)
+    args.scene_crops = args.scene_crops or bool(args.scannet)
+    if args.modelnet:
+        args.num_class = len(datasets.modelnet_files(args.modelnet, "train")[2])
     if args.shape_set and (args.model == "sem_seg" or args.ragged or args.scene_crops):
         raise SystemExit("--shape-set trains the cls / part models on their own ragged batches (no --ragged)")
     if args.votes and (not args.shape_set or args.model not in ("cls_ssg", "cls_msg", "cls_basic")):
@@ -170,12 +190,21 @@ def main() -> None:
 
     rs = np.random.RandomState(1234)  # the same global batch stream on every rank; each takes its slice
     if args.scene_crops:  # every rank builds the same set; only the crops' seeds differ between ranks
-        rooms = [W.scene_room(60000 + 20000 * k, 500 + k) for k in range(args.rooms)]
-        scenes = scene.SceneSet([r[0] for r in rooms], [r[1] for r in rooms], num_class=21, device=dev)
+        if args.scannet:
+            scenes = datasets.load_scannet(args.scannet, "train", device=dev)
+        else:
+            rooms = [W.scene_room(60000 + 20000 * k, 500 + k) for k in range(args.rooms)]
+            scenes = scene.SceneSet([r[0] for r in rooms], [r[1] for r in rooms], num_class=21, device=dev)
         label_w = scenes.train_label_weights()
         order = np.zeros(0, np.int64)
     if args.shape_set:  # every rank builds the same set; only the batches' seeds differ between ranks
-        if part:
+        if args.shapenet_part:
+            shape_set = datasets.load_shapenet_part(args.shapenet_part, "trainval", device=dev)[0]
+            recipe = dict(subset="random", rotate=False, perturb=False, scale=None, shift=0, with_normals=True)
+        elif args.modelnet:
+            shape_set = datasets.load_modelnet(args.modelnet, "train", npoints=args.num_point, device=dev)[0]
+            recipe = {}
+        elif part:
             pts6, cat, parts = W.part_shapes(args.set_shapes, args.set_points, 77, nets.PART_OFFSETS)
             shape_set = shapes.ShapeSet(list(pts6[:, :, :3]), cat, list(pts6[:, :, 3:]), list(parts), num_class=16,
                                         normalize=False, device=dev)
@@ -261,8 +290,11 @@ def main() -> None:
 
     voted = None
     if args.votes:  # a held-out set of the same kinds of shapes, 16 shapes per call as evaluate.py's BATCH_SIZE
-        pts, cat = synthetic_shapes(args.set_shapes, args.set_points, args.num_class, np.random.RandomState(99))
-        test_set = shapes.ShapeSet(list(pts), cat, num_class=args.num_class, device=dev)
+        if args.modelnet:
+            test_set = datasets.load_modelnet(args.modelnet, "test", npoints=args.num_point, device=dev)[0]
+        else:
+            pts, cat = synthetic_shapes(args.set_shapes, args.set_points, args.num_class, np.random.RandomState(99))
+            test_set = shapes.ShapeSet(list(pts), cat, num_class=args.num_class, device=dev)
         model.eval()
         preds = []
         for b0 in range(0, len(test_set), 16):
@@ -276,8 +308,12 @@ def main() -> None:
 
     scanned = None
     if args.scan_eval:  # train on crops of whole rooms, test on virtual scans (the paper's ScanNet robustness check)
-        held = [W.scene_room(60000 + 20000 * k, 900 + k) for k in range(3)]
-        test_scenes = scene.SceneSet([r[0] for r in held], [r[1] for r in held], num_class=21, device=dev)
+        if args.scannet:
+            test_scenes = datasets.load_scannet(args.scannet, "test", device=dev)
+            held = range(len(test_scenes))
+        else:
+            held = [W.scene_room(60000 + 20000 * k, 900 + k) for k in range(3)]
+            test_scenes = scene.SceneSet([r[0] for r in held], [r[1] for r in held], num_class=21, device=dev)
         views = scene.SCAN_VIEWS
         scans = scene.sample_virtual_scans(test_scenes, torch.arange(len(held) * views, device=dev) // views,
                                            torch.arange(views, device=dev).repeat(len(held)), 1 << 41,
@@ -318,7 +354,10 @@ def main() -> None:
                "steps": args.steps, "loss_first": first, "loss_last": last, "loss_decreased": last < first,
                "weights_identical_across_ranks": same, "ms_per_step_wallclock": 1e3 * float(np.median(steady)),
                "clouds_per_s": args.batch / float(np.median(steady)),
-               "data": ("synthetic room crops" if args.scene_crops else
+               "data": (f"ModelNet at {args.modelnet}" if args.modelnet else
+                        f"ShapeNet-part at {args.shapenet_part}" if args.shapenet_part else
+                        f"ScanNet at {args.scannet}" if args.scannet else
+                        "synthetic room crops" if args.scene_crops else
                         "synthetic part shapes" if part else "synthetic parametric shapes"),
                "deterministic": args.deterministic, "compile": args.compile, "ragged": args.ragged, "scene_crops": args.scene_crops,
                "shape_set": args.shape_set}
