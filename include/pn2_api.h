@@ -684,6 +684,27 @@ int pn2_render_balls_counted(int b, int n, int h, int w, const int* xyz, const f
 int pn2_project_points(int b, int n, int v, const double* xyz, const int* lengths, const double* rotations, int size,
                        void* workspace, size_t workspace_bytes, int* out, void* stream);
 
+/* ---- voxel and pillar grouping (utils/pc_util.py point_cloud_to_volume[_v2], point_cloud_to_image; DESIGN.md
+ * §6.19) ------------------------------------------------------------------------------------------------------------
+ * The cells of a grid over [-radius, radius] as centroids: dims = 3, dim^3 voxels (cell (i*dim + j)*dim + k), or dims =
+ * 2, dim^2 xy pillars (cell i*dim + j).  xyz (b, n, 3) f32, lengths (b,) int32 on the device (NULL: n), clamped to
+ * [0, n]; padding rows are never read.  Along each axis a point's quotient q = (p + radius_f) / voxel_f is computed in
+ * float32 (radius_f, voxel_f: radius and the double 2 * radius / dim, each rounded to float32), and its cell index is q
+ * truncated toward zero when -1 < q < dim; a point with any other (or NaN) quotient is in no cell.  Outputs:
+ * count (b, cells) int32, the rows in the cell; idx (b, cells, nsample) int32, its member rows; grouped (b, cells,
+ * nsample, 3) f64, those rows normalised, (p - ((c + 0.5) * voxel - radius)) / voxel in double for cell coordinate c
+ * (pillars: x and y rounded once to float32, z the raw coordinate).  A cell of count c <= nsample holds its rows
+ * ascending, the last one repeated; c > nsample: the nsample rows of smallest rng_row_key(seed, 9, b*cells + cell, row)
+ * (DESIGN.md §6.10's draws, the seed *seed_dev when seed_dev is not NULL, read on the device, else `seed`), in that
+ * order; c = 0: idx 0, grouped 0.  1 <= nsample <= 16384, b*n < 2^31, b*cells < 2^31.  The workspace is
+ * pn2_voxel_group_workspace_bytes(b, n, dim, dims) bytes, 256-byte aligned (0 = invalid shape).  Same bits on every
+ * run; nothing is read back, so the call can be captured in a CUDA graph.  Invalid arguments (radius not positive
+ * and finite in float32 too) return cudaErrorInvalidValue without a launch. */
+size_t pn2_voxel_group_workspace_bytes(int b, int n, int dim, int dims);
+int pn2_voxel_group(int b, int n, const float* xyz, const int* lengths, int dim, int dims, double radius, int nsample,
+                    long long seed, const long long* seed_dev, int* count, int* idx, double* grouped, void* workspace,
+                    size_t workspace_bytes, void* stream);
+
 /* ---- host-buffer entry point (the reference feeds numpy through feed_dict) ----------------- */
 
 /* One SSG set-abstraction sampling+grouping layer (farthest_point_sample + gather_point +

@@ -17,7 +17,7 @@ INCLUDE = os.path.join(REPO_ROOT, "include")
 BUILD_DIR = os.path.join(PKG_DIR, "build")
 LIB_PATH = os.path.join(PKG_DIR, "libpn2_b200.so")
 
-SOURCES = ["api.cu", "fps.cu", "ball_query.cu", "ball_query_grid.cu", "sa_fused.cu", "knn.cu", "group.cu", "interpolate.cu", "scatter_det.cu", "prob_sample.cu", "masked_bn.cu", "sa_mlp.cu", "fp_mlp.cu", "scene.cu", "crops.cu", "shapes.cu", "vscan.cu", "render.cu", "textparse.cu"]
+SOURCES = ["api.cu", "fps.cu", "ball_query.cu", "ball_query_grid.cu", "sa_fused.cu", "knn.cu", "group.cu", "interpolate.cu", "scatter_det.cu", "prob_sample.cu", "masked_bn.cu", "sa_mlp.cu", "fp_mlp.cu", "scene.cu", "crops.cu", "shapes.cu", "vscan.cu", "render.cu", "textparse.cu", "voxel.cu"]
 HEADERS = [os.path.join(CSRC, "pn2_common.cuh"), os.path.join(CSRC, "mlp_tile.cuh"), os.path.join(CSRC, "knn_warp.cuh"), os.path.join(INCLUDE, "pn2_api.h")]
 
 NVCC_FLAGS = [

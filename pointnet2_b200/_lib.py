@@ -126,6 +126,10 @@ _SIGNATURES = {
     # dataset text files parsed into float32 rows, or marked for the host
     "pn2_text_rows_scan": (c_int, [c_int, _P, _P, c_longlong, c_int, c_int, _P, _P, _P]),
     "pn2_text_rows_parse": (c_int, [c_int, _P, _P, c_longlong, c_int, c_int, _P, c_longlong, _P, _P, c_longlong, _P]),
+    # voxel and pillar grouping: grid cells as centroids of up to nsample member rows each
+    "pn2_voxel_group_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "pn2_voxel_group": (c_int, [c_int, c_int, _P, _P, c_int, c_int, c_double, c_int, c_longlong, _P, _P, _P, _P, _P,
+                                c_size_t, _P]),
     "pn2_sa_layer_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
     "pn2_sa_layer_host": (c_int, [c_int, c_int, c_int, c_float, c_int, _P, _P, _P, _P, _P, _P, c_size_t, _P]),
     "pn2_sa_layer_host_ragged_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),

@@ -85,6 +85,36 @@ def device_lengths(lengths, b: int, n: int, device: torch.device, op: str):
     return host.to(torch.int32).to(device)
 
 
+def as_int(v, name: str, op: str) -> int:
+    """``v`` as a Python int; TypeError for anything but an int or a numpy integer (bool included)."""
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+        raise TypeError(f"{op} expects an integer {name}, got {type(v).__name__}")
+    return int(v)
+
+
+def device_lengths0(lengths, b: int, n: int, device: torch.device, op: str):
+    """(b,) int32 lengths on ``device`` or None.  A CUDA tensor is used as is (the kernels clamp to [0, n]); a host
+    value is checked here (0 <= l <= n) and copied."""
+    if lengths is None:
+        return None
+    if isinstance(lengths, torch.Tensor) and lengths.is_cuda:
+        if lengths.device != device:
+            raise RuntimeError(f"all tensors must be on the same device ({device} vs {lengths.device})")
+        if lengths.dtype not in _INT_DTYPES:
+            raise TypeError(f"{op} expects integer lengths, got {lengths.dtype}")
+        if tuple(lengths.shape) != (b,):
+            raise ValueError(f"{op} expects (batch_size,) lengths shape ({b},), got {tuple(lengths.shape)}")
+        return lengths.to(torch.int32).contiguous()
+    host = np.asarray(lengths.cpu() if isinstance(lengths, torch.Tensor) else lengths)
+    if host.size and not np.issubdtype(host.dtype, np.integer):
+        raise TypeError(f"{op} expects integer lengths, got {host.dtype}")
+    if host.shape != (b,):
+        raise ValueError(f"{op} expects (batch_size,) lengths shape ({b},), got {host.shape}")
+    if b and (host.min() < 0 or host.max() > n):
+        raise ValueError(f"{op} expects 0 <= lengths <= {n} (the padded number of points), got {host.tolist()}")
+    return torch.from_numpy(host.astype(np.int32)).to(device)
+
+
 I31 = 2 ** 31
 SELECT_MAX_ROWS = 16384  # npoints cap of the samplers: their row sort is npoints x 8 bytes of shared memory
 

@@ -141,6 +141,11 @@ __device__ __forceinline__ int cloud_length(const int* __restrict__ lengths, int
     return lengths ? min(max(__ldg(lengths + cloud), 1), n) : n;
 }
 
+// The same with lengths clamped to [0, n], for the ops where an empty cloud is legal (render.cu, voxel.cu).
+__device__ __forceinline__ int cloud_length0(const int* __restrict__ lengths, int cloud, int n) {
+    return lengths ? min(max(__ldg(lengths + cloud), 0), n) : n;
+}
+
 // ---- warp helpers ----------------------------------------------------------------------------
 // Batch-level rule of the uniform-grid ball query, evaluated identically by the grid kernel and by
 // the brute-force kernel (each warp on its own, no barrier): the two kernels run back to back on one
@@ -201,6 +206,23 @@ __device__ __forceinline__ int cta_exclusive_sum_1024(int v, int* s_w) {
         if (lane >= o) winc += t;
     }
     return __shfl_sync(kFullMask, winc - wv, warp) + incl - v;
+}
+
+// Exclusive prefix sum of src[0 .. n) into dst[0 .. n) (dst may be src) by a 1024-thread CTA, 1024 values per pass;
+// returns the total to every thread.  Every thread must call it; s_w (32 ints) and s_carry (one int) are shared scratch.
+__device__ __forceinline__ int cta_exclusive_scan_1024(const int* src, int* dst, int n, int* s_w, int* s_carry) {
+    int carry = 0;
+    for (int base = 0; base < n; base += 1024) {
+        const int k = base + threadIdx.x;
+        const int v = k < n ? src[k] : 0;
+        const int ex = cta_exclusive_sum_1024(v, s_w);
+        if (k < n) dst[k] = carry + ex;
+        if (threadIdx.x == 1023) *s_carry = ex + v;
+        __syncthreads();  // s_carry written; s_w free for the next chunk
+        carry += *s_carry;
+        __syncthreads();
+    }
+    return carry;
 }
 
 // ---- counter-based random draws (DESIGN.md §6.10; crops.cu, shapes.cu, vscan.cu) ----------------------------------
@@ -434,9 +456,10 @@ __device__ __forceinline__ GridGeometry grid_geometry(const float* __restrict__ 
     return g;
 }
 
-// Ascending bitonic sort of 32*K ints held K per lane (element i = register i/32 of lane i%32; K <= KMAX, a power of 2).
-template <int K, int KMAX>
-__device__ __forceinline__ void bitonic_sort_keys(int (&key)[KMAX], int lane) {
+// Ascending bitonic sort of 32*K keys (int or unsigned long long) held K per lane (element i = register i/32 of lane
+// i%32; K <= KMAX, a power of 2).
+template <int K, int KMAX, typename Key>
+__device__ __forceinline__ void bitonic_sort_keys(Key (&key)[KMAX], int lane) {
 #pragma unroll
     for (int size = 2; size <= 32 * K; size <<= 1) {
 #pragma unroll
@@ -447,7 +470,7 @@ __device__ __forceinline__ void bitonic_sort_keys(int (&key)[KMAX], int lane) {
                 for (int j = 0; j < K; ++j) {
                     if ((j & js) == 0) {
                         const bool up = (((32 * j) & size) == 0);  // lane bits are below 32 <= stride < size: direction depends on j only
-                        const int a = key[j], b = key[j | js];
+                        const Key a = key[j], b = key[j | js];
                         const bool sw = up ? (a > b) : (a < b);
                         key[j] = sw ? b : a;
                         key[j | js] = sw ? a : b;
@@ -457,7 +480,7 @@ __device__ __forceinline__ void bitonic_sort_keys(int (&key)[KMAX], int lane) {
 #pragma unroll
                 for (int j = 0; j < K; ++j) {
                     const int i = 32 * j + lane;
-                    const int other = __shfl_xor_sync(kFullMask, key[j], stride);
+                    const Key other = __shfl_xor_sync(kFullMask, key[j], stride);
                     const bool up = ((i & size) == 0), lower = ((lane & stride) == 0);
                     // the lower element of an ascending pair keeps the minimum
                     key[j] = (up == lower) ? min(key[j], other) : max(key[j], other);

@@ -34,12 +34,6 @@ constexpr double kMaxCoord = 1073741824.0;  // 2^30: projected coordinates are c
 __device__ __forceinline__ unsigned bias(int v) { return (unsigned)v ^ 0x80000000u; }
 __device__ __forceinline__ int unbias(unsigned u) { return (int)(u ^ 0x80000000u); }
 
-__device__ __forceinline__ int cloud_len(const int* lengths, int img, int n) {
-    if (!lengths) return n;
-    const int l = __ldg(lengths + img);
-    return l < 0 ? 0 : (l > n ? n : l);
-}
-
 // floor(sqrt(k)) for 0 < k < 2^24 (k and the square root are exact in float up to one step, fixed by the test).  It
 // equals the reference's int(sqrt(double(k))): below 2^24 no sqrt(m^2 - 1) rounds up to m in double.
 __device__ __forceinline__ int isqrt(int k) {
@@ -67,7 +61,7 @@ struct RenderArgs {
 
 __global__ void __launch_bounds__(kRenderThreads) render_zrange_kernel(RenderArgs a) {
     const int img = blockIdx.y;
-    const int len = cloud_len(a.lengths, img, a.n);
+    const int len = cloud_length0(a.lengths, img, a.n);
     const int p0 = blockIdx.x * kZrangeChunk;
     if (p0 >= len) return;
     const int p1 = min(len, p0 + kZrangeChunk);
@@ -91,7 +85,7 @@ template <bool kCount>
 __global__ void __launch_bounds__(kRenderThreads) render_splat_kernel(RenderArgs a, int per_cta,
                                                                       unsigned long long* counters) {
     const int img = blockIdx.y;
-    const int len = cloud_len(a.lengths, img, a.n);
+    const int len = cloud_length0(a.lengths, img, a.n);
     const int p0 = blockIdx.x * per_cta;
     if (p0 >= len) return;
     const int r = a.r, side = 2 * r + 1, r2 = r * r;
@@ -178,7 +172,7 @@ __global__ void __launch_bounds__(kStatsThreads) project_stats_kernel(const doub
     __shared__ double mean[3];
     __shared__ double wmax[kStatsThreads / 32];
     const int b = blockIdx.x, tid = threadIdx.x;
-    const int len = cloud_len(lengths, b, n);
+    const int len = cloud_length0(lengths, b, n);
     const double* x = xyz + (size_t)b * n * 3;
     double sx = 0.0, sy = 0.0, sz = 0.0;
     for (int i = tid; i < len; i += kStatsThreads) {
@@ -230,7 +224,7 @@ __global__ void __launch_bounds__(kProjectThreads) project_points_kernel(const d
     const int b = blockIdx.y;
     const int i = blockIdx.x * kProjectThreads + threadIdx.x;
     if (i >= n) return;
-    const int len = cloud_len(lengths, b, n);
+    const int len = cloud_length0(lengths, b, n);
     double c[3] = {0.0, 0.0, 0.0};
     if (i < len) {
         const double* s = stats + (size_t)b * 4;

@@ -126,18 +126,8 @@ __global__ void __launch_bounds__(1024) scene_scan_kernel(int nblk, int tiles, i
     const int blk = blockIdx.x;
     const int* src = blk < nblk ? hist + (size_t)blk * tiles : tile_core;
     int* dst = blk < nblk ? hist + (size_t)blk * tiles : tile_core_off;
-    int carry = 0;
-    for (int base = 0; base < tiles; base += 1024) {
-        const int k = base + threadIdx.x;
-        const int v = k < tiles ? src[k] : 0;
-        const int ex = cta_exclusive_sum_1024(v, s_w);
-        if (k < tiles) dst[k] = carry + ex;
-        if (threadIdx.x == 1023) s_carry = ex + v;
-        __syncthreads();  // s_carry written; s_w free for the next chunk
-        carry += s_carry;
-        __syncthreads();
-    }
-    if (blk < nblk && threadIdx.x == 0) counts[blk] = carry;
+    const int total = cta_exclusive_scan_1024(src, dst, tiles, s_w, &s_carry);
+    if (blk < nblk && threadIdx.x == 0) counts[blk] = total;
 }
 
 // One warp per tile.  Its points are taken 32 at a time in ascending order; the group's (point, block) pairs are

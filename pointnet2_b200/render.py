@@ -15,39 +15,10 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._tensor import _INT_DTYPES, on_device, ptr, require_cuda, stream_ptr
+from ._tensor import as_int as _int, device_lengths0 as _lengths, on_device, ptr, require_cuda, stream_ptr
 
 MAX_RADIUS = 4096     # pn2_api.h: r <= 4096
 MAX_IMAGES = 65535    # images per call (B, or B * V for show_points)
-
-
-def _int(v, name: str, op: str) -> int:
-    if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
-        raise TypeError(f"{op} expects an integer {name}, got {type(v).__name__}")
-    return int(v)
-
-
-def _lengths(lengths, b: int, n: int, device: torch.device, op: str):
-    """(b,) int32 lengths on ``device`` or None.  A CUDA tensor is used as is (the kernels clamp to [0, n]); a host
-    value is checked here (0 <= l <= n) and copied."""
-    if lengths is None:
-        return None
-    if isinstance(lengths, torch.Tensor) and lengths.is_cuda:
-        if lengths.device != device:
-            raise RuntimeError(f"all tensors must be on the same device ({device} vs {lengths.device})")
-        if lengths.dtype not in _INT_DTYPES:
-            raise TypeError(f"{op} expects integer lengths, got {lengths.dtype}")
-        if tuple(lengths.shape) != (b,):
-            raise ValueError(f"{op} expects (batch_size,) lengths shape ({b},), got {tuple(lengths.shape)}")
-        return lengths.to(torch.int32).contiguous()
-    host = np.asarray(lengths.cpu() if isinstance(lengths, torch.Tensor) else lengths)
-    if host.size and not np.issubdtype(host.dtype, np.integer):
-        raise TypeError(f"{op} expects integer lengths, got {host.dtype}")
-    if host.shape != (b,):
-        raise ValueError(f"{op} expects (batch_size,) lengths shape ({b},), got {host.shape}")
-    if b and (host.min() < 0 or host.max() > n):
-        raise ValueError(f"{op} expects 0 <= lengths <= {n} (the padded number of points), got {host.tolist()}")
-    return torch.from_numpy(host.astype(np.int32)).to(device)
 
 
 def _background(background, op: str) -> np.ndarray:
