@@ -3,7 +3,8 @@ tools/scene_crop_bench.py (test infrastructure only).
 
 draw / unit      the counter-based random draws, in uint64 wrap-around arithmetic
 crop_attempts    the ten attempts of one crop: context members, core mask, voxel count, validity
-oracle_crops     every output field of sample_crops, one crop at a time, vectorised over points; xyz also in float64
+oracle_crops     every output field of sample_crops, one crop at a time, vectorised over points; xyz also in float64;
+                 a crop whose scene index is outside [0, S) is empty, attempt -1
 """
 from __future__ import annotations
 
@@ -94,6 +95,9 @@ def oracle_crops(xyz, label, offsets, lo, hi, label_weights, crop_scene, seed: i
            "core": np.zeros((bsz, npoints), bool), "attempt": np.zeros(bsz, np.int32), "valid": np.zeros(bsz, bool),
            "context": np.zeros(bsz, np.int64)}
     for b, s in enumerate(np.asarray(crop_scene, np.int64)):
+        if not 0 <= s < len(offsets) - 1:  # a scene index outside [0, S): an empty crop, attempt -1
+            out["attempt"][b] = -1
+            continue
         o0, o1 = int(offsets[s]), int(offsets[s + 1])
         pts, lab = xyz[o0:o1], label[o0:o1]
         att = crop_attempts(pts, lab, lo[s][2], hi[s][2], seed, b)
